@@ -2,6 +2,7 @@
 """bench.py — RGBD frames/s integrated (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config C2|C3|C4|C5]
+                    [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[1] (C2: TUM1-shape 640x480, 5 mm voxels, tau 0.04 m, 300 synthetic frames
 per step).  `--config C3` (Replica shape 1200x680 + class labels), `C4` (ScanNet shape, 4 mm, meant for 4 GPUs) and
@@ -16,7 +17,7 @@ configuration (16^3 volume units, stride 4): results are bit-identical to the Op
             overlapped with the kernels) -> `b2v_integrate_batch`; one D2H read of the step's result per step.
   roofline  the dominant kernel of the timed region (`integrate_group_kernel`): achieved = bytes it MOVES
             (2*S*512 per block visit + 16 B per texel of the group's frames) / CUDA-event launch durations, against
-            MEASURED_PEAKS.json; `per_frame_equivalent` is SURVEY.md 8d's formula (2*S*512*A_f + 7*W*H per frame,
+            the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s); `per_frame_equivalent` is SURVEY.md 8d's formula (2*S*512*A_f + 7*W*H per frame,
             what frame-by-frame integration must move) over the same time.  `per_frame_kernel` gives the un-fused
             HBM-bound `integrate_kernel` warm (consecutive frames share L2-resident blocks) and cold (L2 flushed).
   cpu_baseline / --impl reference   the Open3D-order CPU port (oracle/open3d_order.c, OpenMP over volume units, the
@@ -26,6 +27,11 @@ configuration (16^3 volume units, stride 4): results are bit-identical to the Op
 N > 1 (torchrun): the voxel-block hash space is sharded by BlockKeyHash % N; every rank integrates every frame into
 the blocks it owns.  Total work is fixed ("strong" scaling).  The union of the shards is checked against an
 unsharded volume on rank 0 by per-block checksums (`parity`).
+
+--dump-outputs DIR writes what the timed path computed in its last timed step: the volume's block keys and voxel
+planes (a fixed, seeded sample of at most 4096 blocks, sorted by key) as DIR/<name>.npy.  The map is reset after the
+clock sampler comes up, so with the same arguments the volume has integrated the same frames the same number of times
+whenever it is dumped.
 """
 
 from __future__ import annotations
@@ -33,8 +39,10 @@ from __future__ import annotations
 import argparse
 import json
 import os
+import atexit
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -69,7 +77,7 @@ def load_frames(cfg_name: str, n_frames: int, rank: int, world: int, barrier=Non
     n_frames = min(n_frames, cfg.n_frames)
     step = max(cfg.n_frames // n_frames, 1)
     idx = [k * step for k in range(n_frames)]
-    cache = f"/tmp/b2v_frames_{cfg_name}_{n_frames}_{step}.npz"
+    cache = os.path.join(tempfile.gettempdir(), f"b2v_frames_{cfg_name}_{n_frames}_{step}.npz")
     if rank == 0 and not os.path.exists(cache):
         import multiprocessing as mp
         procs = max(1, min(len(os.sched_getaffinity(0)), 48))
@@ -86,7 +94,7 @@ def load_frames(cfg_name: str, n_frames: int, rank: int, world: int, barrier=Non
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md "clocks line")
+# clocks sampling (SM clock, power draw and limit, throttle reasons under load)
 # ------------------------------------------------------------------------------------------------
 
 class ClockSampler:
@@ -98,11 +106,12 @@ class ClockSampler:
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}",
                                           "--format=csv,noheader,nounits", "-lms", "20"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self._kill)   # no sampler outlives the benchmark, even when it fails
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -112,15 +121,19 @@ class ClockSampler:
         for line in self.proc.stdout:
             self.rows.append([x.strip() for x in line.split(",")])
 
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            try:
+                self.proc.wait(timeout=2)
+            except Exception:
+                self.proc.kill()
+
     def stop(self):
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
-        self.proc.terminate()
-        try:
-            self.proc.wait(timeout=2)
-        except Exception:
-            self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        self._kill()
+        sm, mx, plim, reasons = [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
@@ -129,10 +142,12 @@ class ClockSampler:
                 for n, v in zip(names, r[3:7]):
                     if v.lower().startswith("active"):
                         reasons.add(n)
+                plim.append(float(r[7]))
             except Exception:
                 pass
         return {"sm_mhz": float(np.median(sm)) if sm else None,
                 "sm_max_mhz": float(np.max(mx)) if mx else None,
+                "power_limit_w": float(np.max(plim)) if plim else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
@@ -389,10 +404,18 @@ def run_gpu_arm(args, rank, world, local_rank):
         ingest.synchronize()
         return vol.last_frame_stats()  # D2H read of the step's result (the volume's counter block)
 
-    # ---- warm-up (populates the map: steady state afterwards); the clock sampler starts here so that it is up
-    #      (nvidia-smi takes ~0.2 s to deliver its first sample) when the timed regions run ----
+    # ---- the clock sampler starts first so that it is up (nvidia-smi takes ~0.2 s to deliver its first sample) when
+    #      the timed regions run; the GPU is kept under load until it delivers.  How many steps that takes varies, so
+    #      the map is reset afterwards: the timed steps then always follow the same number of integrations ----
     sampler = ClockSampler(local_rank)
     sampler.start()
+    t_load = time.perf_counter()
+    while len(sampler.rows) < 2 and time.perf_counter() - t_load < 1.5:
+        step_resident()
+        torch.cuda.synchronize()
+    vol.reset()
+
+    # ---- warm-up (populates the map: steady state afterwards) ----
     for _ in range(max(args.warmup, 3)):
         step_resident()
     torch.cuda.synchronize()
@@ -402,10 +425,6 @@ def run_gpu_arm(args, rank, world, local_rank):
     # ---- value: inputs resident in HBM, CUDA events on the launching stream ----
     barrier()
     torch.cuda.synchronize()
-    t_load = time.perf_counter()
-    while len(sampler.rows) < 2 and time.perf_counter() - t_load < 1.5:   # under load until the sampler delivers
-        step_resident()
-        torch.cuda.synchronize()
     for _ in range(2):
         step_resident()
     torch.cuda.synchronize()
@@ -421,6 +440,8 @@ def run_gpu_arm(args, rank, world, local_rank):
     ms_max = all_max(e0.elapsed_time(e1))
     upd1, launches1 = vol.counters()
     value = args.steps * F / (ms_max * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, vol.dump_blocks(), rank if world > 1 else None, world)
 
     # ---- e2e: pinned host frames through the public API, H2D (+ NVLink all-gather) inside the timed region ----
     for _ in range(2):
@@ -442,7 +463,8 @@ def run_gpu_arm(args, rank, world, local_rank):
     clocks = sampler.stop()  # sampled under load across the warm-up, the timed regions and the tail above
 
     # ---- roofline: CUDA events around every integrate launch over passes of the same work ----
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # 256 MiB > 126 MB L2
+    l2_mb = torch.cuda.get_device_properties(local_rank).L2_cache_size / 1e6
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # 256 MiB, several times the L2
 
     def profile_pass(overlap, fusion, cold=False):
         vol.set_overlap(overlap)
@@ -476,22 +498,7 @@ def run_gpu_arm(args, rank, world, local_rank):
     cold = profile_pass(False, False, cold=True)
     vol.set_overlap(True)
     vol.set_fusion(True)
-    peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
-    try:
-        mp_ = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        peak, peak_src = float(mp_["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
-    except Exception:
-        pass
-    traffic, traffic_note = None, None
-    if world == 1 and args.config == "C2" and args.frames == 300 and shards == 1:
-        try:
-            prof = json.load(open(os.path.join(ROOT, "profiles", "latest.json")))
-            ent = prof.get("integrate_group_kernel", {})
-            if ent.get("workload") == "C2x300":
-                traffic = ent.get("dram_bytes_per_launch")
-                traffic_note = ent.get("source")
-        except Exception:
-            pass
+    peak, peak_src = 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not a measured peak)"
 
     # ---- parity evidence at N > 1: union of the shards == an unsharded volume (per-block checksums) ----
     parity = None
@@ -593,13 +600,14 @@ def run_gpu_arm(args, rank, world, local_rank):
     n_l = max(situ["launches"], 1)
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
+        "gpu": torch.cuda.get_device_name(local_rank),
         "warmup": max(args.warmup, 3), "ms_per_step": ms_max / args.steps, "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": workload_config(cfg, F, world, {
             "blocks_in_map": int(nb), "active_blocks_per_frame": situ["updates"] / max(situ["frames"], 1),
             "frames_per_fused_group": group,
             "l2": (f"no flush in the timed region: each step streams {nb * 10240 / 1e6:.0f} MB of voxel blocks "
-                   f"(> 126 MB L2) between two visits of the same block"),
+                   f"({l2_mb:.0f} MB L2) between two visits of the same block"),
             "timing": "CUDA events on the launching stream, max over ranks"}),
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(F * H * W * 7),
                 "h2d_bytes_per_step_per_rank": int(h2d_rank), "nvlink_gather_bytes_per_step_per_rank": int(gather_rank),
@@ -612,7 +620,6 @@ def run_gpu_arm(args, rank, world, local_rank):
             "kernel": f"integrate_group_kernel (up to {group} frames applied per block visit)", "bound": "hbm",
             "achieved": situ["moved_gbs"], "peak": peak, "peak_source": peak_src, "unit": "GB/s",
             "frac": situ["moved_gbs"] / peak if peak else None,
-            "traffic": traffic, "traffic_source": traffic_note,
             "bytes_moved_per_launch": situ["moved_bytes"] / n_l,
             "avg_launch_us": 1e3 * situ["integ_ms"] / n_l,
             "frames_per_launch": situ["frames"] / n_l,
@@ -622,7 +629,7 @@ def run_gpu_arm(args, rank, world, local_rank):
                 "algorithmic_bytes_per_launch": situ["survey_bytes"] / n_l,
                 "note": "SURVEY.md 8d formula 2*S*512*A_f + 7*W*H summed over the frames of a launch = what "
                         "frame-by-frame integration must move; the fused kernel reads / writes a block once per group, "
-                        "so this is NOT bytes it moves (it is limited by instruction issue, see profiles/)"},
+                        "so this is NOT bytes it moves"},
             "measured": "in situ: CUDA events around every launch in the timed-region schedule "
                         "(allocate kernels of the next group run beside it)",
             "allocate_group_kernel_avg_us_in_situ": 1e3 * situ["alloc_ms"] / n_l,
@@ -631,7 +638,7 @@ def run_gpu_arm(args, rank, world, local_rank):
                 "bound": "hbm",
                 "warm_l2": {"achieved": iso["gbs"], "frac": iso["gbs"] / peak if peak else None,
                             "avg_launch_us": 1e3 * iso["integ_ms"] / max(iso["launches"], 1),
-                            "note": "consecutive frames: most of a frame's blocks are still in the 126 MB L2"},
+                            "note": f"consecutive frames: most of a frame's blocks are still in the {l2_mb:.0f} MB L2"},
                 "cold_l2": {"achieved": cold["gbs"], "frac": cold["gbs"] / peak if peak else None,
                             "avg_launch_us": 1e3 * cold["integ_ms"] / max(cold["launches"], 1),
                             "note": "256 MiB written between frames: every block comes from HBM"},
@@ -648,6 +655,26 @@ def run_gpu_arm(args, rank, world, local_rank):
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_MAX_BLOCKS = 4096   # 4096 blocks x 10 KiB of voxel planes: 42 MB in all, whatever the number of ranks
+
+
+def dump_outputs(out_dir, dump, rank=None, world=1):
+    """Write a block dump (what `dump_blocks()` hands a caller) as DIR/<name>.npy: block keys (float64, exact) and
+    the five voxel planes (float32), sorted by key; above DUMP_MAX_BLOCKS / world blocks per rank a fixed, seeded
+    sample of them."""
+    os.makedirs(out_dir, exist_ok=True)
+    keys = dump["keys"]
+    order = np.lexsort((keys[:, 2], keys[:, 1], keys[:, 0]))
+    cap = DUMP_MAX_BLOCKS // world
+    if len(order) > cap:
+        order = order[np.sort(np.random.default_rng(0).choice(len(order), cap, replace=False))]
+    sfx = "" if rank is None else f"_rank{rank}"
+    np.save(os.path.join(out_dir, f"num_blocks{sfx}.npy"), np.array([len(keys)], np.float64))
+    np.save(os.path.join(out_dir, f"block_keys{sfx}.npy"), keys[order].astype(np.float64))
+    for i, name in enumerate(("tsdf", "weight", "red", "green", "blue")):
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), np.ascontiguousarray(dump["vox"][order, i]))
 
 
 def grid_leg(cfg, depth, color, Tcw, d_dev, c_dev, peak, device):
@@ -723,6 +750,8 @@ def main():
     ap.add_argument("--chunk", type=int, default=64, help="frames per ingest chunk (upload + all-gather granularity)")
     ap.add_argument("--mesh", action="store_true", help="N > 1: also time the distributed mesh extraction")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the volume after the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     ap.add_argument("--shard-of", type=int, default=0,
                     help="diagnostic (N=1 only): act as rank 0 of a --shard-of-way sharded job on one GPU; ranks share "
                          "nothing, so this is the per-rank work of that job")

@@ -1,7 +1,7 @@
-"""pyslam_b200 — B200-native volumetric TSDF integrator behind pySLAM's dense-mapping plugin API.
+"""pyslam_b200 — H100-native volumetric TSDF integrator behind pySLAM's dense-mapping plugin API.
 
 Scope: the hot path of SURVEY.md §8 only (voxel-block hash allocation, projective TSDF + colour
-update, per-block marching cubes, and the point-average compat grid).  `csrc/` holds the sm_100a
+update, per-block marching cubes, and the point-average compat grid).  `csrc/` holds the sm_90a
 CUDA kernels and the C ABI (include/b2v.h); the Python modules mirror the reference's interface.
 """
 

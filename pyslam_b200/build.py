@@ -1,7 +1,7 @@
-"""Build `pyslam_b200/libb2v.so` (the C-ABI library of include/b2v.h) in-tree with nvcc for sm_100a.
+"""Build `pyslam_b200/libb2v.so` (the C-ABI library of include/b2v.h) in-tree with nvcc for sm_90a (H100).
 
-nvcc cross-compiles without a GPU; the resulting .so travels with the repo snapshot to the GPU
-box.  `python -m pyslam_b200.build` or `pyslam_b200.build.build()`.
+nvcc cross-compiles without a GPU; the library is built once, on any machine with the CUDA
+toolkit, and loaded on the GPU host.  `python -m pyslam_b200.build` or `pyslam_b200.build.build()`.
 """
 
 from __future__ import annotations
@@ -18,7 +18,7 @@ SOURCES = ["b2v_api.cu", "b2v_tsdf.cu", "b2v_mesh.cu", "b2v_grid.cu", "b2v_prep.
 HEADERS = ["b2v_device.cuh", "b2v_internal.h", "b2v_scan.cuh", "mc_tables.h", "../../include/b2v.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     # IEEE everywhere: no fast-math, no flush-to-zero, correctly rounded div/sqrt; FMA contraction is
     # left on for non-contract code only (contract code uses explicit-rounding intrinsics)
@@ -43,7 +43,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every .cu for sm_100a and link libb2v.so.  Returns the library path."""
+    """Compile every .cu for sm_90a and link libb2v.so.  Returns the library path."""
     if not force and not _stale():
         return LIB
     nvcc = _nvcc()
@@ -70,7 +70,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         f.write("\n".join(log))
     if verbose:
         print("\n".join(log))
-    cmd = [nvcc, "-ccbin", ccbin, "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc, "-ccbin", ccbin, "-shared", "-gencode", "arch=compute_90a,code=sm_90a",
            *objs, "-o", LIB]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
     if r.returncode != 0:

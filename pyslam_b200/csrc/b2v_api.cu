@@ -280,14 +280,15 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
                                 v->compute));
     int rc = volume_clear_device(v);
     if (rc != B2V_OK) return rc;
-    const int sms = b2v_device_sm_count(cfg->device);
+    int sms = 0;
+    B2V_CUDA(v, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
     // persistent grid: exactly one wave of resident CTAs (B2V_INT_CTAS_PER_SM overrides, for tuning)
     int per_sm = integrate_max_resident_ctas_per_sm();
     if (const char *e = std::getenv("B2V_INT_CTAS_PER_SM")) {
         const int n = std::atoi(e);
         if (n >= 1 && n <= 32) per_sm = n;
     }
-    v->grid_ctas = (sms > 0 ? sms : 148) * per_sm;
+    v->grid_ctas = sms * per_sm;
     v->sm_count = sms;
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     return B2V_OK;
@@ -860,7 +861,7 @@ extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float 
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[2], cs));
-        B2V_CUDA(v, launch_integrate_group(args, v->table, v->meta, buf, v->grid_ctas, cs));
+        B2V_CUDA(v, launch_integrate_group(args, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[3], cs));
         B2V_CUDA(v, cudaEventRecord(v->ev_group_done[buf], cs));
         v->launches += 3;
@@ -1208,7 +1209,7 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     if (rc != B2V_OK) return rc;
     v->mb.n_blocks = nb;
     cudaStream_t cs = v->compute;
-    const int sms = v->sm_count > 0 ? v->sm_count : 148;
+    const int sms = v->sm_count;
     if (mesh) {
         B2V_CUDA(v, launch_mesh_classify(v->table, v->meta, v->mb, sms, cs));
     } else {

@@ -1,4 +1,4 @@
-// b2v_device.cuh — device-side building blocks shared by the sm_100a kernels.
+// b2v_device.cuh — device-side building blocks shared by the sm_90a kernels.
 //
 // Key arithmetic follows pySLAM's cpp/volumetric bit for bit:
 //   voxel coord  v = (int32)floor(x * inv_voxel_size)            voxel_hashing.h:69-75
@@ -25,7 +25,7 @@ constexpr uint32_t kPending = 0xFFFFFFFEu;  // inserted in this launch, pool ind
 constexpr uint32_t kNoBlock = 0xFFFFFFFDu;  // pool overflowed: key present but no storage
 
 // Open-addressing table: entry = {key.x, key.y, key.z, pool index}.  16-byte entries are read
-// with one LDG.128 and inserted with one 128-bit CAS (ATOMG.E.CAS.128 on sm_100a).
+// with one LDG.128 and inserted with one 128-bit CAS (ATOMG.E.CAS.128 on sm_90a).
 struct HashTable {
     uint4 *entries;
     uint32_t *stamp;  // frame id of the last frame that touched the slot

@@ -1,4 +1,4 @@
-// b2v_grid.cu — point-average voxel block grid (pySLAM's own `volumetric.VoxelBlockGrid`), sm_100a.
+// b2v_grid.cu — point-average voxel block grid (pySLAM's own `volumetric.VoxelBlockGrid`), sm_90a.
 //
 // Replaces VoxelBlockGridT<VoxelData>::integrate_raw / get_voxels / remove_low_count_voxels
 // (cpp/volumetric/voxel_block_grid.hpp:115-136, 524-614, 625-647, 717-819).  Per voxel the

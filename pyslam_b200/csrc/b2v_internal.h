@@ -165,7 +165,7 @@ int integrate_max_resident_ctas_per_sm();
 cudaError_t launch_selftest_division(unsigned long long *d_bad, uint64_t pairs, cudaStream_t stream);
 // fused update of a group of frames (each block is read and written once per group)
 cudaError_t launch_integrate_group(const GroupArgs &args, const HashTable &table, const PoolMeta &meta,
-                                   int group_buf, int grid_ctas, cudaStream_t stream);
+                                   int group_buf, int grid_ctas, int sm_count, cudaStream_t stream);
 // hashes[i] = BlockKeyHash(block_keys[i])
 cudaError_t launch_block_hashes(const int4 *block_keys, uint64_t *hashes, uint32_t n,
                                 cudaStream_t stream);

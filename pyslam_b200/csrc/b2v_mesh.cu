@@ -1,4 +1,4 @@
-// b2v_mesh.cu — per-block marching-cubes triangle emission (sm_100a).
+// b2v_mesh.cu — per-block marching-cubes triangle emission (sm_90a).
 //
 // Replaces Open3D ScalableTSDFVolume::ExtractTriangleMesh / ExtractPointCloud, called from
 // pyslam/dense/volumetric_integrator_tsdf.py:239,246,260,267.  Semantics (SURVEY.md A.4):

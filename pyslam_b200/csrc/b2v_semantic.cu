@@ -1,4 +1,4 @@
-// b2v_semantic.cu — semantic voxel-block grids on sm_100a (SURVEY.md §8(f) rank 2, Appendix D).
+// b2v_semantic.cu — semantic voxel-block grids on sm_90a (SURVEY.md §8(f) rank 2, Appendix D).
 //
 // Replaces, for the `integrate(points, colors, class_ids, instance_ids, depths)` path and its read-outs,
 //   VoxelBlockSemanticGrid               = VoxelBlockSemanticGridT<VoxelSemanticData>               (voting)

@@ -82,7 +82,7 @@ def make_integrator_class(Base, api):
     TaskType = api.VolumetricIntegrationTaskType
 
     class VolumetricIntegratorB200(Base):
-        """TSDF + colour integration on a B200 (replaces VolumetricIntegratorTsdf + Open3D)."""
+        """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):

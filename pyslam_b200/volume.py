@@ -67,7 +67,7 @@ class PointCloud:
 
 
 class B200TsdfVolume:
-    """B200-native TSDF + colour volume on 8^3 voxel blocks in a GPU hash table.
+    """H100-native TSDF + colour volume on 8^3 voxel blocks in a GPU hash table.
 
     Parameters mirror `o3d.pipelines.integration.ScalableTSDFVolume(voxel_length, sdf_trunc, ...)`
     as constructed at volumetric_integrator_tsdf.py:104-108, plus the depth truncation the reference
@@ -447,7 +447,7 @@ class BoundingBox3D:
 
 class TBBUtils:
     """`volumetric.TBBUtils` of the reference module (cpp/volumetric/volumetric_module.cpp:43-50): the integrators call
-    `TBBUtils.set_max_threads(n)` to size the CPU thread pool of the voxel grids.  The B200 grids have no CPU pool; the
+    `TBBUtils.set_max_threads(n)` to size the CPU thread pool of the voxel grids.  The GPU grids have no CPU pool; the
     value is kept so that `get_max_threads()` answers what was set."""
     _max_threads = 0
 

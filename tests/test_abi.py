@@ -28,7 +28,7 @@ def test_header_symbols_all_exported():
     assert L.b2v_version() >= 100
 
 
-def test_library_is_sm100a_and_uses_128bit_cas():
+def test_library_is_sm90a_and_uses_128bit_cas():
     import shutil
     import subprocess
     from pyslam_b200 import _lib
@@ -36,7 +36,7 @@ def test_library_is_sm100a_and_uses_128bit_cas():
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out and "sm_100" not in out
     sass = subprocess.run([cuobjdump, "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert "allocate_kernel" in sass and "integrate_kernel" in sass
     assert "ATOMG.E.CAS.128" in sass  # 16-byte hash-table entries are inserted with one 128-bit CAS

@@ -155,6 +155,7 @@ def _blobs(rng):
     return out
 
 
+@needs_ref
 def test_pca_oriented_box_equals_the_compiled_reference():
     """The product's OrientedBoundingBox3D.compute_from_points (numpy) against the boxes the UNMODIFIED reference
     attaches to its object segments (bounding_boxes_3d.cpp:373-556 via voxel_block_semantic_grid.hpp:248-252):
@@ -176,7 +177,10 @@ def test_pca_oriented_box_equals_the_compiled_reference():
                        [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
         assert np.abs(np.abs(np.sum(b.R * Rr, axis=0)) - 1.0).max() < 1e-9     # same axes, sign aside
         assert s["class_id"] == s["id"] + 10 and len(s["points"]) > 1000
-    # degenerate inputs
+
+
+def test_pca_oriented_box_of_degenerate_inputs():
+    from pyslam_b200.volume import OrientedBoundingBox3D
     assert np.array_equal(OrientedBoundingBox3D.compute_from_points(np.zeros((0, 3))).size, np.zeros(3))
     b1 = OrientedBoundingBox3D.compute_from_points([[1.0, 2.0, 3.0]])
     assert np.array_equal(b1.center, [1.0, 2.0, 3.0]) and np.array_equal(b1.size, np.zeros(3))

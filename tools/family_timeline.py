@@ -1,5 +1,5 @@
-"""Run every kernel family once or twice on C2-shape frames: the command the ncu captures of the grid_*, sem_*,
-remap_*, shadow_*, depth_u16_*, mesh_* and lambda kernels are taken from (profiles/).
+"""Run every kernel family once or twice on C2-shape frames, a short timeline of the grid_*, sem_*, remap_*,
+shadow_*, depth_u16_*, mesh_* and lambda kernels for a profiler.
     python tools/family_timeline.py"""
 import os
 import sys
