@@ -51,6 +51,7 @@ void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], 
     I.inv_tau = 1.0f / g.tau;
     I.W = W;
     I.tex = nullptr;
+    I.lam = nullptr;
     p->inv_fx = 1.0f / I.fxf;
     p->inv_fy = 1.0f / I.fyf;
     p->inv_vs = 1.0f / g.vs;  // voxel_block_grid.hpp:6
@@ -111,11 +112,9 @@ struct b2v_volume {
     bool inputs_fenced = false;          // batch call: device inputs already ordered before the alloc stream
     bool fuse = true;                    // b2v_integrate_batch fuses groups of up to kMaxGroup frames
     int group_frames = 16;               // frames per fused group (1..kMaxGroup), b2v_set_group_size
-    LambdaMap lam_map{};
-    bool lam_map_ok = false;
     cudaEvent_t input_event = nullptr;   // b2v_set_input_event: readiness of the next batch's device inputs
     bool rings_stale = false;            // a fused batch advanced frame_id: the per-frame ring counters must be re-armed
-    float4 *d_gtex[kGroupBufs * kMaxGroup] = {};  // texel images of the group buffers
+    Texel *d_gtex[kGroupBufs * kMaxGroup] = {};   // texel images of the group buffers
     size_t gtex_pixels = 0;
     uint32_t group_id = 0;
     cudaEvent_t ev_galloc[kGroupBufs] = {}, ev_group_done[kGroupBufs] = {};
@@ -129,7 +128,6 @@ struct b2v_volume {
     // TMA descriptors are cached per image address (encoding costs ~1 us of host time each)
     std::unordered_map<uintptr_t, FrameMaps> map_cache;
     int map_H = 0, map_W = 0;
-    const float *map_lam = nullptr;
     cudaEvent_t ev_in = nullptr, ev_alloc_done[kActiveRing] = {}, ev_int_done[kActiveRing] = {};
     // raw 16-bit depth input (b2v_integrate_u16 / b2v_integrate_batch_u16): uploaded as is, widened on the device
     uint16_t *d_depth16[kStage] = {};   // same slot layout as d_depth; allocated on first use
@@ -137,8 +135,8 @@ struct b2v_volume {
     float in_u16_scale = 0.0f;          // > 0 while a *_u16 entry point runs: `depth` pointers are uint16_t
     float *d_depth[kStage] = {};
     uint8_t *d_color[kStage] = {};
-    float4 *d_texel[kStage] = {};   // packed {depth, lambda, rgbx} frames read by integrate_kernel
-    float *d_lambda = nullptr;      // lambda image of the cached intrinsics
+    Texel *d_texel[kStage] = {};    // texel images of the frames read by integrate_kernel
+    float *d_lambda = nullptr;      // lambda image of the cached intrinsics, read by the update kernels
     double lam_K[4] = {0, 0, 0, 0};
     int lam_H = 0, lam_W = 0;
     size_t stage_pixels = 0;
@@ -316,7 +314,7 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaFree(v->d_rdepth[0]);
     cudaFree(v->d_rcolor[0]);
     cudaFree(v->d_depth16[0]);
-    for (float4 *t : v->d_gtex) cudaFree(t);
+    for (Texel *t : v->d_gtex) cudaFree(t);
     for (int b = 0; b < kGroupBufs; ++b) {
         if (v->ev_galloc[b]) cudaEventDestroy(v->ev_galloc[b]);
         if (v->ev_group_done[b]) cudaEventDestroy(v->ev_group_done[b]);
@@ -396,10 +394,8 @@ extern "C" int b2v_reset(b2v_volume *v) {
 
 static int ensure_staging(b2v_volume *v, size_t pixels) {
     if (pixels <= v->stage_pixels) return B2V_OK;
-    B2V_CUDA(v, cudaStreamSynchronize(v->compute));
-    B2V_CUDA(v, cudaStreamSynchronize(v->copy));
-    B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
-    if (v->last_stream) B2V_CUDA(v, cudaStreamSynchronize(v->last_stream));
+    // the lambda image freed below is read by update kernels on the library's streams and on callers' streams
+    B2V_CUDA(v, cudaDeviceSynchronize());
     // raw staging slots are carved out of two contiguous allocations, so the frames of a group (which
     // are contiguous in the caller's arrays) upload with ONE copy per image type
     cudaFree(v->d_depth[0]);
@@ -421,7 +417,7 @@ static int ensure_staging(b2v_volume *v, size_t pixels) {
         v->d_depth[s] = dbase + pixels * s;
         v->d_color[s] = cbase + pixels * 3 * s;
         if (s >= kGroupStage)  // texel images of the per-frame path (the group buffers have their own)
-            B2V_CUDA(v, cudaMalloc(&v->d_texel[s], pixels * sizeof(float4)));
+            B2V_CUDA(v, cudaMalloc(&v->d_texel[s], pixels * sizeof(Texel)));
     }
     cudaFree(v->d_lambda);
     v->d_lambda = nullptr;
@@ -442,15 +438,12 @@ static int grow_profile_events(b2v_volume *v, size_t need) {
 
 // cached TMA descriptors of a frame (keyed by the depth image address; colour address is checked)
 static const FrameMaps *frame_maps(b2v_volume *v, const float *d_depth, const uint8_t *d_color, int H, int W) {
-    if (!v->use_tma || !tma_tiles_usable(W, v->cfg.depth_stride, d_depth, d_color, v->d_lambda)) return nullptr;
-    if (v->map_H != H || v->map_W != W || v->map_lam != v->d_lambda || v->map_cache.size() > 4096) {
+    if (!v->use_tma || !tma_tiles_usable(W, v->cfg.depth_stride, d_depth, d_color)) return nullptr;
+    if (v->map_H != H || v->map_W != W || v->map_cache.size() > 4096) {
         v->map_cache.clear();
         v->map_H = H;
         v->map_W = W;
-        v->map_lam = v->d_lambda;
-        v->lam_map_ok = encode_lambda_map(&v->lam_map, v->d_lambda, H, W, 32);
     }
-    if (!v->lam_map_ok) return nullptr;
     auto it = v->map_cache.find(reinterpret_cast<uintptr_t>(d_depth));
     if (it != v->map_cache.end() && it->second.color_ptr == d_color) return &it->second;
     FrameMaps m;
@@ -567,9 +560,9 @@ static int integrate_frame(b2v_volume *v, const float *depth, const uint8_t *col
     FrameParams P;
     fill_frame_params(&P, K, Tcw, height, width, v->geo, v->frame_id + 1);
     if (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0) {
-        if (v->overlap) {  // the lambda image is read by allocate kernels that may still be in flight
-            B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
-        }
+        // the lambda image is read by update kernels of earlier frames that may still run, on the library's streams
+        // or on a caller's; new intrinsics are rare, so the whole device is drained before the image is rewritten
+        B2V_CUDA(v, cudaDeviceSynchronize());
         B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
         std::memcpy(v->lam_K, K, sizeof(v->lam_K));
         v->lam_H = height;
@@ -584,10 +577,11 @@ static int integrate_frame(b2v_volume *v, const float *depth, const uint8_t *col
         v->prof_used += 4;
         B2V_CUDA(v, cudaEventRecord(pe[0], as));
     }
-    float4 *tex = v->d_texel[s];
+    Texel *tex = v->d_texel[s];
     P.I.tex = tex;
-    B2V_CUDA(v, launch_allocate(P, d_depth, d_color, v->d_lambda, tex, v->table, v->meta, ring,
-                                frame_maps(v, d_depth, d_color, height, width), &v->lam_map, as));
+    P.I.lam = v->d_lambda;
+    B2V_CUDA(v, launch_allocate(P, d_depth, d_color, tex, v->table, v->meta, ring,
+                                frame_maps(v, d_depth, d_color, height, width), as));
     if (staged || u16) B2V_CUDA(v, cudaEventRecord(v->ev_free[s], as));  // the raw frame is consumed by allocate only
     v->launches += 1;
     v->frame_id += 1;
@@ -702,10 +696,10 @@ static int ensure_group_buffers(b2v_volume *v, size_t pixels) {
     if (pixels <= v->gtex_pixels) return B2V_OK;
     B2V_CUDA(v, cudaDeviceSynchronize());
     v->gtex_pixels = 0;  // stays 0 if an allocation below fails
-    for (float4 *&t : v->d_gtex) {
+    for (Texel *&t : v->d_gtex) {
         cudaFree(t);
         t = nullptr;
-        B2V_CUDA(v, cudaMalloc(&t, pixels * sizeof(float4)));
+        B2V_CUDA(v, cudaMalloc(&t, pixels * sizeof(Texel)));
     }
     v->gtex_pixels = pixels;
     return B2V_OK;
@@ -815,18 +809,20 @@ extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float 
                 aargs.frame_id0 = v->frame_id + 1;
             }
             if (k == 0 && (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0)) {
-                if (v->overlap) B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
+                // as in integrate_frame: update kernels of earlier batches may still read the lambda image
+                B2V_CUDA(v, cudaDeviceSynchronize());
                 B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
                 std::memcpy(v->lam_K, K, sizeof(v->lam_K));
                 v->lam_H = height;
                 v->lam_W = width;
                 v->launches += 1;
             }
-            float4 *tex = v->d_gtex[buf * kMaxGroup + k];
+            Texel *tex = v->d_gtex[buf * kMaxGroup + k];
             aargs.depth[k] = d_depth;
             aargs.color[k] = d_color;
             aargs.tex[k] = tex;
             P.I.tex = tex;
+            P.I.lam = v->d_lambda;
             args.f[k] = P.I;
             v->frame_id += 1;
         }
@@ -855,8 +851,7 @@ extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float 
             v->prof_int_launches += 1;
             B2V_CUDA(v, cudaEventRecord(pe[0], as));
         }
-        aargs.lmap = v->lam_map;
-        B2V_CUDA(v, launch_allocate_group(aargs, v->d_lambda, v->table, v->meta, as));
+        B2V_CUDA(v, launch_allocate_group(aargs, v->table, v->meta, as));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));

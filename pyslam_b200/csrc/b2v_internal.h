@@ -10,6 +10,25 @@
 
 namespace b2v {
 
+// Texel of the update kernels, one per pixel of a frame, packed by the allocate kernels: {depth, r | g << 8 | b << 16}.
+// depth is 0 where the pixel is invalid (0, or beyond depth_trunc).  The depth-to-camera-distance multiplier is not
+// in the texel: the update kernels read it from the lambda image at the same pixel (one image per set of intrinsics).
+struct alignas(8) Texel {
+    float depth;
+    uint32_t rgb;
+};
+__device__ __forceinline__ Texel make_texel(float depth, uint8_t r, uint8_t g, uint8_t b) {
+    return Texel{depth, static_cast<uint32_t>(r) | (static_cast<uint32_t>(g) << 8) | (static_cast<uint32_t>(b) << 16)};
+}
+__device__ __forceinline__ Texel load_texel(const Texel *p) {  // read-only path, one 8-byte load
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p));
+    return Texel{__uint_as_float(u.x), u.y};
+}
+// colour channel c (0 = r, 1 = g, 2 = b) as float32, exactly: (2^23 + c) - 2^23
+__device__ __forceinline__ float texel_channel(const Texel &t, int c) {
+    return __fsub_rn(__uint_as_float(0x4B000000u | ((t.rgb >> (8 * c)) & 0xFFu)), 8388608.0f);
+}
+
 // Constants of the projective update of one frame (Open3D UniformTSDFVolume::IntegrateWithDepthToCameraDistance-
 // Multiplier): passed in kernel-parameter space, so the kernels read them as constant-bank operands.
 struct IntFrame {
@@ -19,7 +38,8 @@ struct IntFrame {
     float safe_w, safe_h;   // W - 0.0001f, H - 0.0001f
     float tau, inv_tau;
     int32_t W;
-    const float4 *tex;      // packed {valid depth | 0, lambda, rgbx, 0} texels of the frame
+    const Texel *tex;       // texels of the frame
+    const float *lam;       // lambda image of the frame's intrinsics, same pixel index as tex
 };
 
 // camera -> world of one frame, float64 (allocation samples)
@@ -121,26 +141,22 @@ VolumeConsts volume_consts(const VolumeGeometry &g);
 // ---- kernels (b2v_tsdf.cu) ----
 // lambda image (Open3D's depth-to-camera-distance multiplier) for the current intrinsics
 cudaError_t launch_lambda(const FrameParams &p, float *lam, cudaStream_t stream);
-// TMA descriptors of one frame's images (2-D tiled: depth f32, colour u8 x3 interleaved, lambda f32)
+// TMA descriptors of one frame's images (2-D tiled: depth f32, colour u8 x3 interleaved)
 struct FrameMaps {
     alignas(64) CUtensorMap depth;
     alignas(64) CUtensorMap color;
     const void *color_ptr = nullptr;  // host-side cache validation only
 };
-struct LambdaMap {
-    alignas(64) CUtensorMap lam;
-};
 // TMA tile staging needs 16-byte aligned bases and row pitches (W % 16 == 0) and the 32x32 tile
-bool tma_tiles_usable(int W, int stride, const void *depth, const void *color, const void *lam);
+bool tma_tiles_usable(int W, int stride, const void *depth, const void *color);
 // returns false if the driver entry point is unavailable or encoding fails
 bool encode_frame_maps(FrameMaps *maps, const float *depth, const uint8_t *color, int H, int W, int tile);
-bool encode_lambda_map(LambdaMap *map, const float *lam, int H, int W, int tile);
-// frame packing ({valid depth, lambda, rgbx} texels) + allocation + touched-set of one frame;
+// frame packing (texels) + allocation + touched-set of one frame;
 // zeroes the next frame's ring counters.  maps != nullptr: the image tiles are staged into shared
 // memory with TMA (cp.async.bulk.tensor.2d); nullptr: plain loads.
 cudaError_t launch_allocate(const FrameParams &p, const float *depth, const uint8_t *color,
-                            const float *lam, float4 *texels, const HashTable &table,
-                            const PoolMeta &meta, int ring, const FrameMaps *maps, const LambdaMap *lmap,
+                            Texel *texels, const HashTable &table, const PoolMeta &meta, int ring,
+                            const FrameMaps *maps,
                             cudaStream_t stream);
 // projective TSDF + colour update of every block touched by the frame
 cudaError_t launch_integrate(const FrameParams &p, const VolumeConsts &vc, const HashTable &table,
@@ -151,14 +167,13 @@ struct GroupAllocArgs {
     FramePose pose[kMaxGroup];
     const float *depth[kMaxGroup];
     const uint8_t *color[kMaxGroup];
-    float4 *tex[kMaxGroup];
+    Texel *tex[kMaxGroup];
     FrameMaps maps[kMaxGroup];
-    LambdaMap lmap;
     uint32_t frame_id0;            // frame id of the group's first frame
     int32_t count, use_tma;
 };
 static_assert(sizeof(GroupAllocArgs) < 32000, "kernel parameter space");
-cudaError_t launch_allocate_group(const GroupAllocArgs &args, const float *lam, const HashTable &table,
+cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &table,
                                   const PoolMeta &meta, cudaStream_t stream);
 int integrate_max_resident_ctas_per_sm();
 // d_bad[0]: reciprocals (3 x 2^23 inputs), d_bad[1]: quotients (`pairs` inputs) whose fast path differs from IEEE
