@@ -50,6 +50,7 @@ void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], 
     I.tau = g.tau;
     I.inv_tau = 1.0f / g.tau;
     I.W = W;
+    I.pixels = W * H;
     I.tex = nullptr;
     I.lam = nullptr;
     p->inv_fx = 1.0f / I.fxf;
@@ -416,12 +417,16 @@ static int ensure_staging(b2v_volume *v, size_t pixels) {
     for (int s = 0; s < kStage; ++s) {
         v->d_depth[s] = dbase + pixels * s;
         v->d_color[s] = cbase + pixels * 3 * s;
-        if (s >= kGroupStage)  // texel images of the per-frame path (the group buffers have their own)
-            B2V_CUDA(v, cudaMalloc(&v->d_texel[s], pixels * sizeof(Texel)));
+        if (s >= kGroupStage) {  // texel images of the per-frame path (the group buffers have their own)
+            B2V_CUDA(v, cudaMalloc(&v->d_texel[s], (pixels + 1) * sizeof(Texel)));   // + the out-of-image texel
+            B2V_CUDA(v, cudaMemsetAsync(v->d_texel[s] + pixels, 0, sizeof(Texel), v->compute));
+        }
     }
     cudaFree(v->d_lambda);
     v->d_lambda = nullptr;
-    B2V_CUDA(v, cudaMalloc(&v->d_lambda, pixels * sizeof(float)));
+    // + the out-of-image element, which launch_lambda sets to kLambdaSentinel at index W * H of each image it writes
+    B2V_CUDA(v, cudaMalloc(&v->d_lambda, (pixels + 1) * sizeof(float)));
+    B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     v->lam_H = v->lam_W = 0;
     v->stage_pixels = pixels;
     return B2V_OK;
@@ -699,8 +704,10 @@ static int ensure_group_buffers(b2v_volume *v, size_t pixels) {
     for (Texel *&t : v->d_gtex) {
         cudaFree(t);
         t = nullptr;
-        B2V_CUDA(v, cudaMalloc(&t, pixels * sizeof(Texel)));
+        B2V_CUDA(v, cudaMalloc(&t, (pixels + 1) * sizeof(Texel)));   // + the out-of-image texel
+        B2V_CUDA(v, cudaMemsetAsync(t + pixels, 0, sizeof(Texel), v->compute));
     }
+    B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     v->gtex_pixels = pixels;
     return B2V_OK;
 }

@@ -24,9 +24,10 @@ __device__ __forceinline__ Texel load_texel(const Texel *p) {  // read-only path
     const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p));
     return Texel{__uint_as_float(u.x), u.y};
 }
-// colour channel c (0 = r, 1 = g, 2 = b) as float32, exactly: (2^23 + c) - 2^23
+// colour channel c (0 = r, 1 = g, 2 = b) as float32, exactly: (2^23 + c) - 2^23.  One byte permute builds the bits
+// 0x4B0000cc: byte 0 = byte c of rgb, bytes 1, 2 = 0x00 and byte 3 = 0x4B of the constant.
 __device__ __forceinline__ float texel_channel(const Texel &t, int c) {
-    return __fsub_rn(__uint_as_float(0x4B000000u | ((t.rgb >> (8 * c)) & 0xFFu)), 8388608.0f);
+    return __fsub_rn(__uint_as_float(__byte_perm(t.rgb, 0x4B000000u, 0x7440u + c)), 8388608.0f);
 }
 
 // Constants of the projective update of one frame (Open3D UniformTSDFVolume::IntegrateWithDepthToCameraDistance-
@@ -38,9 +39,15 @@ struct IntFrame {
     float safe_w, safe_h;   // W - 0.0001f, H - 0.0001f
     float tau, inv_tau;
     int32_t W;
+    int32_t pixels;         // W * H: the index that voxels projecting outside the image gather (see below)
     const Texel *tex;       // texels of the frame
     const float *lam;       // lambda image of the frame's intrinsics, same pixel index as tex
 };
+// Texel and lambda images hold one element past the W * H pixels.  The update kernels gather it, instead of
+// predicating the loads, for a voxel outside the image.  Its lambda is NaN (written with the lambda image), so the
+// voxel's sdf is NaN and the update skips it whatever the texel there holds; the texel buffers are allocated for the
+// largest frame so far and reused for smaller ones, where index W * H is a pixel of an earlier frame.
+constexpr float kLambdaSentinel = __builtin_nanf("");
 
 // camera -> world of one frame, float64 (allocation samples)
 struct FramePose {
@@ -76,7 +83,7 @@ struct VolumeConsts {
 
 // Fused group integration: up to kMaxGroup consecutive frames are applied to a block while it is
 // resident in registers.
-constexpr int kMaxGroup = 32;   // frames per fused group (bits of the membership mask); the default group is 8
+constexpr int kMaxGroup = 32;   // frames per fused group (bits of the membership mask); the default group is 16
 // group state (masks, union list, texel images, counters) is kGroupBufs-deep: the allocation of group g+3 may
 // run while group g is still being integrated
 constexpr int kGroupBufs = 4;
