@@ -1,11 +1,13 @@
 // b2v_api.cu — the C ABI (include/b2v.h): volume / grid lifetime, frame staging and stream
 // pipelining, parity hooks.  Host code only; kernels live in b2v_tsdf.cu, b2v_mesh.cu, b2v_grid.cu.
 //
-// Per frame (b2v_integrate):   copy stream:    H2D depth, colour  -> event ready[s]
-//                              compute stream: wait ready[s]; allocate_kernel; integrate_kernel;
-//                                              event free[s]
-// with a ring of kStage device staging slots, so the upload of frame f+1 overlaps the kernels of
-// frame f.  Nothing synchronises with the host until b2v_synchronize / an inspection call.
+// Frames are enqueued in groups (enqueue_frames): b2v_integrate_batch fuses groups of up to kMaxGroup frames, and a
+// single frame is a group of one on the frame-by-frame kernels.  Group g uses group buffer buf = g % kGroupBufs:
+//   copy stream:    H2D depth, colour of the group's host frames         -> event ready[buf]
+//   alloc stream:   wait ready[buf]; allocate kernel                      -> event galloc[buf]
+//   compute stream: wait galloc[buf]; update kernel                       -> event group_done[buf]
+// so the upload and allocation of the next groups overlap the update of this one.  Nothing synchronises with
+// the host until b2v_synchronize / an inspection call.
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -26,7 +28,7 @@ namespace b2v {
 // Host-side pose algebra, same operation order as the oracle (and -ffp-contract=off on the host
 // compiler), so allocation keys agree bit for bit.
 void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], int H, int W,
-                       const VolumeGeometry &g, uint32_t frame_id) {
+                       const VolumeGeometry &g) {
     p->fx = K[0];
     p->fy = K[1];
     p->cx = K[2];
@@ -61,10 +63,8 @@ void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], 
     p->H = H;
     p->W = W;
     p->stride = g.stride;
-    p->frame_id = frame_id;
     p->shard_rank = g.shard_rank;
     p->shard_count = g.shard_count;
-    p->group_bit = -1;
     p->group_buf = 0;
 }
 
@@ -81,10 +81,8 @@ VolumeConsts volume_consts(const VolumeGeometry &g) {
 
 namespace {
 
-static_assert(kCtrNew0 == kCtrActive0 + kActiveRing, "the ring counters are cleared with one memset");
-constexpr int kFrameStage = 4;                       // staging ring of the frame-by-frame path
-constexpr int kGroupStage = kGroupBufs * kMaxGroup;  // group buffers x kMaxGroup frames
-constexpr int kStage = kGroupStage + kFrameStage;    // raw-frame staging slots (device copies of host frames)
+// staging and texel slots: slot buf * kMaxGroup + k holds frame k of the group in group buffer buf
+constexpr int kStage = kGroupBufs * kMaxGroup;
 
 uint32_t next_pow2(uint64_t v) {
     uint64_t p = 1;
@@ -108,18 +106,15 @@ struct b2v_volume {
     VolumeGeometry geo{};
     cudaStream_t compute = nullptr, copy = nullptr, alloc = nullptr;
     cudaStream_t last_stream = nullptr;  // caller stream of the most recent frame (synchronised on reads)
-    bool overlap = true;                 // allocate(f+1) on its own stream, concurrent with integrate(f)
+    bool overlap = true;                 // allocate(g+1) on its own stream, concurrent with the update of group g
     bool use_tma = true;                 // stage image tiles with TMA when the layout allows it
-    bool inputs_fenced = false;          // batch call: device inputs already ordered before the alloc stream
     bool fuse = true;                    // b2v_integrate_batch fuses groups of up to kMaxGroup frames
     int group_frames = 16;               // frames per fused group (1..kMaxGroup), b2v_set_group_size
     cudaEvent_t input_event = nullptr;   // b2v_set_input_event: readiness of the next batch's device inputs
-    bool rings_stale = false;            // a fused batch advanced frame_id: the per-frame ring counters must be re-armed
-    Texel *d_gtex[kGroupBufs * kMaxGroup] = {};   // texel images of the group buffers
-    size_t gtex_pixels = 0;
-    uint32_t group_id = 0;
-    cudaEvent_t ev_galloc[kGroupBufs] = {}, ev_group_done[kGroupBufs] = {};
-    int last_group_buf = -1, last_group_count = 0;  // most recent frame came from a fused group
+    uint32_t group_id = 0;               // groups enqueued since reset; group g uses group buffer g % kGroupBufs
+    int last_group_count = 0;            // frames of the most recent group
+    cudaEvent_t ev_in = nullptr;         // input fence recorded on the caller's stream
+    cudaEvent_t ev_ready[kGroupBufs] = {}, ev_galloc[kGroupBufs] = {}, ev_group_done[kGroupBufs] = {};
     int64_t prof_frames = 0, prof_int_launches = 0;
     // optional rectification stage (b2v_set_rectification)
     float *d_mapx = nullptr, *d_mapy = nullptr;
@@ -129,22 +124,19 @@ struct b2v_volume {
     // TMA descriptors are cached per image address (encoding costs ~1 us of host time each)
     std::unordered_map<uintptr_t, FrameMaps> map_cache;
     int map_H = 0, map_W = 0;
-    cudaEvent_t ev_in = nullptr, ev_alloc_done[kActiveRing] = {}, ev_int_done[kActiveRing] = {};
     // raw 16-bit depth input (b2v_integrate_u16 / b2v_integrate_batch_u16): uploaded as is, widened on the device
     uint16_t *d_depth16[kStage] = {};   // same slot layout as d_depth; allocated on first use
     size_t stage16_pixels = 0;
     float in_u16_scale = 0.0f;          // > 0 while a *_u16 entry point runs: `depth` pointers are uint16_t
     float *d_depth[kStage] = {};
     uint8_t *d_color[kStage] = {};
-    Texel *d_texel[kStage] = {};    // texel images of the frames read by integrate_kernel
+    Texel *d_tex[kStage] = {};      // texel images, written by the allocate kernels and read by the update kernels
     float *d_lambda = nullptr;      // lambda image of the cached intrinsics, read by the update kernels
     double lam_K[4] = {0, 0, 0, 0};
     int lam_H = 0, lam_W = 0;
     size_t stage_pixels = 0;
-    cudaEvent_t ev_ready[kStage] = {}, ev_free[kStage] = {};
     HashTable table{};
     PoolMeta meta{};
-    uint32_t frame_id = 0;  // frames integrated since reset (stamp = frame_id + 1)
     int grid_ctas = 0;
     int sm_count = 0;
     int64_t launches = 0;
@@ -174,7 +166,6 @@ struct b2v_volume {
 static int volume_clear_device(b2v_volume *v) {
     const size_t tcap = static_cast<size_t>(v->table.mask) + 1;
     B2V_CUDA(v, cudaMemsetAsync(v->table.entries, 0xFF, tcap * sizeof(uint4), v->compute));
-    B2V_CUDA(v, cudaMemsetAsync(v->table.stamp, 0, tcap * sizeof(uint32_t), v->compute));
     B2V_CUDA(v, cudaMemsetAsync(v->meta.group_mask, 0, tcap * kGroupBufs * sizeof(uint32_t), v->compute));
     B2V_CUDA(v, cudaMemsetAsync(v->meta.counters, 0, kNumCounters * sizeof(uint32_t), v->compute));
     return B2V_OK;
@@ -239,10 +230,6 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     B2V_CUDA(v, cudaStreamCreateWithFlags(&v->copy, cudaStreamNonBlocking));
     B2V_CUDA(v, cudaStreamCreateWithFlags(&v->alloc, cudaStreamNonBlocking));
     B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_in, cudaEventDisableTiming));
-    for (int r = 0; r < kActiveRing; ++r) {
-        B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_alloc_done[r], cudaEventDisableTiming));
-        B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_int_done[r], cudaEventDisableTiming));
-    }
     if (const char *e = std::getenv("B2V_OVERLAP")) v->overlap = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_TMA")) v->use_tma = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_FUSE")) v->fuse = std::atoi(e) != 0;
@@ -251,23 +238,18 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
         if (n >= 1 && n <= kMaxGroup) v->group_frames = n;
     }
     for (int b = 0; b < kGroupBufs; ++b) {
+        B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_ready[b], cudaEventDisableTiming));
         B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_galloc[b], cudaEventDisableTiming));
         B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_group_done[b], cudaEventDisableTiming));
-    }
-    for (int s = 0; s < kStage; ++s) {
-        B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_ready[s], cudaEventDisableTiming));
-        B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_free[s], cudaEventDisableTiming));
     }
     const uint32_t cap = cfg->capacity_blocks;
     const uint32_t tcap = next_pow2(static_cast<uint64_t>(cap) * 2);
     v->table.mask = tcap - 1;
     v->meta.capacity = cap;
     B2V_CUDA(v, cudaMalloc(&v->table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
-    B2V_CUDA(v, cudaMalloc(&v->table.stamp, static_cast<size_t>(tcap) * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.pool, static_cast<size_t>(cap) * kBlockFloats * sizeof(float)));
     B2V_CUDA(v, cudaMalloc(&v->meta.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
     B2V_CUDA(v, cudaMalloc(&v->meta.counters, kNumCounters * sizeof(uint32_t)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.active_slots, static_cast<size_t>(cap) * kActiveRing * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.group_mask, static_cast<size_t>(tcap) * kGroupBufs * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.union_slots, static_cast<size_t>(cap) * kGroupBufs * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.block_flags, static_cast<size_t>(cap) * sizeof(uint32_t)));
@@ -298,25 +280,17 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaSetDevice(v->cfg.device);
     cudaDeviceSynchronize();
     if (v->ev_in) cudaEventDestroy(v->ev_in);
-    for (int r = 0; r < kActiveRing; ++r) {
-        if (v->ev_alloc_done[r]) cudaEventDestroy(v->ev_alloc_done[r]);
-        if (v->ev_int_done[r]) cudaEventDestroy(v->ev_int_done[r]);
-    }
-    cudaFree(v->d_depth[0]);  // slots 1.. point into the same two allocations
+    cudaFree(v->d_depth[0]);  // slots 1.. point into the same three allocations
     cudaFree(v->d_color[0]);
-    for (int s = 0; s < kStage; ++s) {
-        cudaFree(v->d_texel[s]);
-        if (v->ev_ready[s]) cudaEventDestroy(v->ev_ready[s]);
-        if (v->ev_free[s]) cudaEventDestroy(v->ev_free[s]);
-    }
+    cudaFree(v->d_tex[0]);
     cudaFree(v->d_lambda);
     cudaFree(v->d_mapx);
     cudaFree(v->d_mapy);
     cudaFree(v->d_rdepth[0]);
     cudaFree(v->d_rcolor[0]);
     cudaFree(v->d_depth16[0]);
-    for (Texel *t : v->d_gtex) cudaFree(t);
     for (int b = 0; b < kGroupBufs; ++b) {
+        if (v->ev_ready[b]) cudaEventDestroy(v->ev_ready[b]);
         if (v->ev_galloc[b]) cudaEventDestroy(v->ev_galloc[b]);
         if (v->ev_group_done[b]) cudaEventDestroy(v->ev_group_done[b]);
     }
@@ -324,11 +298,9 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaFree(v->meta.union_slots);
     cudaFree(v->meta.block_flags);
     cudaFree(v->table.entries);
-    cudaFree(v->table.stamp);
     cudaFree(v->meta.pool);
     cudaFree(v->meta.block_keys);
     cudaFree(v->meta.counters);
-    cudaFree(v->meta.active_slots);
     cudaFree(v->mb.nbr);
     cudaFree(v->mb.cube);
     cudaFree(v->mb.edge_mask);
@@ -384,43 +356,45 @@ extern "C" int b2v_reset(b2v_volume *v) {
     B2V_CUDA(v, cudaMemsetAsync(v->meta.block_flags, 0, static_cast<size_t>(nb) * sizeof(uint32_t), v->compute));
     rc = volume_clear_device(v);
     if (rc != B2V_OK) return rc;
-    v->frame_id = 0;
     v->group_id = 0;
-    v->last_group_buf = -1;
-    v->rings_stale = false;
+    v->last_group_count = 0;
     v->err.clear();
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     return B2V_OK;
 }
 
+// Raw staging, texel images and the lambda image for frames of up to `pixels` pixels.
 static int ensure_staging(b2v_volume *v, size_t pixels) {
     if (pixels <= v->stage_pixels) return B2V_OK;
-    // the lambda image freed below is read by update kernels on the library's streams and on callers' streams
+    // the texel and lambda images freed below are read by update kernels on the library's streams and on callers'
     B2V_CUDA(v, cudaDeviceSynchronize());
-    // raw staging slots are carved out of two contiguous allocations, so the frames of a group (which
-    // are contiguous in the caller's arrays) upload with ONE copy per image type
+    // slots are carved out of contiguous allocations, so the frames of a group (which are contiguous in the caller's
+    // arrays) upload with ONE copy per image type
     cudaFree(v->d_depth[0]);
     cudaFree(v->d_color[0]);
+    cudaFree(v->d_tex[0]);
     for (int s = 0; s < kStage; ++s) {
-        cudaFree(v->d_texel[s]);
         v->d_depth[s] = nullptr;
         v->d_color[s] = nullptr;
-        v->d_texel[s] = nullptr;
+        v->d_tex[s] = nullptr;
     }
     v->stage_pixels = 0;  // stays 0 if an allocation below fails
     float *dbase = nullptr;
     uint8_t *cbase = nullptr;
+    Texel *tbase = nullptr;
     B2V_CUDA(v, cudaMalloc(&dbase, pixels * sizeof(float) * kStage));
     v->d_depth[0] = dbase;
     B2V_CUDA(v, cudaMalloc(&cbase, pixels * 3 * kStage));
     v->d_color[0] = cbase;
+    // a texel slot holds the image + the out-of-image texel (zeroed once, here), rounded up to 256 bytes
+    const size_t tex_pitch = (pixels + 32) & ~static_cast<size_t>(31);
+    B2V_CUDA(v, cudaMalloc(&tbase, tex_pitch * sizeof(Texel) * kStage));
+    v->d_tex[0] = tbase;
+    B2V_CUDA(v, cudaMemsetAsync(tbase, 0, tex_pitch * sizeof(Texel) * kStage, v->compute));
     for (int s = 0; s < kStage; ++s) {
         v->d_depth[s] = dbase + pixels * s;
         v->d_color[s] = cbase + pixels * 3 * s;
-        if (s >= kGroupStage) {  // texel images of the per-frame path (the group buffers have their own)
-            B2V_CUDA(v, cudaMalloc(&v->d_texel[s], (pixels + 1) * sizeof(Texel)));   // + the out-of-image texel
-            B2V_CUDA(v, cudaMemsetAsync(v->d_texel[s] + pixels, 0, sizeof(Texel), v->compute));
-        }
+        v->d_tex[s] = tbase + tex_pitch * s;
     }
     cudaFree(v->d_lambda);
     v->d_lambda = nullptr;
@@ -458,9 +432,6 @@ static const FrameMaps *frame_maps(b2v_volume *v, const float *d_depth, const ui
     return &res.first->second;
 }
 
-static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d_color, int H, int W, int slot,
-                         cudaStream_t stream);
-
 // raw uint16 staging, one contiguous allocation carved into the same slots as the float staging
 static int ensure_staging16(b2v_volume *v, size_t pixels) {
     if (pixels <= v->stage16_pixels) return B2V_OK;
@@ -476,140 +447,6 @@ static int ensure_staging16(b2v_volume *v, size_t pixels) {
     for (int s = 0; s < kStage; ++s) v->d_depth16[s] = base + pixels * s;
     v->stage16_pixels = pixels;
     return B2V_OK;
-}
-
-static int integrate_frame(b2v_volume *v, const float *depth, const uint8_t *color, int32_t height,
-                           int32_t width, const double K[4], const double Tcw[16], void *stream,
-                           int dev_hint = -1) {
-    if (!depth || !color || !K || !Tcw || height <= 0 || width <= 0) {
-        v->err = "b2v_integrate: null pointer or non-positive image size";
-        return B2V_ERR_INVALID_ARGUMENT;
-    }
-    if (!(K[0] > 0.0) || !(K[1] > 0.0)) {
-        v->err = "b2v_integrate: focal lengths must be positive";
-        return B2V_ERR_INVALID_ARGUMENT;
-    }
-    const size_t pixels = static_cast<size_t>(height) * width;
-    bool dev_depth, dev_color;
-    if (dev_hint >= 0) {  // batch call: queried once for the whole batch
-        dev_depth = dev_color = dev_hint != 0;
-    } else {
-        B2V_CUDA(v, cudaSetDevice(v->cfg.device));
-        dev_depth = is_device_pointer(depth);
-        dev_color = is_device_pointer(color);
-    }
-    if (stream != nullptr && !(dev_depth && dev_color)) {
-        v->err = "b2v_integrate: a caller stream requires device image pointers";
-        return B2V_ERR_INVALID_ARGUMENT;
-    }
-    cudaStream_t cs = stream ? static_cast<cudaStream_t>(stream) : v->compute;
-    cudaStream_t as = v->overlap ? v->alloc : cs;  // stream of the allocate kernel
-    v->last_stream = stream ? cs : nullptr;
-    const int s = kGroupStage + static_cast<int>(v->frame_id % kFrameStage);
-    const int ring = static_cast<int>(v->frame_id % kActiveRing);
-    const float *d_depth = depth;
-    const uint8_t *d_color = color;
-    const bool staged = !(dev_depth && dev_color);
-    const bool u16 = v->in_u16_scale > 0.0f;  // `depth` is really const uint16_t *
-    {
-        int rc = ensure_staging(v, pixels);
-        if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
-        if (rc != B2V_OK) return rc;
-    }
-    if (staged) {
-        B2V_CUDA(v, cudaStreamWaitEvent(v->copy, v->ev_free[s], 0));
-        if (!dev_depth) {
-            if (u16)
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth16[s], depth, pixels * sizeof(uint16_t), cudaMemcpyHostToDevice,
-                                            v->copy));
-            else
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth[s], depth, pixels * sizeof(float),
-                                            cudaMemcpyHostToDevice, v->copy));
-            d_depth = v->d_depth[s];
-        }
-        if (!dev_color) {
-            B2V_CUDA(v, cudaMemcpyAsync(v->d_color[s], color, pixels * 3, cudaMemcpyHostToDevice, v->copy));
-            d_color = v->d_color[s];
-        }
-        B2V_CUDA(v, cudaEventRecord(v->ev_ready[s], v->copy));
-        B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_ready[s], 0));
-    } else if (v->overlap && !v->inputs_fenced) {
-        // device inputs were produced by earlier work on the caller's stream (a batch call fences once:
-        // an event recorded now would also wait for the previous frame's integrate kernel)
-        B2V_CUDA(v, cudaEventRecord(v->ev_in, cs));
-        B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_in, 0));
-    }
-    if (v->rings_stale) {
-        // first single frame after a fused batch: the batch advanced frame_id without passing through the
-        // per-frame rings, so the ring this frame counts into may still hold an old frame's counts (only the
-        // previous per-frame allocate re-arms the next ring).  Rare transition: order it after everything on the
-        // compute stream and clear all ring counters.
-        B2V_CUDA(v, cudaEventRecord(v->ev_in, cs));
-        B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_in, 0));
-        B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + kCtrActive0, 0, 2 * kActiveRing * sizeof(uint32_t), as));
-        v->rings_stale = false;
-    } else if (v->overlap && v->frame_id >= 3) {
-        // allocate(f) recycles the ring slot / texel buffer last read by integrate(f - 3) .. (f - 4)
-        B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_int_done[(v->frame_id - 3) % kActiveRing], 0));
-    }
-    if (u16) {  // widen the raw depth into the float staging slot: float(u16) * scale, one rounding
-        const uint16_t *src = dev_depth ? reinterpret_cast<const uint16_t *>(depth) : v->d_depth16[s];
-        B2V_CUDA(v, launch_depth_u16_to_f32(src, v->d_depth[s], pixels, v->in_u16_scale, as));
-        d_depth = v->d_depth[s];
-        v->launches += 1;
-    }
-    {
-        const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s, as);
-        if (rc != B2V_OK) return rc;
-    }
-    FrameParams P;
-    fill_frame_params(&P, K, Tcw, height, width, v->geo, v->frame_id + 1);
-    if (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0) {
-        // the lambda image is read by update kernels of earlier frames that may still run, on the library's streams
-        // or on a caller's; new intrinsics are rare, so the whole device is drained before the image is rewritten
-        B2V_CUDA(v, cudaDeviceSynchronize());
-        B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
-        std::memcpy(v->lam_K, K, sizeof(v->lam_K));
-        v->lam_H = height;
-        v->lam_W = width;
-        v->launches += 1;
-    }
-    cudaEvent_t *pe = nullptr;
-    if (v->prof_enabled) {
-        const int rc = grow_profile_events(v, 4);
-        if (rc != B2V_OK) return rc;
-        pe = &v->prof_events[v->prof_used];
-        v->prof_used += 4;
-        B2V_CUDA(v, cudaEventRecord(pe[0], as));
-    }
-    Texel *tex = v->d_texel[s];
-    P.I.tex = tex;
-    P.I.lam = v->d_lambda;
-    B2V_CUDA(v, launch_allocate(P, d_depth, d_color, tex, v->table, v->meta, ring,
-                                frame_maps(v, d_depth, d_color, height, width), as));
-    if (staged || u16) B2V_CUDA(v, cudaEventRecord(v->ev_free[s], as));  // the raw frame is consumed by allocate only
-    v->launches += 1;
-    v->frame_id += 1;
-    if (v->prof_enabled) v->prof_frames += 1;
-    v->last_group_buf = -1;
-    if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
-    if (v->overlap) {
-        B2V_CUDA(v, cudaEventRecord(v->ev_alloc_done[ring], as));
-        B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_alloc_done[ring], 0));
-    }
-    if (pe) B2V_CUDA(v, cudaEventRecord(pe[2], cs));
-    B2V_CUDA(v, launch_integrate(P, volume_consts(v->geo), v->table, v->meta, ring, v->grid_ctas, cs));
-    if (pe) B2V_CUDA(v, cudaEventRecord(pe[3], cs));
-    if (v->overlap) B2V_CUDA(v, cudaEventRecord(v->ev_int_done[ring], cs));
-    v->launches += 1;
-    if (v->prof_enabled) v->prof_int_launches += 1;
-    return B2V_OK;
-}
-
-extern "C" int b2v_integrate(b2v_volume *v, const float *depth, const uint8_t *color, int32_t height,
-                             int32_t width, const double K[4], const double Tcw[16], void *stream) {
-    if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    return integrate_frame(v, depth, color, height, width, K, Tcw, stream);
 }
 
 extern "C" int b2v_set_rectification(b2v_volume *v, const float *map_x, const float *map_y, int32_t height,
@@ -697,181 +534,160 @@ static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d
     return B2V_OK;
 }
 
-static int ensure_group_buffers(b2v_volume *v, size_t pixels) {
-    if (pixels <= v->gtex_pixels) return B2V_OK;
-    B2V_CUDA(v, cudaDeviceSynchronize());
-    v->gtex_pixels = 0;  // stays 0 if an allocation below fails
-    for (Texel *&t : v->d_gtex) {
-        cudaFree(t);
-        t = nullptr;
-        B2V_CUDA(v, cudaMalloc(&t, (pixels + 1) * sizeof(Texel)));   // + the out-of-image texel
-        B2V_CUDA(v, cudaMemsetAsync(t + pixels, 0, sizeof(Texel), v->compute));
-    }
-    B2V_CUDA(v, cudaStreamSynchronize(v->compute));
-    v->gtex_pixels = pixels;
-    return B2V_OK;
-}
-
-extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float *depth,
-                                   const uint8_t *color, int32_t height, int32_t width,
-                                   const double K[4], const double *Tcw, void *stream) {
-    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+// Enqueues n_frames frames, contiguous in the caller's arrays, as groups in the group buffers: groups of up to
+// group_frames frames on the fused kernels when fusion is on and there are two frames or more, else groups of one
+// frame on the frame-by-frame kernels.  inputs_ready: an event after which device frames are ready, or nullptr.
+static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, const float *depth, const uint8_t *color,
+                          int32_t height, int32_t width, const double K[4], const double *Tcw, void *stream,
+                          cudaEvent_t inputs_ready) {
     if (n_frames < 0 || (n_frames > 0 && (!depth || !color || !Tcw || !K)) || height <= 0 || width <= 0) {
-        v->err = "b2v_integrate_batch: bad arguments";
+        v->err = std::string(what) + ": bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     if (n_frames == 0) return B2V_OK;
     if (!(K[0] > 0.0) || !(K[1] > 0.0)) {
-        v->err = "b2v_integrate_batch: focal lengths must be positive";
+        v->err = std::string(what) + ": focal lengths must be positive";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
     const size_t pixels = static_cast<size_t>(height) * width;
-    const bool dd = is_device_pointer(depth), dc = is_device_pointer(color);
-    const int dev_hint = dd == dc ? (dd ? 1 : 0) : -1;
-    if (stream != nullptr && dev_hint != 1) {
-        v->err = "b2v_integrate_batch: a caller stream requires device image pointers";
+    const bool dev_depth = is_device_pointer(depth), dev_color = is_device_pointer(color);
+    if (stream != nullptr && !(dev_depth && dev_color)) {
+        v->err = std::string(what) + ": a caller stream requires device image pointers";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     cudaStream_t cs = stream ? static_cast<cudaStream_t>(stream) : v->compute;
-    cudaStream_t as = v->overlap ? v->alloc : cs;
-    struct FenceGuard {  // every exit path (errors included) drops the batch-wide input fence
-        b2v_volume *v;
-        ~FenceGuard() { v->inputs_fenced = false; }
-    } fence_guard{v};
-    if (v->overlap) {
-        // one fence for the whole batch: by default everything enqueued on the caller's stream so far (the inputs'
-        // producers, earlier per-frame work) happens before the batch's allocate kernels.  A caller that knows better
-        // (b2v_set_input_event: "the inputs are ready when this event fires") keeps the allocate kernels of this batch
-        // from also waiting for the update kernels of the previous one.
-        if (v->input_event && dev_hint == 1) {
-            B2V_CUDA(v, cudaStreamWaitEvent(v->alloc, v->input_event, 0));
-        } else {
-            B2V_CUDA(v, cudaEventRecord(v->ev_in, cs));
-            B2V_CUDA(v, cudaStreamWaitEvent(v->alloc, v->ev_in, 0));
-        }
-        v->inputs_fenced = true;
-    } else if (v->input_event && dev_hint == 1) {
-        B2V_CUDA(v, cudaStreamWaitEvent(cs, v->input_event, 0));
-    }
-    v->input_event = nullptr;
-    int rc = B2V_OK;
-    const bool u16 = v->in_u16_scale > 0.0f;  // `depth` is really const uint16_t *
+    cudaStream_t as = v->overlap ? v->alloc : cs;  // stream of the allocate kernels
+    const bool u16 = v->in_u16_scale > 0.0f;       // `depth` is really const uint16_t *
     const uint16_t *depth16 = reinterpret_cast<const uint16_t *>(depth);
-    if (!v->fuse || n_frames < 2) {
-        for (int32_t f = 0; f < n_frames && rc == B2V_OK; ++f)
-            rc = integrate_frame(v, u16 ? reinterpret_cast<const float *>(depth16 + pixels * f) : depth + pixels * f,
-                                 color + pixels * 3 * f, height, width, K, Tcw + 16 * static_cast<size_t>(f), stream,
-                                 dev_hint);
-        return rc;
+    {
+        int rc = ensure_staging(v, pixels);
+        if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
+        if (rc != B2V_OK) return rc;
     }
-    rc = ensure_group_buffers(v, pixels);
-    if (rc == B2V_OK) rc = ensure_staging(v, pixels);
-    if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
-    if (rc != B2V_OK) return rc;
-    v->rings_stale = true;
     v->last_stream = stream ? cs : nullptr;
-    const bool staged = dev_hint != 1;
-    const int gsz = std::max(1, std::min(v->group_frames, kMaxGroup));
+    if (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0) {
+        // the lambda image is read by update kernels of earlier frames that may still run, on the library's streams
+        // or on a caller's; new intrinsics are rare, so the whole device is drained before the image is rewritten
+        FrameParams P;
+        fill_frame_params(&P, K, Tcw, height, width, v->geo);
+        B2V_CUDA(v, cudaDeviceSynchronize());
+        B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
+        std::memcpy(v->lam_K, K, sizeof(v->lam_K));
+        v->lam_H = height;
+        v->lam_W = width;
+        v->launches += 1;
+    }
+    const bool fused = v->fuse && n_frames >= 2;
+    const int gsz = fused ? std::max(1, std::min(v->group_frames, kMaxGroup)) : 1;
     for (int32_t g0 = 0; g0 < n_frames; g0 += gsz) {
         const int count = std::min<int32_t>(gsz, n_frames - g0);
         const int buf = static_cast<int>(v->group_id % kGroupBufs);
-        // the group buffer (masks, union list, texel images) was last used by group id - kGroupBufs
+        const int s0 = buf * kMaxGroup;  // the buffer's staging and texel slots
+        // the group buffer (masks, union list, counters, texel images) was last used by group id - kGroupBufs
         B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_group_done[buf], 0));
         B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + group_ctr(buf, 0), 0, kGroupCtrStride * sizeof(uint32_t), as));
+        if (g0 == 0 && (dev_depth || dev_color)) {
+            // one input fence per call: by default everything enqueued on the caller's stream so far (the inputs'
+            // producers, earlier frames) happens before the allocate kernels.  A caller that knows better
+            // (b2v_set_input_event: "the inputs are ready when this event fires") keeps the allocate kernels of this
+            // call from also waiting for the update kernels of the previous one.  The counter memset above does not
+            // read the inputs, so it stays off that path.  Host frames are ordered by their uploads.
+            if (inputs_ready) {
+                B2V_CUDA(v, cudaStreamWaitEvent(as, inputs_ready, 0));
+            } else if (v->overlap) {
+                B2V_CUDA(v, cudaEventRecord(v->ev_in, cs));
+                B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_in, 0));
+            }
+        }
+        if (!dev_depth || !dev_color) {
+            // the raw staging slots of this buffer were consumed by the allocate launch of group id - kGroupBufs;
+            // the group's frames are contiguous on both sides: one H2D copy per image type
+            B2V_CUDA(v, cudaStreamWaitEvent(v->copy, v->ev_galloc[buf], 0));
+            if (!dev_depth && u16)
+                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth16[s0], depth16 + pixels * g0, pixels * sizeof(uint16_t) * count,
+                                            cudaMemcpyHostToDevice, v->copy));
+            else if (!dev_depth)
+                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth[s0], depth + pixels * g0, pixels * sizeof(float) * count,
+                                            cudaMemcpyHostToDevice, v->copy));
+            if (!dev_color)
+                B2V_CUDA(v, cudaMemcpyAsync(v->d_color[s0], color + pixels * 3 * g0, pixels * 3 * count,
+                                            cudaMemcpyHostToDevice, v->copy));
+            B2V_CUDA(v, cudaEventRecord(v->ev_ready[buf], v->copy));
+            B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_ready[buf], 0));
+        }
+        if (u16) {  // widen the group's raw depth into its (contiguous) float staging slots in one launch
+            const uint16_t *src = dev_depth ? depth16 + pixels * g0 : v->d_depth16[s0];
+            B2V_CUDA(v, launch_depth_u16_to_f32(src, v->d_depth[s0], pixels * count, v->in_u16_scale, as));
+            v->launches += 1;
+        }
         static thread_local GroupAllocArgs aargs;  // ~15 KB: keep it off the stack
         static thread_local GroupArgs args;
         std::memset(&args, 0, sizeof(args));
         args.V = volume_consts(v->geo);
-        args.count = count;
-        aargs.count = count;
+        args.count = aargs.count = count;
         aargs.use_tma = 1;
-        if (staged) {
-            // the raw staging slots of this buffer were consumed by the allocate launch of group id - kGroupBufs;
-            // the group's frames are contiguous on both sides: one H2D copy per image type
-            B2V_CUDA(v, cudaStreamWaitEvent(v->copy, v->ev_galloc[buf], 0));
-            const int s0 = buf * kMaxGroup;
-            if (u16)
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth16[s0], depth16 + pixels * g0, pixels * sizeof(uint16_t) * count,
-                                            cudaMemcpyHostToDevice, v->copy));
-            else
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth[s0], depth + pixels * g0, pixels * sizeof(float) * count,
-                                            cudaMemcpyHostToDevice, v->copy));
-            B2V_CUDA(v, cudaMemcpyAsync(v->d_color[s0], color + pixels * 3 * g0, pixels * 3 * count,
-                                        cudaMemcpyHostToDevice, v->copy));
-        }
         for (int k = 0; k < count; ++k) {
             const size_t f = static_cast<size_t>(g0 + k);
-            const float *d_depth = u16 ? nullptr : depth + pixels * f;
-            const uint8_t *d_color = color + pixels * 3 * f;
-            if (staged || u16) d_depth = v->d_depth[buf * kMaxGroup + k];  // (widened) float staging slot
-            if (staged) d_color = v->d_color[buf * kMaxGroup + k];
+            const float *d_depth = dev_depth && !u16 ? depth + pixels * f : v->d_depth[s0 + k];  // (widened) staging
+            const uint8_t *d_color = dev_color ? color + pixels * 3 * f : v->d_color[s0 + k];
+            const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s0 + k, as);
+            if (rc != B2V_OK) return rc;
             FrameParams P;
-            fill_frame_params(&P, K, Tcw + 16 * f, height, width, v->geo, v->frame_id + 1);
-            P.group_bit = k;
+            fill_frame_params(&P, K, Tcw + 16 * f, height, width, v->geo);
             P.group_buf = buf;
+            P.I.tex = v->d_tex[s0 + k];
+            P.I.lam = v->d_lambda;
+            if (k == 0) aargs.P = P;
             aargs.pose[k] = P.pose;
-            if (k == 0) {
-                aargs.P = P;
-                aargs.frame_id0 = v->frame_id + 1;
-            }
-            if (k == 0 && (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0)) {
-                // as in integrate_frame: update kernels of earlier batches may still read the lambda image
-                B2V_CUDA(v, cudaDeviceSynchronize());
-                B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
-                std::memcpy(v->lam_K, K, sizeof(v->lam_K));
-                v->lam_H = height;
-                v->lam_W = width;
-                v->launches += 1;
-            }
-            Texel *tex = v->d_gtex[buf * kMaxGroup + k];
             aargs.depth[k] = d_depth;
             aargs.color[k] = d_color;
-            aargs.tex[k] = tex;
-            P.I.tex = tex;
-            P.I.lam = v->d_lambda;
-            args.f[k] = P.I;
-            v->frame_id += 1;
-        }
-        if (staged) {
-            B2V_CUDA(v, cudaEventRecord(v->ev_ready[buf], v->copy));  // all frames of the group uploaded
-            B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_ready[buf], 0));
-        }
-        if (u16) {  // widen the group's raw depth into its (contiguous) float staging slots in one launch
-            const uint16_t *src = staged ? v->d_depth16[buf * kMaxGroup] : depth16 + pixels * g0;
-            B2V_CUDA(v, launch_depth_u16_to_f32(src, v->d_depth[buf * kMaxGroup], pixels * count, v->in_u16_scale, as));
-            v->launches += 1;
-        }
-        for (int k = 0; k < count; ++k) {  // optional rectification, then the TMA descriptors of the final images
-            const int rrc = rectify_frame(v, &aargs.depth[k], &aargs.color[k], height, width, buf * kMaxGroup + k, as);
-            if (rrc != B2V_OK) return rrc;
-            const FrameMaps *fm = frame_maps(v, aargs.depth[k], aargs.color[k], height, width);
+            aargs.tex[k] = v->d_tex[s0 + k];
+            const FrameMaps *fm = frame_maps(v, d_depth, d_color, height, width);
             if (fm) aargs.maps[k] = *fm; else aargs.use_tma = 0;
+            args.f[k] = P.I;
         }
         cudaEvent_t *pe = nullptr;
         if (v->prof_enabled) {
-            const int prc = grow_profile_events(v, 4);
-            if (prc != B2V_OK) return prc;
+            const int rc = grow_profile_events(v, 4);
+            if (rc != B2V_OK) return rc;
             pe = &v->prof_events[v->prof_used];
             v->prof_used += 4;
             v->prof_frames += count;
             v->prof_int_launches += 1;
             B2V_CUDA(v, cudaEventRecord(pe[0], as));
         }
-        B2V_CUDA(v, launch_allocate_group(aargs, v->table, v->meta, as));
+        B2V_CUDA(v, fused ? launch_allocate_group(aargs, v->table, v->meta, as)
+                          : launch_allocate(aargs, v->table, v->meta, as));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[2], cs));
-        B2V_CUDA(v, launch_integrate_group(args, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs));
+        B2V_CUDA(v, fused ? launch_integrate_group(args, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs)
+                          : launch_integrate(args.f[0], args.V, v->table, v->meta, buf, v->grid_ctas, cs));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[3], cs));
         B2V_CUDA(v, cudaEventRecord(v->ev_group_done[buf], cs));
-        v->launches += 3;
-        v->last_group_buf = buf;
+        v->launches += fused ? 3 : 2;  // allocate, update (+ the mask clear of a fused group)
         v->last_group_count = count;
         v->group_id += 1;
     }
     return B2V_OK;
+}
+
+extern "C" int b2v_integrate(b2v_volume *v, const float *depth, const uint8_t *color, int32_t height,
+                             int32_t width, const double K[4], const double Tcw[16], void *stream) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    return enqueue_frames(v, "b2v_integrate", 1, depth, color, height, width, K, Tcw, stream, nullptr);
+}
+
+extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float *depth,
+                                   const uint8_t *color, int32_t height, int32_t width,
+                                   const double K[4], const double *Tcw, void *stream) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    cudaEvent_t inputs_ready = v->input_event;  // one-shot
+    v->input_event = nullptr;
+    return enqueue_frames(v, "b2v_integrate_batch", n_frames, depth, color, height, width, K, Tcw, stream,
+                          inputs_ready);
 }
 
 // Raw 16-bit depth (e.g. TUM / ScanNet PNGs): uploaded as uint16 (2 instead of 4 bytes per pixel over PCIe) and
@@ -901,7 +717,7 @@ extern "C" int b2v_integrate_u16(b2v_volume *v, const uint16_t *depth, float dep
         return B2V_ERR_INVALID_ARGUMENT;
     }
     v->in_u16_scale = depth_scale;
-    const int rc = integrate_frame(v, reinterpret_cast<const float *>(depth), color, height, width, K, Tcw, stream);
+    const int rc = b2v_integrate(v, reinterpret_cast<const float *>(depth), color, height, width, K, Tcw, stream);
     v->in_u16_scale = 0.0f;
     return rc;
 }
@@ -948,23 +764,11 @@ extern "C" int b2v_last_frame_stats(b2v_volume *v, int64_t *touched_blocks, int6
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
     const int rc = read_counters(v);
     if (rc == B2V_ERR_CUDA) return rc;
-    const int ring = v->frame_id ? static_cast<int>((v->frame_id - 1) % kActiveRing) : 0;
-    if (touched_blocks) {
-        if (v->frame_id == 0)
-            *touched_blocks = 0;
-        else if (v->last_group_buf >= 0)
-            *touched_blocks = v->h_counters[group_ctr(v->last_group_buf, kGcTouched0) + v->last_group_count - 1];
-        else
-            *touched_blocks = v->h_counters[kCtrActive0 + ring];
-    }
-    if (new_blocks) {
-        if (v->frame_id == 0)
-            *new_blocks = 0;
-        else if (v->last_group_buf >= 0)  // after a fused batch: blocks allocated by the last group
-            *new_blocks = v->h_counters[group_ctr(v->last_group_buf, kGcNew)];
-        else
-            *new_blocks = v->h_counters[kCtrNew0 + ring];
-    }
+    const int buf = static_cast<int>((v->group_id - 1) % kGroupBufs);  // the most recent group
+    // touched: by the group's last frame; new: allocated by the whole group
+    if (touched_blocks)
+        *touched_blocks = v->group_id ? v->h_counters[group_ctr(buf, kGcTouched0) + v->last_group_count - 1] : 0;
+    if (new_blocks) *new_blocks = v->group_id ? v->h_counters[group_ctr(buf, kGcNew)] : 0;
     return rc;
 }
 
@@ -1152,10 +956,9 @@ extern "C" int b2v_import_blocks_device(b2v_volume *v, int64_t n_blocks, const i
 extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys, int64_t max_keys) {
     if (!v) return -1;
     if (read_counters(v) == B2V_ERR_CUDA) return -1;
-    if (v->frame_id == 0) return 0;
-    const int ring = static_cast<int>((v->frame_id - 1) % kActiveRing);
-    const bool grp = v->last_group_buf >= 0;  // after a fused batch: the last group's union of touched blocks
-    uint32_t n = grp ? v->h_counters[group_ctr(v->last_group_buf, kGcUnion)] : v->h_counters[kCtrActive0 + ring];
+    if (v->group_id == 0) return 0;
+    const int buf = static_cast<int>((v->group_id - 1) % kGroupBufs);  // the most recent group's touched blocks
+    uint32_t n = v->h_counters[group_ctr(buf, kGcUnion)];
     if (n > v->meta.capacity) n = v->meta.capacity;
     if (!keys) return n;
     if (static_cast<int64_t>(n) > max_keys) n = static_cast<uint32_t>(max_keys);
@@ -1163,8 +966,7 @@ extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys, int64_t m
     int4 *d_k = nullptr;
     if (cudaMalloc(&d_k, n * sizeof(int4)) != cudaSuccess) return -1;
     std::vector<int4> tmp(n);
-    const uint32_t *list = grp ? v->meta.union_slots + static_cast<size_t>(v->last_group_buf) * v->meta.capacity
-                               : v->meta.active_slots + static_cast<size_t>(ring) * v->meta.capacity;
+    const uint32_t *list = v->meta.union_slots + static_cast<size_t>(buf) * v->meta.capacity;
     cudaError_t e = launch_gather_active_keys(v->table, list, n, d_k, v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
     if (e == cudaSuccess) e = cudaMemcpy(tmp.data(), d_k, n * sizeof(int4), cudaMemcpyDeviceToHost);
@@ -1326,7 +1128,6 @@ extern "C" int b2v_grid_create(float voxel_size, int32_t block_size, uint32_t ca
     B2V_CUDA(g, cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
     const uint32_t tcap = next_pow2(static_cast<uint64_t>(capacity_blocks) * 2);
     g->table.mask = tcap - 1;
-    g->table.stamp = nullptr;
     g->meta.capacity = capacity_blocks;
     B2V_CUDA(g, cudaMalloc(&g->table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
     B2V_CUDA(g, cudaMalloc(&g->meta.pool, static_cast<size_t>(capacity_blocks) * kGridBlockWordsHost * sizeof(uint32_t)));

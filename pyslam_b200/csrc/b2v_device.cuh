@@ -28,7 +28,6 @@ constexpr uint32_t kNoBlock = 0xFFFFFFFDu;  // pool overflowed: key present but 
 // with one LDG.128 and inserted with one 128-bit CAS (ATOMG.E.CAS.128 on sm_90a).
 struct HashTable {
     uint4 *entries;
-    uint32_t *stamp;  // frame id of the last frame that touched the slot
     uint32_t mask;    // capacity - 1 (capacity is a power of two)
 };
 

@@ -55,7 +55,7 @@ struct FramePose {
     double twc[3];
 };
 
-// Per-frame constants of the allocate kernels (+ the update constants of the frame-by-frame path).
+// Per-frame constants of the allocate kernels (+ the update constants of the frame-by-frame kernels).
 struct FrameParams {
     // f64 back-projection of the allocation samples (Open3D CreatePointCloudFromFloatDepthImage)
     double fx, fy, cx, cy;
@@ -67,11 +67,8 @@ struct FrameParams {
     float inv_vs, depth_trunc;
     int32_t unit_shift;     // log2(blocks per unit side): 0 = 8^3 units (D1 allocation), 1 = Open3D's 16^3 units
     int32_t H, W, stride;
-    uint32_t frame_id;
     int32_t shard_rank, shard_count;
-    // fused group mode (b2v_integrate_batch): this frame is bit `group_bit` of group buffer
-    // `group_buf`; -1 = per-frame mode (frame stamps + per-frame active lists)
-    int32_t group_bit, group_buf;
+    int32_t group_buf;      // group buffer the allocation records into (membership masks, union list, counters)
 };
 
 // Volume-wide constants of the update kernels (frame independent).
@@ -81,11 +78,11 @@ struct VolumeConsts {
     int32_t unit_shift;
 };
 
-// Fused group integration: up to kMaxGroup consecutive frames are applied to a block while it is
-// resident in registers.
+// Frames are integrated in groups.  Fused groups of up to kMaxGroup consecutive frames are applied to a block while
+// it is resident in registers; a single frame is a group of one on the frame-by-frame kernels.
 constexpr int kMaxGroup = 32;   // frames per fused group (bits of the membership mask); the default group is 16
-// group state (masks, union list, texel images, counters) is kGroupBufs-deep: the allocation of group g+3 may
-// run while group g is still being integrated
+// group state (masks, union list, staging, texel images, counters) is kGroupBufs-deep: the allocation of group g+3
+// may run while group g is still being integrated
 constexpr int kGroupBufs = 4;
 struct GroupArgs {
     IntFrame f[kMaxGroup];
@@ -98,7 +95,6 @@ struct PoolMeta {
     float *pool;              // [capacity][5][512] float32 planes: tsdf, weight, r, g, b
     int4 *block_keys;         // [capacity] key of pool block i (w unused)
     uint32_t *counters;       // device counters, see Counter
-    uint32_t *active_slots;   // [kActiveRing][capacity] table slots touched by a frame
     uint32_t *group_mask;     // [kGroupBufs][table capacity] bit k: the slot is touched by frame k of the group
     uint32_t *union_slots;    // [kGroupBufs][capacity] slots touched by any frame of the group
     uint32_t *block_flags;    // [capacity] sign summary for the mesh extraction's tile filter: bit 0 = some store left
@@ -112,8 +108,6 @@ enum Counter : int {
     kCtrError = 1,           // sticky error flag (1 = pool overflow, 2 = table full)
     kCtrUpdatesLo = 2,       // 64-bit total of (block, frame) updates since reset (8-byte aligned)
     kCtrUpdatesHi = 3,
-    kCtrActive0 = 4,         // [kActiveRing] per-frame counts of touched blocks
-    kCtrNew0 = 8,            // [kActiveRing] per-frame counts of newly allocated blocks
     kCtrVisitsLo = 12,       // 64-bit total of block visits (one block read + written) since reset
     kCtrVisitsHi = 13,
     kCtrGroup0 = 16,         // [kGroupBufs][kGroupCtrStride] per-group-buffer counters, contiguous so that ONE
@@ -131,7 +125,6 @@ constexpr int kGroupCtrStride = 4 + kMaxGroup;
 __host__ __device__ __forceinline__ constexpr int group_ctr(int buf, int which) {
     return kCtrGroup0 + buf * kGroupCtrStride + which;
 }
-constexpr int kActiveRing = 4;
 static_assert(kGcTouched0 + kMaxGroup <= kGroupCtrStride && kCtrGroup0 + kGroupBufs * kGroupCtrStride <= kNumCounters,
               "counter layout");
 
@@ -142,7 +135,7 @@ struct VolumeGeometry {   // set once per volume (b2v_create)
     int32_t shard_rank, shard_count;
 };
 void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], int H, int W,
-                       const VolumeGeometry &g, uint32_t frame_id);
+                       const VolumeGeometry &g);
 VolumeConsts volume_consts(const VolumeGeometry &g);
 
 // ---- kernels (b2v_tsdf.cu) ----
@@ -158,30 +151,28 @@ struct FrameMaps {
 bool tma_tiles_usable(int W, int stride, const void *depth, const void *color);
 // returns false if the driver entry point is unavailable or encoding fails
 bool encode_frame_maps(FrameMaps *maps, const float *depth, const uint8_t *color, int H, int W, int tile);
-// frame packing (texels) + allocation + touched-set of one frame;
-// zeroes the next frame's ring counters.  maps != nullptr: the image tiles are staged into shared
-// memory with TMA (cp.async.bulk.tensor.2d); nullptr: plain loads.
-cudaError_t launch_allocate(const FrameParams &p, const float *depth, const uint8_t *color,
-                            Texel *texels, const HashTable &table, const PoolMeta &meta, int ring,
-                            const FrameMaps *maps,
-                            cudaStream_t stream);
-// projective TSDF + colour update of every block touched by the frame
-cudaError_t launch_integrate(const FrameParams &p, const VolumeConsts &vc, const HashTable &table,
-                             const PoolMeta &meta, int ring, int grid_ctas, cudaStream_t stream);
-// all frames of a group in ONE launch (blockIdx.z = frame): the per-frame latency chains overlap
+// Frame packing (texels) + allocation + touched set of the frames of a group, recorded in group buffer
+// P.group_buf.  use_tma: the image tiles are staged into shared memory with TMA (cp.async.bulk.tensor.2d); else
+// plain loads.
 struct GroupAllocArgs {
-    FrameParams P;                 // constants shared by the frames of the group (P.pose / P.I unused)
+    FrameParams P;                 // constants shared by the frames of the group (P.pose / P.I: frame 0's)
     FramePose pose[kMaxGroup];
     const float *depth[kMaxGroup];
     const uint8_t *color[kMaxGroup];
     Texel *tex[kMaxGroup];
     FrameMaps maps[kMaxGroup];
-    uint32_t frame_id0;            // frame id of the group's first frame
     int32_t count, use_tma;
 };
 static_assert(sizeof(GroupAllocArgs) < 32000, "kernel parameter space");
+// a one-frame group (frame 0 of args), with the frame-by-frame allocate_kernel
+cudaError_t launch_allocate(const GroupAllocArgs &args, const HashTable &table, const PoolMeta &meta,
+                            cudaStream_t stream);
+// all frames of a group in ONE launch (blockIdx.z = frame): the per-frame latency chains overlap
 cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &table,
                                   const PoolMeta &meta, cudaStream_t stream);
+// projective TSDF + colour update of every block touched by the one-frame group in group buffer group_buf
+cudaError_t launch_integrate(const IntFrame &f, const VolumeConsts &vc, const HashTable &table,
+                             const PoolMeta &meta, int group_buf, int grid_ctas, cudaStream_t stream);
 int integrate_max_resident_ctas_per_sm();
 // d_bad[0]: reciprocals (3 x 2^23 inputs), d_bad[1]: quotients (`pairs` inputs) whose fast path differs from IEEE
 cudaError_t launch_selftest_division(unsigned long long *d_bad, uint64_t pairs, cudaStream_t stream);
@@ -191,8 +182,8 @@ cudaError_t launch_integrate_group(const GroupArgs &args, const HashTable &table
 // hashes[i] = BlockKeyHash(block_keys[i])
 cudaError_t launch_block_hashes(const int4 *block_keys, uint64_t *hashes, uint32_t n,
                                 cudaStream_t stream);
-// keys of the slots in an active list
-cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *active_slots,
+// keys of the slots in a touched list
+cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *slots,
                                       uint32_t n, int4 *out, cudaStream_t stream);
 
 // find-or-create the blocks of `keys` (unique) and copy `vox` [n][5][512] into them

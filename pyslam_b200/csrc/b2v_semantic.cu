@@ -729,7 +729,6 @@ extern "C" int b2v_sgrid_create(double voxel_size, int32_t block_size, uint32_t 
     uint64_t tcap = 1;
     while (tcap < static_cast<uint64_t>(capacity_blocks) * 2) tcap <<= 1;
     g->table.mask = static_cast<uint32_t>(tcap - 1);
-    g->table.stamp = nullptr;
     const size_t nv = static_cast<size_t>(capacity_blocks) * kVox;
     SG_CUDA(g, cudaMalloc(&g->table.entries, tcap * sizeof(uint4)));
     SG_CUDA(g, cudaMalloc(&g->G.counters, kSemNumCounters * sizeof(uint32_t)));
