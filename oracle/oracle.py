@@ -450,6 +450,75 @@ def numpy_touched_blocks(depth, K, Tcw, voxel_size, sdf_trunc, depth_trunc, bloc
     return out
 
 
+def numpy_point_cloud(dump, voxel_length, unit_resolution=16):
+    """A.4 ExtractPointCloud restated in numpy from a block dump (keys int32 [nb,3], vox float32 [nb,5,512]): the
+    formulas DESIGN §3 and b2v_mesh.cu state, evaluated with numpy's IEEE operations (float64 positions, float32
+    weights of the blend and float32 colours).  It pins that documented formula, not a running Open3D; whether
+    Open3D also re-evaluates the two off-axis coordinates through the blend is not pinned.
+      selection  w != 0 and -0.98 <= f < 0.98 at both ends of an edge along +x / +y / +z (across block borders;
+                 a missing neighbour is unobserved) and f0 * f1 < 0 in float32
+      position   p0 = (vl/2 + vl * x_in_unit) + unit * L (float64, L = vl * unit_resolution); on the edge's axis
+                 p = (p0 r1 + (p0 + vl) r0) / rs with r0 = |f0|, r1 = |f1|, rs = r0 + r1 in float32
+      colour     ((c0 r1 + c1 r0) / rs) / 255 in float32, widened
+    Returns dict(points f64 [n,3], colors f64 [n,3], edges int32 [n,4] = global voxel (x, y, z) + axis)."""
+    keys = np.asarray(dump["keys"], np.int64)
+    vox = np.asarray(dump["vox"], np.float32)
+    nb = len(keys)
+    S = {8: 0, 16: 1, 32: 2}[int(unit_resolution)]
+    vl = float(voxel_length)
+    half = vl * 0.5
+    L = vl * float(8 << S)
+    idx = {tuple(k): i for i, k in enumerate(keys.tolist())}
+    f = vox[:, 0].reshape(nb, 8, 8, 8)      # [b, z, y, x]
+    w = vox[:, 1].reshape(nb, 8, 8, 8)
+    c = vox[:, 2:].reshape(nb, 3, 8, 8, 8)
+    lz, ly, lx = np.meshgrid(np.arange(8), np.arange(8), np.arange(8), indexing="ij")
+    loc = (lx, ly, lz)
+    pts, cols, edges = [], [], []
+    a98 = np.float32(0.98)
+    for a in range(3):
+        # the voxel at +1 along axis a: shift inside the block, the first slab of the neighbour at the border
+        ax = 3 - a                          # array axis of spatial axis a in [b, z, y, x] (c: one more)
+        nbr = np.array([idx.get((k[0] + (a == 0), k[1] + (a == 1), k[2] + (a == 2)), -1) for k in keys.tolist()],
+                       np.int64)
+        has = nbr >= 0
+        nsafe = np.where(has, nbr, 0)
+
+        def shifted(arr, axis):
+            inner = np.take(arr, range(1, 8), axis=axis)
+            border = np.take(arr[nsafe], [0], axis=axis)
+            return np.concatenate([inner, border], axis=axis)
+
+        f1, w1, c1 = shifted(f, ax), shifted(w, ax), shifted(c, ax + 1)
+        border_missing = np.zeros((nb, 8, 8, 8), bool)
+        sl = [slice(None)] * 4
+        sl[ax] = slice(7, 8)
+        border_missing[tuple(sl)] = ~has[:, None, None, None]
+        ok0 = (w != 0) & (f < a98) & (f >= -a98)
+        ok1 = (w1 != 0) & (f1 < a98) & (f1 >= -a98) & ~border_missing
+        sel = ok0 & ok1 & (f * f1 < np.float32(0))
+        b, z, y, x = np.nonzero(sel)
+        l3 = np.stack([x, y, z], 1)
+        k3 = keys[b]
+        u = k3 >> S
+        xin = (k3 - (u << S)) * 8 + l3
+        p0 = (half + vl * xin.astype(np.float64)) + u.astype(np.float64) * L
+        r0 = np.abs(f[b, z, y, x])
+        r1 = np.abs(f1[b, z, y, x])
+        rs = r0 + r1                                    # float32
+        pa = p0[:, a]
+        p = p0.copy()
+        p[:, a] = (pa * r1.astype(np.float64) + (pa + vl) * r0.astype(np.float64)) / rs.astype(np.float64)
+        col = np.empty((len(b), 3), np.float64)
+        for k in range(3):
+            num = c[b, k, z, y, x] * r1 + c1[b, k, z, y, x] * r0   # float32 products and sum
+            col[:, k] = ((num / rs) / np.float32(255.0)).astype(np.float64)
+        pts.append(p)
+        cols.append(col)
+        edges.append(np.concatenate([k3 * 8 + l3, np.full((len(b), 1), a)], 1).astype(np.int32))
+    return dict(points=np.concatenate(pts), colors=np.concatenate(cols), edges=np.concatenate(edges))
+
+
 def numpy_integrate_block(vox, key, depth, color, K, Tcw, voxel_size, sdf_trunc, depth_trunc,
                           block_size=8):
     """A.3 update of one block in float32 numpy (no FMA, true divisions): an independent second
