@@ -16,10 +16,12 @@ legs may import this package; the product (`pyslam_b200/`) never does.
                   truth the twin above and the kernels are measured against, with the tolerances of SURVEY.md 8c.
 * `numpy_tsdf`  - a second, independent numpy restatement of A.3 used to pin the C oracle.
 * `numpy_point_cloud` - numpy restatement of the documented ExtractPointCloud formulas (DESIGN §3) on a block dump.
+* `numpy_grid`  - numpy restatement of the point-average `VoxelBlockGrid` (keys, sums, queries, carve).
+* `numpy_shadow_filter` - numpy restatement of the reference's `filter_shadow_points` (median threshold).
 """
 
-from .oracle import (EigenOps, Open3DOrderVolume, have_eigen_ops, open3d_order_inverse4, RefGrid, RefSemanticGrid, TsdfOracle, build, canonical_mesh, have_ref, have_ref_semantic, numpy_integrate_block,
-                     numpy_point_cloud, numpy_touched_blocks, ref_block_key_hash, ref_floor_div, ref_keys)
+from .oracle import (EigenOps, Open3DOrderVolume, have_eigen_ops, open3d_order_inverse4, RefGrid, RefSemanticGrid, TsdfOracle, build, canonical_mesh, have_ref, have_ref_semantic, numpy_grid, numpy_integrate_block,
+                     numpy_point_cloud, numpy_shadow_filter, numpy_touched_blocks, ref_block_key_hash, ref_floor_div, ref_keys)
 
-__all__ = ["EigenOps", "have_eigen_ops", "open3d_order_inverse4", "Open3DOrderVolume", "RefGrid", "RefSemanticGrid", "TsdfOracle", "build", "canonical_mesh", "have_ref", "have_ref_semantic", "numpy_integrate_block",
-           "numpy_point_cloud", "numpy_touched_blocks", "ref_block_key_hash", "ref_floor_div", "ref_keys"]
+__all__ = ["EigenOps", "have_eigen_ops", "open3d_order_inverse4", "Open3DOrderVolume", "RefGrid", "RefSemanticGrid", "TsdfOracle", "build", "canonical_mesh", "have_ref", "have_ref_semantic", "numpy_grid", "numpy_integrate_block",
+           "numpy_point_cloud", "numpy_shadow_filter", "numpy_touched_blocks", "ref_block_key_hash", "ref_floor_div", "ref_keys"]

@@ -519,6 +519,190 @@ def numpy_point_cloud(dump, voxel_length, unit_resolution=16):
     return dict(points=np.concatenate(pts), colors=np.concatenate(cols), edges=np.concatenate(edges))
 
 
+class numpy_grid:
+    """The point-average `VoxelBlockGrid` (b2v_grid.cu, voxel_block_grid.hpp) restated in numpy, voxel by voxel.
+      keys       float32 points: floor(float32(x * inv_vs)), inv_vs = float32(1 / voxel_size);
+                 float64 points: floor(x * float64(inv_vs)); block = floor_div(voxel, 8)
+      sums       count += 1, pos += float32(x), col += c (float32 c, or float32(c) * float32(1/255) for uint8),
+                 accumulated in input order in float32 (np.add.at)
+      means      sum / float32(count)
+      queries    count >= min_count, voxel key inside the float64 key bounds floor(bb * float64(inv_vs)), then the
+                 float64 box test or the frustum test of CameraFrustrum::contains (R p + t in float64, in the kernel's
+                 order; u = float32(fx * (x / z) + cx), 0 <= u < W, depth = float32(z) in [depth_min, depth_max])
+      carve      the depth at truncated (v, u); skipped when <= 0 or not finite; reset when depth < image - thr
+    A block exists once a point lands in it; resetting voxels (remove_low_count_voxels, carve) keeps the block."""
+
+    def __init__(self, voxel_size):
+        self.inv_vs = np.float32(1.0) / np.float32(voxel_size)
+        self.clear()
+
+    def clear(self):
+        self.keys = np.zeros((0, 3), np.int64)      # voxel keys, one row per voxel ever touched
+        self.count = np.zeros(0, np.int64)
+        self.pos = np.zeros((0, 3), np.float32)
+        self.col = np.zeros((0, 3), np.float32)
+
+    def voxel_keys(self, points):
+        p = np.asarray(points)
+        if p.dtype == np.float64:
+            return np.floor(p * np.float64(self.inv_vs)).astype(np.int64)
+        assert p.dtype == np.float32
+        return np.floor(p * self.inv_vs).astype(np.int64)
+
+    def integrate(self, points, colors=None):
+        p = np.asarray(points)
+        if len(p) == 0:
+            return
+        vk = self.voxel_keys(p)
+        allk, inv = np.unique(np.concatenate([self.keys, vk]), axis=0, return_inverse=True)
+        inv = inv.reshape(-1)
+        old, new = inv[:len(self.keys)], inv[len(self.keys):]
+        count = np.zeros(len(allk), np.int64)
+        pos = np.zeros((len(allk), 3), np.float32)
+        col = np.zeros((len(allk), 3), np.float32)
+        count[old], pos[old], col[old] = self.count, self.pos, self.col
+        np.add.at(count, new, 1)
+        np.add.at(pos, new, p.astype(np.float32))
+        if colors is not None:
+            c = np.asarray(colors)
+            c = c.astype(np.float32) * (np.float32(1.0) / np.float32(255.0)) if c.dtype == np.uint8 else \
+                c.astype(np.float32)
+            np.add.at(col, new, c)
+        self.keys, self.count, self.pos, self.col = allk, count, pos, col
+
+    def block_keys(self):
+        return np.unique(self.keys // 8, axis=0).astype(np.int32).reshape(-1, 3)
+
+    def dump(self):
+        """Like `sort_dump(grid.dump_blocks())` without the hashes: keys [nb,3] sorted, count [nb,512],
+        pos_sum / col_sum [nb,512,3]."""
+        bk = self.block_keys()
+        nb = len(bk)
+        count = np.zeros((nb, 512), np.int32)
+        pos = np.zeros((nb, 512, 3), np.float32)
+        col = np.zeros((nb, 512, 3), np.float32)
+        if nb:
+            b = np.searchsorted(self._block_ids(bk), self._block_ids(self.keys // 8))
+            lk = self.keys - (self.keys // 8) * 8
+            l = lk[:, 0] + 8 * lk[:, 1] + 64 * lk[:, 2]
+            count[b, l], pos[b, l], col[b, l] = self.count, self.pos, self.col
+        return dict(keys=bk, count=count, pos_sum=pos, col_sum=col)
+
+    @staticmethod
+    def _block_ids(k):
+        k = np.asarray(k, np.int64) + (1 << 20)
+        return (k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2]
+
+    def remove_low_count_voxels(self, min_count):
+        low = self.count < min_count
+        self.count[low] = 0
+        self.pos[low] = 0
+        self.col[low] = 0
+
+    def _means(self, sel):
+        c = self.count[sel].astype(np.float32)[:, None]
+        return self.pos[sel] / c, self.col[sel] / c
+
+    def get_voxels(self, min_count=1):
+        """(points, colours) of the voxels with count >= min_count (min_count >= 1), in voxel-key order."""
+        return self._means(self.count >= min_count)
+
+    def _key_bounds(self, bb):
+        bb = np.asarray(bb, np.float64)
+        return (np.floor(bb[:3] * np.float64(self.inv_vs)).astype(np.int64),
+                np.floor(bb[3:] * np.float64(self.inv_vs)).astype(np.int64))
+
+    def _in_keys(self, bb, min_count):
+        lo, hi = self._key_bounds(bb)
+        return (self.count >= min_count) & np.all((self.keys >= lo) & (self.keys <= hi), axis=1)
+
+    def get_voxels_in_bb(self, bbox, min_count=1):
+        bb = np.asarray(bbox, np.float64).reshape(6)
+        sel = np.flatnonzero(self._in_keys(bb, min_count))
+        p, c = self._means(sel)
+        q = p.astype(np.float64)
+        ok = np.all((q >= bb[:3]) & (q <= bb[3:]), axis=1)
+        return p[ok], c[ok]
+
+    @staticmethod
+    def frustum_bounds(K, W, H, Tcw, depth_max, depth_min):
+        """fill_frustum_query: the world AABB [6] of the 8 frustum corners, float64, in the kernel's order."""
+        fx, fy, cx, cy = [np.float64(np.float32(v)) for v in K]
+        T = np.asarray(Tcw, np.float64).reshape(4, 4)
+        R, t = T[:3, :3], T[:3, 3]
+        twc = [-((R[0, i] * t[0] + R[1, i] * t[1]) + R[2, i] * t[2]) for i in range(3)]
+        lo, hi = np.full(3, 1e300), np.full(3, -1e300)
+        for u, v in ((0.0, 0.0), (float(W), 0.0), (float(W), float(H)), (0.0, float(H))):
+            xn, yn = (u - cx) / fx, (v - cy) / fy
+            for d in (np.float64(np.float32(depth_min)), np.float64(np.float32(depth_max))):
+                pc = (xn * d, yn * d, d)
+                for a in range(3):
+                    w = ((R[0, a] * pc[0] + R[1, a] * pc[1]) + R[2, a] * pc[2]) + twc[a]
+                    lo[a], hi[a] = min(lo[a], w), max(hi[a], w)
+        return np.concatenate([lo, hi])
+
+    @staticmethod
+    def project(points, K, W, H, Tcw, depth_max, depth_min):
+        """CameraFrustrum::contains on float32 points -> (inside, u, v, depth) with u, v, depth float32."""
+        fx, fy, cx, cy = [np.float64(np.float32(v)) for v in K]
+        T = np.asarray(Tcw, np.float64).reshape(4, 4)
+        p = np.asarray(points, np.float32).astype(np.float64)
+        pc = [((T[a, 0] * p[:, 0] + T[a, 1] * p[:, 1]) + T[a, 2] * p[:, 2]) + T[a, 3] for a in range(3)]
+        depth = pc[2].astype(np.float32)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            u = (fx * (pc[0] / pc[2]) + cx).astype(np.float32)
+            v = (fy * (pc[1] / pc[2]) + cy).astype(np.float32)
+        ok = (depth >= np.float32(depth_min)) & (depth <= np.float32(depth_max))
+        ok &= (u >= 0) & (u < np.float32(W)) & (v >= 0) & (v < np.float32(H))
+        return ok, u, v, depth
+
+    def _frustum_select(self, K, W, H, Tcw, depth_max, depth_min, min_count):
+        bb = self.frustum_bounds(K, W, H, Tcw, depth_max, depth_min)
+        sel = np.flatnonzero(self._in_keys(bb, min_count))
+        p, c = self._means(sel)
+        ok, u, v, depth = self.project(p, K, W, H, Tcw, depth_max, depth_min)
+        return sel[ok], p[ok], c[ok], u[ok], v[ok], depth[ok]
+
+    def get_voxels_in_frustum(self, K, W, H, Tcw, depth_max=10.0, depth_min=1e-2, min_count=1):
+        _, p, c, _, _, _ = self._frustum_select(K, W, H, Tcw, depth_max, depth_min, min_count)
+        return p, c
+
+    def carve(self, K, W, H, Tcw, depth_image, depth_threshold, depth_max=10.0, depth_min=1e-2):
+        """Resets the carved voxels; returns their indices into `keys`."""
+        sel, _, _, u, v, depth = self._frustum_select(K, W, H, Tcw, depth_max, depth_min, 1)
+        img = np.asarray(depth_image, np.float32)[v.astype(np.int64), u.astype(np.int64)]
+        with np.errstate(invalid="ignore"):
+            cut = (img > 0) & np.isfinite(img) & (depth < img - np.float32(depth_threshold))
+        gone = sel[cut]
+        self.count[gone] = 0
+        self.pos[gone] = 0
+        self.col[gone] = 0
+        return gone
+
+
+def numpy_shadow_filter(depth, delta_x=2, delta_y=2, fill_value=-1.0):
+    """`filter_shadow_points(depth, delta_depth=None)` (pyslam/utilities/depth.py:103-146) restated in numpy 2:
+    deltas |d[dy:] - d[:-dy]| and |d[:, dx:] - d[:, :-dx]| in float32, threshold 3 * (1.4826 * median of the
+    positive deltas) in float32 (NaN without positive deltas: nothing is filtered), both pixels of an
+    over-threshold pair set to fill_value.  Returns (filtered, threshold)."""
+    d = np.asarray(depth, np.float32)
+    assert d.ndim == 2 and 1 <= delta_y < d.shape[0] and 1 <= delta_x < d.shape[1]
+    with np.errstate(invalid="ignore"):
+        dv = np.abs(d[delta_y:] - d[:-delta_y])
+        dh = np.abs(d[:, delta_x:] - d[:, :-delta_x])
+        vals = np.concatenate([dv.ravel(), dh.ravel()])
+        pos = vals[vals > 0]
+        mad = np.median(pos) if len(pos) else np.float32(np.nan)
+        thr = np.float32(3.0) * (np.float32(1.4826) * np.float32(mad))
+        mv, mh = dv > thr, dh > thr
+    mask = np.zeros(d.shape, bool)
+    mask[delta_y:] |= mv
+    mask[:-delta_y] |= mv
+    mask[:, delta_x:] |= mh
+    mask[:, :-delta_x] |= mh
+    return np.where(mask, np.float32(fill_value), d), thr
+
+
 def numpy_integrate_block(vox, key, depth, color, K, Tcw, voxel_size, sdf_trunc, depth_trunc,
                           block_size=8):
     """A.3 update of one block in float32 numpy (no FMA, true divisions): an independent second

@@ -6,7 +6,8 @@
 // here each block stores the same seven fields as 512-wide planes so a warp's accesses coalesce.
 //   keys: voxel = floor(p * inv_vs) (voxel_hashing.h:69-75), block = floor_div(voxel, 8),
 //         local index lx + 8 ly + 64 lz (voxel_block.h:67-70) -- bit exact.
-//   sums: float atomics => same values as the reference up to summation order.
+//   sums: float atomics => same values as the reference up to summation order; sub-normal addends are kept
+//         (sum_add), as the reference's float adds keep them.
 #include "b2v_internal.h"
 #include "b2v_scan.cuh"
 
@@ -67,6 +68,23 @@ grid_insert_kernel(const Tp *__restrict__ pts, const int64_t n, const float inv_
 }
 
 // ---- pass 2: accumulate ----------------------------------------------------------------------
+// running float sum += x as the reference's float add does it.  Float atomics (red.global.add.f32) flush sub-normal
+// operands and results to zero.  An addend of magnitude >= 2^-100 can neither make a sub-normal sum nor lose anything
+// but a sub-normal sum that rounding would drop anyway, so it takes the atomic; smaller non-zero addends go through a
+// compare-and-swap of an IEEE add.  Adding +-0 leaves every sum unchanged (sums start at +0).
+__device__ __forceinline__ void sum_add(float *p, float x) {
+    if (fabsf(x) >= 0x1p-100f) {
+        atomicAdd(p, x);
+    } else if (x != 0.0f) {
+        unsigned int *u = reinterpret_cast<unsigned int *>(p);
+        unsigned int old = *u, assumed;
+        do {
+            assumed = old;
+            old = atomicCAS(u, assumed, __float_as_uint(__fadd_rn(__uint_as_float(assumed), x)));
+        } while (old != assumed);
+    }
+}
+
 // colour of a point as the voxel accumulates it: float passthrough, uint8 * (1.0f / 255.0f) (voxel_data.h:79-97)
 __device__ __forceinline__ float color_value(float c) { return c; }
 __device__ __forceinline__ float color_value(uint8_t c) { return __fmul_rn(static_cast<float>(c), 1.0f / 255.0f); }
@@ -88,13 +106,13 @@ grid_accumulate_kernel(const Tp *__restrict__ pts, const Tc *__restrict__ cols, 
     const int l = local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6);
     uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords;
     float *fb = reinterpret_cast<float *>(blk);
-    atomicAdd(fb + 1 * kVox + l, x);
-    atomicAdd(fb + 2 * kVox + l, y);
-    atomicAdd(fb + 3 * kVox + l, z);
+    sum_add(fb + 1 * kVox + l, x);
+    sum_add(fb + 2 * kVox + l, y);
+    sum_add(fb + 3 * kVox + l, z);
     if (cols != nullptr) {
-        atomicAdd(fb + 4 * kVox + l, color_value(cols[3 * i + 0]));
-        atomicAdd(fb + 5 * kVox + l, color_value(cols[3 * i + 1]));
-        atomicAdd(fb + 6 * kVox + l, color_value(cols[3 * i + 2]));
+        sum_add(fb + 4 * kVox + l, color_value(cols[3 * i + 0]));
+        sum_add(fb + 5 * kVox + l, color_value(cols[3 * i + 1]));
+        sum_add(fb + 6 * kVox + l, color_value(cols[3 * i + 2]));
     }
     atomicAdd(reinterpret_cast<int *>(blk) + l, 1);
 }
@@ -173,12 +191,12 @@ grid_rgbd_accumulate_kernel(const RgbdParams P, const float *__restrict__ depth,
     const int l = local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6);
     uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords;
     float *fb = reinterpret_cast<float *>(blk);
-    atomicAdd(fb + 1 * kVox + l, pt[0]);
-    atomicAdd(fb + 2 * kVox + l, pt[1]);
-    atomicAdd(fb + 3 * kVox + l, pt[2]);
+    sum_add(fb + 1 * kVox + l, pt[0]);
+    sum_add(fb + 2 * kVox + l, pt[1]);
+    sum_add(fb + 3 * kVox + l, pt[2]);
 #pragma unroll
     for (int c = 0; c < 3; ++c)  // image[valid] / 255.0 in float64, then float32 (depth.py:76, voxel_grid.py:271-273)
-        atomicAdd(fb + (4 + c) * kVox + l, __double2float_rn(__ddiv_rn(static_cast<double>(rgb[3 * i + c]), 255.0)));
+        sum_add(fb + (4 + c) * kVox + l, __double2float_rn(__ddiv_rn(static_cast<double>(rgb[3 * i + c]), 255.0)));
     atomicAdd(reinterpret_cast<int *>(blk) + l, 1);
 }
 

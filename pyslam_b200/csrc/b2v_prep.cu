@@ -197,14 +197,19 @@ cudaError_t launch_filter_shadow_points(const float *depth, int H, int W, int dx
 //   linear (8-bit): sx = round_half_even(mapx * 32), pixel = sx >> 5, fraction a = sx & 31;
 //                   weights (32-ay)(32-ax)*32, ... (sum 32768); out = (sum w*p + 16384) >> 15
 //   nearest:        pixel = round_half_even(mapx)
+// A NaN map coordinate converts to INT_MIN, as OpenCV's cvRound does on x86 (cvtss2si), so the pixel lies outside
+// the image and takes the zero border; the PTX conversion alone would give 0 and read column / row 0.
 // ------------------------------------------------------------------------------------------------
+constexpr int kNanMapCoord = INT_MIN;
+
 __global__ void remap_u8c3_linear_kernel(const uint8_t *__restrict__ src, int H, int W,
                                          const float *__restrict__ mapx, const float *__restrict__ mapy,
                                          uint8_t *__restrict__ dst, int swap_rb) {
     const int64_t n = static_cast<int64_t>(H) * W;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int sx = __float2int_rn(__fmul_rn(mapx[i], 32.0f)), sy = __float2int_rn(__fmul_rn(mapy[i], 32.0f));
+        const float fx = __fmul_rn(mapx[i], 32.0f), fy = __fmul_rn(mapy[i], 32.0f);
+        const int sx = isnan(fx) ? kNanMapCoord : __float2int_rn(fx), sy = isnan(fy) ? kNanMapCoord : __float2int_rn(fy);
         const int x0 = sx >> 5, y0 = sy >> 5, ax = sx & 31, ay = sy & 31;
         const int w00 = (32 - ay) * (32 - ax) * 32, w01 = (32 - ay) * ax * 32, w10 = ay * (32 - ax) * 32,
                   w11 = ay * ax * 32;
@@ -233,7 +238,8 @@ __global__ void remap_b32_nearest_kernel(const uint32_t *__restrict__ src, int H
     const int64_t n = static_cast<int64_t>(H) * W;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int x = __float2int_rn(mapx[i]), y = __float2int_rn(mapy[i]);
+        const int x = isnan(mapx[i]) ? kNanMapCoord : __float2int_rn(mapx[i]),
+                  y = isnan(mapy[i]) ? kNanMapCoord : __float2int_rn(mapy[i]);
         dst[i] = (x >= 0 && x < W && y >= 0 && y < H) ? src[static_cast<int64_t>(y) * W + x] : 0u;
     }
 }
