@@ -26,7 +26,8 @@ VOXEL_PLANES = 5
 #: every symbol include/b2v.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
     "b2v_create", "b2v_destroy", "b2v_reset", "b2v_last_error", "b2v_integrate",
-    "b2v_integrate_batch", "b2v_integrate_u16", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_num_blocks", "b2v_last_frame_stats", "b2v_last_mesh_stats",
+    "b2v_integrate_batch", "b2v_integrate_u16", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_capacity",
+    "b2v_num_blocks", "b2v_last_frame_stats", "b2v_last_mesh_stats",
     "b2v_counters", "b2v_set_overlap", "b2v_set_fusion", "b2v_set_group_size", "b2v_set_input_event", "b2v_set_rectification", "b2v_remap", "b2v_profile_enable", "b2v_profile_read", "b2v_dump_blocks", "b2v_upload_blocks", "b2v_export_blocks_device", "b2v_import_blocks_device", "b2v_last_touched_keys", "b2v_extract_mesh", "b2v_copy_mesh",
     "b2v_extract_points", "b2v_copy_points", "b2v_grid_create", "b2v_grid_destroy", "b2v_grid_clear",
     "b2v_grid_last_error", "b2v_grid_integrate", "b2v_grid_integrate_f64", "b2v_grid_integrate_ex", "b2v_grid_integrate_rgbd", "b2v_filter_shadow_points", "b2v_grid_synchronize", "b2v_grid_num_blocks",
@@ -59,6 +60,7 @@ class B2VConfig(C.Structure):
         ("unit_resolution", C.c_int32),
         ("voxel_length", C.c_double),
         ("sdf_trunc_d", C.c_double),
+        ("max_capacity_blocks", C.c_uint32),
     ]
 
 
@@ -98,6 +100,8 @@ def load() -> C.CDLL:
     L.b2v_integrate_batch.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp]
     L.b2v_synchronize.restype = C.c_int
     L.b2v_synchronize.argtypes = [vp]
+    L.b2v_capacity.restype = C.c_int
+    L.b2v_capacity.argtypes = [vp, p_i64, p_i64]
     L.b2v_num_blocks.restype = i64
     L.b2v_num_blocks.argtypes = [vp]
     L.b2v_last_mesh_stats.restype = C.c_int

@@ -15,7 +15,9 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/b2v.h"
@@ -137,6 +139,17 @@ struct b2v_volume {
     size_t stage_pixels = 0;
     HashTable table{};
     PoolMeta meta{};
+    // The pool is one virtual-address reservation for meta.capacity blocks; physical chunks are mapped as it grows
+    // (fixed volumes map it whole at create), so the pool address the kernels see never changes.
+    bool growable = false;               // max_capacity_blocks > capacity_blocks
+    CUdeviceptr pool_va = 0;
+    size_t pool_reserved = 0, pool_mapped = 0, pool_gran = 0;   // bytes
+    std::vector<std::pair<size_t, size_t>> pool_chunks;         // (offset, bytes) of each mapping
+    int64_t growths = 0;
+    // update launch of the group in each buffer, kept for the replay of a skipped group
+    GroupArgs gargs[kGroupBufs];
+    bool gfused[kGroupBufs] = {};
+    uint32_t *h_skip = nullptr;          // pinned [kGroupBufs]: counters[kCtrSkipping] after the gate of the buffer's group
     int grid_ctas = 0;
     int sm_count = 0;
     int64_t launches = 0;
@@ -163,6 +176,120 @@ struct b2v_volume {
         }                                                                                  \
     } while (0)
 
+// ---- the block pool: virtual memory management entry points of the driver ----
+
+namespace {
+struct VmmApi {
+    decltype(&cuMemGetAllocationGranularity) granularity;
+    decltype(&cuMemAddressReserve) reserve;
+    decltype(&cuMemAddressFree) address_free;
+    decltype(&cuMemCreate) create;
+    decltype(&cuMemRelease) release;
+    decltype(&cuMemMap) map;
+    decltype(&cuMemUnmap) unmap;
+    decltype(&cuMemSetAccess) set_access;
+};
+
+const VmmApi *vmm_api() {
+    static VmmApi api{};
+    static const bool ok = [] {
+        auto get = [](const char *name, auto *fn) {
+            void *sym = nullptr;
+            cudaDriverEntryPointQueryResult st;
+            if (cudaGetDriverEntryPoint(name, &sym, cudaEnableDefault, &st) != cudaSuccess ||
+                st != cudaDriverEntryPointSuccess || !sym)
+                return false;
+            *fn = reinterpret_cast<std::remove_pointer_t<decltype(fn)>>(sym);
+            return true;
+        };
+        return get("cuMemGetAllocationGranularity", &api.granularity) && get("cuMemAddressReserve", &api.reserve) &&
+               get("cuMemAddressFree", &api.address_free) && get("cuMemCreate", &api.create) &&
+               get("cuMemRelease", &api.release) && get("cuMemMap", &api.map) && get("cuMemUnmap", &api.unmap) &&
+               get("cuMemSetAccess", &api.set_access);
+    }();
+    return ok ? &api : nullptr;
+}
+
+CUmemAllocationProp pool_prop(int device) {
+    CUmemAllocationProp p{};
+    p.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    p.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    p.location.id = device;
+    return p;
+}
+
+constexpr size_t kBlockBytes = static_cast<size_t>(kBlockFloats) * sizeof(float);
+}  // namespace
+
+#define B2V_CU(v, call)                                                                    \
+    do {                                                                                   \
+        CUresult r_ = (call);                                                              \
+        if (r_ != CUDA_SUCCESS) {                                                          \
+            (v)->err = std::string(#call) + ": CUresult " + std::to_string(r_);            \
+            return B2V_ERR_CUDA;                                                           \
+        }                                                                                  \
+    } while (0)
+
+// reserve the address range of meta.capacity blocks
+static int pool_reserve(b2v_volume *v) {
+    const VmmApi *api = vmm_api();
+    if (!api) {
+        v->err = "the driver's virtual memory management entry points are unavailable";
+        return B2V_ERR_CUDA;
+    }
+    const CUmemAllocationProp prop = pool_prop(v->cfg.device);
+    B2V_CU(v, api->granularity(&v->pool_gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM));
+    const size_t g = v->pool_gran;
+    v->pool_reserved = (static_cast<size_t>(v->meta.capacity) * kBlockBytes + g - 1) / g * g;
+    B2V_CU(v, api->reserve(&v->pool_va, v->pool_reserved, 0, 0, 0));
+    v->meta.pool = reinterpret_cast<float *>(v->pool_va);
+    return B2V_OK;
+}
+
+// map (and zero) storage for at least `blocks` blocks, in whole granules, up to the reservation; pool_capacity follows
+static int pool_map(b2v_volume *v, uint64_t blocks) {
+    const size_t g = v->pool_gran;
+    const size_t want = std::min(v->pool_reserved, (static_cast<size_t>(blocks) * kBlockBytes + g - 1) / g * g);
+    if (want > v->pool_mapped) {
+        const VmmApi *api = vmm_api();
+        const size_t off = v->pool_mapped, bytes = want - off;
+        const CUmemAllocationProp prop = pool_prop(v->cfg.device);
+        CUmemGenericAllocationHandle h;
+        B2V_CU(v, api->create(&h, bytes, &prop, 0));
+        const CUresult r = api->map(v->pool_va + off, bytes, 0, h, 0);
+        api->release(h);  // the mapping keeps the memory until it is unmapped
+        B2V_CU(v, r);
+        v->pool_chunks.emplace_back(off, bytes);
+        CUmemAccessDesc acc{};
+        acc.location = prop.location;
+        acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+        B2V_CU(v, api->set_access(v->pool_va + off, bytes, &acc, 1));
+        v->pool_mapped = want;
+        // allocation relies on a zeroed pool
+        B2V_CUDA(v, cudaMemsetAsync(reinterpret_cast<char *>(v->meta.pool) + off, 0, bytes, v->compute));
+    }
+    v->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(v->meta.capacity, v->pool_mapped / kBlockBytes));
+    return B2V_OK;
+}
+
+static void pool_release(b2v_volume *v) {
+    const VmmApi *api = vmm_api();
+    if (!api || !v->pool_va) return;
+    for (const auto &c : v->pool_chunks) api->unmap(v->pool_va + c.first, c.second);
+    api->address_free(v->pool_va, v->pool_reserved);
+    v->pool_chunks.clear();
+    v->pool_va = 0;
+}
+
+// growth policy: at least double, at least `need` blocks, at most the maximum
+static int pool_grow(b2v_volume *v, uint64_t need) {
+    const uint32_t old = v->meta.pool_capacity;
+    if (need <= old || old >= v->meta.capacity) return B2V_OK;
+    const int rc = pool_map(v, std::min<uint64_t>(v->meta.capacity, std::max<uint64_t>(need, 2ull * old)));
+    if (v->meta.pool_capacity > old) v->growths += 1;
+    return rc;
+}
+
 static int volume_clear_device(b2v_volume *v) {
     const size_t tcap = static_cast<size_t>(v->table.mask) + 1;
     B2V_CUDA(v, cudaMemsetAsync(v->table.entries, 0xFF, tcap * sizeof(uint4), v->compute));
@@ -171,7 +298,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 100; }
+extern "C" int b2v_version(void) { return 101; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -202,6 +329,8 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
         !(cfg->depth_trunc > 0.0f) || cfg->capacity_blocks == 0 || cfg->shard_count < 1 ||
         cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_count ||
         (cfg->unit_resolution != 0 && cfg->unit_resolution != 8 && cfg->unit_resolution != 16) ||
+        (cfg->max_capacity_blocks != 0 &&
+         (cfg->max_capacity_blocks < cfg->capacity_blocks || cfg->max_capacity_blocks > (1u << 30))) ||
         static_cast<float>(cfg->voxel_length > 0.0 ? cfg->voxel_length : cfg->voxel_size) != cfg->voxel_size ||
         static_cast<float>(cfg->sdf_trunc_d > 0.0 ? cfg->sdf_trunc_d : cfg->sdf_trunc) != cfg->sdf_trunc)
         return B2V_ERR_INVALID_ARGUMENT;
@@ -242,12 +371,21 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
         B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_galloc[b], cudaEventDisableTiming));
         B2V_CUDA(v, cudaEventCreateWithFlags(&v->ev_group_done[b], cudaEventDisableTiming));
     }
-    const uint32_t cap = cfg->capacity_blocks;
+    // the table and everything indexed by slot or pool index are sized for the maximum; only the pool's storage grows
+    const uint32_t cap = std::max(cfg->capacity_blocks, cfg->max_capacity_blocks);
+    v->growable = cap > cfg->capacity_blocks;
     const uint32_t tcap = next_pow2(static_cast<uint64_t>(cap) * 2);
     v->table.mask = tcap - 1;
     v->meta.capacity = cap;
     B2V_CUDA(v, cudaMalloc(&v->table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.pool, static_cast<size_t>(cap) * kBlockFloats * sizeof(float)));
+    {
+        int rc = pool_reserve(v);
+        if (rc == B2V_OK) rc = pool_map(v, cfg->capacity_blocks);
+        if (rc != B2V_OK) return rc;
+        v->meta.pool_capacity = cfg->capacity_blocks;   // the rest of the last granule is used only after a growth
+    }
+    B2V_CUDA(v, cudaMallocHost(&v->h_skip, kGroupBufs * sizeof(uint32_t)));
+    std::memset(v->h_skip, 0, kGroupBufs * sizeof(uint32_t));
     B2V_CUDA(v, cudaMalloc(&v->meta.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
     B2V_CUDA(v, cudaMalloc(&v->meta.counters, kNumCounters * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.group_mask, static_cast<size_t>(tcap) * kGroupBufs * sizeof(uint32_t)));
@@ -257,8 +395,6 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     B2V_CUDA(v, cudaMallocHost(&v->h_counters, kNumCounters * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMallocHost(&v->h_totals, kNumMeshTotals * sizeof(uint32_t)));
     std::memset(v->h_totals, 0, kNumMeshTotals * sizeof(uint32_t));
-    B2V_CUDA(v, cudaMemsetAsync(v->meta.pool, 0, static_cast<size_t>(cap) * kBlockFloats * sizeof(float),
-                                v->compute));
     int rc = volume_clear_device(v);
     if (rc != B2V_OK) return rc;
     int sms = 0;
@@ -298,7 +434,8 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaFree(v->meta.union_slots);
     cudaFree(v->meta.block_flags);
     cudaFree(v->table.entries);
-    cudaFree(v->meta.pool);
+    pool_release(v);
+    cudaFreeHost(v->h_skip);
     cudaFree(v->meta.block_keys);
     cudaFree(v->meta.counters);
     cudaFree(v->mb.nbr);
@@ -325,7 +462,8 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     return B2V_OK;
 }
 
-static int read_counters(b2v_volume *v) {
+// waits for the volume's streams and the caller stream of the most recent frames, then mirrors the counters
+static int drain_and_copy_counters(b2v_volume *v) {
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
     B2V_CUDA(v, cudaStreamSynchronize(v->copy));
     B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
@@ -333,6 +471,51 @@ static int read_counters(b2v_volume *v) {
     B2V_CUDA(v, cudaMemcpyAsync(v->h_counters, v->meta.counters, kNumCounters * sizeof(uint32_t),
                                 cudaMemcpyDeviceToHost, v->compute));
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
+    return B2V_OK;
+}
+
+static int launch_group_update(b2v_volume *v, int buf, cudaStream_t cs) {
+    const GroupArgs &a = v->gargs[buf];
+    B2V_CUDA(v, v->gfused[buf] ? launch_integrate_group(a, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs)
+                               : launch_integrate(a.f[0], a.V, v->table, v->meta, buf, v->grid_ctas, cs));
+    v->launches += v->gfused[buf] ? 2 : 1;  // update (+ the mask clear of a fused group)
+    return B2V_OK;
+}
+
+// Growable volumes: if groups were skipped because they were handed pool indices past the storage, map storage for
+// every handed-out index and apply the skipped groups in order.  Called at quiescent points (it drains every stream first) and before
+// anything the skipped groups still read is overwritten: their texel images, the lambda image.
+static int resolve_skipped(b2v_volume *v) {
+    int rc = drain_and_copy_counters(v);
+    if (rc != B2V_OK || !v->h_counters[kCtrSkipping]) return rc;
+    // the allocate kernels handed out the dense indices [0, kCtrPool) below the maximum; map storage for them
+    const int grow_rc = pool_grow(v, v->h_counters[kCtrPool]);
+    if (v->h_counters[kCtrPool] > v->meta.pool_capacity && v->meta.pool_capacity < v->meta.capacity) {
+        B2V_CUDA(v, launch_drop_unbacked_blocks(v->table, v->meta, v->compute));  // the storage could not grow
+        v->launches += 1;
+    }
+    B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + kCtrSkipping, 0, sizeof(uint32_t), v->compute));
+    // the skipped groups are a suffix of the enqueued ones, and the enqueue throttle keeps the first of them among the
+    // last kGroupBufs groups
+    bool skipping = false;
+    for (uint32_t g = v->group_id > kGroupBufs ? v->group_id - kGroupBufs : 0; g < v->group_id; ++g) {
+        const int buf = static_cast<int>(g % kGroupBufs);
+        skipping = skipping || v->h_skip[buf] != 0;
+        if (!skipping) continue;
+        B2V_CUDA(v, cudaMemcpyAsync(v->meta.counters + group_ctr(buf, kGcUnion), v->meta.counters + kCtrSavedUnion0 + buf,
+                                    sizeof(uint32_t), cudaMemcpyDeviceToDevice, v->compute));
+        B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + group_ctr(buf, kGcNext), 0, sizeof(uint32_t), v->compute));
+        rc = launch_group_update(v, buf, v->compute);
+        if (rc != B2V_OK) return rc;
+    }
+    std::memset(v->h_skip, 0, kGroupBufs * sizeof(uint32_t));
+    rc = drain_and_copy_counters(v);
+    return rc != B2V_OK ? rc : grow_rc;
+}
+
+static int read_counters(b2v_volume *v) {
+    const int rc = v->growable ? resolve_skipped(v) : drain_and_copy_counters(v);
+    if (rc != B2V_OK) return rc;
     if (v->h_counters[kCtrError]) {
         v->err = (v->h_counters[kCtrError] & 2u) ? "hash table full: raise capacity_blocks"
                                                  : "block pool full: raise capacity_blocks";
@@ -343,13 +526,15 @@ static int read_counters(b2v_volume *v) {
 
 static uint32_t block_count(const b2v_volume *v) {
     const uint32_t n = v->h_counters[kCtrPool];
-    return n < v->meta.capacity ? n : v->meta.capacity;
+    return n < v->meta.pool_capacity ? n : v->meta.pool_capacity;
 }
 
 extern "C" int b2v_reset(b2v_volume *v) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    int rc = read_counters(v);
-    if (rc == B2V_ERR_CUDA) return rc;
+    // pending skipped groups are discarded, not replayed; the grown pool is kept
+    int rc = drain_and_copy_counters(v);
+    if (rc != B2V_OK) return rc;
+    std::memset(v->h_skip, 0, kGroupBufs * sizeof(uint32_t));
     const uint32_t nb = block_count(v);
     B2V_CUDA(v, cudaMemsetAsync(v->meta.pool, 0, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
                                 v->compute));
@@ -368,6 +553,10 @@ static int ensure_staging(b2v_volume *v, size_t pixels) {
     if (pixels <= v->stage_pixels) return B2V_OK;
     // the texel and lambda images freed below are read by update kernels on the library's streams and on callers'
     B2V_CUDA(v, cudaDeviceSynchronize());
+    if (v->growable) {  // and by the replay of skipped groups
+        const int rc = resolve_skipped(v);
+        if (rc == B2V_ERR_CUDA) return rc;
+    }
     // slots are carved out of contiguous allocations, so the frames of a group (which are contiguous in the caller's
     // arrays) upload with ONE copy per image type
     cudaFree(v->d_depth[0]);
@@ -572,6 +761,10 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         FrameParams P;
         fill_frame_params(&P, K, Tcw, height, width, v->geo);
         B2V_CUDA(v, cudaDeviceSynchronize());
+        if (v->growable) {  // a skipped group is replayed with the lambda image it was enqueued with
+            const int rc = resolve_skipped(v);
+            if (rc == B2V_ERR_CUDA) return rc;
+        }
         B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
         std::memcpy(v->lam_K, K, sizeof(v->lam_K));
         v->lam_H = height;
@@ -584,6 +777,16 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         const int count = std::min<int32_t>(gsz, n_frames - g0);
         const int buf = static_cast<int>(v->group_id % kGroupBufs);
         const int s0 = buf * kMaxGroup;  // the buffer's staging and texel slots
+        // growable volumes: the group that last used this buffer may have been skipped, and its replay needs the
+        // buffer's state; the host waits for that group (so it runs at most kGroupBufs groups ahead) and resolves first
+        if (v->growable) {
+            B2V_CUDA(v, cudaEventSynchronize(v->ev_group_done[buf]));
+            if (v->h_skip[buf]) {
+                const int rc = resolve_skipped(v);
+                if (rc == B2V_ERR_CUDA) return rc;
+            }
+            v->h_skip[buf] = 0;
+        }
         // the group buffer (masks, union list, counters, texel images) was last used by group id - kGroupBufs
         B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_group_done[buf], 0));
         B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + group_ctr(buf, 0), 0, kGroupCtrStride * sizeof(uint32_t), as));
@@ -622,8 +825,9 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             v->launches += 1;
         }
         static thread_local GroupAllocArgs aargs;  // ~15 KB: keep it off the stack
-        static thread_local GroupArgs args;
+        GroupArgs &args = v->gargs[buf];
         std::memset(&args, 0, sizeof(args));
+        v->gfused[buf] = fused;
         args.V = volume_consts(v->geo);
         args.count = aargs.count = count;
         aargs.use_tma = 1;
@@ -661,13 +865,23 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
                           : launch_allocate(aargs, v->table, v->meta, as));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
+        v->launches += 1;
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
+        if (v->growable && v->meta.pool_capacity < v->meta.capacity) {
+            // in group order on one stream, each after its own allocation: the first group skipped is the first that
+            // overflowed, and every later one is skipped too, which keeps each block's frame order for the replay
+            B2V_CUDA(v, launch_group_gate(v->meta, buf, cs));
+            B2V_CUDA(v, cudaMemcpyAsync(v->h_skip + buf, v->meta.counters + kCtrSkipping, sizeof(uint32_t),
+                                        cudaMemcpyDeviceToHost, cs));
+            v->launches += 1;
+        }
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[2], cs));
-        B2V_CUDA(v, fused ? launch_integrate_group(args, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs)
-                          : launch_integrate(args.f[0], args.V, v->table, v->meta, buf, v->grid_ctas, cs));
+        {
+            const int rc = launch_group_update(v, buf, cs);
+            if (rc != B2V_OK) return rc;
+        }
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[3], cs));
         B2V_CUDA(v, cudaEventRecord(v->ev_group_done[buf], cs));
-        v->launches += fused ? 3 : 2;  // allocate, update (+ the mask clear of a fused group)
         v->last_group_count = count;
         v->group_id += 1;
     }
@@ -751,6 +965,15 @@ extern "C" int b2v_set_fusion(b2v_volume *v, int32_t enable) {
 extern "C" int b2v_synchronize(b2v_volume *v) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
     return read_counters(v);
+}
+
+extern "C" int b2v_capacity(b2v_volume *v, int64_t *capacity_blocks, int64_t *growths) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    const int rc = read_counters(v);
+    if (rc == B2V_ERR_CUDA) return rc;
+    if (capacity_blocks) *capacity_blocks = v->meta.pool_capacity;
+    if (growths) *growths = v->growths;
+    return rc;
 }
 
 extern "C" int64_t b2v_num_blocks(b2v_volume *v) {
@@ -872,6 +1095,14 @@ extern "C" int64_t b2v_dump_blocks(b2v_volume *v, int32_t *keys, uint64_t *hashe
     return nb;
 }
 
+// growable volumes: before n blocks are uploaded (new or not), storage for all of them after the current ones
+static int grow_for_blocks(b2v_volume *v, int64_t n_blocks) {
+    if (!v->growable) return B2V_OK;
+    const int rc = read_counters(v);
+    if (rc == B2V_ERR_CUDA) return rc;
+    return pool_grow(v, static_cast<uint64_t>(v->h_counters[kCtrPool]) + static_cast<uint64_t>(n_blocks));
+}
+
 extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t *keys, const float *voxels) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
     if (n_blocks < 0 || (n_blocks > 0 && (!keys || !voxels))) {
@@ -880,6 +1111,10 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
     }
     if (n_blocks == 0) return B2V_OK;
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
+    {
+        const int rc = grow_for_blocks(v, n_blocks);
+        if (rc == B2V_ERR_CUDA) return rc;
+    }
     const size_t n = static_cast<size_t>(n_blocks);
     std::vector<int4> k4(n);
     for (size_t i = 0; i < n; ++i) k4[i] = make_int4(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2], 0);
@@ -938,6 +1173,10 @@ extern "C" int b2v_import_blocks_device(b2v_volume *v, int64_t n_blocks, const i
     }
     if (n_blocks == 0) return B2V_OK;
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
+    {
+        const int rc = grow_for_blocks(v, n_blocks);
+        if (rc == B2V_ERR_CUDA) return rc;
+    }
     uint32_t *d_i = nullptr;
     cudaError_t e = cudaMalloc(&d_i, static_cast<size_t>(n_blocks) * sizeof(uint32_t));
     if (e == cudaSuccess)

@@ -90,9 +90,10 @@ struct GroupArgs {
     int32_t count;
 };
 
-// Device-resident bookkeeping of one volume.
+// Device-resident bookkeeping of one volume.  Everything indexed by table slot or pool index is sized for the
+// maximum capacity; only the pool's storage grows (a growable volume maps it on demand, see b2v_api.cu).
 struct PoolMeta {
-    float *pool;              // [capacity][5][512] float32 planes: tsdf, weight, r, g, b
+    float *pool;              // [pool_capacity][5][512] float32 planes: tsdf, weight, r, g, b
     int4 *block_keys;         // [capacity] key of pool block i (w unused)
     uint32_t *counters;       // device counters, see Counter
     uint32_t *group_mask;     // [kGroupBufs][table capacity] bit k: the slot is touched by frame k of the group
@@ -100,14 +101,21 @@ struct PoolMeta {
     uint32_t *block_flags;    // [capacity] sign summary for the mesh extraction's tile filter: bit 0 = some store left
                               // an observed voxel (w != 0) with tsdf < 0, bit 1 = with tsdf >= 0; bits are only ever
                               // set, so the union over a tile is a superset of the signs present now
-    uint32_t capacity;
+    uint32_t capacity;        // maximum capacity: stride of the union lists; allocation hands out pool indices below
+                              // it (the others get kNoBlock)
+    uint32_t pool_capacity;   // blocks with storage now (<= capacity).  A growable volume skips every group from the
+                              // first that was handed an index past it, until the host has mapped storage for them
 };
 
 enum Counter : int {
-    kCtrPool = 0,            // number of allocated blocks (may exceed capacity on overflow)
+    kCtrPool = 0,            // number of allocated blocks (may exceed pool_capacity on overflow)
     kCtrError = 1,           // sticky error flag (1 = pool overflow, 2 = table full)
     kCtrUpdatesLo = 2,       // 64-bit total of (block, frame) updates since reset (8-byte aligned)
     kCtrUpdatesHi = 3,
+    kCtrSkipping = 4,        // growable volumes: sticky, set by the gate of the first group that saw kCtrPool pass
+                             // pool_capacity; every later group is skipped too until the host grows the pool and
+                             // replays them
+    kCtrSavedUnion0 = 5,     // [kGroupBufs] kGcUnion of the skipped group of each buffer (restored for the replay)
     kCtrVisitsLo = 12,       // 64-bit total of block visits (one block read + written) since reset
     kCtrVisitsHi = 13,
     kCtrGroup0 = 16,         // [kGroupBufs][kGroupCtrStride] per-group-buffer counters, contiguous so that ONE
@@ -127,6 +135,7 @@ __host__ __device__ __forceinline__ constexpr int group_ctr(int buf, int which) 
 }
 static_assert(kGcTouched0 + kMaxGroup <= kGroupCtrStride && kCtrGroup0 + kGroupBufs * kGroupCtrStride <= kNumCounters,
               "counter layout");
+static_assert(kCtrSavedUnion0 + kGroupBufs <= kCtrVisitsLo, "counter layout");
 
 struct VolumeGeometry {   // set once per volume (b2v_create)
     float vs, tau, depth_trunc;
@@ -189,6 +198,14 @@ cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *sl
 // find-or-create the blocks of `keys` (unique) and copy `vox` [n][5][512] into them
 cudaError_t launch_upload_blocks(const int4 *keys, const float *vox, uint32_t n, uint32_t *scratch_idx,
                                  const HashTable &table, const PoolMeta &meta, cudaStream_t stream);
+
+// ---- pool growth (growable volumes) ----
+// one thread, between a group's allocation and its update: if pool indices past the storage were handed out
+// (kCtrPool > pool_capacity), or an earlier group is being skipped, mark the volume as skipping, save the group's union
+// count and zero it (the update kernels then do nothing and leave the group's masks and list in place for the replay)
+cudaError_t launch_group_gate(const PoolMeta &meta, int group_buf, cudaStream_t stream);
+// when the storage could not grow: entries holding an index past it lose it (kNoBlock, "block pool full")
+cudaError_t launch_drop_unbacked_blocks(const HashTable &table, const PoolMeta &meta, cudaStream_t stream);
 
 // ---- mesh (b2v_mesh.cu) ----
 // Scratch and outputs of one extraction.  Per-voxel scratch is indexed [pool block][voxel].

@@ -33,6 +33,9 @@ DEFAULT_PARAMETERS = {
     "kVolumetricIntegrationOutputTimeInterval": 1.0,
     "kVolumetricIntegrationTsdfExtractMesh": True,
     "kVolumetricIntegrationB200CapacityBlocks": 1 << 19,
+    # growth ceiling of the block pool: > CapacityBlocks starts with CapacityBlocks blocks and maps more on demand,
+    # bit-identical to a pool of this size from the start; 0 = fixed pool of CapacityBlocks
+    "kVolumetricIntegrationB200MaxCapacityBlocks": 0,
     "kVolumetricIntegrationB200Device": 0,
     # undistort + BGR->RGB on the GPU (b2v_set_rectification) instead of the base class's cv2.remap / cvtColor
     "kVolumetricIntegrationB200GpuRectify": True,
@@ -110,6 +113,7 @@ def make_integrator_class(Base, api):
                 sdf_trunc=p["kVolumetricIntegrationTSdfTrunc"],
                 depth_trunc=self.volumetric_integration_depth_trunc,
                 capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
+                max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None,
                 device=int(p["kVolumetricIntegrationB200Device"]),
                 volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]))
             self.last_output = None

@@ -77,10 +77,13 @@ class B200TsdfVolume:
     def __init__(self, voxel_length: float, sdf_trunc: float, depth_trunc: float = 4.0,
                  capacity_blocks: int = 1 << 18, device: int = 0, depth_sampling_stride: int = 4,
                  block_size: int = BLOCK_SIZE, shard_rank: int = 0, shard_count: int = 1,
-                 volume_unit_resolution: int = 16):
+                 volume_unit_resolution: int = 16, max_capacity_blocks: int | None = None):
         """`volume_unit_resolution`: Open3D's parameter of that name.  16 (the reference's value) allocates every
         8^3 block of each 16^3 unit `ScalableTSDFVolume::LocateVolumeUnit` touches - the same voxels Open3D updates;
-        8 is SURVEY decision D1 (the float32 pyslam key range of the +-sdf_trunc box, ~9 % fewer blocks)."""
+        8 is SURVEY decision D1 (the float32 pyslam key range of the +-sdf_trunc box, ~9 % fewer blocks).
+        `max_capacity_blocks`: growth ceiling of the block pool.  Above `capacity_blocks`, the pool starts with
+        `capacity_blocks` blocks of storage and grows on demand; the volume then holds, bit for bit, what a volume
+        created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the pool fixed."""
         self._L = _lib.load()
         self._h = C.c_void_p()
         self.voxel_length = float(voxel_length)
@@ -88,12 +91,13 @@ class B200TsdfVolume:
         self.depth_trunc = float(depth_trunc)
         self.block_size = int(block_size)
         self.capacity_blocks = int(capacity_blocks)
+        self.max_capacity_blocks = int(max_capacity_blocks or 0)
         self.device = int(device)
         self.shard_rank, self.shard_count = int(shard_rank), int(shard_count)
         self.volume_unit_resolution = int(volume_unit_resolution)
         cfg = B2VConfig(voxel_length, block_size, sdf_trunc, depth_trunc, depth_sampling_stride,
                         capacity_blocks, device, shard_rank, shard_count, int(volume_unit_resolution),
-                        float(voxel_length), float(sdf_trunc))
+                        float(voxel_length), float(sdf_trunc), self.max_capacity_blocks)
         rc = self._L.b2v_create(C.byref(cfg), C.byref(self._h))
         if rc != _lib.B2V_OK:
             msg = self._L.b2v_last_error(self._h).decode() if self._h else "invalid configuration"
@@ -219,6 +223,12 @@ class B200TsdfVolume:
     def synchronize(self):
         self._check(self._L.b2v_synchronize(self._h), "b2v_synchronize")
         self._keepalive.clear()
+
+    def capacity(self):
+        """(blocks the pool has storage for now, growths since creation); synchronises."""
+        n, g = C.c_int64(0), C.c_int64(0)
+        self._check(self._L.b2v_capacity(self._h, C.byref(n), C.byref(g)), "b2v_capacity")
+        return int(n.value), int(g.value)
 
     def reset(self):
         """`self.volume.reset()` (tsdf.py:156; base.py:642)."""
