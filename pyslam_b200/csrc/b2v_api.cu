@@ -142,9 +142,7 @@ struct b2v_volume {
     // The pool is one virtual-address reservation for meta.capacity blocks; physical chunks are mapped as it grows
     // (fixed volumes map it whole at create), so the pool address the kernels see never changes.
     bool growable = false;               // max_capacity_blocks > capacity_blocks
-    CUdeviceptr pool_va = 0;
-    size_t pool_reserved = 0, pool_mapped = 0, pool_gran = 0;   // bytes
-    std::vector<std::pair<size_t, size_t>> pool_chunks;         // (offset, bytes) of each mapping
+    VmmRange pool;
     int64_t growths = 0;
     // update launch of the group in each buffer, kept for the replay of a skipped group
     GroupArgs gargs[kGroupBufs];
@@ -219,67 +217,85 @@ CUmemAllocationProp pool_prop(int device) {
 }
 
 constexpr size_t kBlockBytes = static_cast<size_t>(kBlockFloats) * sizeof(float);
+
+bool cu_failed(CUresult r, const char *what, std::string *err) {
+    if (r == CUDA_SUCCESS) return false;
+    *err = std::string(what) + ": CUresult " + std::to_string(r);
+    return true;
+}
 }  // namespace
 
-#define B2V_CU(v, call)                                                                    \
-    do {                                                                                   \
-        CUresult r_ = (call);                                                              \
-        if (r_ != CUDA_SUCCESS) {                                                          \
-            (v)->err = std::string(#call) + ": CUresult " + std::to_string(r_);            \
-            return B2V_ERR_CUDA;                                                           \
-        }                                                                                  \
-    } while (0)
+bool b2v::vmm_reserve(VmmRange *r, size_t bytes, int device, std::string *err) {
+    const VmmApi *api = vmm_api();
+    if (!api) {
+        *err = "the driver's virtual memory management entry points are unavailable";
+        return false;
+    }
+    r->device = device;
+    const CUmemAllocationProp prop = pool_prop(device);
+    if (cu_failed(api->granularity(&r->gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM), "cuMemGetAllocationGranularity",
+                  err))
+        return false;
+    const size_t g = r->gran;
+    const size_t reserved = (std::max<size_t>(bytes, 1) + g - 1) / g * g;
+    if (cu_failed(api->reserve(&r->va, reserved, 0, 0, 0), "cuMemAddressReserve", err)) return false;
+    r->reserved = reserved;
+    return true;
+}
+
+bool b2v::vmm_map(VmmRange *r, size_t bytes, cudaStream_t stream, std::string *err) {
+    const size_t g = r->gran;
+    const size_t want = std::min(r->reserved, (bytes + g - 1) / g * g);
+    if (want <= r->mapped) return true;
+    const VmmApi *api = vmm_api();
+    const size_t off = r->mapped, len = want - off;
+    const CUmemAllocationProp prop = pool_prop(r->device);
+    CUmemGenericAllocationHandle h;
+    if (cu_failed(api->create(&h, len, &prop, 0), "cuMemCreate", err)) return false;
+    const CUresult m = api->map(r->va + off, len, 0, h, 0);
+    api->release(h);  // the mapping keeps the memory until it is unmapped
+    if (cu_failed(m, "cuMemMap", err)) return false;
+    r->chunks.emplace_back(off, len);
+    CUmemAccessDesc acc{};
+    acc.location = prop.location;
+    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    if (cu_failed(api->set_access(r->va + off, len, &acc, 1), "cuMemSetAccess", err)) return false;
+    r->mapped = want;
+    const cudaError_t e = cudaMemsetAsync(reinterpret_cast<void *>(r->va + off), 0, len, stream);
+    if (e != cudaSuccess) {
+        *err = std::string("cudaMemsetAsync: ") + cudaGetErrorString(e);
+        return false;
+    }
+    return true;
+}
+
+void b2v::vmm_release(VmmRange *r) {
+    const VmmApi *api = vmm_api();
+    if (!api || !r->va) return;
+    for (const auto &c : r->chunks) api->unmap(r->va + c.first, c.second);
+    api->address_free(r->va, r->reserved);
+    r->chunks.clear();
+    r->va = 0;
+    r->reserved = r->mapped = 0;
+}
 
 // reserve the address range of meta.capacity blocks
 static int pool_reserve(b2v_volume *v) {
-    const VmmApi *api = vmm_api();
-    if (!api) {
-        v->err = "the driver's virtual memory management entry points are unavailable";
+    if (!vmm_reserve(&v->pool, static_cast<size_t>(v->meta.capacity) * kBlockBytes, v->cfg.device, &v->err))
         return B2V_ERR_CUDA;
-    }
-    const CUmemAllocationProp prop = pool_prop(v->cfg.device);
-    B2V_CU(v, api->granularity(&v->pool_gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM));
-    const size_t g = v->pool_gran;
-    v->pool_reserved = (static_cast<size_t>(v->meta.capacity) * kBlockBytes + g - 1) / g * g;
-    B2V_CU(v, api->reserve(&v->pool_va, v->pool_reserved, 0, 0, 0));
-    v->meta.pool = reinterpret_cast<float *>(v->pool_va);
+    v->meta.pool = reinterpret_cast<float *>(v->pool.va);
     return B2V_OK;
 }
 
-// map (and zero) storage for at least `blocks` blocks, in whole granules, up to the reservation; pool_capacity follows
+// map (and zero: allocation relies on a zeroed pool) storage for at least `blocks` blocks, in whole granules, up to
+// the reservation; pool_capacity follows
 static int pool_map(b2v_volume *v, uint64_t blocks) {
-    const size_t g = v->pool_gran;
-    const size_t want = std::min(v->pool_reserved, (static_cast<size_t>(blocks) * kBlockBytes + g - 1) / g * g);
-    if (want > v->pool_mapped) {
-        const VmmApi *api = vmm_api();
-        const size_t off = v->pool_mapped, bytes = want - off;
-        const CUmemAllocationProp prop = pool_prop(v->cfg.device);
-        CUmemGenericAllocationHandle h;
-        B2V_CU(v, api->create(&h, bytes, &prop, 0));
-        const CUresult r = api->map(v->pool_va + off, bytes, 0, h, 0);
-        api->release(h);  // the mapping keeps the memory until it is unmapped
-        B2V_CU(v, r);
-        v->pool_chunks.emplace_back(off, bytes);
-        CUmemAccessDesc acc{};
-        acc.location = prop.location;
-        acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-        B2V_CU(v, api->set_access(v->pool_va + off, bytes, &acc, 1));
-        v->pool_mapped = want;
-        // allocation relies on a zeroed pool
-        B2V_CUDA(v, cudaMemsetAsync(reinterpret_cast<char *>(v->meta.pool) + off, 0, bytes, v->compute));
-    }
-    v->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(v->meta.capacity, v->pool_mapped / kBlockBytes));
+    if (!vmm_map(&v->pool, static_cast<size_t>(blocks) * kBlockBytes, v->compute, &v->err)) return B2V_ERR_CUDA;
+    v->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(v->meta.capacity, v->pool.mapped / kBlockBytes));
     return B2V_OK;
 }
 
-static void pool_release(b2v_volume *v) {
-    const VmmApi *api = vmm_api();
-    if (!api || !v->pool_va) return;
-    for (const auto &c : v->pool_chunks) api->unmap(v->pool_va + c.first, c.second);
-    api->address_free(v->pool_va, v->pool_reserved);
-    v->pool_chunks.clear();
-    v->pool_va = 0;
-}
+static void pool_release(b2v_volume *v) { vmm_release(&v->pool); }
 
 // growth policy: at least double, at least `need` blocks, at most the maximum
 static int pool_grow(b2v_volume *v, uint64_t need) {
@@ -298,7 +314,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 101; }
+extern "C" int b2v_version(void) { return 102; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -1326,6 +1342,11 @@ struct b2v_grid {
     cudaStream_t stream = nullptr;
     HashTable table{};
     GridMeta meta{};
+    // the pool is a reservation for meta.capacity blocks with storage mapped for meta.pool_capacity (a fixed grid maps
+    // it whole at create); a growable grid maps more inside the integrate call that needs it
+    bool growable = false;
+    VmmRange pool;
+    int64_t growths = 0;
     uint32_t *h_counters = nullptr;
     float *d_pts = nullptr, *d_cols = nullptr;
     size_t stage_points = 0;
@@ -1338,6 +1359,7 @@ struct b2v_grid {
 };
 
 constexpr int kGridBlockWordsHost = 7 * kVox;
+constexpr size_t kGridBlockBytes = static_cast<size_t>(kGridBlockWordsHost) * sizeof(uint32_t);
 
 extern "C" const char *b2v_grid_last_error(const b2v_grid *g) { return g ? g->err.c_str() : "null grid"; }
 
@@ -1353,9 +1375,15 @@ static int grid_clear_device(b2v_grid *g, uint32_t used_blocks) {
 
 extern "C" int b2v_grid_create(float voxel_size, int32_t block_size, uint32_t capacity_blocks,
                                int32_t device, b2v_grid **out) {
+    return b2v_grid_create_ex(voxel_size, block_size, capacity_blocks, 0, device, out);
+}
+
+extern "C" int b2v_grid_create_ex(float voxel_size, int32_t block_size, uint32_t capacity_blocks,
+                                  uint32_t max_capacity_blocks, int32_t device, b2v_grid **out) {
     if (!out) return B2V_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    if (block_size != B2V_BLOCK_SIZE || !(voxel_size > 0.0f) || capacity_blocks == 0)
+    if (block_size != B2V_BLOCK_SIZE || !(voxel_size > 0.0f) || capacity_blocks == 0 ||
+        (max_capacity_blocks != 0 && (max_capacity_blocks < capacity_blocks || max_capacity_blocks > (1u << 22))))
         return B2V_ERR_INVALID_ARGUMENT;
     b2v_grid *g = new (std::nothrow) b2v_grid();
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
@@ -1365,12 +1393,19 @@ extern "C" int b2v_grid_create(float voxel_size, int32_t block_size, uint32_t ca
     *out = g;
     B2V_CUDA(g, cudaSetDevice(device));
     B2V_CUDA(g, cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
-    const uint32_t tcap = next_pow2(static_cast<uint64_t>(capacity_blocks) * 2);
+    // the table and the block keys are sized for the maximum; only the pool's storage grows
+    const uint32_t cap = std::max(capacity_blocks, max_capacity_blocks);
+    g->growable = cap > capacity_blocks;
+    const uint32_t tcap = next_pow2(static_cast<uint64_t>(cap) * 2);
     g->table.mask = tcap - 1;
-    g->meta.capacity = capacity_blocks;
+    g->meta.capacity = cap;
     B2V_CUDA(g, cudaMalloc(&g->table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
-    B2V_CUDA(g, cudaMalloc(&g->meta.pool, static_cast<size_t>(capacity_blocks) * kGridBlockWordsHost * sizeof(uint32_t)));
-    B2V_CUDA(g, cudaMalloc(&g->meta.block_keys, static_cast<size_t>(capacity_blocks) * sizeof(int4)));
+    if (!vmm_reserve(&g->pool, static_cast<size_t>(cap) * kGridBlockBytes, device, &g->err) ||
+        !vmm_map(&g->pool, static_cast<size_t>(capacity_blocks) * kGridBlockBytes, g->stream, &g->err))
+        return B2V_ERR_CUDA;
+    g->meta.pool = reinterpret_cast<uint32_t *>(g->pool.va);
+    g->meta.pool_capacity = capacity_blocks;   // the rest of the last granule is used only after a growth
+    B2V_CUDA(g, cudaMalloc(&g->meta.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
     B2V_CUDA(g, cudaMalloc(&g->meta.counters, kNumCounters * sizeof(uint32_t)));
     B2V_CUDA(g, cudaMalloc(&g->d_total, sizeof(uint32_t)));
     B2V_CUDA(g, cudaMallocHost(&g->h_counters, kNumCounters * sizeof(uint32_t)));
@@ -1385,7 +1420,7 @@ extern "C" int b2v_grid_destroy(b2v_grid *g) {
     cudaSetDevice(g->device);
     if (g->stream) cudaStreamSynchronize(g->stream);
     cudaFree(g->table.entries);
-    cudaFree(g->meta.pool);
+    vmm_release(&g->pool);
     cudaFree(g->meta.block_keys);
     cudaFree(g->meta.counters);
     cudaFree(g->d_pts);
@@ -1416,7 +1451,44 @@ static int grid_read_counters(b2v_grid *g) {
 
 static uint32_t grid_block_count(const b2v_grid *g) {
     const uint32_t n = g->h_counters[kCtrPool];
-    return n < g->meta.capacity ? n : g->meta.capacity;
+    return n < g->meta.pool_capacity ? n : g->meta.pool_capacity;
+}
+
+// Growable grids, at the end of an integrate call: the call's accumulate pass skipped the points of blocks handed a
+// pool index past the storage.  Map storage for every handed-out index (at least doubling, at most the maximum), then
+// replay(lo, hi) repeats the pass over the blocks that just got storage, from the same inputs, which must still be
+// alive.  All observations of a voxel in one call belong to one block, and a block's index never changes, so every
+// voxel is updated by exactly one of the two passes.  If the storage cannot grow, the blocks past it are dropped
+// ("block pool full").
+template <typename Replay>
+static int grid_resolve(b2v_grid *g, Replay replay) {
+    B2V_CUDA(g, cudaMemcpyAsync(g->h_counters, g->meta.counters, kNumCounters * sizeof(uint32_t),
+                                cudaMemcpyDeviceToHost, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    const uint32_t used = g->h_counters[kCtrPool], old = g->meta.pool_capacity;
+    if (used <= old || old >= g->meta.capacity) return B2V_OK;
+    const uint64_t want = std::min<uint64_t>(g->meta.capacity, std::max<uint64_t>(used, 2ull * old));
+    std::string map_err;   // a failed mapping surfaces as "block pool full" below
+    vmm_map(&g->pool, static_cast<size_t>(want) * kGridBlockBytes, g->stream, &map_err);
+    g->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(g->meta.capacity, g->pool.mapped / kGridBlockBytes));
+    if (g->meta.pool_capacity > old) {
+        g->growths += 1;
+        B2V_CUDA(g, replay(old, g->meta.pool_capacity));
+    }
+    if (used > g->meta.pool_capacity)   // the storage could not grow far enough
+        B2V_CUDA(g, launch_drop_unbacked_slots(g->table, g->meta.pool_capacity, g->meta.capacity,
+                                               g->meta.counters + kCtrError, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return B2V_OK;
+}
+
+extern "C" int b2v_grid_capacity(b2v_grid *g, int64_t *capacity_blocks, int64_t *growths) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    if (capacity_blocks) *capacity_blocks = g->meta.pool_capacity;
+    if (growths) *growths = g->growths;
+    return B2V_OK;
 }
 
 extern "C" int b2v_grid_clear(b2v_grid *g) {
@@ -1461,7 +1533,11 @@ static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const v
         }
     }
     B2V_CUDA(g, launch_grid_integrate(d_p, f64, d_c, u8, n_points, g->inv_voxel_size, g->table, g->meta, g->stream));
-    return B2V_OK;
+    if (!g->growable) return B2V_OK;
+    return grid_resolve(g, [&](uint32_t lo, uint32_t hi) {
+        return launch_grid_accumulate(d_p, f64, d_c, u8, n_points, g->inv_voxel_size, g->table, g->meta, lo, hi,
+                                      g->stream);
+    });
 }
 
 extern "C" int b2v_grid_integrate(b2v_grid *g, const float *points, const float *colors, int64_t n_points) {
@@ -1538,6 +1614,7 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         if (e == cudaSuccess) e = launch_filter_shadow_points(d_depth, height, width, 2, 2, -1.0f, filtered, scratch, g->stream);
         d_depth = filtered;
     }
+    int rc = B2V_OK;
     if (e == cudaSuccess) {
         RgbdParams P;
         P.fx_inv = 1.0 / K[0];
@@ -1553,6 +1630,12 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         P.H = height;
         P.W = width;
         e = launch_grid_integrate_rgbd(P, d_depth, d_color, g->inv_voxel_size, g->table, g->meta, g->stream);
+        // the replay reads the temporaries freed below
+        if (e == cudaSuccess && g->growable)
+            rc = grid_resolve(g, [&](uint32_t lo, uint32_t hi) {
+                return launch_grid_rgbd_accumulate(P, d_depth, d_color, g->inv_voxel_size, g->table, g->meta, lo, hi,
+                                                   g->stream);
+            });
     }
     if (e == cudaSuccess && (tmp_d || tmp_c || filtered)) e = cudaStreamSynchronize(g->stream);
     cudaFree(tmp_d);
@@ -1563,7 +1646,7 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         g->err = std::string("b2v_grid_integrate_rgbd: ") + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
     }
-    return B2V_OK;
+    return rc;
 }
 
 extern "C" int b2v_grid_synchronize(b2v_grid *g) {

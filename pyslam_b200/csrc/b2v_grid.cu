@@ -89,10 +89,13 @@ __device__ __forceinline__ void sum_add(float *p, float x) {
 __device__ __forceinline__ float color_value(float c) { return c; }
 __device__ __forceinline__ float color_value(uint8_t c) { return __fmul_rn(static_cast<float>(c), 1.0f / 255.0f); }
 
+// Only the points whose block has a pool index in [lo, hi) are accumulated: the first pass of a call covers the blocks
+// with storage, [0, pool_capacity); after a growth the same pass is replayed over the blocks that just got storage.
+// A voxel's observations of one call all belong to one block, so each voxel is updated in exactly one of the passes.
 template <typename Tp, typename Tc>
 __global__ void __launch_bounds__(256)
 grid_accumulate_kernel(const Tp *__restrict__ pts, const Tc *__restrict__ cols, const int64_t n,
-                       const float inv_vs, const HashTable T, const GridMeta G) {
+                       const float inv_vs, const HashTable T, const GridMeta G, const uint32_t lo, const uint32_t hi) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const Tp xp = pts[3 * i + 0], yp = pts[3 * i + 1], zp = pts[3 * i + 2];
@@ -102,7 +105,7 @@ grid_accumulate_kernel(const Tp *__restrict__ pts, const Tc *__restrict__ cols, 
     const uint32_t slot = table_find(T, block_coord(vx), block_coord(vy), block_coord(vz));
     if (slot == kEmpty) return;
     const uint32_t idx = T.entries[slot].w;
-    if (idx >= G.capacity) return;
+    if (idx < lo || idx >= hi) return;   // kNoBlock is past every window
     const int l = local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6);
     uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords;
     float *fb = reinterpret_cast<float *>(blk);
@@ -178,7 +181,8 @@ grid_rgbd_insert_kernel(const RgbdParams P, const float *__restrict__ depth, con
 
 __global__ void __launch_bounds__(256)
 grid_rgbd_accumulate_kernel(const RgbdParams P, const float *__restrict__ depth, const uint8_t *__restrict__ rgb,
-                            const float inv_vs, const HashTable T, const GridMeta G) {
+                            const float inv_vs, const HashTable T, const GridMeta G, const uint32_t lo,
+                            const uint32_t hi) {
     const int64_t n = static_cast<int64_t>(P.H) * P.W;
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     float pt[3];
@@ -187,7 +191,7 @@ grid_rgbd_accumulate_kernel(const RgbdParams P, const float *__restrict__ depth,
     const uint32_t slot = table_find(T, block_coord(vx), block_coord(vy), block_coord(vz));
     if (slot == kEmpty) return;
     const uint32_t idx = T.entries[slot].w;
-    if (idx >= G.capacity) return;
+    if (idx < lo || idx >= hi) return;   // the window of grid_accumulate_kernel
     const int l = local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6);
     uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords;
     float *fb = reinterpret_cast<float *>(blk);
@@ -207,7 +211,17 @@ cudaError_t launch_grid_integrate_rgbd(const RgbdParams &p, const float *depth, 
     if (n <= 0) return cudaSuccess;
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
     grid_rgbd_insert_kernel<<<grid, 256, 0, stream>>>(p, depth, inv_vs, table, meta);
-    grid_rgbd_accumulate_kernel<<<grid, 256, 0, stream>>>(p, depth, rgb, inv_vs, table, meta);
+    grid_rgbd_accumulate_kernel<<<grid, 256, 0, stream>>>(p, depth, rgb, inv_vs, table, meta, 0u, meta.pool_capacity);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_grid_rgbd_accumulate(const RgbdParams &p, const float *depth, const uint8_t *rgb, float inv_vs,
+                                        const HashTable &table, const GridMeta &meta, uint32_t lo, uint32_t hi,
+                                        cudaStream_t stream) {
+    const int64_t n = static_cast<int64_t>(p.H) * p.W;
+    if (n <= 0) return cudaSuccess;
+    grid_rgbd_accumulate_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(p, depth, rgb, inv_vs,
+                                                                                            table, meta, lo, hi);
     return cudaGetLastError();
 }
 
@@ -398,24 +412,38 @@ cudaError_t launch_grid_carve(const GridMeta &meta, uint32_t n_blocks, const Gri
 
 // ---- launchers -------------------------------------------------------------------------------
 template <typename Tp>
-static void launch_grid_integrate_t(const Tp *p, const void *cols, bool cols_u8, int64_t n, float inv_vs,
-                                    const HashTable &table, const GridMeta &meta, cudaStream_t stream) {
+static void launch_grid_accumulate_t(const Tp *p, const void *cols, bool cols_u8, int64_t n, float inv_vs,
+                                     const HashTable &table, const GridMeta &meta, uint32_t lo, uint32_t hi,
+                                     cudaStream_t stream) {
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    grid_insert_kernel<Tp><<<grid, 256, 0, stream>>>(p, n, inv_vs, table, meta);
     if (cols_u8)
-        grid_accumulate_kernel<Tp, uint8_t><<<grid, 256, 0, stream>>>(p, static_cast<const uint8_t *>(cols), n, inv_vs, table, meta);
+        grid_accumulate_kernel<Tp, uint8_t><<<grid, 256, 0, stream>>>(p, static_cast<const uint8_t *>(cols), n, inv_vs,
+                                                                      table, meta, lo, hi);
     else
-        grid_accumulate_kernel<Tp, float><<<grid, 256, 0, stream>>>(p, static_cast<const float *>(cols), n, inv_vs, table, meta);
+        grid_accumulate_kernel<Tp, float><<<grid, 256, 0, stream>>>(p, static_cast<const float *>(cols), n, inv_vs,
+                                                                    table, meta, lo, hi);
+}
+
+cudaError_t launch_grid_accumulate(const void *pts, bool pts_f64, const void *cols, bool cols_u8, int64_t n,
+                                   float inv_vs, const HashTable &table, const GridMeta &meta, uint32_t lo, uint32_t hi,
+                                   cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    if (pts_f64)
+        launch_grid_accumulate_t(static_cast<const double *>(pts), cols, cols_u8, n, inv_vs, table, meta, lo, hi, stream);
+    else
+        launch_grid_accumulate_t(static_cast<const float *>(pts), cols, cols_u8, n, inv_vs, table, meta, lo, hi, stream);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_grid_integrate(const void *pts, bool pts_f64, const void *cols, bool cols_u8, int64_t n, float inv_vs,
                                   const HashTable &table, const GridMeta &meta, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
     if (pts_f64)
-        launch_grid_integrate_t(static_cast<const double *>(pts), cols, cols_u8, n, inv_vs, table, meta, stream);
+        grid_insert_kernel<double><<<grid, 256, 0, stream>>>(static_cast<const double *>(pts), n, inv_vs, table, meta);
     else
-        launch_grid_integrate_t(static_cast<const float *>(pts), cols, cols_u8, n, inv_vs, table, meta, stream);
-    return cudaGetLastError();
+        grid_insert_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float *>(pts), n, inv_vs, table, meta);
+    return launch_grid_accumulate(pts, pts_f64, cols, cols_u8, n, inv_vs, table, meta, 0u, meta.pool_capacity, stream);
 }
 
 cudaError_t launch_grid_count(const GridMeta &meta, uint32_t n_blocks, int min_count, uint32_t *sums,

@@ -5,10 +5,28 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <string>
+#include <utility>
+#include <vector>
 
 #include "b2v_device.cuh"
 
 namespace b2v {
+
+// ---- device storage that grows in place (b2v_api.cu) ----
+// One virtual-address range reserved for the maximum size; physical memory is mapped into it in whole granules with
+// the driver's virtual memory management entry points, so the address the kernels see never changes and a growth
+// copies nothing.  Fixed-size storage takes the same path with the whole reservation mapped at create.
+struct VmmRange {
+    CUdeviceptr va = 0;
+    size_t reserved = 0, mapped = 0, gran = 0;      // bytes
+    int device = 0;
+    std::vector<std::pair<size_t, size_t>> chunks;  // (offset, bytes) of each mapping
+};
+// reserve at least `bytes`, rounded up to the granularity; false (and *err) on failure
+bool vmm_reserve(VmmRange *r, size_t bytes, int device, std::string *err);
+// map at least `bytes` (whole granules, capped at the reservation); the newly mapped bytes are zeroed on `stream`
+bool vmm_map(VmmRange *r, size_t bytes, cudaStream_t stream, std::string *err);
+void vmm_release(VmmRange *r);
 
 // Texel of the update kernels, one per pixel of a frame, packed by the allocate kernels: {depth, r | g << 8 | b << 16}.
 // depth is 0 where the pixel is invalid (0, or beyond depth_trunc).  The depth-to-camera-distance multiplier is not
@@ -206,6 +224,9 @@ cudaError_t launch_upload_blocks(const int4 *keys, const float *vox, uint32_t n,
 cudaError_t launch_group_gate(const PoolMeta &meta, int group_buf, cudaStream_t stream);
 // when the storage could not grow: entries holding an index past it lose it (kNoBlock, "block pool full")
 cudaError_t launch_drop_unbacked_blocks(const HashTable &table, const PoolMeta &meta, cudaStream_t stream);
+// the same for any block table: entries with a pool index in [storage, capacity) get kNoBlock and set bit 0 of *error
+cudaError_t launch_drop_unbacked_slots(const HashTable &table, uint32_t storage, uint32_t capacity, uint32_t *error,
+                                       cudaStream_t stream);
 
 // ---- mesh (b2v_mesh.cu) ----
 // Scratch and outputs of one extraction.  Per-voxel scratch is indexed [pool block][voxel].
@@ -244,13 +265,19 @@ cudaError_t launch_mesh_triangles(const MeshBuffers &mb, uint32_t work_blocks, c
 
 // ---- point-average grid (b2v_grid.cu) ----
 struct GridMeta {
-    uint32_t *pool;        // [capacity][7][512] planes: count(int32), px, py, pz, cr, cg, cb (float32)
+    uint32_t *pool;        // [pool_capacity][7][512] planes: count(int32), px, py, pz, cr, cg, cb (float32)
     int4 *block_keys;      // [capacity]
     uint32_t *counters;    // kCtrPool, kCtrError
-    uint32_t capacity;
+    uint32_t capacity;     // maximum capacity: allocation hands out pool indices below it (the others get kNoBlock)
+    uint32_t pool_capacity;   // blocks with storage now (<= capacity); a growable grid maps more within the call
 };
+// insert + accumulate; the accumulate pass skips the points of blocks without storage (index >= pool_capacity)
 cudaError_t launch_grid_integrate(const void *pts, bool pts_f64, const void *cols, bool cols_u8, int64_t n, float inv_vs,
                                   const HashTable &table, const GridMeta &meta, cudaStream_t stream);
+// the accumulate pass alone, restricted to the points whose block's pool index lies in [lo, hi) (replay after growth)
+cudaError_t launch_grid_accumulate(const void *pts, bool pts_f64, const void *cols, bool cols_u8, int64_t n,
+                                   float inv_vs, const HashTable &table, const GridMeta &meta, uint32_t lo, uint32_t hi,
+                                   cudaStream_t stream);
 cudaError_t launch_grid_count(const GridMeta &meta, uint32_t n_blocks, int min_count, uint32_t *sums,
                               uint32_t *offs, uint32_t *total, cudaStream_t stream);
 cudaError_t launch_grid_emit(const GridMeta &meta, uint32_t n_blocks, int min_count,
@@ -271,6 +298,9 @@ struct RgbdParams {
 cudaError_t launch_grid_integrate_rgbd(const RgbdParams &p, const float *depth, const uint8_t *rgb,
                                        float inv_vs, const HashTable &table, const GridMeta &meta,
                                        cudaStream_t stream);
+cudaError_t launch_grid_rgbd_accumulate(const RgbdParams &p, const float *depth, const uint8_t *rgb, float inv_vs,
+                                        const HashTable &table, const GridMeta &meta, uint32_t lo, uint32_t hi,
+                                        cudaStream_t stream);
 
 // raw uint16 depth -> float32 metres (b2v_prep.cu)
 cudaError_t launch_depth_u16_to_f32(const uint16_t *src, float *dst, size_t n, float scale, cudaStream_t stream);

@@ -24,6 +24,7 @@
 // deviation that no test or reference KAT reaches.
 #include <cub/device/device_radix_sort.cuh>
 
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstring>
@@ -57,7 +58,8 @@ struct SemGrid {
     float *conf;        // [V]            Bayesian: cached confidence
     int32_t *lab_obj, *lab_cls;  // [V][kSemLabels]
     float *lab_logp;             // [V][kSemLabels]
-    uint32_t capacity;
+    uint32_t capacity;           // maximum capacity: allocation hands out pool indices below it (others get kNoBlock)
+    uint32_t pool_capacity;      // blocks with storage now (<= capacity): the per-voxel arrays hold pool_capacity * 512
     int32_t kind;
     float depth_threshold, depth_decay_rate;
 };
@@ -117,10 +119,14 @@ sem_insert_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, 
 }
 
 // ---- 2. sort keys --------------------------------------------------------------------------------------------
+// Only points whose block has a pool index in [lo, hi) get a key; the others get kBadVid, sort last and are left out
+// by the runs.  The first pass of a call covers the blocks with storage, [0, pool_capacity); after a growth the
+// keys -> sort -> runs passes are replayed over the blocks that just got storage.
 template <typename T>
 __global__ void __launch_bounds__(256)
 sem_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, const int64_t n, const float inv_vs,
-                const HashTable H, const SemGrid G, uint32_t *__restrict__ vid, uint32_t *__restrict__ order) {
+                const HashTable H, const SemGrid G, const uint32_t lo, const uint32_t hi, uint32_t *__restrict__ vid,
+                uint32_t *__restrict__ order) {
     const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int vx = PointKey<T>::coord(pts[3 * i + 0], inv_vs), vy = PointKey<T>::coord(pts[3 * i + 1], inv_vs),
@@ -131,7 +137,7 @@ sem_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, co
                               : kEmpty;
     if (slot != kEmpty) {
         const uint32_t idx = H.entries[slot].w;
-        if (idx < G.capacity)
+        if (idx >= lo && idx < hi)   // kNoBlock is past every window
             key = idx * kVox + static_cast<uint32_t>(local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6));
     }
     vid[i] = key;
@@ -623,8 +629,9 @@ sem_assoc_apply_kernel(const SemGrid G, const int32_t *__restrict__ pend, const 
     }
 }
 
-__global__ void sem_fill_kernel(const SemGrid G, const size_t n_vox) {
-    for (size_t v = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < n_vox;
+// the non-zero fields of a cleared voxel, for the voxels [v0, v1)
+__global__ void sem_fill_kernel(const SemGrid G, const size_t v0, const size_t v1) {
+    for (size_t v = v0 + static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; v < v1;
          v += static_cast<size_t>(gridDim.x) * blockDim.x) {
         G.obj[v] = -1;
         G.cls[v] = -1;
@@ -639,6 +646,8 @@ __global__ void sem_fill_kernel(const SemGrid G, const size_t n_vox) {
 // ====================================================================================================================
 using namespace b2v;
 
+constexpr int kSemArrays = 11;   // per-voxel arrays of a Bayesian grid (a voting grid has the first 6)
+
 struct b2v_sgrid {
     double voxel_size = 0.0;
     float inv_voxel_size = 0.0f;
@@ -646,6 +655,11 @@ struct b2v_sgrid {
     cudaStream_t stream = nullptr;
     HashTable table{};
     SemGrid G{};
+    // each per-voxel array of G is a reservation for G.capacity blocks with storage mapped on demand (a fixed grid
+    // maps it whole at create); G.pool_capacity is the least any array holds
+    bool growable = false;
+    VmmRange store[kSemArrays];
+    int64_t growths = 0;
     uint32_t *h_counters = nullptr;
     // staging
     void *d_pts = nullptr, *d_cols = nullptr;
@@ -700,17 +714,65 @@ static int sgrid_clear_device(b2v_sgrid *g, uint32_t used_blocks) {
     SG_CUDA(g, cudaMemsetAsync(g->G.col, 0, nv * 3 * sizeof(float), g->stream));
     SG_CUDA(g, cudaMemsetAsync(g->G.counter, 0, nv * sizeof(int32_t), g->stream));
     if (g->G.kind == B2V_SEM_PROBABILISTIC) SG_CUDA(g, cudaMemsetAsync(g->G.conf, 0, nv * sizeof(float), g->stream));
-    sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->G, nv);
+    sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->G, 0, nv);
     SG_CUDA(g, cudaGetLastError());
     return B2V_OK;
 }
 
+// the per-voxel arrays of the grid's kind and the bytes each holds per voxel
+struct SemArray {
+    void **ptr;
+    size_t voxel_bytes;
+};
+static int sgrid_arrays(b2v_sgrid *g, SemArray out[kSemArrays]) {
+    SemGrid &G = g->G;
+    const SemArray all[kSemArrays] = {
+        {reinterpret_cast<void **>(&G.count), sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.pos), 3 * sizeof(double)},
+        {reinterpret_cast<void **>(&G.col), 3 * sizeof(float)},
+        {reinterpret_cast<void **>(&G.obj), sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.cls), sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.counter), sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.ml_logp), sizeof(float)},
+        {reinterpret_cast<void **>(&G.conf), sizeof(float)},
+        {reinterpret_cast<void **>(&G.lab_obj), kSemLabels * sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.lab_cls), kSemLabels * sizeof(int32_t)},
+        {reinterpret_cast<void **>(&G.lab_logp), kSemLabels * sizeof(float)},
+    };
+    const int n = G.kind == B2V_SEM_PROBABILISTIC ? kSemArrays : 6;
+    for (int k = 0; k < n; ++k) out[k] = all[k];
+    return n;
+}
+
+// map (zeroed) storage for at least `blocks` blocks in every array; G.pool_capacity becomes the least any array holds.
+// Voxels entering the storage are set to the cleared state by the caller.  False if a mapping failed.
+static bool sgrid_map_storage(b2v_sgrid *g, uint64_t blocks, std::string *err) {
+    SemArray arr[kSemArrays];
+    const int na = sgrid_arrays(g, arr);
+    bool ok = true;
+    uint64_t storage = g->G.capacity;
+    for (int k = 0; k < na; ++k) {
+        const size_t block_bytes = arr[k].voxel_bytes * kVox;
+        ok = ok && vmm_map(&g->store[k], static_cast<size_t>(blocks) * block_bytes, g->stream, err);
+        storage = std::min<uint64_t>(storage, g->store[k].mapped / block_bytes);
+    }
+    g->G.pool_capacity = static_cast<uint32_t>(storage);
+    return ok;
+}
+
 extern "C" int b2v_sgrid_create(double voxel_size, int32_t block_size, uint32_t capacity_blocks, int32_t kind,
                                 int32_t device, b2v_sgrid **out) {
+    return b2v_sgrid_create_ex(voxel_size, block_size, capacity_blocks, 0, kind, device, out);
+}
+
+extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32_t capacity_blocks,
+                                   uint32_t max_capacity_blocks, int32_t kind, int32_t device, b2v_sgrid **out) {
     if (!out) return B2V_ERR_INVALID_ARGUMENT;
     *out = nullptr;
+    // the sort key pool_index * 512 + voxel must stay below kBadVid: at most 2^22 blocks
     if (block_size != B2V_BLOCK_SIZE || !(voxel_size > 0.0) || capacity_blocks == 0 ||
-        capacity_blocks > (1u << 22) || (kind != B2V_SEM_VOTING && kind != B2V_SEM_PROBABILISTIC))
+        capacity_blocks > (1u << 22) || (kind != B2V_SEM_VOTING && kind != B2V_SEM_PROBABILISTIC) ||
+        (max_capacity_blocks != 0 && (max_capacity_blocks < capacity_blocks || max_capacity_blocks > (1u << 22))))
         return B2V_ERR_INVALID_ARGUMENT;
     b2v_sgrid *g = new (std::nothrow) b2v_sgrid();
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
@@ -719,7 +781,10 @@ extern "C" int b2v_sgrid_create(double voxel_size, int32_t block_size, uint32_t 
     g->inv_voxel_size = 1.0f / static_cast<float>(voxel_size);
     g->device = device;
     g->G.kind = kind;
-    g->G.capacity = capacity_blocks;
+    // the table, the block keys and the arrays' reservations are sized for the maximum; only storage grows
+    const uint32_t cap = std::max(capacity_blocks, max_capacity_blocks);
+    g->growable = cap > capacity_blocks;
+    g->G.capacity = cap;
     // class defaults (voxel_data_semantic.h:107-108, 251-254)
     g->G.depth_threshold = kind == B2V_SEM_VOTING ? 10.0f : 5.0f;
     g->G.depth_decay_rate = 0.07f;
@@ -727,25 +792,20 @@ extern "C" int b2v_sgrid_create(double voxel_size, int32_t block_size, uint32_t 
     SG_CUDA(g, cudaSetDevice(device));
     SG_CUDA(g, cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
     uint64_t tcap = 1;
-    while (tcap < static_cast<uint64_t>(capacity_blocks) * 2) tcap <<= 1;
+    while (tcap < static_cast<uint64_t>(cap) * 2) tcap <<= 1;
     g->table.mask = static_cast<uint32_t>(tcap - 1);
-    const size_t nv = static_cast<size_t>(capacity_blocks) * kVox;
     SG_CUDA(g, cudaMalloc(&g->table.entries, tcap * sizeof(uint4)));
     SG_CUDA(g, cudaMalloc(&g->G.counters, kSemNumCounters * sizeof(uint32_t)));
-    SG_CUDA(g, cudaMalloc(&g->G.block_keys, static_cast<size_t>(capacity_blocks) * sizeof(int4)));
-    SG_CUDA(g, cudaMalloc(&g->G.count, nv * sizeof(int32_t)));
-    SG_CUDA(g, cudaMalloc(&g->G.pos, nv * 3 * sizeof(double)));
-    SG_CUDA(g, cudaMalloc(&g->G.col, nv * 3 * sizeof(float)));
-    SG_CUDA(g, cudaMalloc(&g->G.obj, nv * sizeof(int32_t)));
-    SG_CUDA(g, cudaMalloc(&g->G.cls, nv * sizeof(int32_t)));
-    SG_CUDA(g, cudaMalloc(&g->G.counter, nv * sizeof(int32_t)));
-    if (kind == B2V_SEM_PROBABILISTIC) {
-        SG_CUDA(g, cudaMalloc(&g->G.ml_logp, nv * sizeof(float)));
-        SG_CUDA(g, cudaMalloc(&g->G.conf, nv * sizeof(float)));
-        SG_CUDA(g, cudaMalloc(&g->G.lab_obj, nv * kSemLabels * sizeof(int32_t)));
-        SG_CUDA(g, cudaMalloc(&g->G.lab_cls, nv * kSemLabels * sizeof(int32_t)));
-        SG_CUDA(g, cudaMalloc(&g->G.lab_logp, nv * kSemLabels * sizeof(float)));
+    SG_CUDA(g, cudaMalloc(&g->G.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
+    SemArray arr[kSemArrays];
+    const int na = sgrid_arrays(g, arr);
+    for (int k = 0; k < na; ++k) {
+        if (!vmm_reserve(&g->store[k], static_cast<size_t>(cap) * kVox * arr[k].voxel_bytes, device, &g->err))
+            return B2V_ERR_CUDA;
+        *arr[k].ptr = reinterpret_cast<void *>(g->store[k].va);
     }
+    if (!sgrid_map_storage(g, capacity_blocks, &g->err)) return B2V_ERR_CUDA;
+    g->G.pool_capacity = capacity_blocks;   // the rest of the last granules is used only after a growth
     SG_CUDA(g, cudaMalloc(&g->d_total, sizeof(uint32_t)));
     SG_CUDA(g, cudaMallocHost(&g->h_counters, kSemNumCounters * sizeof(uint32_t)));
     const int rc = sgrid_clear_device(g, capacity_blocks);
@@ -758,8 +818,8 @@ extern "C" int b2v_sgrid_destroy(b2v_sgrid *g) {
     if (!g) return B2V_OK;
     cudaSetDevice(g->device);
     if (g->stream) cudaStreamSynchronize(g->stream);
-    void *ptrs[] = {g->table.entries, g->G.counters, g->G.block_keys, g->G.count, g->G.pos, g->G.col, g->G.obj,
-                    g->G.cls, g->G.counter, g->G.ml_logp, g->G.conf, g->G.lab_obj, g->G.lab_cls, g->G.lab_logp,
+    for (VmmRange &r : g->store) vmm_release(&r);
+    void *ptrs[] = {g->table.entries, g->G.counters, g->G.block_keys,
                     g->d_pts, g->d_cols, g->d_cls, g->d_inst, g->d_depths, g->d_vid[0], g->d_vid[1], g->d_ord[0],
                     g->d_ord[1], g->d_sort_tmp, g->d_sums, g->d_offs, g->d_total, g->d_out_pts, g->d_out_cols,
                     g->d_out_conf, g->d_out_cls, g->d_out_obj, g->d_img_depth, g->d_img_filtered, g->d_img_rgb,
@@ -791,7 +851,7 @@ extern "C" int b2v_sgrid_clear(b2v_sgrid *g) {
     SG_CUDA(g, cudaMemcpyAsync(g->h_counters, g->G.counters, kSemNumCounters * sizeof(uint32_t),
                                cudaMemcpyDeviceToHost, g->stream));
     SG_CUDA(g, cudaStreamSynchronize(g->stream));
-    const uint32_t used = g->h_counters[kSemPool] < g->G.capacity ? g->h_counters[kSemPool] : g->G.capacity;
+    const uint32_t used = std::min(g->h_counters[kSemPool], g->G.pool_capacity);   // the storage is kept
     const int rc = sgrid_clear_device(g, used);
     if (rc != B2V_OK) return rc;
     SG_CUDA(g, cudaStreamSynchronize(g->stream));
@@ -841,21 +901,16 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
     return B2V_OK;
 }
 
-// insert -> keys -> sort -> runs over the staged point records (valid: optional per-point mask)
-static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
+// keys -> sort -> runs over the staged point records, for the points whose block's pool index lies in [lo, hi)
+static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid, uint32_t lo, uint32_t hi) {
     cudaStream_t s = g->stream;
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    if (in.pts_f64) {
-        sem_insert_kernel<double><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n,
-                                                       g->inv_voxel_size, g->table, g->G);
+    if (in.pts_f64)
         sem_keys_kernel<double><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n, g->inv_voxel_size,
-                                                     g->table, g->G, g->d_vid[0], g->d_ord[0]);
-    } else {
-        sem_insert_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n, g->inv_voxel_size,
-                                                      g->table, g->G);
+                                                     g->table, g->G, lo, hi, g->d_vid[0], g->d_ord[0]);
+    else
         sem_keys_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n, g->inv_voxel_size,
-                                                    g->table, g->G, g->d_vid[0], g->d_ord[0]);
-    }
+                                                    g->table, g->G, lo, hi, g->d_vid[0], g->d_ord[0]);
     SG_CUDA(g, cudaGetLastError());
     size_t tmp = g->sort_tmp_bytes;  // all 32 key bits: kBadVid (points without storage) must sort last
     SG_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp, tmp, g->d_vid[0], g->d_vid[1], g->d_ord[0], g->d_ord[1],
@@ -863,6 +918,52 @@ static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const
     sem_runs_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1], g->d_ord[1], n, in, g->G);
     SG_CUDA(g, cudaGetLastError());
     return B2V_OK;
+}
+
+// Growable grids, at the end of an integrate call: the call's first pass skipped the points of blocks handed a pool
+// index past the storage.  Map storage for every handed-out index (at least doubling, at most the maximum), set the
+// new voxels to the cleared state and replay keys -> sort -> runs over the blocks that just got storage, from the
+// same staged inputs.  All observations of a voxel in one call belong to one block and a block's index never
+// changes, so every voxel is updated by exactly one of the passes, from the cleared state, in input order (the sort
+// is stable): the grid equals one created at the maximum.  If the storage cannot grow, the blocks past it are dropped
+// ("block pool full").
+static int sgrid_resolve(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
+    SG_CUDA(g, cudaMemcpyAsync(g->h_counters, g->G.counters, kSemNumCounters * sizeof(uint32_t),
+                               cudaMemcpyDeviceToHost, g->stream));
+    SG_CUDA(g, cudaStreamSynchronize(g->stream));
+    const uint32_t used = g->h_counters[kSemPool], old = g->G.pool_capacity;
+    if (used <= old || old >= g->G.capacity) return B2V_OK;
+    std::string map_err;   // a failed mapping surfaces as "block pool full" below
+    sgrid_map_storage(g, std::min<uint64_t>(g->G.capacity, std::max<uint64_t>(used, 2ull * old)), &map_err);
+    const uint32_t now = g->G.pool_capacity;
+    if (now > old) {
+        g->growths += 1;
+        sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->G, static_cast<size_t>(old) * kVox,
+                                                    static_cast<size_t>(now) * kVox);
+        SG_CUDA(g, cudaGetLastError());
+        const int rc = sgrid_apply(g, n, in, valid, old, now);
+        if (rc != B2V_OK) return rc;
+    }
+    if (used > now)   // the storage could not grow far enough
+        SG_CUDA(g, launch_drop_unbacked_slots(g->table, now, g->G.capacity, g->G.counters + kSemError, g->stream));
+    return B2V_OK;
+}
+
+// insert -> keys -> sort -> runs over the staged point records (valid: optional per-point mask); a growable grid
+// resolves an overflow before returning, so the staged inputs must stay alive until the call ends
+static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
+    cudaStream_t s = g->stream;
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+    if (in.pts_f64)
+        sem_insert_kernel<double><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n,
+                                                       g->inv_voxel_size, g->table, g->G);
+    else
+        sem_insert_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n, g->inv_voxel_size,
+                                                      g->table, g->G);
+    SG_CUDA(g, cudaGetLastError());
+    const int rc = sgrid_apply(g, n, in, valid, 0, g->G.pool_capacity);
+    if (rc != B2V_OK || !g->growable) return rc;
+    return sgrid_resolve(g, n, in, valid);
 }
 
 extern "C" int b2v_sgrid_integrate(b2v_sgrid *g, int64_t n, const void *points, int32_t points_f64,
@@ -988,7 +1089,16 @@ extern "C" int64_t b2v_sgrid_num_blocks(b2v_sgrid *g) {
         cudaStreamSynchronize(g->stream) != cudaSuccess)
         return -1;
     const uint32_t p = g->h_counters[kSemPool];
-    return p < g->G.capacity ? p : g->G.capacity;
+    return p < g->G.pool_capacity ? p : g->G.pool_capacity;
+}
+
+extern "C" int b2v_sgrid_capacity(b2v_sgrid *g, int64_t *capacity_blocks, int64_t *growths) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    SG_CUDA(g, cudaSetDevice(g->device));
+    SG_CUDA(g, cudaStreamSynchronize(g->stream));
+    if (capacity_blocks) *capacity_blocks = g->G.pool_capacity;
+    if (growths) *growths = g->growths;
+    return B2V_OK;
 }
 
 extern "C" int b2v_sgrid_label_overflows(b2v_sgrid *g, uint64_t *out) {

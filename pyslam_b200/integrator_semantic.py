@@ -54,6 +54,9 @@ DEFAULT_PARAMETERS = {
     "kVolumetricSemanticIntegrationMinVoteRatio": 0.5,
     "kVolumetricSemanticIntegrationMinVotes": 3,
     "kVolumetricIntegrationB200CapacityBlocks": 1 << 15,
+    # growth ceiling of the grid's storage: > CapacityBlocks starts with CapacityBlocks blocks and maps more on
+    # demand, holding what a grid of this size from the start holds; 0 = fixed storage of CapacityBlocks
+    "kVolumetricIntegrationB200MaxCapacityBlocks": 0,
     "kVolumetricIntegrationB200Device": 0,
     "kVolumetricIntegrationB200GenerateObjects": True,   # kGenerateObjectsDefault (reference :84)
 }
@@ -91,7 +94,8 @@ def make_semantic_integrator_class(Base, api):
             self.volume = grid_t(voxel_size=p["kVolumetricIntegrationVoxelLength"],
                                  block_size=p["kVolumetricIntegrationBlockSize"],
                                  capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
-                                 device=int(p["kVolumetricIntegrationB200Device"]))
+                                 device=int(p["kVolumetricIntegrationB200Device"]),
+                                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None)
             self.volume.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
             self.volume.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
             fx, fy, cx, cy = self._intrinsics()
@@ -263,7 +267,9 @@ def make_voxel_grid_integrator_class(Base, api):
             self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{side}"]
             self.volume = VoxelBlockGrid(p["kVolumetricIntegrationVoxelLength"], p["kVolumetricIntegrationBlockSize"],
                                          capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
-                                         device=int(p["kVolumetricIntegrationB200Device"]))
+                                         device=int(p["kVolumetricIntegrationB200Device"]),
+                                         max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"])
+                                         or None)
             fx, fy, cx, cy = self._intrinsics()
             self.camera_frustrum = CameraFrustrum(
                 fx, fy, cx, cy, self.camera.width, self.camera.height, np.eye(4),

@@ -486,12 +486,18 @@ class VoxelBlockGrid:
     """GPU drop-in for pySLAM's `volumetric.VoxelBlockGrid(voxel_size, block_size=8)`."""
 
     def __init__(self, voxel_size: float, block_size: int = 8, capacity_blocks: int = 1 << 17,
-                 device: int = 0):
+                 device: int = 0, max_capacity_blocks: int | None = None):
+        """`max_capacity_blocks`: growth ceiling of the block pool.  Above `capacity_blocks`, the pool starts with
+        `capacity_blocks` blocks of storage and grows inside the integrate call that needs more; the grid then holds
+        what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the
+        pool fixed."""
         self._L = _lib.load()
         self._h = C.c_void_p()
         self.voxel_size = float(voxel_size)
         self._block_size = int(block_size)
-        rc = self._L.b2v_grid_create(voxel_size, block_size, capacity_blocks, device, C.byref(self._h))
+        self.max_capacity_blocks = int(max_capacity_blocks or 0)
+        rc = self._L.b2v_grid_create_ex(voxel_size, block_size, capacity_blocks, self.max_capacity_blocks, device,
+                                        C.byref(self._h))
         if rc != _lib.B2V_OK:
             msg = self._L.b2v_grid_last_error(self._h).decode() if self._h else "invalid configuration"
             if self._h:
@@ -587,7 +593,14 @@ class VoxelBlockGrid:
         return self.get_voxels(1).colors
 
     def clear(self):
+        """Empties the grid; a grown pool keeps its storage."""
         self._check(self._L.b2v_grid_clear(self._h), "b2v_grid_clear")
+
+    def capacity(self):
+        """(blocks the pool has storage for now, growths since creation); synchronises."""
+        n, g = C.c_int64(0), C.c_int64(0)
+        self._check(self._L.b2v_grid_capacity(self._h, C.byref(n), C.byref(g)), "b2v_grid_capacity")
+        return int(n.value), int(g.value)
 
     reset = clear
 
@@ -788,13 +801,18 @@ class VoxelBlockSemanticGrid:
     KIND = _lib.B2V_SEM_VOTING
 
     def __init__(self, voxel_size: float = 0.05, block_size: int = 8, capacity_blocks: int = 1 << 14,
-                 device: int = 0):
+                 device: int = 0, max_capacity_blocks: int | None = None):
+        """`max_capacity_blocks`: growth ceiling (at most 2^22 blocks).  Above `capacity_blocks`, the per-voxel storage
+        starts with `capacity_blocks` blocks and grows inside the integrate call that needs more; the grid then holds,
+        bit for bit, what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or
+        `capacity_blocks`) keeps the storage fixed."""
         self._L = _lib.load()
         self._h = C.c_void_p()
         self.voxel_size = float(voxel_size)
         self._block_size = int(block_size)
-        rc = self._L.b2v_sgrid_create(float(voxel_size), int(block_size), int(capacity_blocks), self.KIND,
-                                      int(device), C.byref(self._h))
+        self.max_capacity_blocks = int(max_capacity_blocks or 0)
+        rc = self._L.b2v_sgrid_create_ex(float(voxel_size), int(block_size), int(capacity_blocks),
+                                         self.max_capacity_blocks, self.KIND, int(device), C.byref(self._h))
         if rc != _lib.B2V_OK:
             msg = self._L.b2v_sgrid_last_error(self._h).decode() if self._h else "invalid configuration"
             if self._h:
@@ -1002,7 +1020,14 @@ class VoxelBlockSemanticGrid:
         return self.num_blocks() == 0
 
     def clear(self):
+        """Empties the grid; grown storage is kept."""
         self._check(self._L.b2v_sgrid_clear(self._h), "b2v_sgrid_clear")
+
+    def capacity(self):
+        """(blocks the storage holds now, growths since creation); synchronises."""
+        n, g = C.c_int64(0), C.c_int64(0)
+        self._check(self._L.b2v_sgrid_capacity(self._h, C.byref(n), C.byref(g)), "b2v_sgrid_capacity")
+        return int(n.value), int(g.value)
 
     reset = clear
 
