@@ -29,7 +29,8 @@ EXPORTED_SYMBOLS = [
     "b2v_integrate_batch", "b2v_integrate_u16", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_capacity",
     "b2v_num_blocks", "b2v_last_frame_stats", "b2v_last_mesh_stats",
     "b2v_counters", "b2v_set_overlap", "b2v_set_fusion", "b2v_set_group_size", "b2v_set_input_event", "b2v_set_rectification", "b2v_remap", "b2v_profile_enable", "b2v_profile_read", "b2v_dump_blocks", "b2v_upload_blocks", "b2v_export_blocks_device", "b2v_import_blocks_device", "b2v_last_touched_keys", "b2v_extract_mesh", "b2v_copy_mesh",
-    "b2v_extract_points", "b2v_copy_points", "b2v_grid_create", "b2v_grid_create_ex", "b2v_grid_capacity",
+    "b2v_extract_points", "b2v_copy_points", "b2v_export_halo_device", "b2v_extract_mesh_with_halo",
+    "b2v_extract_points_with_halo", "b2v_weld_mesh_device", "b2v_weld_last_error", "b2v_grid_create", "b2v_grid_create_ex", "b2v_grid_capacity",
     "b2v_grid_destroy", "b2v_grid_clear",
     "b2v_grid_last_error", "b2v_grid_integrate", "b2v_grid_integrate_f64", "b2v_grid_integrate_ex", "b2v_grid_integrate_rgbd", "b2v_filter_shadow_points", "b2v_grid_synchronize", "b2v_grid_num_blocks",
     "b2v_grid_size", "b2v_grid_get_voxels", "b2v_grid_copy_voxels",
@@ -190,6 +191,16 @@ def load() -> C.CDLL:
     L.b2v_extract_points.argtypes = [vp, p_i64]
     L.b2v_copy_points.restype = C.c_int
     L.b2v_copy_points.argtypes = [vp, vp, vp]
+    L.b2v_export_halo_device.restype = C.c_int
+    L.b2v_export_halo_device.argtypes = [vp, i32, vp, vp, vp, vp, i64, i64]
+    L.b2v_extract_mesh_with_halo.restype = C.c_int
+    L.b2v_extract_mesh_with_halo.argtypes = [vp, i64, vp, vp, p_i64, p_i64]
+    L.b2v_extract_points_with_halo.restype = C.c_int
+    L.b2v_extract_points_with_halo.argtypes = [vp, i64, vp, vp, p_i64]
+    L.b2v_weld_mesh_device.restype = C.c_int
+    L.b2v_weld_mesh_device.argtypes = [i32, i32, vp, vp] + [vp] * 8 + [p_i64]
+    L.b2v_weld_last_error.restype = C.c_char_p
+    L.b2v_weld_last_error.argtypes = []
 
     L.b2v_grid_create.restype = C.c_int
     L.b2v_grid_create.argtypes = [C.c_float, i32, u32, i32, C.POINTER(vp)]

@@ -159,6 +159,11 @@ struct b2v_volume {
     size_t mesh_v_cap = 0, mesh_t_cap = 0;
     int64_t last_nv = 0, last_nt = 0;
     uint32_t *h_totals = nullptr;
+    // sharded extraction (b2v_extract_*_with_halo): an unsharded scratch volume holding this volume's blocks at the
+    // same pool indices plus the received halo blocks after them, kept between extractions.  The most recent
+    // extraction's output lives in it when last_from_halo is set.
+    b2v_volume *halo = nullptr;
+    bool last_from_halo = false;
     // optional per-kernel timing (b2v_profile_*)
     bool prof_enabled = false;
     std::vector<cudaEvent_t> prof_events;  // quadruples: allocate begin/end, integrate begin/end
@@ -314,7 +319,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 102; }
+extern "C" int b2v_version(void) { return 103; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -429,6 +434,7 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
 
 extern "C" int b2v_destroy(b2v_volume *v) {
     if (!v) return B2V_OK;
+    b2v_destroy(v->halo);
     cudaSetDevice(v->cfg.device);
     cudaDeviceSynchronize();
     if (v->ev_in) cudaEventDestroy(v->ev_in);
@@ -1267,6 +1273,7 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     rc = ensure_mesh_scratch(v, nb);
     if (rc != B2V_OK) return rc;
     v->mb.n_blocks = nb;
+    v->last_from_halo = false;
     cudaStream_t cs = v->compute;
     const int sms = v->sm_count;
     if (mesh) {
@@ -1301,6 +1308,7 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
 
 extern "C" int b2v_last_mesh_stats(b2v_volume *v, int64_t stats[5]) {
     if (!v || !stats) return B2V_ERR_INVALID_ARGUMENT;
+    if (v->last_from_halo && v->halo) return b2v_last_mesh_stats(v->halo, stats);
     stats[0] = v->mb.n_blocks;
     stats[1] = v->h_totals[kMtCandidates];
     stats[2] = v->h_totals[kMtTiles];
@@ -1317,6 +1325,11 @@ extern "C" int b2v_extract_mesh(b2v_volume *v, int64_t *n_vertices, int64_t *n_t
 extern "C" int b2v_copy_mesh(b2v_volume *v, double *vertices, double *colors, int32_t *edge_ids,
                              int32_t *triangles) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    if (v->last_from_halo && v->halo) {
+        const int rc = b2v_copy_mesh(v->halo, vertices, colors, edge_ids, triangles);
+        if (rc != B2V_OK) v->err = v->halo->err;
+        return rc;
+    }
     const size_t nv = static_cast<size_t>(v->last_nv), nt = static_cast<size_t>(v->last_nt);
     if (vertices && nv) B2V_CUDA(v, cudaMemcpy(vertices, v->mb.vertices, nv * 3 * sizeof(double), cudaMemcpyDeviceToHost));
     if (colors && nv) B2V_CUDA(v, cudaMemcpy(colors, v->mb.colors, nv * 3 * sizeof(double), cudaMemcpyDeviceToHost));
@@ -1332,6 +1345,262 @@ extern "C" int b2v_extract_points(b2v_volume *v, int64_t *n_points) {
 
 extern "C" int b2v_copy_points(b2v_volume *v, double *points, double *colors) {
     return b2v_copy_mesh(v, points, colors, nullptr, nullptr);
+}
+
+// ---- sharded extraction: face-halo exchange (b2v_shard.cu) --------------------------------------------------------
+
+extern "C" int b2v_export_halo_device(b2v_volume *v, int32_t world, int64_t *records, int64_t *payload_voxels,
+                                      int32_t *d_headers, float *d_payload, int64_t max_records,
+                                      int64_t max_payload_voxels) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    if (world < 1 || !records || !payload_voxels || ((d_headers == nullptr) != (d_payload == nullptr))) {
+        v->err = "b2v_export_halo_device: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    const int rc = read_counters(v);
+    if (rc == B2V_ERR_CUDA) return rc;
+    B2V_CUDA(v, cudaSetDevice(v->cfg.device));
+    const uint32_t nb = block_count(v);
+    for (int r = 0; r < world; ++r) records[r] = payload_voxels[r] = 0;
+    if (nb == 0 || world == 1) return B2V_OK;
+    const uint64_t n = static_cast<uint64_t>(world) * nb;
+    if (n >= (1ull << 31)) {
+        v->err = "b2v_export_halo_device: world size x blocks must stay below 2^31";
+        return B2V_ERR_UNSUPPORTED;
+    }
+    const uint64_t chunks = (n + 1023) / 1024;
+    uint32_t *d_counts = nullptr, *d_offs = nullptr, *d_part = nullptr, *d_tot = nullptr, *d_dest = nullptr;
+    std::vector<uint32_t> dest(2 * (static_cast<size_t>(world) + 1));
+    cudaStream_t cs = v->compute;
+    cudaError_t e = cudaMalloc(&d_counts, 2 * n * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_offs, 2 * n * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_part, 2 * chunks * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_tot, 2 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_dest, dest.size() * sizeof(uint32_t));
+    if (e == cudaSuccess) e = launch_halo_count(v->meta, nb, world, d_counts, d_offs, d_part, d_tot, d_dest, cs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dest.data(), d_dest, dest.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+    int out = B2V_OK;
+    if (e == cudaSuccess) {
+        const uint32_t *dr = dest.data(), *dp = dest.data() + world + 1;
+        for (int r = 0; r < world; ++r) {
+            records[r] = dr[r + 1] - dr[r];
+            payload_voxels[r] = dp[r + 1] - dp[r];
+        }
+        if (d_headers) {
+            if (static_cast<int64_t>(dr[world]) > max_records || static_cast<int64_t>(dp[world]) > max_payload_voxels) {
+                v->err = "b2v_export_halo_device: destination too small";
+                out = B2V_ERR_INVALID_ARGUMENT;
+            } else {
+                e = launch_halo_emit(v->meta, nb, world, d_offs, d_headers, d_payload, cs);
+                if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+            }
+        }
+    }
+    cudaFree(d_counts);
+    cudaFree(d_offs);
+    cudaFree(d_part);
+    cudaFree(d_tot);
+    cudaFree(d_dest);
+    if (e != cudaSuccess) {
+        v->err = std::string("b2v_export_halo_device: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    return out;
+}
+
+// the unsharded scratch of the halo extraction, with room for `blocks` blocks (recreated larger when needed)
+static int ensure_halo_scratch(b2v_volume *v, uint64_t blocks) {
+    if (v->halo && v->halo->meta.capacity >= blocks) return B2V_OK;
+    b2v_destroy(v->halo);
+    v->halo = nullptr;
+    const uint64_t cap = std::max<uint64_t>(1024, blocks + blocks / 2);
+    if (cap > (1ull << 30)) {
+        v->err = "halo extraction: more than 2^30 blocks";
+        return B2V_ERR_UNSUPPORTED;
+    }
+    b2v_config c = v->cfg;
+    c.shard_rank = 0;
+    c.shard_count = 1;
+    c.capacity_blocks = static_cast<uint32_t>(cap);
+    c.max_capacity_blocks = 0;
+    b2v_volume *h = nullptr;
+    const int rc = b2v_create(&c, &h);
+    if (rc != B2V_OK) {
+        v->err = std::string("halo extraction scratch: ") + (h ? h->err : "invalid configuration");
+        b2v_destroy(h);
+        return rc;
+    }
+    v->halo = h;
+    return B2V_OK;
+}
+
+static int extract_with_halo(b2v_volume *v, bool mesh, int64_t n_records, const int32_t *d_headers,
+                             const float *d_payload, int64_t *n_vertices, int64_t *n_triangles) {
+    if (n_records < 0 || (n_records > 0 && (!d_headers || !d_payload))) {
+        v->err = "b2v_extract_*_with_halo: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    int rc = read_counters(v);
+    if (rc == B2V_ERR_CUDA) return rc;
+    B2V_CUDA(v, cudaSetDevice(v->cfg.device));
+    const uint32_t nb = block_count(v);
+    rc = ensure_halo_scratch(v, static_cast<uint64_t>(nb) + static_cast<uint64_t>(n_records));
+    if (rc != B2V_OK) return rc;
+    b2v_volume *h = v->halo;
+    const uint32_t nr = static_cast<uint32_t>(n_records);
+    cudaStream_t cs = h->compute;
+    uint32_t *d_sizes = nullptr, *d_offs = nullptr, *d_part = nullptr, *d_tot = nullptr;
+    uint32_t head[2] = {nb + nr, 0u};   // the scratch's block count; its error flag after the import
+    cudaError_t e = cudaMalloc(&d_sizes, (nr ? nr : 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_offs, (nr ? nr : 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_part, ((nr + 1023) / 1024 + 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_tot, sizeof(uint32_t));
+    if (e == cudaSuccess)
+        e = cudaMemsetAsync(h->table.entries, 0xFF, (static_cast<size_t>(h->table.mask) + 1) * sizeof(uint4), cs);
+    if (e == cudaSuccess) e = cudaMemsetAsync(h->meta.counters, 0, kNumCounters * sizeof(uint32_t), cs);
+    if (e == cudaSuccess)
+        e = launch_halo_import(v->meta, nb, d_headers, d_payload, nr, d_sizes, d_offs, d_part, d_tot, h->table, h->meta, cs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->meta.counters + kCtrPool, &head[0], sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&head[1], h->meta.counters + kCtrError, sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+    cudaFree(d_sizes);
+    cudaFree(d_offs);
+    cudaFree(d_part);
+    cudaFree(d_tot);
+    if (e != cudaSuccess) {
+        v->err = std::string("halo import: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    if (head[1]) {
+        v->err = (head[1] & 4u) ? "halo import: a record has an invalid mask"
+                 : (head[1] & 8u) ? "halo import: a block key arrived twice (records of another world size?)"
+                                  : "halo import: scratch table full";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    rc = extract_common(h, mesh, n_vertices, n_triangles);
+    if (rc != B2V_OK) {
+        v->err = h->err;
+        return rc;
+    }
+    if (!mesh && nb < h->mb.n_blocks) {
+        // the point pass roots at the own blocks only: their points come first (output order is by pool index)
+        uint32_t owned = 0;
+        B2V_CUDA(v, cudaMemcpy(&owned, h->mb.offs + nb, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        h->last_nv = owned;
+        if (n_vertices) *n_vertices = owned;
+    }
+    v->last_from_halo = true;
+    return B2V_OK;
+}
+
+extern "C" int b2v_extract_mesh_with_halo(b2v_volume *v, int64_t n_records, const int32_t *d_headers,
+                                          const float *d_payload, int64_t *n_vertices, int64_t *n_triangles) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    return extract_with_halo(v, true, n_records, d_headers, d_payload, n_vertices, n_triangles);
+}
+
+extern "C" int b2v_extract_points_with_halo(b2v_volume *v, int64_t n_records, const int32_t *d_headers,
+                                            const float *d_payload, int64_t *n_points) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    return extract_with_halo(v, false, n_records, d_headers, d_payload, n_points, nullptr);
+}
+
+static thread_local std::string g_weld_err;
+
+extern "C" const char *b2v_weld_last_error(void) { return g_weld_err.c_str(); }
+
+extern "C" int b2v_weld_mesh_device(int32_t device, int32_t n_pieces, const int64_t *piece_vertices,
+                                    const int64_t *piece_triangles, const double *d_vertices, const double *d_colors,
+                                    const int32_t *d_edge_ids, const int32_t *d_triangles, double *d_out_vertices,
+                                    double *d_out_colors, int32_t *d_out_edge_ids, int32_t *d_out_triangles,
+                                    int64_t *n_out_vertices) {
+    g_weld_err.clear();
+    if (n_pieces < 1 || !piece_vertices || !piece_triangles || !n_out_vertices) {
+        g_weld_err = "b2v_weld_mesh_device: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    std::vector<uint32_t> base(2 * (static_cast<size_t>(n_pieces) + 1), 0u);
+    uint64_t nv = 0, nt = 0;
+    for (int p = 0; p < n_pieces; ++p) {
+        if (piece_vertices[p] < 0 || piece_triangles[p] < 0) {
+            g_weld_err = "b2v_weld_mesh_device: negative piece size";
+            return B2V_ERR_INVALID_ARGUMENT;
+        }
+        base[p] = static_cast<uint32_t>(nv);
+        base[n_pieces + 1 + p] = static_cast<uint32_t>(nt);
+        nv += static_cast<uint64_t>(piece_vertices[p]);
+        nt += static_cast<uint64_t>(piece_triangles[p]);
+    }
+    if (nv >= (1ull << 30) || nt >= (1ull << 31)) {
+        g_weld_err = "b2v_weld_mesh_device: mesh too large";
+        return B2V_ERR_UNSUPPORTED;
+    }
+    base[n_pieces] = static_cast<uint32_t>(nv);
+    base[2 * static_cast<size_t>(n_pieces) + 1] = static_cast<uint32_t>(nt);
+    if ((nv && (!d_vertices || !d_colors || !d_edge_ids || !d_out_vertices || !d_out_colors || !d_out_edge_ids)) ||
+        (nt && (!d_triangles || !d_out_triangles))) {
+        g_weld_err = "b2v_weld_mesh_device: missing buffers";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    *n_out_vertices = 0;
+    if (cudaSetDevice(device) != cudaSuccess) {
+        g_weld_err = "b2v_weld_mesh_device: bad device";
+        return B2V_ERR_CUDA;
+    }
+    WeldArgs a{};
+    a.nv = static_cast<uint32_t>(nv);
+    a.nt = static_cast<uint32_t>(nt);
+    a.n_pieces = n_pieces;
+    a.vertices = d_vertices;
+    a.colors = d_colors;
+    a.edge_ids = d_edge_ids;
+    a.triangles = d_triangles;
+    a.out_vertices = d_out_vertices;
+    a.out_colors = d_out_colors;
+    a.out_edge_ids = d_out_edge_ids;
+    a.out_triangles = d_out_triangles;
+    const uint32_t scap = next_pow2(std::max<uint64_t>(1024, 2 * nv));
+    a.set.mask = scap - 1;
+    uint32_t *d_base = nullptr;
+    uint32_t host_tot[2] = {0u, 0u};
+    cudaStream_t cs = nullptr;
+    const size_t n1 = nv ? nv : 1;
+    cudaError_t e = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaMalloc(&a.set.entries, static_cast<size_t>(scap) * sizeof(uint4));
+    if (e == cudaSuccess) e = cudaMalloc(&a.first, static_cast<size_t>(scap) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&a.slot_of, n1 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&a.keep, n1 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&a.newidx, n1 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&a.partials, ((n1 + 1023) / 1024) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&a.totals, 2 * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMalloc(&d_base, base.size() * sizeof(uint32_t));
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(d_base, base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
+    a.vbase = d_base;
+    a.tbase = d_base + n_pieces + 1;
+    if (e == cudaSuccess) e = launch_weld(a, cs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(host_tot, a.totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
+    cudaFree(a.set.entries);
+    cudaFree(a.first);
+    cudaFree(a.slot_of);
+    cudaFree(a.keep);
+    cudaFree(a.newidx);
+    cudaFree(a.partials);
+    cudaFree(a.totals);
+    cudaFree(d_base);
+    if (cs) cudaStreamDestroy(cs);
+    if (e != cudaSuccess) {
+        g_weld_err = std::string("b2v_weld_mesh_device: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    if (host_tot[1]) {
+        g_weld_err = "b2v_weld_mesh_device: edge-id set full";
+        return B2V_ERR_CUDA;
+    }
+    *n_out_vertices = nv ? host_tot[0] : 0;
+    return B2V_OK;
 }
 
 // ---- point-average grid (duck type B) ---------------------------------------------------------

@@ -38,6 +38,13 @@ __host__ __device__ __forceinline__ uint64_t block_key_hash(int x, int y, int z)
     return h1 ^ (h2 << 1) ^ (h3 << 2);
 }
 
+// owner rank of a block: BlockKeyHash % n (SURVEY.md 8e).  64-bit division is emulated (~60 instructions); the
+// allocate kernels test ~1000 candidate keys per tile, so a power-of-two rank count takes the mask instead
+__host__ __device__ __forceinline__ uint32_t block_owner(int x, int y, int z, uint32_t n) {
+    const uint64_t h = block_key_hash(x, y, z);
+    return (n & (n - 1u)) == 0u ? static_cast<uint32_t>(h) & (n - 1u) : static_cast<uint32_t>(h % static_cast<uint64_t>(n));
+}
+
 __host__ __device__ __forceinline__ uint32_t mix32(uint32_t h) {
     h ^= h >> 16;
     h *= 0x85ebca6bu;

@@ -263,6 +263,38 @@ cudaError_t launch_mesh_vertices(const PoolMeta &meta, const MeshBuffers &mb, do
                                  bool points, uint32_t work_blocks, cudaStream_t stream);
 cudaError_t launch_mesh_triangles(const MeshBuffers &mb, uint32_t work_blocks, cudaStream_t stream);
 
+// ---- face-halo exchange of a sharded volume (b2v_shard.cu) ----
+// a halo record carries the union of the faces / lines / corner a rank needs of a block: at most the 512 - 7^3 = 169
+// voxels with some local coordinate 0
+constexpr int kHaloMaxVoxels = 169;
+// counts [2][world * nb] (zeroed here), offs the same, partials [2][ceil(world * nb / 1024)], totals [2];
+// dest_offs [2][world + 1]: the first record / payload voxel of each destination (index world: the totals)
+cudaError_t launch_halo_count(const PoolMeta &meta, uint32_t nb, uint32_t world, uint32_t *counts, uint32_t *offs,
+                              uint32_t *partials, uint32_t *totals, uint32_t *dest_offs, cudaStream_t stream);
+// headers int32 [records][4] = {key x, y, z, mask}, payload float32 [voxels][5], at the positions of launch_halo_count
+cudaError_t launch_halo_emit(const PoolMeta &meta, uint32_t nb, uint32_t world, const uint32_t *offs, int32_t *headers,
+                             float *payload, cudaStream_t stream);
+// scratch dst := src blocks [0, n_owned) at the same pool indices + the records as zero-filled halo blocks at
+// [n_owned, n_owned + n_records); the table must be empty.  sizes / offs [n_records], partials, totals: scan scratch.
+// dst.counters[kCtrError]: bit 1 table full, bit 2 a record with a bad mask, bit 3 a key imported twice
+cudaError_t launch_halo_import(const PoolMeta &src, uint32_t n_owned, const int32_t *headers, const float *payload,
+                               uint32_t n_records, uint32_t *sizes, uint32_t *offs, uint32_t *partials,
+                               uint32_t *totals, const HashTable &table, const PoolMeta &dst, cudaStream_t stream);
+// weld of concatenated mesh pieces by edge id: vertices in order of first occurrence, triangles remapped
+struct WeldArgs {
+    uint32_t nv, nt;
+    int32_t n_pieces;
+    const double *vertices, *colors;
+    const int32_t *edge_ids, *triangles;   // triangles hold piece-local vertex indices
+    const uint32_t *vbase, *tbase;         // [n_pieces + 1] first vertex / triangle of each piece
+    HashTable set;                         // edge-id set, >= 2 nv slots
+    uint32_t *first, *slot_of, *keep, *newidx, *partials;
+    uint32_t *totals;                      // [2]: kept vertices, set-full flag
+    double *out_vertices, *out_colors;
+    int32_t *out_edge_ids, *out_triangles;
+};
+cudaError_t launch_weld(const WeldArgs &args, cudaStream_t stream);
+
 // ---- point-average grid (b2v_grid.cu) ----
 struct GridMeta {
     uint32_t *pool;        // [pool_capacity][7][512] planes: count(int32), px, py, pz, cr, cg, cb (float32)

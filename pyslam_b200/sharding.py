@@ -7,9 +7,12 @@ integrates every frame into the blocks it owns (`b2v_config.shard_rank / shard_c
 * Ingest (`FrameIngest`): a frame crosses PCIe ONCE in the whole job - rank r uploads 1/world of every chunk of
   frames over its own link and the chunk is completed GPU <-> GPU by an NCCL all-gather over NVLink / NVSwitch on a
   side stream, overlapped with the kernels of the previous chunk.
-* Mesh extraction needs the +1-voxel halos of blocks that may live on another rank; `gather_blocks_device` collects
-  all shards on one rank GPU-to-GPU over NCCL (`gather_blocks` is the host-array variant used with gloo in the CPU
-  tests), which then meshes the union.
+* Mesh extraction needs the +1-voxel halos of blocks that may live on another rank.  `extract_mesh_sharded` /
+  `extract_point_cloud_sharded` exchange only those faces (one all_to_all of halo records) and mesh every shard on its
+  own GPU; the pieces are welded on one rank (DESIGN.md §7).  The per-rank steps are public (`halo_records`,
+  `mesh_piece`, `point_piece`, `weld`) so that N shards held in one process can run them too.
+  `extract_mesh_distributed` is the older route: `gather_blocks_device` collects all shards on one rank GPU-to-GPU over
+  NCCL (`gather_blocks` is the host-array variant used with gloo in the CPU tests), which then meshes the union.
 """
 
 from __future__ import annotations
@@ -260,3 +263,148 @@ def extract_mesh_distributed(volume, dst: int = 0, group=None, device=None, capa
     else:
         scratch.upload_blocks(keys, vox)
     return scratch.extract_mesh()
+
+
+# ---- sharded extraction: face-halo exchange ----------------------------------------------------------------------
+
+def halo_records(volume, world: int):
+    """The halo records `volume` (one shard of a `world`-rank sharding) sends each rank: a list of `world` pairs
+    (headers int32 [n,4] = {x,y,z,mask}, payload float32 [m,5]) of CUDA tensors; the volume's own rank gets empty ones."""
+    headers, payload, nrec, nvox = volume.export_halo_torch(world)
+    return list(zip(headers.split(nrec), payload.split(nvox)))
+
+
+def _concat_records(records):
+    """`records`: one (headers, payload) pair or a list of them (the records a rank received, any order)."""
+    import torch
+    if isinstance(records, tuple) and len(records) == 2 and not isinstance(records[0], tuple):
+        return records
+    records = list(records)
+    if not records:
+        return torch.zeros((0, 4), dtype=torch.int32), torch.zeros((0, 5), dtype=torch.float32)
+    return torch.cat([torch.as_tensor(h).reshape(-1, 4) for h, _ in records]), \
+        torch.cat([torch.as_tensor(x).reshape(-1, 5) for _, x in records])
+
+
+def mesh_piece(volume, records):
+    """The mesh of the cubes rooted in `volume`'s blocks, given the halo records the other shards sent it: a
+    TriangleMesh with edge_ids; seam vertices may repeat across pieces (`weld` merges them)."""
+    h, x = _concat_records(records)
+    return volume.extract_mesh_with_halo(h, x)
+
+
+def point_piece(volume, records):
+    """The zero crossings rooted in `volume`'s blocks: a PointCloud with edge_ids; pieces of different shards are
+    disjoint."""
+    h, x = _concat_records(records)
+    return volume.extract_point_cloud_with_halo(h, x)
+
+
+def weld(pieces, device: int = 0):
+    """One mesh from the mesh pieces of every shard, in rank order: the first vertex of each edge id is kept, in order
+    of first occurrence, and the triangles (rank-major) are re-indexed (b2v_weld_mesh_device, on `device`)."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    from .volume import TriangleMesh
+    L = _lib.load()
+    pieces = list(pieces)
+    dev = torch.device("cuda", device)
+    nv = (C.c_int64 * len(pieces))(*[len(p.vertices) for p in pieces])
+    nt = (C.c_int64 * len(pieces))(*[len(p.triangles) for p in pieces])
+
+    def cat(name, dtype, width):
+        arrs = [np.asarray(getattr(p, name), dtype).reshape(-1, width) for p in pieces]
+        return torch.from_numpy(np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros((0, width), dtype))).to(dev)
+
+    V, Cc = cat("vertices", np.float64, 3), cat("vertex_colors", np.float64, 3)
+    E, T = cat("edge_ids", np.int32, 4), cat("triangles", np.int32, 3)
+    oV, oC, oE, oT = torch.empty_like(V), torch.empty_like(Cc), torch.empty_like(E), torch.empty_like(T)
+    torch.cuda.current_stream(dev).synchronize()
+    n = C.c_int64(0)
+    rc = L.b2v_weld_mesh_device(device, len(pieces), nv, nt, V.data_ptr(), Cc.data_ptr(), E.data_ptr(), T.data_ptr(),
+                                oV.data_ptr(), oC.data_ptr(), oE.data_ptr(), oT.data_ptr(), C.byref(n))
+    if rc != _lib.B2V_OK:
+        raise RuntimeError(f"b2v_weld_mesh_device failed (status {rc}): {L.b2v_weld_last_error().decode()}")
+    k = n.value
+    return TriangleMesh(oV[:k].cpu().numpy(), oT.cpu().numpy(), oC[:k].cpu().numpy(), oE[:k].cpu().numpy())
+
+
+def _exchange_halo(volume, group):
+    """All-to-all of the halo records: -> (headers, payload) this rank received (on the volume's GPU), and the halo
+    bytes each rank sent."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    rank = dist.get_rank(group)
+    on_device = dist.get_backend(group) == "nccl"
+    headers, payload, nrec, nvox = volume.export_halo_torch(world)
+    dev = headers.device if on_device else torch.device("cpu")
+    headers, payload = headers.to(dev), payload.to(dev)
+    mine = torch.tensor([nrec, nvox], dtype=torch.int64, device=dev)
+    sizes = [torch.zeros_like(mine) for _ in range(world)]
+    dist.all_gather(sizes, mine, group=group)
+    sizes = [s.cpu() for s in sizes]
+    in_rec = [int(sizes[s][0, rank]) for s in range(world)]
+    in_vox = [int(sizes[s][1, rank]) for s in range(world)]
+    rh = torch.empty((sum(in_rec), 4), dtype=torch.int32, device=dev)
+    rx = torch.empty((sum(in_vox), payload.shape[1]), dtype=torch.float32, device=dev)
+    dist.all_to_all_single(rh, headers, output_split_sizes=in_rec, input_split_sizes=nrec, group=group)
+    dist.all_to_all_single(rx, payload, output_split_sizes=in_vox, input_split_sizes=nvox, group=group)
+    sent = [int(sizes[s][0].sum()) * 16 + int(sizes[s][1].sum()) * 20 for s in range(world)]
+    return rh, rx, sent
+
+
+def _gather_rows(arr, dst, group, on_device, device):
+    """Variable-length row arrays of every rank, on dst (list in rank order), None elsewhere."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    dev = torch.device("cuda", device) if on_device else torch.device("cpu")
+    t = torch.from_numpy(np.ascontiguousarray(arr)).to(dev)
+    n = torch.tensor([t.shape[0]], dtype=torch.int64, device=dev)
+    sizes = [torch.zeros_like(n) for _ in range(world)]
+    dist.all_gather(sizes, n, group=group)
+    sizes = [int(s.item()) for s in sizes]
+    pad = torch.zeros((max(max(sizes), 1),) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+    pad[:t.shape[0]] = t
+    bufs = [torch.zeros_like(pad) for _ in range(world)] if dist.get_rank(group) == dst else None
+    dist.gather(pad, bufs, dst=dst, group=group)
+    if bufs is None:
+        return None
+    return [bufs[r][:sizes[r]].cpu().numpy() for r in range(world)]
+
+
+def _sharded(volume, dst, group, gather, points):
+    import torch.distributed as dist
+    from .volume import PointCloud, TriangleMesh
+    rh, rx, sent = _exchange_halo(volume, group)
+    volume.last_halo_bytes = sent
+    piece = point_piece(volume, (rh, rx)) if points else mesh_piece(volume, (rh, rx))
+    if not gather:
+        return piece
+    on_device = dist.get_backend(group) == "nccl"
+    names = (("points", "colors", "edge_ids") if points else ("vertices", "vertex_colors", "edge_ids", "triangles"))
+    parts = {k: _gather_rows(getattr(piece, k), dst, group, on_device, volume.device) for k in names}
+    if dist.get_rank(group) != dst:
+        return None
+    if points:
+        return PointCloud(*(np.concatenate(parts[k]) for k in names))
+    ranks = range(len(parts["edge_ids"]))
+    return weld([TriangleMesh(parts["vertices"][r], parts["triangles"][r], parts["vertex_colors"][r],
+                              parts["edge_ids"][r]) for r in ranks], device=volume.device)
+
+
+def extract_mesh_sharded(volume, dst: int = 0, group=None, gather: bool = True):
+    """Mesh of a hash-sharded volume with each rank meshing its own blocks: one all-gather of the per-destination
+    sizes, one all_to_all of halo headers and one of halo voxels (GPU to GPU with NCCL, host tensors with any other
+    backend), the mesh piece of the rank's blocks on its GPU, then the pieces gathered to `dst` and welded there.
+    Returns the welded TriangleMesh (with edge_ids) on dst and None elsewhere; `gather=False` returns every rank's own
+    piece instead.  `volume.last_halo_bytes` lists the halo bytes each rank sent."""
+    return _sharded(volume, dst, group, gather, points=False)
+
+
+def extract_point_cloud_sharded(volume, dst: int = 0, group=None, gather: bool = True):
+    """Point cloud of a hash-sharded volume, like `extract_mesh_sharded`: each rank extracts the zero crossings rooted
+    in its own blocks; the disjoint pieces are concatenated in rank order on `dst` (a PointCloud with edge_ids)."""
+    return _sharded(volume, dst, group, gather, points=True)

@@ -61,9 +61,10 @@ class TriangleMesh:
 class PointCloud:
     """Arrays shaped like `VolumetricIntegrationPointCloud` (volumetric_integrator_base.py:159-210)."""
 
-    def __init__(self, points, colors):
+    def __init__(self, points, colors, edge_ids=None):
         self.points = points
         self.colors = colors
+        self.edge_ids = edge_ids                 # [N,4] int32 voxel (x,y,z) + axis of each zero crossing, if known
 
 
 class B200TsdfVolume:
@@ -373,6 +374,60 @@ class B200TsdfVolume:
         return TriangleMesh(V, T, Cc, E)
 
     extract_triangle_mesh = extract_mesh
+
+    # ---- sharded extraction: face-halo exchange (pyslam_b200.sharding.extract_mesh_sharded) ----
+    def export_halo_torch(self, world: int):
+        """Halo records this shard sends the other ranks of a `world`-rank sharding (b2v_export_halo_device):
+        (headers int32 [R,4] = {x,y,z,mask}, payload float32 [P,5] = {tsdf, weight, r, g, b}, records per destination
+        rank, payload voxels per destination rank), CUDA tensors grouped by destination rank.  Only reads the volume."""
+        import torch
+        world = int(world)
+        rec, pay = (C.c_int64 * world)(), (C.c_int64 * world)()
+        self._check(self._L.b2v_export_halo_device(self._h, world, rec, pay, None, None, 0, 0), "b2v_export_halo_device")
+        nrec, nvox = [int(x) for x in rec], [int(x) for x in pay]
+        dev = torch.device("cuda", self.device)
+        headers = torch.empty((sum(nrec), 4), dtype=torch.int32, device=dev)
+        payload = torch.empty((sum(nvox), VOXEL_PLANES), dtype=torch.float32, device=dev)
+        if headers.shape[0]:
+            self._check(self._L.b2v_export_halo_device(self._h, world, rec, pay, headers.data_ptr(), payload.data_ptr(),
+                                                       headers.shape[0], payload.shape[0]), "b2v_export_halo_device")
+        return headers, payload, nrec, nvox
+
+    def _halo_args(self, headers, payload):
+        import torch
+        dev = torch.device("cuda", self.device)
+        h = torch.as_tensor(headers, dtype=torch.int32).to(dev).contiguous().reshape(-1, 4)
+        x = torch.as_tensor(payload, dtype=torch.float32).to(dev).contiguous().reshape(-1, VOXEL_PLANES)
+        torch.cuda.current_stream(dev).synchronize()
+        return h, x
+
+    def extract_mesh_with_halo(self, headers, payload) -> TriangleMesh:
+        """The mesh piece rooted in this shard's blocks, given the halo records the other ranks sent it
+        (b2v_extract_mesh_with_halo).  Seam vertices may repeat in other ranks' pieces; `sharding.weld` merges them."""
+        h, x = self._halo_args(headers, payload)
+        nv, nt = C.c_int64(0), C.c_int64(0)
+        self._check(self._L.b2v_extract_mesh_with_halo(self._h, h.shape[0], h.data_ptr(), x.data_ptr(), C.byref(nv),
+                                                       C.byref(nt)), "b2v_extract_mesh_with_halo")
+        return self._copy_mesh(nv.value, nt.value)
+
+    def extract_point_cloud_with_halo(self, headers, payload) -> PointCloud:
+        """The zero crossings rooted in this shard's blocks (b2v_extract_points_with_halo): the ranks' pieces are
+        disjoint and together make the unsharded volume's point cloud."""
+        h, x = self._halo_args(headers, payload)
+        n = C.c_int64(0)
+        self._check(self._L.b2v_extract_points_with_halo(self._h, h.shape[0], h.data_ptr(), x.data_ptr(), C.byref(n)),
+                    "b2v_extract_points_with_halo")
+        m = self._copy_mesh(n.value, 0)
+        return PointCloud(m.vertices, m.vertex_colors, m.edge_ids)
+
+    def _copy_mesh(self, nv: int, nt: int) -> TriangleMesh:
+        V = np.zeros((nv, 3), np.float64)
+        Cc = np.zeros((nv, 3), np.float64)
+        E = np.zeros((nv, 4), np.int32)
+        T = np.zeros((nt, 3), np.int32)
+        self._check(self._L.b2v_copy_mesh(self._h, V.ctypes.data, Cc.ctypes.data, E.ctypes.data, T.ctypes.data),
+                    "b2v_copy_mesh")
+        return TriangleMesh(V, T, Cc, E)
 
     def extract_point_cloud(self) -> PointCloud:
         n = C.c_int64(0)
