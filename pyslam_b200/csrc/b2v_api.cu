@@ -139,6 +139,7 @@ struct b2v_volume {
     size_t stage_pixels = 0;
     HashTable table{};
     PoolMeta meta{};
+    UnitSet units{};                     // group unit sets of the fused allocation, one per group buffer
     // The pool is one virtual-address reservation for meta.capacity blocks; physical chunks are mapped as it grows
     // (fixed volumes map it whole at create), so the pool address the kernels see never changes.
     bool growable = false;               // max_capacity_blocks > capacity_blocks
@@ -316,6 +317,8 @@ static int volume_clear_device(b2v_volume *v) {
     B2V_CUDA(v, cudaMemsetAsync(v->table.entries, 0xFF, tcap * sizeof(uint4), v->compute));
     B2V_CUDA(v, cudaMemsetAsync(v->meta.group_mask, 0, tcap * kGroupBufs * sizeof(uint32_t), v->compute));
     B2V_CUDA(v, cudaMemsetAsync(v->meta.counters, 0, kNumCounters * sizeof(uint32_t), v->compute));
+    B2V_CUDA(v, cudaMemsetAsync(v->units.entries, 0, (static_cast<size_t>(v->units.mask) + 1) * kGroupBufs * sizeof(uint4),
+                                v->compute));
     return B2V_OK;
 }
 
@@ -412,6 +415,20 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     B2V_CUDA(v, cudaMalloc(&v->meta.group_mask, static_cast<size_t>(tcap) * kGroupBufs * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.union_slots, static_cast<size_t>(cap) * kGroupBufs * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMalloc(&v->meta.block_flags, static_cast<size_t>(cap) * sizeof(uint32_t)));
+    {
+        // Group unit sets: 2^16 entries (1 MB) per group buffer, L2-resident.  The largest union of 32-frame groups
+        // on the bench configs is ~2.6 k 16^3 units on C2 (~21 k under decision D1's 8^3 units); units that find no
+        // entry take the direct path, exactly.  B2V_GROUP_UNIT_SET (a power of two) overrides the size, for tuning
+        // and for tests of that path.
+        uint32_t entries = 1u << 16;
+        if (const char *e = std::getenv("B2V_GROUP_UNIT_SET")) {
+            const long n = std::atol(e);
+            if (n >= 1 && n <= (1l << 24) && (n & (n - 1)) == 0) entries = static_cast<uint32_t>(n);
+        }
+        v->units.mask = entries - 1;
+        B2V_CUDA(v, cudaMalloc(&v->units.entries, static_cast<size_t>(entries) * kGroupBufs * sizeof(uint4)));
+        B2V_CUDA(v, cudaMalloc(&v->units.list, static_cast<size_t>(entries) * kGroupBufs * sizeof(uint32_t)));
+    }
     B2V_CUDA(v, cudaMemsetAsync(v->meta.block_flags, 0, static_cast<size_t>(cap) * sizeof(uint32_t), v->compute));
     B2V_CUDA(v, cudaMallocHost(&v->h_counters, kNumCounters * sizeof(uint32_t)));
     B2V_CUDA(v, cudaMallocHost(&v->h_totals, kNumMeshTotals * sizeof(uint32_t)));
@@ -455,6 +472,8 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaFree(v->meta.group_mask);
     cudaFree(v->meta.union_slots);
     cudaFree(v->meta.block_flags);
+    cudaFree(v->units.entries);
+    cudaFree(v->units.list);
     cudaFree(v->table.entries);
     pool_release(v);
     cudaFreeHost(v->h_skip);
@@ -883,11 +902,12 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             v->prof_int_launches += 1;
             B2V_CUDA(v, cudaEventRecord(pe[0], as));
         }
-        B2V_CUDA(v, fused ? launch_allocate_group(aargs, v->table, v->meta, as)
+        aargs.units = v->units;
+        B2V_CUDA(v, fused ? launch_allocate_group(aargs, v->table, v->meta, v->sm_count, as)
                           : launch_allocate(aargs, v->table, v->meta, as));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
-        v->launches += 1;
+        v->launches += fused ? 2 : 1;  // (+ the expand kernel of a fused group)
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
         if (v->growable && v->meta.pool_capacity < v->meta.capacity) {
             // in group order on one stream, each after its own allocation: the first group skipped is the first that

@@ -136,6 +136,8 @@ enum Counter : int {
     kCtrSavedUnion0 = 5,     // [kGroupBufs] kGcUnion of the skipped group of each buffer (restored for the replay)
     kCtrVisitsLo = 12,       // 64-bit total of block visits (one block read + written) since reset
     kCtrVisitsHi = 13,
+    kCtrUnitSetFull = 14,    // (unit, frame) pairs of fused groups that found no entry in the group unit set within
+                             // its probe limit and touched their blocks directly, since reset
     kCtrGroup0 = 16,         // [kGroupBufs][kGroupCtrStride] per-group-buffer counters, contiguous so that ONE
                              // memset re-arms a buffer: see GroupCounter
     kNumCounters = 16 + 4 * (4 + 32)
@@ -145,6 +147,7 @@ enum GroupCounter : int {
     kGcUnion = 0,    // number of slots in the group's union list
     kGcNext = 1,     // work-stealing cursor of the fused kernel
     kGcNew = 2,      // blocks newly allocated by the group
+    kGcUnits = 3,    // entries of the group unit set (fused groups)
     kGcTouched0 = 4  // [kMaxGroup] blocks touched by frame k of the group
 };
 constexpr int kGroupCtrStride = 4 + kMaxGroup;
@@ -178,6 +181,14 @@ struct FrameMaps {
 bool tma_tiles_usable(int W, int stride, const void *depth, const void *color);
 // returns false if the driver entry point is unavailable or encoding fails
 bool encode_frame_maps(FrameMaps *maps, const float *depth, const uint8_t *color, int H, int W, int tile);
+// The allocation units a fused group touches and, per unit, the frames that touch it: one set per group buffer, filled
+// by allocate_group_kernel (per frame and tile) and read and cleared by allocate_group_expand_kernel (per group).
+// Entry {ux, uy, uz, frame mask}; mask 0 = empty.  Sized for the largest union with slack (b2v_api.cu).
+struct UnitSet {
+    uint4 *entries;   // [kGroupBufs][mask + 1]
+    uint32_t *list;   // [kGroupBufs][mask + 1] entry positions of the group's units, in insertion order
+    uint32_t mask;    // entries per buffer - 1 (a power of two)
+};
 // Frame packing (texels) + allocation + touched set of the frames of a group, recorded in group buffer
 // P.group_buf.  use_tma: the image tiles are staged into shared memory with TMA (cp.async.bulk.tensor.2d); else
 // plain loads.
@@ -188,15 +199,17 @@ struct GroupAllocArgs {
     const uint8_t *color[kMaxGroup];
     Texel *tex[kMaxGroup];
     FrameMaps maps[kMaxGroup];
+    UnitSet units;                 // fused groups
     int32_t count, use_tma;
 };
 static_assert(sizeof(GroupAllocArgs) < 32000, "kernel parameter space");
 // a one-frame group (frame 0 of args), with the frame-by-frame allocate_kernel
 cudaError_t launch_allocate(const GroupAllocArgs &args, const HashTable &table, const PoolMeta &meta,
                             cudaStream_t stream);
-// all frames of a group in ONE launch (blockIdx.z = frame): the per-frame latency chains overlap
+// all frames of a group in ONE launch (blockIdx.z = frame): the per-frame latency chains overlap.  It collects the
+// group's units in args.units; a second kernel then touches each block of those units once for the whole group.
 cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &table,
-                                  const PoolMeta &meta, cudaStream_t stream);
+                                  const PoolMeta &meta, int sm_count, cudaStream_t stream);
 // projective TSDF + colour update of every block touched by the one-frame group in group buffer group_buf
 cudaError_t launch_integrate(const IntFrame &f, const VolumeConsts &vc, const HashTable &table,
                              const PoolMeta &meta, int group_buf, int grid_ctas, cudaStream_t stream);
