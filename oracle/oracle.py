@@ -626,7 +626,7 @@ class numpy_grid:
 
     @staticmethod
     def frustum_bounds(K, W, H, Tcw, depth_max, depth_min):
-        """fill_frustum_query: the world AABB [6] of the 8 frustum corners, float64, in the kernel's order."""
+        """BlockGridCore::frustum_query: the world AABB [6] of the 8 frustum corners, float64, in the kernel's order."""
         fx, fy, cx, cy = [np.float64(np.float32(v)) for v in K]
         T = np.asarray(Tcw, np.float64).reshape(4, 4)
         R, t = T[:3, :3], T[:3, 3]

@@ -16,7 +16,7 @@ CSRC = os.path.join(_DIR, "csrc")
 LIB = os.path.join(_DIR, "libb2v.so")
 SOURCES = ["b2v_api.cu", "b2v_tsdf.cu", "b2v_mesh.cu", "b2v_grid.cu", "b2v_prep.cu", "b2v_semantic.cu",
            "b2v_shard.cu"]
-HEADERS = ["b2v_device.cuh", "b2v_internal.h", "b2v_scan.cuh", "mc_tables.h", "../../include/b2v.h"]
+HEADERS = ["b2v_block_grid.cuh", "b2v_device.cuh", "b2v_internal.h", "b2v_scan.cuh", "mc_tables.h", "../../include/b2v.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -147,4 +147,17 @@ static __device__ __forceinline__ uint32_t block_excl_scan_512(uint32_t v, uint3
     return x - v + (wid ? s_warp[wid - 1] : 0u);
 }
 
+// the number of threads of a 512-thread CTA with `keep` set, stored by thread 0 to *out; s_warp: 16 words
+static __device__ __forceinline__ void block_count_512(bool keep, uint32_t *s_warp, uint32_t *out) {
+    const int t = threadIdx.x;
+    const uint32_t x = __reduce_add_sync(0xffffffffu, keep ? 1u : 0u);
+    if ((t & 31) == 0) s_warp[t >> 5] = x;
+    __syncthreads();
+    if (t == 0) {
+        uint32_t s = 0;
+        for (int k = 0; k < 16; ++k) s += s_warp[k];
+        *out = s;
+    }
+}
+
 }  // namespace b2v
