@@ -44,8 +44,22 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_remove_low_count_voxels", "b2v_sgrid_remove_low_confidence_segments", "b2v_sgrid_merge_segments",
     "b2v_sgrid_remove_segment", "b2v_sgrid_label_overflows", "b2v_sgrid_dump_blocks", "b2v_sgrid_carve",
     "b2v_sgrid_assign_object_ids_to_instance_ids", "b2v_sgrid_copy_instance_map", "b2v_sgrid_set_next_object_id",
-    "b2v_sgrid_get_next_object_id",
+    "b2v_sgrid_get_next_object_id", "b2v_grid_set_rectification", "b2v_grid_set_frame", "b2v_sgrid_set_rectification",
+    "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids",
 ]
+
+
+class B2VFrame(C.Structure):
+    """`b2v_frame`: the staged images of one frame (device pointers)."""
+    _fields_ = [
+        ("depth", C.c_void_p),
+        ("filtered_depth", C.c_void_p),
+        ("color", C.c_void_p),
+        ("class_image", C.c_void_p),
+        ("instance_image", C.c_void_p),
+        ("height", C.c_int32),
+        ("width", C.c_int32),
+    ]
 
 
 class B2VConfig(C.Structure):
@@ -244,5 +258,15 @@ def load() -> C.CDLL:
     L.b2v_grid_get_voxels_in_bb.argtypes = [vp, vp, i32]
     L.b2v_grid_dump_blocks.restype = i64
     L.b2v_grid_dump_blocks.argtypes = [vp, vp, vp, vp, vp, vp]
+    for prefix in ("b2v_grid", "b2v_sgrid"):
+        fn = getattr(L, prefix + "_set_rectification")
+        fn.restype = C.c_int
+        fn.argtypes = [vp, vp, vp, i32, i32, i32]
+    L.b2v_grid_set_frame.restype = C.c_int
+    L.b2v_grid_set_frame.argtypes = [vp, vp, i32, C.c_float, vp, i32, i32, i32, C.POINTER(B2VFrame)]
+    L.b2v_sgrid_set_frame.restype = C.c_int
+    L.b2v_sgrid_set_frame.argtypes = [vp, vp, i32, C.c_float, vp, vp, vp, i32, i32, i32, C.POINTER(B2VFrame)]
+    L.b2v_sgrid_remap_instance_ids.restype = C.c_int
+    L.b2v_sgrid_remap_instance_ids.argtypes = [vp, C.POINTER(vp)]
     _lib = L
     return L

@@ -318,6 +318,7 @@ void BlockGridCore::destroy() {
     if (stream) cudaStreamSynchronize(stream);
     void *ptrs[] = {table.entries, index.block_keys, index.counters, d_sums, d_offs, d_total};
     for (void *p : ptrs) cudaFree(p);
+    free_frame();
     cudaFreeHost(h_counters);
     if (stream) cudaStreamDestroy(stream);
 }
@@ -447,6 +448,134 @@ cudaError_t BlockGridCore::device_input(const void *src, size_t bytes, void **tm
     if (e == cudaSuccess) e = cudaMemcpyAsync(*tmp, src, bytes, cudaMemcpyHostToDevice, stream);
     *out = *tmp;
     return e;
+}
+
+void BlockGridCore::free_frame() {
+    void *ptrs[] = {frame.mapx, frame.mapy, frame.raw, frame.depth, frame.filtered, frame.rgb, frame.shadow_scratch,
+                    frame.cls, frame.inst, frame.obj};
+    for (void *p : ptrs) cudaFree(p);
+    frame = FrameStage{};
+}
+
+int BlockGridCore::set_rectification(const float *map_x, const float *map_y, int H, int W, int swap_rb) {
+    if (map_x && map_y && (H <= 0 || W <= 0)) {
+        err = "set_rectification: bad image size";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(this, cudaSetDevice(device));
+    B2V_CUDA(this, cudaStreamSynchronize(stream));
+    cudaFree(frame.mapx);
+    cudaFree(frame.mapy);
+    frame.mapx = frame.mapy = nullptr;
+    frame.map_h = frame.map_w = 0;
+    frame.swap_rb = swap_rb;
+    if (!map_x || !map_y) return B2V_OK;
+    const size_t bytes = static_cast<size_t>(H) * W * sizeof(float);
+    B2V_CUDA(this, cudaMalloc(&frame.mapx, bytes));
+    B2V_CUDA(this, cudaMalloc(&frame.mapy, bytes));
+    B2V_CUDA(this, cudaMemcpy(frame.mapx, map_x, bytes, cudaMemcpyDefault));
+    B2V_CUDA(this, cudaMemcpy(frame.mapy, map_y, bytes, cudaMemcpyDefault));
+    frame.map_h = H;
+    frame.map_w = W;
+    return B2V_OK;
+}
+
+int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scale, const uint8_t *color,
+                             const int32_t *cls, const int32_t *inst, int H, int W, bool filter_shadow_points,
+                             b2v_frame *out) {
+    const char *bad = nullptr;
+    if (!depth || !color || !out || H <= 0 || W <= 0) bad = "set_frame: bad arguments";
+    else if (depth_u16 && !(depth_scale > 0.0f)) bad = "set_frame: uint16 depth needs a positive depth_scale";
+    else if (inst && !cls) bad = "set_frame: an instance image needs a class image";
+    else if (frame.mapx && (H != frame.map_h || W != frame.map_w))
+        bad = "set_frame: rectification maps were installed for a different image size";
+    else if (filter_shadow_points && (H <= 2 || W <= 2)) bad = "set_frame: image too small for the shadow filter";
+    if (bad) {
+        err = bad;
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(this, cudaSetDevice(device));
+    frame.staged = b2v_frame{};
+    const size_t pixels = static_cast<size_t>(H) * W;
+    if (pixels > frame.pixels) {
+        B2V_CUDA(this, cudaStreamSynchronize(stream));
+        void **bufs[] = {&frame.raw, reinterpret_cast<void **>(&frame.depth), reinterpret_cast<void **>(&frame.filtered),
+                         reinterpret_cast<void **>(&frame.rgb), &frame.shadow_scratch};
+        for (void **b : bufs) {
+            cudaFree(*b);
+            *b = nullptr;
+        }
+        frame.pixels = 0;   // stays 0 if an allocation below fails
+        B2V_CUDA(this, cudaMalloc(&frame.raw, pixels * sizeof(float)));
+        B2V_CUDA(this, cudaMalloc(&frame.depth, pixels * sizeof(float)));
+        B2V_CUDA(this, cudaMalloc(&frame.filtered, pixels * sizeof(float)));
+        B2V_CUDA(this, cudaMalloc(&frame.rgb, pixels * 3));
+        B2V_CUDA(this, cudaMalloc(&frame.shadow_scratch, kShadowScratchBytes));
+        frame.pixels = pixels;
+    }
+    if (cls && pixels > frame.label_pixels) {
+        B2V_CUDA(this, cudaStreamSynchronize(stream));
+        int32_t **bufs[] = {&frame.cls, &frame.inst, &frame.obj};
+        for (int32_t **b : bufs) {
+            cudaFree(*b);
+            *b = nullptr;
+        }
+        frame.label_pixels = 0;
+        for (int32_t **b : bufs) B2V_CUDA(this, cudaMalloc(b, pixels * sizeof(int32_t)));
+        frame.label_pixels = pixels;
+    }
+    cudaStream_t s = stream;
+    const bool rect = frame.mapx != nullptr;
+    cudaError_t e = cudaSuccess;
+    // a host image is uploaded into `dst`, a device image is read in place.  Uploads through frame.raw are ordered
+    // after the kernels that read the previous one (one stream).
+    auto input = [&](const void *src, size_t bytes, void *dst) -> const void * {
+        if (e != cudaSuccess || is_device_pointer(src)) return src;
+        e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s);
+        return dst;
+    };
+    // 32-bit image (depth, labels) into its staged buffer: nearest remap, or a copy without maps
+    auto place_b32 = [&](const void *src, void *dst) {
+        if (e != cudaSuccess) return;
+        if (rect)
+            e = launch_remap_b32_nearest(src, H, W, frame.mapx, frame.mapy, dst, s);
+        else if (src != dst)
+            e = cudaMemcpyAsync(dst, src, pixels * 4, cudaMemcpyDeviceToDevice, s);
+    };
+    // depth: upload -> widen (uint16; into `filtered`, free until the filter runs, when the remap follows) -> remap
+    const void *d = input(depth, pixels * (depth_u16 ? 2 : 4), (depth_u16 || rect) ? frame.raw : frame.depth);
+    if (depth_u16 && e == cudaSuccess) {
+        float *wide = rect ? frame.filtered : frame.depth;
+        e = launch_depth_u16_to_f32(static_cast<const uint16_t *>(d), wide, pixels, depth_scale, s);
+        d = wide;
+    }
+    place_b32(d, frame.depth);
+    const void *c = input(color, pixels * 3, rect ? frame.raw : frame.rgb);
+    if (e == cudaSuccess) {
+        if (rect)
+            e = launch_remap_u8c3_linear(static_cast<const uint8_t *>(c), H, W, frame.mapx, frame.mapy, frame.rgb,
+                                         frame.swap_rb, s);
+        else if (c != frame.rgb)
+            e = cudaMemcpyAsync(frame.rgb, c, pixels * 3, cudaMemcpyDeviceToDevice, s);
+    }
+    if (cls) place_b32(input(cls, pixels * 4, rect ? frame.raw : frame.cls), frame.cls);
+    if (inst) place_b32(input(inst, pixels * 4, rect ? frame.raw : frame.inst), frame.inst);
+    if (e == cudaSuccess && filter_shadow_points)
+        e = launch_filter_shadow_points(frame.depth, H, W, 2, 2, -1.0f, frame.filtered, frame.shadow_scratch, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        err = std::string("set_frame: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    frame.staged.depth = frame.depth;
+    frame.staged.filtered_depth = filter_shadow_points ? frame.filtered : frame.depth;
+    frame.staged.color = frame.rgb;
+    frame.staged.class_image = cls ? frame.cls : nullptr;
+    frame.staged.instance_image = inst ? frame.inst : nullptr;
+    frame.staged.height = H;
+    frame.staged.width = W;
+    *out = frame.staged;
+    return B2V_OK;
 }
 
 }  // namespace b2v
@@ -675,6 +804,20 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         return B2V_ERR_CUDA;
     }
     return rc;
+}
+
+extern "C" int b2v_grid_set_rectification(b2v_grid *g, const float *map_x, const float *map_y, int32_t height,
+                                          int32_t width, int32_t swap_rb) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_rectification(map_x, map_y, height, width, swap_rb);
+}
+
+extern "C" int b2v_grid_set_frame(b2v_grid *g, const void *depth, int32_t depth_u16, float depth_scale,
+                                  const uint8_t *color, int32_t height, int32_t width, int32_t filter_shadow_points,
+                                  b2v_frame *out) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame(depth, depth_u16 != 0, depth_scale, color, nullptr, nullptr, height, width,
+                        filter_shadow_points != 0, out);
 }
 
 extern "C" int b2v_grid_synchronize(b2v_grid *g) {

@@ -425,6 +425,27 @@ struct BlockGridCore {
                             int min_count) const;
     // `src` in place if it is device memory, else a copy in a fresh device allocation *tmp (the caller frees it)
     cudaError_t device_input(const void *src, size_t bytes, void **tmp, const void **out);
+
+    // Per-frame preparation (b2v_grid_set_frame / b2v_sgrid_set_frame): the rectification maps and the staged images
+    // of the last frame, in buffers sized for the largest frame so far.
+    struct FrameStage {
+        float *mapx = nullptr, *mapy = nullptr;   // NULL: no rectification
+        int32_t map_h = 0, map_w = 0, swap_rb = 0;
+        void *raw = nullptr;                      // upload of one host image at a time (4 bytes per pixel)
+        float *depth = nullptr, *filtered = nullptr;
+        uint8_t *rgb = nullptr;
+        void *shadow_scratch = nullptr;
+        size_t pixels = 0;                        // capacity of the buffers above
+        int32_t *cls = nullptr, *inst = nullptr, *obj = nullptr;   // label images (semantic grids)
+        size_t label_pixels = 0;
+        b2v_frame staged{};                       // the last staged frame (all NULL: none)
+    } frame;
+    int set_rectification(const float *map_x, const float *map_y, int H, int W, int swap_rb);   // synchronises
+    // upload once -> widen uint16 depth -> rectify -> shadow filter; *out = frame.staged.  Synchronises.  Arguments
+    // are checked before anything is touched.
+    int set_frame(const void *depth, bool depth_u16, float depth_scale, const uint8_t *color, const int32_t *cls,
+                  const int32_t *inst, int H, int W, bool filter_shadow_points, b2v_frame *out);
+    void free_frame();
 };
 
 template <typename MapStorage, typename Replay> int BlockGridCore::resolve(MapStorage map_storage, Replay replay) {
@@ -458,5 +479,9 @@ cudaError_t launch_remap_u8c3_linear(const uint8_t *src, int H, int W, const flo
                                      uint8_t *dst, int swap_rb, cudaStream_t stream);
 cudaError_t launch_remap_b32_nearest(const void *src, int H, int W, const float *mapx, const float *mapy, void *dst,
                                      cudaStream_t stream);
+// remap_instance_ids (image_utils.h:69-163): dst[i] = map_obj[k] where map_inst[k] == src[i] (map_inst sorted
+// ascending), else -1; n_map == 0 gives -1 everywhere
+cudaError_t launch_remap_instance_ids(const int32_t *src, size_t n, const int32_t *map_inst, const int32_t *map_obj,
+                                      int n_map, int32_t *dst, cudaStream_t stream);
 
 }  // namespace b2v

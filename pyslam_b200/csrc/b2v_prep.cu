@@ -252,6 +252,35 @@ __global__ void depth_u16_to_f32_kernel(const uint16_t *__restrict__ src, float 
         dst[i] = __fmul_rn(static_cast<float>(src[i]), scale);
 }
 
+// instance id -> object id of the last association; one binary search over the sorted map per pixel
+__global__ void remap_instance_ids_kernel(const int32_t *__restrict__ src, const size_t n,
+                                          const int32_t *__restrict__ map_inst, const int32_t *__restrict__ map_obj,
+                                          const int n_map, int32_t *__restrict__ dst) {
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const int32_t id = src[i];
+        int32_t out = -1;
+        int lo = 0, hi = n_map - 1;
+        while (lo <= hi) {
+            const int mid = (lo + hi) >> 1;
+            const int32_t m = __ldg(map_inst + mid);
+            if (m == id) {
+                out = __ldg(map_obj + mid);
+                break;
+            }
+            if (m < id) lo = mid + 1; else hi = mid - 1;
+        }
+        dst[i] = out;
+    }
+}
+
+cudaError_t launch_remap_instance_ids(const int32_t *src, size_t n, const int32_t *map_inst, const int32_t *map_obj,
+                                      int n_map, int32_t *dst, cudaStream_t stream) {
+    if (n == 0) return cudaSuccess;
+    remap_instance_ids_kernel<<<1184, 256, 0, stream>>>(src, n, map_inst, map_obj, n_map, dst);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_depth_u16_to_f32(const uint16_t *src, float *dst, size_t n, float scale, cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
     depth_u16_to_f32_kernel<<<1184, 256, 0, stream>>>(src, dst, n, scale);

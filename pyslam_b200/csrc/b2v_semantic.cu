@@ -552,6 +552,9 @@ struct b2v_sgrid : BlockGridCore {
     size_t records_cap = 0;
     int32_t next_object_id = 1;  // VoxelSemanticSharedData::next_object_id (process-wide in the reference)
     std::vector<int32_t> map_inst, map_obj;
+    bool has_instance_map = false;   // the last association succeeded (map_inst / map_obj are its map)
+    int32_t *d_map = nullptr;        // map_inst then map_obj on the device, room for 2 * map_cap (remap_instance_ids)
+    size_t map_cap = 0;
     // read-out
     double *d_out_pts = nullptr;
     float *d_out_cols = nullptr, *d_out_conf = nullptr;
@@ -669,7 +672,7 @@ extern "C" int b2v_sgrid_destroy(b2v_sgrid *g) {
     void *ptrs[] = {g->d_pts, g->d_cols, g->d_cls, g->d_inst, g->d_depths, g->d_vid[0], g->d_vid[1], g->d_ord[0],
                     g->d_ord[1], g->d_sort_tmp, g->d_out_pts, g->d_out_cols, g->d_out_conf, g->d_out_cls,
                     g->d_out_obj, g->d_img_depth, g->d_img_filtered, g->d_img_rgb, g->d_valid, g->d_img_cls,
-                    g->d_img_obj, g->d_shadow_scratch, g->d_pend, g->d_records, g->d_n_records};
+                    g->d_img_obj, g->d_shadow_scratch, g->d_pend, g->d_records, g->d_n_records, g->d_map};
     for (void *p : ptrs) cudaFree(p);
     delete g;
     return B2V_OK;
@@ -842,11 +845,19 @@ extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const 
         g->img_pixels = pixels;
     }
     cudaStream_t s = g->stream;
-    B2V_CUDA(g, cudaMemcpyAsync(g->d_img_depth, depth, pixels * sizeof(float), cudaMemcpyDefault, s));
-    B2V_CUDA(g, cudaMemcpyAsync(g->d_img_rgb, color, pixels * 3, cudaMemcpyDefault, s));
-    if (class_image) B2V_CUDA(g, cudaMemcpyAsync(g->d_img_cls, class_image, pixels * sizeof(int32_t), cudaMemcpyDefault, s));
-    if (object_image) B2V_CUDA(g, cudaMemcpyAsync(g->d_img_obj, object_image, pixels * sizeof(int32_t), cudaMemcpyDefault, s));
-    const float *d_depth = g->d_img_depth;
+    // device images (such as the staged ones of b2v_sgrid_set_frame) are read in place, host images uploaded
+    auto input = [&](const void *src, void *buf, size_t bytes, const void **out) -> cudaError_t {
+        *out = src;
+        if (!src || is_device_pointer(src)) return cudaSuccess;
+        *out = buf;
+        return cudaMemcpyAsync(buf, src, bytes, cudaMemcpyHostToDevice, s);
+    };
+    const void *in_depth, *in_rgb, *in_cls, *in_obj;
+    B2V_CUDA(g, input(depth, g->d_img_depth, pixels * sizeof(float), &in_depth));
+    B2V_CUDA(g, input(color, g->d_img_rgb, pixels * 3, &in_rgb));
+    B2V_CUDA(g, input(class_image, g->d_img_cls, pixels * sizeof(int32_t), &in_cls));
+    B2V_CUDA(g, input(object_image, g->d_img_obj, pixels * sizeof(int32_t), &in_obj));
+    const float *d_depth = static_cast<const float *>(in_depth);
     if (filter_shadow_points) {  // semantic_grid.py:332-341: everything downstream sees the filtered depth
         if (height <= 2 || width <= 2) {
             g->err = "b2v_sgrid_integrate_rgbd: image too small for the shadow filter";
@@ -859,7 +870,8 @@ extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const 
     const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
     const int64_t n = static_cast<int64_t>(pixels);
     sem_rgbd_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(
-        P, d_depth, g->d_img_rgb, class_image ? g->d_img_cls : nullptr, object_image ? g->d_img_obj : nullptr,
+        P, d_depth, static_cast<const uint8_t *>(in_rgb), static_cast<const int32_t *>(in_cls),
+        static_cast<const int32_t *>(in_obj),
         static_cast<float *>(g->d_pts), static_cast<float *>(g->d_cols), g->d_cls, g->d_inst, g->d_depths, g->d_valid);
     B2V_CUDA(g, cudaGetLastError());
     SemInputs in{};
@@ -1127,6 +1139,7 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
     if (!g) return -1;
     g->map_inst.clear();
     g->map_obj.clear();
+    g->has_instance_map = false;
     if (!K || !Tcw || !class_image || !instance_image || width <= 0 || height <= 0) {
         g->err = "b2v_sgrid_assign_object_ids_to_instance_ids: bad arguments";
         return -1;
@@ -1238,7 +1251,49 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
         cudaFree(d_mo);
         if (e != cudaSuccess) return fail("apply", e);
     }
+    g->has_instance_map = true;
     return static_cast<int64_t>(g->map_inst.size());
+}
+
+extern "C" int b2v_sgrid_set_rectification(b2v_sgrid *g, const float *map_x, const float *map_y, int32_t height,
+                                           int32_t width, int32_t swap_rb) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_rectification(map_x, map_y, height, width, swap_rb);
+}
+
+extern "C" int b2v_sgrid_set_frame(b2v_sgrid *g, const void *depth, int32_t depth_u16, float depth_scale,
+                                   const uint8_t *color, const int32_t *class_image, const int32_t *instance_image,
+                                   int32_t height, int32_t width, int32_t filter_shadow_points, b2v_frame *out) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame(depth, depth_u16 != 0, depth_scale, color, class_image, instance_image, height, width,
+                        filter_shadow_points != 0, out);
+}
+
+extern "C" int b2v_sgrid_remap_instance_ids(b2v_sgrid *g, const int32_t **object_image) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    const b2v_frame &f = g->frame.staged;
+    if (!object_image || !f.instance_image || !g->has_instance_map) {
+        g->err = !g->has_instance_map ? "b2v_sgrid_remap_instance_ids: no instance map (run an association first)"
+                                      : "b2v_sgrid_remap_instance_ids: no staged instance image";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    const size_t m = g->map_inst.size();
+    if (m > g->map_cap) {
+        B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+        B2V_CUDA(g, regrow(&g->d_map, 2 * m));
+        g->map_cap = m;
+    }
+    cudaStream_t s = g->stream;
+    if (m) {
+        B2V_CUDA(g, cudaMemcpyAsync(g->d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        B2V_CUDA(g, cudaMemcpyAsync(g->d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    }
+    B2V_CUDA(g, launch_remap_instance_ids(f.instance_image, static_cast<size_t>(f.height) * f.width, g->d_map,
+                                          g->d_map + m, static_cast<int>(m), g->frame.obj, s));
+    B2V_CUDA(g, cudaStreamSynchronize(s));
+    *object_image = g->frame.obj;
+    return B2V_OK;
 }
 
 extern "C" int b2v_sgrid_copy_instance_map(b2v_sgrid *g, int32_t *instance_ids, int32_t *object_ids) {

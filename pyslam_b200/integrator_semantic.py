@@ -13,6 +13,10 @@ loop body (reference :326-461) maps one-to-one onto the C ABI:
 
     get_object_segments(min_count, min_confidence)                          ->  b2v_sgrid_get_voxels + grouping / PCA boxes
 
+With undistortion maps and no depth estimator (kVolumetricIntegrationB200GpuRectify), the base class's host preparation
+(cv2.remap, cvtColor, depth widening) and the host instance remap give way to b2v_sgrid_set_frame (raw images, each
+uploaded once, shadow filter once) and b2v_sgrid_remap_instance_ids; the calls above read the staged images.
+
 Outputs: when 2-D instance ids are integrated, the reference's OBJECTS representation (:523-587:
 `get_object_segments` -> `VolumetricIntegrationObjectList`, one entry per object with its points, colours, class id,
 confidence range and oriented box); otherwise its single-point-cloud representation (:590-700): points, colours,
@@ -59,6 +63,9 @@ DEFAULT_PARAMETERS = {
     "kVolumetricIntegrationB200MaxCapacityBlocks": 0,
     "kVolumetricIntegrationB200Device": 0,
     "kVolumetricIntegrationB200GenerateObjects": True,   # kGenerateObjectsDefault (reference :84)
+    # raw keyframe images to the grid (set_frame): upload once, undistort + BGR->RGB + depth widening + shadow filter
+    # on the GPU instead of the base class's cv2.remap / cvtColor (integrator.py has the same switch)
+    "kVolumetricIntegrationB200GpuRectify": True,
 }
 
 
@@ -106,6 +113,38 @@ def make_semantic_integrator_class(Base, api):
             self.last_output = None
             self.last_integrated_id = -1
             self.last_instance_map = {}
+            self._init_gpu_rectify()
+
+        def _init_gpu_rectify(self):
+            """Raw frames go to the grid when the base class computed undistortion maps (base.py:766-778) and no
+            depth estimator runs (estimated depth needs the host path), as in integrator.py."""
+            self._gpu_rectify = False
+            m1, m2 = getattr(self, "calib_map1", None), getattr(self, "calib_map2", None)
+            if (self.b200_parameters["kVolumetricIntegrationB200GpuRectify"] and m1 is not None and m2 is not None
+                    and getattr(self, "depth_estimator", None) is None):
+                self.volume.set_rectification(m1, m2, swap_rb=True)
+                self._gpu_rectify = True
+
+        def _raw_frame(self, kd):
+            """(depth, depth_scale) of a keyframe for `set_frame`, or None when it takes the host path.  The depth
+            conversion of base.py:1007-1015, as integrator.py::_prepare_frame does it: raw uint16 depth in C++-core
+            mode goes to the GPU with depth_scale = camera.depth_factor and is widened there to the value
+            `depth.astype(np.float32) * depth_factor` has on the host."""
+            if not self._gpu_rectify or kd.depth is None or not kd.depth.size or kd.img is None:
+                return None
+            if kd.depth.shape != (self.camera_frustrum.height, self.camera_frustrum.width):
+                return None   # the frustum's label / carve calls reject such frames: the host path handles them
+            depth, scale = kd.depth, None
+            if depth.dtype != np.float32:
+                if getattr(api, "USE_CPP", False):
+                    factor = float(getattr(self.camera, "depth_factor", 1.0))
+                    if depth.dtype == np.uint16:
+                        scale = np.float32(factor)
+                    else:
+                        depth = depth.astype(np.float32) * factor
+                else:
+                    depth = depth.astype(np.float32)
+            return depth, scale
 
         def _intrinsics(self):
             if hasattr(self, "get_camera_intrinsics_for_depth"):
@@ -113,8 +152,45 @@ def make_semantic_integrator_class(Base, api):
             c = self.camera
             return c.fx, c.fy, c.cx, c.cy
 
+        def _integrate_raw_keyframe(self, kd, depth, scale):
+            """The loop body on the raw images: one set_frame uploads, rectifies and shadow-filters them on the
+            device; association (or carving), the instance remap and the integration read the staged images."""
+            p = self.b200_parameters
+            flt = bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"])
+            classes, instances = kd.semantic_img, kd.semantic_instances_img
+            use_instances = (bool(p["kVolumetricSemanticIntegrationUseInstanceIds"]) and instances is not None
+                             and np.asarray(instances).size > 0 and classes is not None)
+            fr = self.volume.set_frame(depth, kd.img, class_image=classes,
+                                       instance_image=instances if use_instances else None, depth_scale=scale,
+                                       filter_shadow_points=flt)
+            self.integrated_instance_ids = False
+            self.camera_frustrum.set_T_cw(kd.pose)
+            carve_thr = float(p["kVolumetricIntegrationVoxelGridCarvingDepthThreshold"])
+            object_image = None
+            if use_instances:   # association and carving see the filtered depth (:349-362, :371-388)
+                self.last_instance_map = self.volume.assign_object_ids_to_instance_ids(
+                    self.camera_frustrum, fr.class_image, fr.instance_image, fr.filtered_depth,
+                    depth_threshold=carve_thr, do_carving=bool(p["kVolumetricIntegrationVoxelGridUseCarving"]),
+                    min_vote_ratio=float(p["kVolumetricSemanticIntegrationMinVoteRatio"]),
+                    min_votes=int(p["kVolumetricSemanticIntegrationMinVotes"]))
+                object_image = self.volume.remap_instance_ids()
+                self.integrated_instance_ids = True
+            elif p["kVolumetricIntegrationVoxelGridUseCarving"]:
+                self.volume.carve(self.camera_frustrum, fr.filtered_depth, carve_thr)
+            fx, fy, cx, cy = self._intrinsics()
+            Twc = np.linalg.inv(np.asarray(kd.pose, np.float64).reshape(4, 4))
+            self.volume.integrate_rgbd(
+                fr.filtered_depth, fr.color, (fx, fy, cx, cy), Twc, class_image=fr.class_image,
+                object_image=object_image, max_depth=self.volumetric_integration_depth_trunc,
+                use_depths=bool(p["kVolumetricSemanticProbabilisticIntegrationUseDepth"]), filter_shadow_points=False)
+            self.last_integrated_id = kd.id
+            return True
+
         def _integrate_keyframe(self, kd):
             """The reference loop body for one keyframe (:300-461)."""
+            raw = self._raw_frame(kd)
+            if raw is not None:
+                return self._integrate_raw_keyframe(kd, *raw)
             p = self.b200_parameters
             rect = self.estimate_depth_if_needed_and_rectify(kd)
             color, depth = rect[0], rect[1]
@@ -277,8 +353,28 @@ def make_voxel_grid_integrator_class(Base, api):
                 depth_min=p["kVolumetricIntegrationVoxelGridCarvingDepthMin"])
             self.last_output = None
             self.last_integrated_id = -1
+            self._init_gpu_rectify()
+
+        def _integrate_raw_keyframe(self, kd, depth, scale):
+            """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
+            p = self.b200_parameters
+            fr = self.volume.set_frame(depth, kd.img, depth_scale=scale,
+                                       filter_shadow_points=bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"]))
+            if p["kVolumetricIntegrationVoxelGridUseCarving"]:
+                self.camera_frustrum.set_T_cw(kd.pose)
+                self.volume.carve(self.camera_frustrum, fr.depth,
+                                  float(p["kVolumetricIntegrationVoxelGridCarvingDepthThreshold"]))
+            fx, fy, cx, cy = self._intrinsics()
+            Twc = np.linalg.inv(np.asarray(kd.pose, np.float64).reshape(4, 4))
+            self.volume.integrate_rgbd(fr.filtered_depth, fr.color, (fx, fy, cx, cy), Twc,
+                                       max_depth=self.volumetric_integration_depth_trunc, filter_shadow_points=False)
+            self.last_integrated_id = kd.id
+            return True
 
         def _integrate_keyframe(self, kd):
+            raw = self._raw_frame(kd)
+            if raw is not None:
+                return self._integrate_raw_keyframe(kd, *raw)
             p = self.b200_parameters
             rect = self.estimate_depth_if_needed_and_rectify(kd)
             color, depth = rect[0], rect[1]
@@ -313,8 +409,10 @@ def load_pyslam_semantic_plugin():
     from pyslam.config_parameters import Parameters
     from pyslam.dense import volumetric_integrator_base as B
     from pyslam.io.dataset_types import DatasetEnvironmentType
+    from pyslam.slam import USE_CPP   # C++ core: raw depth reaches the integrator unscaled (base.py:29, 1008-1012)
 
     api = SimpleNamespace(
+        USE_CPP=bool(USE_CPP),
         VolumetricIntegrationTaskType=B.VolumetricIntegrationTaskType,
         VolumetricIntegrationOutput=B.VolumetricIntegrationOutput,
         VolumetricIntegrationMesh=B.VolumetricIntegrationMesh,
