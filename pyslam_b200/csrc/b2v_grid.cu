@@ -441,20 +441,69 @@ GridQuery BlockGridCore::frustum_query(const float K[4], int W, int H, const dou
     return q;
 }
 
-cudaError_t BlockGridCore::device_input(const void *src, size_t bytes, void **tmp, const void **out) {
-    *out = src;
-    if (is_device_pointer(src)) return cudaSuccess;
-    cudaError_t e = cudaMalloc(tmp, bytes);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(*tmp, src, bytes, cudaMemcpyHostToDevice, stream);
-    *out = *tmp;
-    return e;
+int BlockGridCore::stage_input(const char *fn, int H, int W, bool filter_shadow_points, const float **depth,
+                               const uint8_t **rgb, const int32_t **cls, const int32_t **obj) {
+    if (filter_shadow_points && (H <= 2 || W <= 2)) {
+        err = std::string(fn) + ": image too small for the shadow filter";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(this, cudaSetDevice(device));
+    const size_t pixels = static_cast<size_t>(H) * W;
+    auto on_host = [](auto **p) { return p && *p && !is_device_pointer(*p); };
+    if ((filter_shadow_points || on_host(depth) || on_host(rgb)) && pixels > input.pixels) {
+        B2V_CUDA(this, cudaStreamSynchronize(stream));
+        void **bufs[] = {reinterpret_cast<void **>(&input.depth), reinterpret_cast<void **>(&input.filtered),
+                         reinterpret_cast<void **>(&input.rgb), &input.shadow_scratch};
+        for (void **b : bufs) {
+            cudaFree(*b);
+            *b = nullptr;
+        }
+        input.pixels = 0;   // stays 0 if an allocation below fails
+        B2V_CUDA(this, cudaMalloc(&input.depth, pixels * sizeof(float)));
+        B2V_CUDA(this, cudaMalloc(&input.filtered, pixels * sizeof(float)));
+        B2V_CUDA(this, cudaMalloc(&input.rgb, pixels * 3));
+        B2V_CUDA(this, cudaMalloc(&input.shadow_scratch, kShadowScratchBytes));
+        input.pixels = pixels;
+    }
+    if ((on_host(cls) || on_host(obj)) && pixels > input.label_pixels) {
+        B2V_CUDA(this, cudaStreamSynchronize(stream));
+        int32_t **bufs[] = {&input.cls, &input.obj};
+        for (int32_t **b : bufs) {
+            cudaFree(*b);
+            *b = nullptr;
+        }
+        input.label_pixels = 0;
+        for (int32_t **b : bufs) B2V_CUDA(this, cudaMalloc(b, pixels * sizeof(int32_t)));
+        input.label_pixels = pixels;
+    }
+    cudaError_t e = cudaSuccess;
+    auto upload = [&](auto **p, void *buf, size_t bytes) {
+        if (e != cudaSuccess || !on_host(p)) return;
+        e = cudaMemcpyAsync(buf, *p, bytes, cudaMemcpyHostToDevice, stream);
+        *p = static_cast<std::remove_reference_t<decltype(*p)>>(buf);
+    };
+    upload(depth, input.depth, pixels * sizeof(float));
+    upload(rgb, input.rgb, pixels * 3);
+    upload(cls, input.cls, pixels * sizeof(int32_t));
+    upload(obj, input.obj, pixels * sizeof(int32_t));
+    if (e == cudaSuccess && filter_shadow_points) {
+        e = launch_filter_shadow_points(*depth, H, W, 2, 2, -1.0f, input.filtered, input.shadow_scratch, stream);
+        *depth = input.filtered;
+    }
+    if (e != cudaSuccess) {
+        err = std::string(fn) + ": " + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    return B2V_OK;
 }
 
 void BlockGridCore::free_frame() {
     void *ptrs[] = {frame.mapx, frame.mapy, frame.raw, frame.depth, frame.filtered, frame.rgb, frame.shadow_scratch,
-                    frame.cls, frame.inst, frame.obj};
+                    frame.cls, frame.inst, frame.obj, input.depth, input.filtered, input.rgb, input.shadow_scratch,
+                    input.cls, input.obj};
     for (void *p : ptrs) cudaFree(p);
     frame = FrameStage{};
+    input = InputStage{};
 }
 
 int BlockGridCore::set_rectification(const float *map_x, const float *map_y, int H, int W, int swap_rb) {
@@ -755,55 +804,30 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         g->err = "b2v_grid_integrate_rgbd: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    B2V_CUDA(g, cudaSetDevice(g->device));
-    const size_t pixels = static_cast<size_t>(height) * width;
-    void *tmp_d = nullptr, *tmp_c = nullptr;
-    const void *in_d = nullptr, *in_c = nullptr;
-    cudaError_t e = g->device_input(depth, pixels * sizeof(float), &tmp_d, &in_d);
-    if (e == cudaSuccess) e = g->device_input(color, pixels * 3, &tmp_c, &in_c);
-    const float *d_depth = static_cast<const float *>(in_d);
-    const uint8_t *d_color = static_cast<const uint8_t *>(in_c);
-    float *filtered = nullptr;
-    void *scratch = nullptr;
-    if (e == cudaSuccess && filter_shadow_points) {  // voxel_grid.py:238-245: depth2pointcloud sees the filtered depth
-        e = cudaMalloc(&filtered, pixels * sizeof(float));
-        if (e == cudaSuccess) e = cudaMalloc(&scratch, kShadowScratchBytes);
-        if (e == cudaSuccess && (height <= 2 || width <= 2)) e = cudaErrorInvalidValue;
-        if (e == cudaSuccess) e = launch_filter_shadow_points(d_depth, height, width, 2, 2, -1.0f, filtered, scratch, g->stream);
-        d_depth = filtered;
-    }
-    int rc = B2V_OK;
-    if (e == cudaSuccess) {
-        const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
-        const unsigned grid = static_cast<unsigned>((pixels + 255) / 256);
-        grid_rgbd_insert_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, g->inv_voxel_size, g->table, g->index);
-        grid_rgbd_accumulate_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, d_color, g->inv_voxel_size, g->table,
-                                                                 g->meta(), 0u, g->index.pool_capacity);
-        e = cudaGetLastError();
-        // the replay reads the temporaries freed below
-        if (e == cudaSuccess && g->growable)
-            rc = g->resolve(
-                [&](uint64_t blocks) {
-                    std::string map_err;   // a failed mapping surfaces as "block pool full"
-                    grid_map_storage(g, blocks, &map_err);
-                },
-                [&](uint32_t lo, uint32_t hi) {
-                    grid_rgbd_accumulate_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, d_color, g->inv_voxel_size,
-                                                                             g->table, g->meta(), lo, hi);
-                    B2V_CUDA(g, cudaGetLastError());
-                    return B2V_OK;
-                });
-    }
-    if (e == cudaSuccess && (tmp_d || tmp_c || filtered)) e = cudaStreamSynchronize(g->stream);
-    cudaFree(tmp_d);
-    cudaFree(tmp_c);
-    cudaFree(filtered);
-    cudaFree(scratch);
-    if (e != cudaSuccess) {
-        g->err = std::string("b2v_grid_integrate_rgbd: ") + cudaGetErrorString(e);
-        return B2V_ERR_CUDA;
-    }
-    return rc;
+    const float *d_depth = depth;
+    const uint8_t *d_color = color;
+    // voxel_grid.py:238-245: depth2pointcloud sees the filtered depth
+    const int rc = g->stage_input("b2v_grid_integrate_rgbd", height, width, filter_shadow_points != 0, &d_depth,
+                                  &d_color);
+    if (rc != B2V_OK) return rc;
+    const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
+    const unsigned grid = static_cast<unsigned>((static_cast<size_t>(height) * width + 255) / 256);
+    grid_rgbd_insert_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, g->inv_voxel_size, g->table, g->index);
+    grid_rgbd_accumulate_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, d_color, g->inv_voxel_size, g->table,
+                                                             g->meta(), 0u, g->index.pool_capacity);
+    B2V_CUDA(g, cudaGetLastError());
+    if (!g->growable) return B2V_OK;
+    return g->resolve(
+        [&](uint64_t blocks) {
+            std::string map_err;   // a failed mapping surfaces as "block pool full"
+            grid_map_storage(g, blocks, &map_err);
+        },
+        [&](uint32_t lo, uint32_t hi) {
+            grid_rgbd_accumulate_kernel<<<grid, 256, 0, g->stream>>>(P, d_depth, d_color, g->inv_voxel_size,
+                                                                     g->table, g->meta(), lo, hi);
+            B2V_CUDA(g, cudaGetLastError());
+            return B2V_OK;
+        });
 }
 
 extern "C" int b2v_grid_set_rectification(b2v_grid *g, const float *map_x, const float *map_y, int32_t height,
@@ -898,24 +922,18 @@ extern "C" int b2v_grid_carve(b2v_grid *g, const float K[4], int32_t width, int3
         g->err = "b2v_grid_carve: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    const int rc = g->read_counters();
+    int rc = g->read_counters();
     if (rc == B2V_ERR_CUDA) return rc;
-    void *tmp = nullptr;
-    const void *d_depth = nullptr;
-    cudaError_t e = g->device_input(depth, static_cast<size_t>(width) * height * sizeof(float), &tmp, &d_depth);
     const uint32_t nb = g->block_count();
-    if (e == cudaSuccess && nb) {
-        grid_carve_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), g->frustum_query(K, width, height, Tcw, depth_max,
-                                                                                  depth_min, 1),
-                                                      static_cast<const float *>(d_depth), depth_threshold);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
-    cudaFree(tmp);
-    if (e != cudaSuccess) {
-        g->err = cudaGetErrorString(e);
-        return B2V_ERR_CUDA;
-    }
+    if (nb == 0) return B2V_OK;
+    const float *d_depth = depth;
+    rc = g->stage_input("b2v_grid_carve", height, width, false, &d_depth);
+    if (rc != B2V_OK) return rc;
+    grid_carve_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), g->frustum_query(K, width, height, Tcw, depth_max,
+                                                                              depth_min, 1),
+                                                  d_depth, depth_threshold);
+    B2V_CUDA(g, cudaGetLastError());
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
 }
 

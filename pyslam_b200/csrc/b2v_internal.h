@@ -423,8 +423,23 @@ struct BlockGridCore {
     // world AABB of the frustum corners (camera_frustrum.cpp:209-260) -> voxel key bounds (voxel_block_grid.hpp:1340-1345)
     GridQuery frustum_query(const float K[4], int W, int H, const double Tcw[16], float depth_max, float depth_min,
                             int min_count) const;
-    // `src` in place if it is device memory, else a copy in a fresh device allocation *tmp (the caller frees it)
-    cudaError_t device_input(const void *src, size_t bytes, void **tmp, const void **out);
+    // Per-call images of integrate_rgbd, carve and the association, in buffers sized for the largest call so far.
+    // Kept apart from `frame`, so a staged frame stays valid across calls made with host images.  A call's buffers
+    // are next written by a later call on the same stream, so the growth replay of the call may read them.
+    struct InputStage {
+        float *depth = nullptr, *filtered = nullptr;
+        uint8_t *rgb = nullptr;
+        void *shadow_scratch = nullptr;
+        size_t pixels = 0;                        // capacity of the buffers above
+        int32_t *cls = nullptr, *obj = nullptr;   // class and object (or instance) images (semantic grids)
+        size_t label_pixels = 0;
+    } input;
+    // The [H][W] images of one call on the device: each non-NULL pointer is read in place if it is device memory, else
+    // replaced by its upload into `input` on the stream.  filter_shadow_points: *depth is then replaced by its
+    // shadow-filtered copy in input.filtered.  Arguments are checked before anything is uploaded; `fn` names the call
+    // in err.
+    int stage_input(const char *fn, int H, int W, bool filter_shadow_points, const float **depth,
+                    const uint8_t **rgb = nullptr, const int32_t **cls = nullptr, const int32_t **obj = nullptr);
 
     // Per-frame preparation (b2v_grid_set_frame / b2v_sgrid_set_frame): the rectification maps and the staged images
     // of the last frame, in buffers sized for the largest frame so far.
@@ -445,7 +460,7 @@ struct BlockGridCore {
     // are checked before anything is touched.
     int set_frame(const void *depth, bool depth_u16, float depth_scale, const uint8_t *color, const int32_t *cls,
                   const int32_t *inst, int H, int W, bool filter_shadow_points, b2v_frame *out);
-    void free_frame();
+    void free_frame();      // frees `frame` and `input`
 };
 
 template <typename MapStorage, typename Replay> int BlockGridCore::resolve(MapStorage map_storage, Replay replay) {

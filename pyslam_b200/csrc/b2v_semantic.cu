@@ -537,14 +537,9 @@ struct b2v_sgrid : BlockGridCore {
     int32_t *d_cls = nullptr, *d_inst = nullptr;
     float *d_depths = nullptr;
     uint32_t *d_vid[2] = {nullptr, nullptr}, *d_ord[2] = {nullptr, nullptr};
+    uint8_t *d_valid = nullptr;   // per-point mask of the fused RGBD front-end
     void *d_sort_tmp = nullptr;
     size_t sort_tmp_bytes = 0, stage_points = 0;
-    // fused RGBD front-end
-    float *d_img_depth = nullptr, *d_img_filtered = nullptr;
-    uint8_t *d_img_rgb = nullptr, *d_valid = nullptr;
-    int32_t *d_img_cls = nullptr, *d_img_obj = nullptr;
-    void *d_shadow_scratch = nullptr;
-    size_t img_pixels = 0;
     // instance -> object association
     int32_t *d_pend = nullptr;
     int2 *d_records = nullptr;
@@ -553,7 +548,7 @@ struct b2v_sgrid : BlockGridCore {
     int32_t next_object_id = 1;  // VoxelSemanticSharedData::next_object_id (process-wide in the reference)
     std::vector<int32_t> map_inst, map_obj;
     bool has_instance_map = false;   // the last association succeeded (map_inst / map_obj are its map)
-    int32_t *d_map = nullptr;        // map_inst then map_obj on the device, room for 2 * map_cap (remap_instance_ids)
+    int32_t *d_map = nullptr;        // its map_inst then map_obj on the device, room for 2 * map_cap
     size_t map_cap = 0;
     // read-out
     double *d_out_pts = nullptr;
@@ -671,8 +666,7 @@ extern "C" int b2v_sgrid_destroy(b2v_sgrid *g) {
     for (VmmRange &r : g->store) vmm_release(&r);
     void *ptrs[] = {g->d_pts, g->d_cols, g->d_cls, g->d_inst, g->d_depths, g->d_vid[0], g->d_vid[1], g->d_ord[0],
                     g->d_ord[1], g->d_sort_tmp, g->d_out_pts, g->d_out_cols, g->d_out_conf, g->d_out_cls,
-                    g->d_out_obj, g->d_img_depth, g->d_img_filtered, g->d_img_rgb, g->d_valid, g->d_img_cls,
-                    g->d_img_obj, g->d_shadow_scratch, g->d_pend, g->d_records, g->d_n_records, g->d_map};
+                    g->d_out_obj, g->d_valid, g->d_pend, g->d_records, g->d_n_records, g->d_map};
     for (void *p : ptrs) cudaFree(p);
     delete g;
     return B2V_OK;
@@ -706,7 +700,7 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
     void **bufs[] = {&g->d_pts, &g->d_cols, reinterpret_cast<void **>(&g->d_cls), reinterpret_cast<void **>(&g->d_inst),
                      reinterpret_cast<void **>(&g->d_depths), reinterpret_cast<void **>(&g->d_vid[0]),
                      reinterpret_cast<void **>(&g->d_vid[1]), reinterpret_cast<void **>(&g->d_ord[0]),
-                     reinterpret_cast<void **>(&g->d_ord[1]), &g->d_sort_tmp};
+                     reinterpret_cast<void **>(&g->d_ord[1]), reinterpret_cast<void **>(&g->d_valid), &g->d_sort_tmp};
     for (void **b : bufs) {
         cudaFree(*b);
         *b = nullptr;
@@ -718,6 +712,7 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
     B2V_CUDA(g, cudaMalloc(&g->d_cls, cap * sizeof(int32_t)));
     B2V_CUDA(g, cudaMalloc(&g->d_inst, cap * sizeof(int32_t)));
     B2V_CUDA(g, cudaMalloc(&g->d_depths, cap * sizeof(float)));
+    B2V_CUDA(g, cudaMalloc(&g->d_valid, cap));
     for (int k = 0; k < 2; ++k) {
         B2V_CUDA(g, cudaMalloc(&g->d_vid[k], cap * sizeof(uint32_t)));
         B2V_CUDA(g, cudaMalloc(&g->d_ord[k], cap * sizeof(uint32_t)));
@@ -820,59 +815,20 @@ extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const 
         g->err = "b2v_sgrid_integrate_rgbd: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    B2V_CUDA(g, cudaSetDevice(g->device));
-    const size_t pixels = static_cast<size_t>(height) * width;
-    int rc = sgrid_ensure_stage(g, pixels);
+    const float *d_depth = depth;
+    const uint8_t *d_rgb = color;
+    const int32_t *d_cls = class_image, *d_obj = object_image;
+    // semantic_grid.py:332-341: everything downstream sees the filtered depth
+    int rc = g->stage_input("b2v_sgrid_integrate_rgbd", height, width, filter_shadow_points != 0, &d_depth, &d_rgb,
+                            &d_cls, &d_obj);
     if (rc != B2V_OK) return rc;
-    if (pixels > g->img_pixels) {
-        B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-        void **bufs[] = {reinterpret_cast<void **>(&g->d_img_depth), reinterpret_cast<void **>(&g->d_img_filtered),
-                         reinterpret_cast<void **>(&g->d_img_rgb), reinterpret_cast<void **>(&g->d_img_cls),
-                         reinterpret_cast<void **>(&g->d_img_obj), reinterpret_cast<void **>(&g->d_valid),
-                         &g->d_shadow_scratch};
-        for (void **b : bufs) {
-            cudaFree(*b);
-            *b = nullptr;
-        }
-        g->img_pixels = 0;  // stays 0 if an allocation below fails
-        B2V_CUDA(g, cudaMalloc(&g->d_img_depth, pixels * sizeof(float)));
-        B2V_CUDA(g, cudaMalloc(&g->d_img_filtered, pixels * sizeof(float)));
-        B2V_CUDA(g, cudaMalloc(&g->d_img_rgb, pixels * 3));
-        B2V_CUDA(g, cudaMalloc(&g->d_img_cls, pixels * sizeof(int32_t)));
-        B2V_CUDA(g, cudaMalloc(&g->d_img_obj, pixels * sizeof(int32_t)));
-        B2V_CUDA(g, cudaMalloc(&g->d_valid, pixels));
-        B2V_CUDA(g, cudaMalloc(&g->d_shadow_scratch, kShadowScratchBytes));
-        g->img_pixels = pixels;
-    }
-    cudaStream_t s = g->stream;
-    // device images (such as the staged ones of b2v_sgrid_set_frame) are read in place, host images uploaded
-    auto input = [&](const void *src, void *buf, size_t bytes, const void **out) -> cudaError_t {
-        *out = src;
-        if (!src || is_device_pointer(src)) return cudaSuccess;
-        *out = buf;
-        return cudaMemcpyAsync(buf, src, bytes, cudaMemcpyHostToDevice, s);
-    };
-    const void *in_depth, *in_rgb, *in_cls, *in_obj;
-    B2V_CUDA(g, input(depth, g->d_img_depth, pixels * sizeof(float), &in_depth));
-    B2V_CUDA(g, input(color, g->d_img_rgb, pixels * 3, &in_rgb));
-    B2V_CUDA(g, input(class_image, g->d_img_cls, pixels * sizeof(int32_t), &in_cls));
-    B2V_CUDA(g, input(object_image, g->d_img_obj, pixels * sizeof(int32_t), &in_obj));
-    const float *d_depth = static_cast<const float *>(in_depth);
-    if (filter_shadow_points) {  // semantic_grid.py:332-341: everything downstream sees the filtered depth
-        if (height <= 2 || width <= 2) {
-            g->err = "b2v_sgrid_integrate_rgbd: image too small for the shadow filter";
-            return B2V_ERR_INVALID_ARGUMENT;
-        }
-        B2V_CUDA(g, launch_filter_shadow_points(d_depth, height, width, 2, 2, -1.0f, g->d_img_filtered,
-                                               g->d_shadow_scratch, s));
-        d_depth = g->d_img_filtered;
-    }
+    const int64_t n = static_cast<int64_t>(height) * width;
+    rc = sgrid_ensure_stage(g, static_cast<size_t>(n));
+    if (rc != B2V_OK) return rc;
     const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
-    const int64_t n = static_cast<int64_t>(pixels);
-    sem_rgbd_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(
-        P, d_depth, static_cast<const uint8_t *>(in_rgb), static_cast<const int32_t *>(in_cls),
-        static_cast<const int32_t *>(in_obj),
-        static_cast<float *>(g->d_pts), static_cast<float *>(g->d_cols), g->d_cls, g->d_inst, g->d_depths, g->d_valid);
+    sem_rgbd_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, g->stream>>>(
+        P, d_depth, d_rgb, d_cls, d_obj, static_cast<float *>(g->d_pts), static_cast<float *>(g->d_cols), g->d_cls,
+        g->d_inst, g->d_depths, g->d_valid);
     B2V_CUDA(g, cudaGetLastError());
     SemInputs in{};
     in.pts = g->d_pts;
@@ -1106,21 +1062,13 @@ extern "C" int b2v_sgrid_carve(b2v_sgrid *g, const float K[4], int32_t width, in
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return B2V_ERR_CUDA;
     if (nb == 0) return B2V_OK;
-    void *tmp = nullptr;
-    const void *d_depth = nullptr;
-    cudaError_t e = g->device_input(depth, static_cast<size_t>(width) * height * sizeof(float), &tmp, &d_depth);
-    if (e == cudaSuccess) {
-        sem_carve_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(
-            g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1),
-            static_cast<const float *>(d_depth), depth_threshold);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
-    cudaFree(tmp);
-    if (e != cudaSuccess) {
-        g->err = std::string("b2v_sgrid_carve: ") + cudaGetErrorString(e);
-        return B2V_ERR_CUDA;
-    }
+    const float *d_depth = depth;
+    const int rc = g->stage_input("b2v_sgrid_carve", height, width, false, &d_depth);
+    if (rc != B2V_OK) return rc;
+    sem_carve_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(
+        g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_depth, depth_threshold);
+    B2V_CUDA(g, cudaGetLastError());
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
 }
 
@@ -1160,20 +1108,16 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
 
     std::vector<int2> rec;
     if (nb > 0) {
-        void *t_cls = nullptr, *t_inst = nullptr, *t_depth = nullptr;
-        const void *d_cls = nullptr, *d_inst = nullptr, *d_depth = nullptr;
-        e = g->device_input(class_image, pixels * sizeof(int32_t), &t_cls, &d_cls);
-        if (e == cudaSuccess) e = g->device_input(instance_image, pixels * sizeof(int32_t), &t_inst, &d_inst);
-        if (e == cudaSuccess && depth_image) e = g->device_input(depth_image, pixels * sizeof(float), &t_depth, &d_depth);
-        if (e == cudaSuccess && nv > g->records_cap) {
-            cudaFree(g->d_pend);
-            cudaFree(g->d_records);
-            g->d_pend = nullptr;
-            g->d_records = nullptr;
+        const float *d_depth = depth_image;
+        const int32_t *d_cls = class_image, *d_inst = instance_image;
+        if (g->stage_input("b2v_sgrid_assign_object_ids_to_instance_ids", height, width, false, &d_depth, nullptr,
+                           &d_cls, &d_inst) != B2V_OK)
+            return -1;
+        if (nv > g->records_cap) {
             g->records_cap = 0;
-            e = cudaMalloc(&g->d_pend, nv * sizeof(int32_t));
-            if (e == cudaSuccess) e = cudaMalloc(&g->d_records, nv * sizeof(int2));
-            if (e == cudaSuccess && !g->d_n_records) e = cudaMalloc(&g->d_n_records, sizeof(uint32_t));
+            e = regrow(&g->d_pend, nv);
+            if (e == cudaSuccess) e = regrow(&g->d_records, nv);
+            if (e == cudaSuccess) e = regrow(&g->d_n_records, 1);
             if (e == cudaSuccess) g->records_cap = nv;
         }
         uint32_t n_rec = 0;
@@ -1181,10 +1125,9 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
         if (e == cudaSuccess) e = cudaMemsetAsync(g->d_n_records, 0, sizeof(uint32_t), g->stream);
         if (e == cudaSuccess) {
             sem_assoc_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(
-                g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1),
-                static_cast<const int32_t *>(d_cls), static_cast<const int32_t *>(d_inst),
-                static_cast<const float *>(d_depth), depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend,
-                g->d_records, g->d_n_records, static_cast<uint32_t>(nv));
+                g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_cls, d_inst, d_depth,
+                depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend, g->d_records, g->d_n_records,
+                static_cast<uint32_t>(nv));
             e = cudaGetLastError();
         }
         if (e == cudaSuccess) e = cudaMemcpyAsync(&n_rec, g->d_n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, g->stream);
@@ -1193,9 +1136,6 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
             rec.resize(n_rec);
             e = cudaMemcpy(rec.data(), g->d_records, n_rec * sizeof(int2), cudaMemcpyDeviceToHost);
         }
-        cudaFree(t_cls);
-        cudaFree(t_inst);
-        cudaFree(t_depth);
         if (e != cudaSuccess) return fail("device pass", e);
     }
 
@@ -1234,23 +1174,24 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
         g->map_inst.push_back(inst);
         g->map_obj.push_back(obj);
     }
-    if (!new_id.empty() && nb > 0) {  // deferred assignment of the pending voxels
-        int32_t *d_mi = nullptr, *d_mo = nullptr;
-        const size_t m = g->map_inst.size();
-        e = cudaMalloc(&d_mi, m * sizeof(int32_t));
-        if (e == cudaSuccess) e = cudaMalloc(&d_mo, m * sizeof(int32_t));
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_mi, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_mo, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
-        if (e == cudaSuccess) {
-            sem_assoc_apply_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(g->dev(), g->d_pend, d_mi, d_mo,
-                                                                                       static_cast<int>(m));
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
-        cudaFree(d_mi);
-        cudaFree(d_mo);
-        if (e != cudaSuccess) return fail("apply", e);
+    // the map on the device, for the deferred assignment below and for b2v_sgrid_remap_instance_ids
+    const size_t m = g->map_inst.size();
+    if (m > g->map_cap) {
+        e = cudaStreamSynchronize(g->stream);
+        if (e == cudaSuccess) e = regrow(&g->d_map, 2 * m);
+        g->map_cap = e == cudaSuccess ? m : 0;
     }
+    if (e == cudaSuccess && m)
+        e = cudaMemcpyAsync(g->d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
+    if (e == cudaSuccess && m)
+        e = cudaMemcpyAsync(g->d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
+    if (e == cudaSuccess && !new_id.empty() && nb > 0) {  // deferred assignment of the pending voxels
+        sem_assoc_apply_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(g->dev(), g->d_pend, g->d_map,
+                                                                                   g->d_map + m, static_cast<int>(m));
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
+    if (e != cudaSuccess) return fail("instance map", e);
     g->has_instance_map = true;
     return static_cast<int64_t>(g->map_inst.size());
 }
@@ -1278,20 +1219,10 @@ extern "C" int b2v_sgrid_remap_instance_ids(b2v_sgrid *g, const int32_t **object
         return B2V_ERR_INVALID_ARGUMENT;
     }
     B2V_CUDA(g, cudaSetDevice(g->device));
-    const size_t m = g->map_inst.size();
-    if (m > g->map_cap) {
-        B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-        B2V_CUDA(g, regrow(&g->d_map, 2 * m));
-        g->map_cap = m;
-    }
-    cudaStream_t s = g->stream;
-    if (m) {
-        B2V_CUDA(g, cudaMemcpyAsync(g->d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-        B2V_CUDA(g, cudaMemcpyAsync(g->d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    }
+    const size_t m = g->map_inst.size();   // the association left its map in d_map
     B2V_CUDA(g, launch_remap_instance_ids(f.instance_image, static_cast<size_t>(f.height) * f.width, g->d_map,
-                                          g->d_map + m, static_cast<int>(m), g->frame.obj, s));
-    B2V_CUDA(g, cudaStreamSynchronize(s));
+                                          g->d_map + m, static_cast<int>(m), g->frame.obj, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     *object_image = g->frame.obj;
     return B2V_OK;
 }

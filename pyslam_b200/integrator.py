@@ -77,6 +77,50 @@ def write_ply_points(path: str, points, colors=None) -> None:
     write_ply_mesh(path, points, np.zeros((0, 3), np.int32), colors)
 
 
+def raw_depth(depth, camera, use_cpp: bool):
+    """(depth, depth_scale) of a raw keyframe depth image for the device, the conversion of base.py:1007-1015.  Raw
+    uint16 depth in C++-core mode goes as is with depth_scale = camera.depth_factor: the device widens it to
+    float32(depth) * factor, the value `depth.astype(np.float32) * camera.depth_factor` has on the host."""
+    if depth.dtype == np.float32:
+        return depth, None
+    if not use_cpp:
+        return depth.astype(np.float32), None
+    factor = float(getattr(camera, "depth_factor", 1.0))
+    if depth.dtype == np.uint16:
+        return depth, np.float32(factor)
+    return depth.astype(np.float32) * factor, None
+
+
+class B200PluginSetup:
+    """Set-up every B200 plugin shares; mixed in before pySLAM's `VolumetricIntegratorBase`."""
+
+    def _merge_parameters(self, defaults, parameters_dict, constructor_kwargs):
+        """self.b200_parameters: `defaults`, overridden by parameters_dict, then by constructor_kwargs (known keys)."""
+        p = dict(defaults)
+        if parameters_dict:
+            p.update({k: parameters_dict[k] for k in defaults if k in parameters_dict})
+        if constructor_kwargs:
+            p.update({k: v for k, v in constructor_kwargs.items() if k in defaults})
+        self.b200_parameters = p
+        return p
+
+    def _init_gpu_rectify(self):
+        """Raw frames go to the device when the base class computed undistortion maps (base.py:766-778) and no depth
+        estimator runs (estimated depth needs the host path): the maps are installed on self.volume once."""
+        self._gpu_rectify = False
+        m1, m2 = getattr(self, "calib_map1", None), getattr(self, "calib_map2", None)
+        if (self.b200_parameters["kVolumetricIntegrationB200GpuRectify"] and m1 is not None and m2 is not None
+                and getattr(self, "depth_estimator", None) is None):
+            self.volume.set_rectification(m1, m2, swap_rb=True)
+            self._gpu_rectify = True
+
+    def _intrinsics(self):
+        if hasattr(self, "get_camera_intrinsics_for_depth"):
+            return self.get_camera_intrinsics_for_depth()
+        c = self.camera
+        return c.fx, c.fy, c.cx, c.cy
+
+
 def make_integrator_class(Base, api):
     """Build the plugin class against a base class and an `api` namespace providing
     `VolumetricIntegrationTaskType`, `VolumetricIntegrationOutput`, `VolumetricIntegrationMesh`,
@@ -84,7 +128,7 @@ def make_integrator_class(Base, api):
 
     TaskType = api.VolumetricIntegrationTaskType
 
-    class VolumetricIntegratorB200(Base):
+    class VolumetricIntegratorB200(B200PluginSetup, Base):
         """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
@@ -95,12 +139,7 @@ def make_integrator_class(Base, api):
         # -- runs inside the integrator process: the CUDA context is created here, never in the parent
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
             Base.init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs)
-            p = dict(DEFAULT_PARAMETERS)
-            if parameters_dict:
-                p.update({k: parameters_dict[k] for k in DEFAULT_PARAMETERS if k in parameters_dict})
-            if constructor_kwargs:
-                p.update({k: v for k, v in constructor_kwargs.items() if k in DEFAULT_PARAMETERS})
-            self.b200_parameters = p
+            p = self._merge_parameters(DEFAULT_PARAMETERS, parameters_dict, constructor_kwargs)
             outdoor = False
             env_t = getattr(api, "DatasetEnvironmentType", None)
             if env_t is not None and hasattr(env_t, "INDOOR"):
@@ -120,42 +159,18 @@ def make_integrator_class(Base, api):
             self.last_integrated_id = -1
             self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call
             self._has_deferred = False
-            # rectification on the GPU: the maps the base class computed (base.py:766-778) go to the device once
-            self._gpu_rectify = False
-            m1, m2 = getattr(self, "calib_map1", None), getattr(self, "calib_map2", None)
-            if (p["kVolumetricIntegrationB200GpuRectify"] and m1 is not None and m2 is not None
-                    and getattr(self, "depth_estimator", None) is None):  # estimated depth needs the CPU path
-                self.volume.set_rectification(m1, m2, swap_rb=True)
-                self._gpu_rectify = True
+            self._init_gpu_rectify()
 
         def _prepare_frame(self, kd):
             """(color RGB or raw BGR when the GPU rectifies, depth, depth_scale).  With GPU rectification and no
             depth estimator the raw images go straight to the device: remap + channel swap happen there,
-            bit-identically to cv2.remap / cvtColor (base.py:1017-1054).  Raw uint16 depth in C++-core mode is
-            passed as is with depth_scale = camera.depth_factor: the GPU widens it to float32(depth) * factor,
-            the value `depth.astype(np.float32) * self.camera.depth_factor` has on the host (base.py:1008-1012)."""
+            bit-identically to cv2.remap / cvtColor (base.py:1017-1054), and the depth is converted by `raw_depth`."""
             if self._gpu_rectify and kd.depth is not None and kd.depth.size and kd.img is not None:
-                depth, scale = kd.depth, None
-                if depth.dtype != np.float32:  # base.py:1007-1015
-                    if getattr(api, "USE_CPP", False):
-                        factor = float(getattr(self.camera, "depth_factor", 1.0))
-                        if depth.dtype == np.uint16:
-                            scale = np.float32(factor)
-                        else:
-                            depth = depth.astype(np.float32) * factor
-                    else:
-                        depth = depth.astype(np.float32)
-                return kd.img, depth, scale
+                return (kd.img, *raw_depth(kd.depth, self.camera, getattr(api, "USE_CPP", False)))
             if self._gpu_rectify:
                 return None, None, None
             rect = self.estimate_depth_if_needed_and_rectify(kd)
             return rect[0], rect[1], None
-
-        def _intrinsics(self):
-            if hasattr(self, "get_camera_intrinsics_for_depth"):
-                return self.get_camera_intrinsics_for_depth()
-            c = self.camera
-            return c.fx, c.fy, c.cx, c.cy
 
         def _make_output(self, task_type):
             p = self.b200_parameters

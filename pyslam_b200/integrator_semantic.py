@@ -30,7 +30,7 @@ import traceback
 
 import numpy as np
 
-from .integrator import write_ply_points
+from .integrator import B200PluginSetup, raw_depth, write_ply_points
 from .volume import (CameraFrustrum, VoxelBlockGrid, VoxelBlockSemanticGrid, VoxelBlockSemanticProbabilisticGrid,
                      filter_shadow_points, remap_instance_ids)
 
@@ -69,12 +69,22 @@ DEFAULT_PARAMETERS = {
 }
 
 
+def _grid_args(p):
+    """Constructor arguments of either grid from the plugin parameters."""
+    return dict(voxel_size=p["kVolumetricIntegrationVoxelLength"], block_size=p["kVolumetricIntegrationBlockSize"],
+                capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
+                device=int(p["kVolumetricIntegrationB200Device"]),
+                max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None)
+
+
 def make_semantic_integrator_class(Base, api):
     """Build the semantic plugin class against a base class and an `api` namespace (see `integrator.py`)."""
     TaskType = api.VolumetricIntegrationTaskType
 
-    class VolumetricIntegratorB200SemanticGrid(Base):
+    class VolumetricIntegratorB200SemanticGrid(B200PluginSetup, Base):
         """GPU semantic voxel-grid integrator; `use_semantic_probabilistic` selects Bayesian fusion (:131-141)."""
+
+        _defaults = DEFAULT_PARAMETERS
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
@@ -84,27 +94,14 @@ def make_semantic_integrator_class(Base, api):
         # -- runs inside the integrator process: the CUDA context is created here, never in the parent
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
             Base.init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs)
-            p = dict(DEFAULT_PARAMETERS)
-            if parameters_dict:
-                p.update({k: parameters_dict[k] for k in DEFAULT_PARAMETERS if k in parameters_dict})
-            if constructor_kwargs:
-                p.update({k: v for k, v in constructor_kwargs.items() if k in DEFAULT_PARAMETERS})
-            self.b200_parameters = p
+            p = self._merge_parameters(self._defaults, parameters_dict, constructor_kwargs)
             indoor = True
             env_t = getattr(api, "DatasetEnvironmentType", None)
             if env_t is not None and hasattr(env_t, "INDOOR"):
                 indoor = environment_type == env_t.INDOOR
             side = "Indoor" if indoor else "Outdoor"
             self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{side}"]
-            probabilistic = bool((constructor_kwargs or {}).get("use_semantic_probabilistic", False))
-            grid_t = VoxelBlockSemanticProbabilisticGrid if probabilistic else VoxelBlockSemanticGrid
-            self.volume = grid_t(voxel_size=p["kVolumetricIntegrationVoxelLength"],
-                                 block_size=p["kVolumetricIntegrationBlockSize"],
-                                 capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
-                                 device=int(p["kVolumetricIntegrationB200Device"]),
-                                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None)
-            self.volume.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
-            self.volume.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
+            self.volume = self._make_grid(p, side, constructor_kwargs or {})
             fx, fy, cx, cy = self._intrinsics()
             self.camera_frustrum = CameraFrustrum(
                 fx, fy, cx, cy, self.camera.width, self.camera.height, np.eye(4),
@@ -115,42 +112,22 @@ def make_semantic_integrator_class(Base, api):
             self.last_instance_map = {}
             self._init_gpu_rectify()
 
-        def _init_gpu_rectify(self):
-            """Raw frames go to the grid when the base class computed undistortion maps (base.py:766-778) and no
-            depth estimator runs (estimated depth needs the host path), as in integrator.py."""
-            self._gpu_rectify = False
-            m1, m2 = getattr(self, "calib_map1", None), getattr(self, "calib_map2", None)
-            if (self.b200_parameters["kVolumetricIntegrationB200GpuRectify"] and m1 is not None and m2 is not None
-                    and getattr(self, "depth_estimator", None) is None):
-                self.volume.set_rectification(m1, m2, swap_rb=True)
-                self._gpu_rectify = True
+        def _make_grid(self, p, side, constructor_kwargs):
+            probabilistic = bool(constructor_kwargs.get("use_semantic_probabilistic", False))
+            grid_t = VoxelBlockSemanticProbabilisticGrid if probabilistic else VoxelBlockSemanticGrid
+            grid = grid_t(**_grid_args(p))
+            grid.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
+            grid.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
+            return grid
 
         def _raw_frame(self, kd):
-            """(depth, depth_scale) of a keyframe for `set_frame`, or None when it takes the host path.  The depth
-            conversion of base.py:1007-1015, as integrator.py::_prepare_frame does it: raw uint16 depth in C++-core
-            mode goes to the GPU with depth_scale = camera.depth_factor and is widened there to the value
-            `depth.astype(np.float32) * depth_factor` has on the host."""
+            """(depth, depth_scale) of a keyframe for `set_frame` (see `raw_depth`), or None when it takes the host
+            path."""
             if not self._gpu_rectify or kd.depth is None or not kd.depth.size or kd.img is None:
                 return None
             if kd.depth.shape != (self.camera_frustrum.height, self.camera_frustrum.width):
                 return None   # the frustum's label / carve calls reject such frames: the host path handles them
-            depth, scale = kd.depth, None
-            if depth.dtype != np.float32:
-                if getattr(api, "USE_CPP", False):
-                    factor = float(getattr(self.camera, "depth_factor", 1.0))
-                    if depth.dtype == np.uint16:
-                        scale = np.float32(factor)
-                    else:
-                        depth = depth.astype(np.float32) * factor
-                else:
-                    depth = depth.astype(np.float32)
-            return depth, scale
-
-        def _intrinsics(self):
-            if hasattr(self, "get_camera_intrinsics_for_depth"):
-                return self.get_camera_intrinsics_for_depth()
-            c = self.camera
-            return c.fx, c.fy, c.cx, c.cy
+            return raw_depth(kd.depth, self.camera, getattr(api, "USE_CPP", False))
 
         def _integrate_raw_keyframe(self, kd, depth, scale):
             """The loop body on the raw images: one set_frame uploads, rectifies and shadow-filters them on the
@@ -326,34 +303,10 @@ def make_voxel_grid_integrator_class(Base, api):
     SemanticCls = make_semantic_integrator_class(Base, api)
 
     class VolumetricIntegratorB200VoxelGrid(SemanticCls):
-        def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
-            Base.init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs)
-            p = dict(DEFAULT_PARAMETERS)
-            p["kVolumetricIntegrationB200CapacityBlocks"] = 1 << 17
-            if parameters_dict:
-                p.update({k: parameters_dict[k] for k in DEFAULT_PARAMETERS if k in parameters_dict})
-            if constructor_kwargs:
-                p.update({k: v for k, v in constructor_kwargs.items() if k in DEFAULT_PARAMETERS})
-            self.b200_parameters = p
-            indoor = True
-            env_t = getattr(api, "DatasetEnvironmentType", None)
-            if env_t is not None and hasattr(env_t, "INDOOR"):
-                indoor = environment_type == env_t.INDOOR
-            side = "Indoor" if indoor else "Outdoor"
-            self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{side}"]
-            self.volume = VoxelBlockGrid(p["kVolumetricIntegrationVoxelLength"], p["kVolumetricIntegrationBlockSize"],
-                                         capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
-                                         device=int(p["kVolumetricIntegrationB200Device"]),
-                                         max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"])
-                                         or None)
-            fx, fy, cx, cy = self._intrinsics()
-            self.camera_frustrum = CameraFrustrum(
-                fx, fy, cx, cy, self.camera.width, self.camera.height, np.eye(4),
-                depth_max=p[f"kVolumetricIntegrationVoxelGridCarvingDepthMax{side}"],
-                depth_min=p["kVolumetricIntegrationVoxelGridCarvingDepthMin"])
-            self.last_output = None
-            self.last_integrated_id = -1
-            self._init_gpu_rectify()
+        _defaults = dict(DEFAULT_PARAMETERS, kVolumetricIntegrationB200CapacityBlocks=1 << 17)
+
+        def _make_grid(self, p, side, constructor_kwargs):
+            return VoxelBlockGrid(**_grid_args(p))
 
         def _integrate_raw_keyframe(self, kd, depth, scale):
             """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
