@@ -18,6 +18,7 @@ B2V_ERR_INVALID_ARGUMENT = 1
 B2V_ERR_CUDA = 2
 B2V_ERR_CAPACITY = 3
 B2V_ERR_UNSUPPORTED = 4
+B2V_ASSOC_PENDING = -(1 << 31)   # object id of a pending vote triple (b2v_sgrid_assoc_votes)
 
 BLOCK_SIZE = 8
 BLOCK_VOXELS = 512
@@ -45,7 +46,8 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_remove_segment", "b2v_sgrid_label_overflows", "b2v_sgrid_dump_blocks", "b2v_sgrid_carve",
     "b2v_sgrid_assign_object_ids_to_instance_ids", "b2v_sgrid_copy_instance_map", "b2v_sgrid_set_next_object_id",
     "b2v_sgrid_get_next_object_id", "b2v_grid_set_rectification", "b2v_grid_set_frame", "b2v_sgrid_set_rectification",
-    "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids",
+    "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids", "b2v_grid_set_shard", "b2v_sgrid_set_shard",
+    "b2v_sgrid_assoc_votes", "b2v_sgrid_copy_assoc_votes", "b2v_sgrid_assoc_resolve",
 ]
 
 
@@ -154,6 +156,12 @@ def load() -> C.CDLL:
     L.b2v_sgrid_assign_object_ids_to_instance_ids.argtypes = [vp, vp, i32, i32, vp, C.c_float, C.c_float, vp, vp, vp,
                                                              C.c_float, i32, C.c_float, i32]
     L.b2v_sgrid_copy_instance_map.argtypes = [vp, vp, vp]
+    L.b2v_sgrid_assoc_votes.restype = C.c_int64
+    L.b2v_sgrid_assoc_votes.argtypes = [vp, vp, i32, i32, vp, C.c_float, C.c_float, vp, vp, vp, C.c_float, i32]
+    L.b2v_sgrid_copy_assoc_votes.restype = C.c_int
+    L.b2v_sgrid_copy_assoc_votes.argtypes = [vp, vp]
+    L.b2v_sgrid_assoc_resolve.restype = C.c_int64
+    L.b2v_sgrid_assoc_resolve.argtypes = [vp, vp, i64, i32, i32, vp, vp, C.c_float, i32]
     L.b2v_sgrid_set_next_object_id.argtypes = [vp, i32]
     L.b2v_sgrid_get_next_object_id.restype = i32
     L.b2v_sgrid_get_next_object_id.argtypes = [vp]
@@ -262,6 +270,9 @@ def load() -> C.CDLL:
         fn = getattr(L, prefix + "_set_rectification")
         fn.restype = C.c_int
         fn.argtypes = [vp, vp, vp, i32, i32, i32]
+        fn = getattr(L, prefix + "_set_shard")
+        fn.restype = C.c_int
+        fn.argtypes = [vp, i32, i32]
     L.b2v_grid_set_frame.restype = C.c_int
     L.b2v_grid_set_frame.argtypes = [vp, vp, i32, C.c_float, vp, i32, i32, i32, C.POINTER(B2VFrame)]
     L.b2v_sgrid_set_frame.restype = C.c_int

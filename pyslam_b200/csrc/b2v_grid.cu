@@ -32,6 +32,8 @@ struct GridMeta {
 // ---- block insert (both grids) ---------------------------------------------------------------
 // Make sure block (bx, by, bz) of every thread with `have` exists: one probe per distinct block per warp
 // (neighbouring points share blocks).  A new block gets the next pool index, or kNoBlock past index.capacity.
+// A sharded grid inserts only the blocks its rank owns; every pass that writes voxels finds its block with
+// table_find and skips the points whose block is absent, so this one test partitions both grids.
 __device__ __forceinline__ void block_insert(bool have, int bx, int by, int bz, const HashTable &T,
                                              const BlockIndex &B) {
     const int lane = threadIdx.x & 31;
@@ -45,6 +47,8 @@ __device__ __forceinline__ void block_insert(bool have, int bx, int by, int bz, 
               lbz = __shfl_sync(0xffffffffu, bz, leader);
     if (!have) return;
     if (leader != lane && lbx == bx && lby == by && lbz == bz) return;
+    // after the warp vote, which needs every lane: one owner test per distinct block
+    if (B.shard_count > 1u && block_owner(bx, by, bz, B.shard_count) != B.shard_rank) return;
     bool is_new;
     const uint32_t slot = table_insert(T, bx, by, bz, &is_new);
     if (slot == kEmpty) {
@@ -347,6 +351,22 @@ int BlockGridCore::capacity(int64_t *capacity_blocks, int64_t *growths_out) {
     B2V_CUDA(this, cudaStreamSynchronize(stream));
     if (capacity_blocks) *capacity_blocks = index.pool_capacity;
     if (growths_out) *growths_out = growths;
+    return B2V_OK;
+}
+
+int BlockGridCore::set_shard(int32_t rank, int32_t count) {
+    if (count < 1 || rank < 0 || rank >= count) {
+        err = "set_shard: need shard_count >= 1 and 0 <= shard_rank < shard_count";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    const int rc = fetch_counters();
+    if (rc != B2V_OK) return rc;
+    if (h_counters[kBgPool] != 0) {   // blocks of another partition may already be in the table
+        err = "set_shard: the grid holds blocks (clear it first)";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    index.shard_rank = static_cast<uint32_t>(rank);
+    index.shard_count = static_cast<uint32_t>(count);
     return B2V_OK;
 }
 
@@ -706,6 +726,11 @@ extern "C" int b2v_grid_destroy(b2v_grid *g) {
 extern "C" int b2v_grid_capacity(b2v_grid *g, int64_t *capacity_blocks, int64_t *growths) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     return g->capacity(capacity_blocks, growths);
+}
+
+extern "C" int b2v_grid_set_shard(b2v_grid *g, int32_t shard_rank, int32_t shard_count) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_shard(shard_rank, shard_count);
 }
 
 extern "C" int b2v_grid_clear(b2v_grid *g) {

@@ -344,6 +344,8 @@ struct BlockIndex {
     uint32_t *counters;       // see BlockGridCounter
     uint32_t capacity;        // maximum capacity: allocation hands out pool indices below it (the others get kNoBlock)
     uint32_t pool_capacity;   // blocks with storage now (<= capacity); a growable grid maps more within the call
+    // hash sharding (SURVEY.md 8e): the grid holds only the blocks with block_owner(key, shard_count) == shard_rank
+    uint32_t shard_rank = 0, shard_count = 1;
 };
 // Block insert of every point (optional per-point mask `valid`): each block a point falls in gets a table entry and a
 // pool index (kNoBlock once the index passes index.capacity).  Points are float or double [n][3].
@@ -405,6 +407,9 @@ struct BlockGridCore {
         return std::min(h_counters[kBgPool], index.pool_capacity);
     }
     int capacity(int64_t *capacity_blocks, int64_t *growths_out);
+    // keep only the blocks rank `rank` of `count` owns from now on; only on a grid without blocks (synchronises).
+    // clear() keeps the setting.
+    int set_shard(int32_t rank, int32_t count);
     int clear_index();      // empty table, zero counters (asynchronous)
     // Growable grids, at the end of an integrate call: the call's first pass skipped the points of blocks handed a
     // pool index past the storage.  map_storage(blocks) maps storage for at least that many blocks and updates

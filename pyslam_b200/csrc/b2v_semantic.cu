@@ -23,6 +23,7 @@
 // that is not the current argmax and bumps the overflow counter (b2v_sgrid_label_overflows) - a documented
 // deviation that no test or reference KAT reaches.
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
 
 #include <algorithm>
 #include <climits>
@@ -44,8 +45,16 @@ constexpr int kSemLabels = B2V_SEM_MAX_LABELS;
 constexpr uint32_t kBadVid = 0xFFFFFFFFu;
 constexpr float kBaseLogProb = 0.10536051565782628f;  // voxel_data_semantic.h:287, -log(0.9)
 
+// the block index as the semantic kernels read it: BlockIndex without the shard fields, which only the block insert
+// reads (the 24-byte layout keeps sem_runs_kernel's label slots in a local-memory frame, as before the shard fields)
+struct SemBlockIndex {
+    int4 *block_keys;
+    uint32_t *counters;
+    uint32_t capacity, pool_capacity;
+};
+
 struct SemGrid {
-    BlockIndex index;
+    SemBlockIndex index;
     int32_t *count;     // [V]            V = capacity * 512, voxel id = pool index * 512 + lx + 8 ly + 64 lz
     double *pos;        // [V][3]
     float *col;         // [V][3]
@@ -448,12 +457,21 @@ sem_carve_kernel(const SemGrid G, const GridQuery Q, const float *__restrict__ d
 // process_point of assign_object_ids_to_instance_ids (voxel_semantic_data_association.h:171-229): every voxel in
 // the frustum whose class equals the pixel's class and that lies on the observed surface votes
 // "image instance id -> my object id".  Voxels without an object id are recorded as pending (pend[v] = instance
-// id); the host turns the vote records into the instance -> object map.
-constexpr int32_t kAssocPending = INT_MIN;
+// id).  The records are reduced on the device to sorted (instance, object, count) triples, from which the host
+// builds the instance -> object map.
+constexpr int32_t kAssocPending = B2V_ASSOC_PENDING;
+static_assert(kAssocPending == INT_MIN, "the pending marker sorts before every object id");
+
+// vote record (instance, object) as one sort key: sign bits flipped, so unsigned order is (instance, object) order
+__device__ __forceinline__ unsigned long long assoc_key(int32_t inst, int32_t obj) {
+    return static_cast<unsigned long long>(static_cast<uint32_t>(inst) ^ 0x80000000u) << 32 |
+           (static_cast<uint32_t>(obj) ^ 0x80000000u);
+}
+
 __global__ void __launch_bounds__(kVox)
 sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__ class_img,
                  const int32_t *__restrict__ inst_img, const float *__restrict__ depth_img, const float thr,
-                 const int do_carving, int32_t *__restrict__ pend, int2 *__restrict__ records,
+                 const int do_carving, int32_t *__restrict__ pend, unsigned long long *__restrict__ records,
                  uint32_t *__restrict__ n_records, const uint32_t cap_records) {
     const uint32_t b = blockIdx.x;
     ImagePoint ip;
@@ -486,7 +504,19 @@ sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__
         }
     }
     const uint32_t r = atomicAdd(n_records, 1u);
-    if (r < cap_records) records[r] = make_int2(image_instance, point_object);
+    if (r < cap_records) records[r] = assoc_key(image_instance, point_object);
+}
+
+// the runs of the sorted records -> triples int32 [n_runs][3] = {instance, object or kAssocPending, count}
+__global__ void __launch_bounds__(256)
+sem_assoc_triples_kernel(const unsigned long long *__restrict__ keys, const uint32_t *__restrict__ counts,
+                         const uint32_t *__restrict__ n_runs, int32_t *__restrict__ triples) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= *n_runs) return;
+    const unsigned long long k = keys[i];
+    triples[3 * static_cast<size_t>(i) + 0] = static_cast<int32_t>(static_cast<uint32_t>(k >> 32) ^ 0x80000000u);
+    triples[3 * static_cast<size_t>(i) + 1] = static_cast<int32_t>(static_cast<uint32_t>(k) ^ 0x80000000u);
+    triples[3 * static_cast<size_t>(i) + 2] = static_cast<int32_t>(counts[i]);
 }
 
 // deferred assignment (voxel_semantic_data_association.h:354-370): pending voxels take their instance's final id
@@ -540,11 +570,21 @@ struct b2v_sgrid : BlockGridCore {
     uint8_t *d_valid = nullptr;   // per-point mask of the fused RGBD front-end
     void *d_sort_tmp = nullptr;
     size_t sort_tmp_bytes = 0, stage_points = 0;
-    // instance -> object association
-    int32_t *d_pend = nullptr;
-    int2 *d_records = nullptr;
-    uint32_t *d_n_records = nullptr;
+    // instance -> object association: votes (records -> sort -> runs -> triples), then resolve
+    int32_t *d_pend = nullptr;                       // [voxels] instance id of a pending voxel, else -1
+    unsigned long long *d_records = nullptr;         // [voxels] vote records (sort keys)
+    uint32_t *d_n_records = nullptr;                 // [2] records, runs
     size_t records_cap = 0;
+    unsigned long long *d_sorted = nullptr, *d_runs = nullptr;   // [votes_cap] sort buffer, run keys
+    uint32_t *d_run_counts = nullptr;                // [votes_cap]
+    int32_t *d_triples = nullptr;                    // [votes_cap][3]
+    uint8_t *d_votes_tmp = nullptr;
+    size_t votes_cap = 0, votes_tmp_bytes = 0;
+    int64_t n_triples = 0;
+    // every call that may change a voxel bumps `generation`; resolve needs the votes of the current state
+    uint64_t generation = 0, votes_generation = 0;
+    bool votes_ready = false;
+    uint32_t votes_blocks = 0;                       // blocks d_pend covers
     int32_t next_object_id = 1;  // VoxelSemanticSharedData::next_object_id (process-wide in the reference)
     std::vector<int32_t> map_inst, map_obj;
     bool has_instance_map = false;   // the last association succeeded (map_inst / map_obj are its map)
@@ -559,7 +599,7 @@ struct b2v_sgrid : BlockGridCore {
 
     SemGrid dev() const {   // the kernels' view
         SemGrid d = G;
-        d.index = index;
+        d.index = SemBlockIndex{index.block_keys, index.counters, index.capacity, index.pool_capacity};
         return d;
     }
 };
@@ -666,14 +706,21 @@ extern "C" int b2v_sgrid_destroy(b2v_sgrid *g) {
     for (VmmRange &r : g->store) vmm_release(&r);
     void *ptrs[] = {g->d_pts, g->d_cols, g->d_cls, g->d_inst, g->d_depths, g->d_vid[0], g->d_vid[1], g->d_ord[0],
                     g->d_ord[1], g->d_sort_tmp, g->d_out_pts, g->d_out_cols, g->d_out_conf, g->d_out_cls,
-                    g->d_out_obj, g->d_valid, g->d_pend, g->d_records, g->d_n_records, g->d_map};
+                    g->d_out_obj, g->d_valid, g->d_pend, g->d_records, g->d_n_records, g->d_map,
+                    g->d_sorted, g->d_runs, g->d_run_counts, g->d_triples, g->d_votes_tmp};
     for (void *p : ptrs) cudaFree(p);
     delete g;
     return B2V_OK;
 }
 
+extern "C" int b2v_sgrid_set_shard(b2v_sgrid *g, int32_t shard_rank, int32_t shard_count) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_shard(shard_rank, shard_count);
+}
+
 extern "C" int b2v_sgrid_clear(b2v_sgrid *g) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    ++g->generation;
     int rc = g->fetch_counters();
     if (rc != B2V_OK) return rc;
     rc = sgrid_clear_device(g, g->block_count());   // the storage is kept
@@ -751,6 +798,7 @@ static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8
 // is updated from the cleared state in input order (the sort is stable) and the grid equals one created at the
 // maximum.  The staged inputs must stay alive until the call ends.
 static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
+    ++g->generation;
     B2V_CUDA(g, launch_point_insert(in.pts, in.pts_f64 != 0, valid, n, g->inv_voxel_size, g->table, g->index,
                                     g->stream));
     const int rc = sgrid_apply(g, n, in, valid, 0, g->index.pool_capacity);
@@ -939,6 +987,7 @@ extern "C" int b2v_sgrid_copy_voxels(b2v_sgrid *g, double *points, float *colors
 
 static int sgrid_edit(b2v_sgrid *g, int op, int a, int b) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    ++g->generation;
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return B2V_ERR_CUDA;
     if (nb == 0) return B2V_OK;
@@ -1059,6 +1108,7 @@ extern "C" int b2v_sgrid_carve(b2v_sgrid *g, const float K[4], int32_t width, in
         g->err = "b2v_sgrid_carve: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
+    ++g->generation;
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return B2V_ERR_CUDA;
     if (nb == 0) return B2V_OK;
@@ -1080,76 +1130,172 @@ extern "C" int b2v_sgrid_set_next_object_id(b2v_sgrid *g, int32_t next_object_id
 
 extern "C" int32_t b2v_sgrid_get_next_object_id(const b2v_sgrid *g) { return g ? g->next_object_id : -1; }
 
-extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
-    b2v_sgrid *g, const float K[4], int32_t width, int32_t height, const double Tcw[16], float depth_max,
-    float depth_min, const int32_t *class_image, const int32_t *instance_image, const float *depth_image,
-    float depth_threshold, int32_t do_carving, float min_vote_ratio, int32_t min_votes) {
-    if (!g) return -1;
+// votes of the association: sem_assoc_kernel (pending marks, optional carving), then the records reduced on the
+// device to sorted unique (instance, object or kAssocPending, count) triples in d_triples.  `fn` names the call in
+// err.  Returns the number of triples, or -1.
+static int64_t sgrid_assoc_votes(b2v_sgrid *g, const char *fn, const float K[4], int32_t width, int32_t height,
+                                 const double Tcw[16], float depth_max, float depth_min, const int32_t *class_image,
+                                 const int32_t *instance_image, const float *depth_image, float depth_threshold,
+                                 int32_t do_carving) {
     g->map_inst.clear();
     g->map_obj.clear();
     g->has_instance_map = false;
+    g->votes_ready = false;
+    g->n_triples = 0;
     if (!K || !Tcw || !class_image || !instance_image || width <= 0 || height <= 0) {
-        g->err = "b2v_sgrid_assign_object_ids_to_instance_ids: bad arguments";
+        g->err = std::string(fn) + ": bad arguments";
         return -1;
     }
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return -1;
-    const size_t pixels = static_cast<size_t>(width) * height;
     const size_t nv = static_cast<size_t>(nb) * kVox;
-    auto fail = [&](const char *what, cudaError_t e) {
-        g->err = std::string("b2v_sgrid_assign_object_ids_to_instance_ids: ") + what + ": " + cudaGetErrorString(e);
-        return static_cast<int64_t>(-1);
-    };
-    // host copies of the label images: the map must cover every (instance >= 0, class >= 0) pixel (:322-352)
-    std::vector<int32_t> h_cls(pixels), h_inst(pixels);
-    cudaError_t e = cudaMemcpy(h_cls.data(), class_image, pixels * sizeof(int32_t), cudaMemcpyDefault);
-    if (e == cudaSuccess) e = cudaMemcpy(h_inst.data(), instance_image, pixels * sizeof(int32_t), cudaMemcpyDefault);
-    if (e != cudaSuccess) return fail("label images", e);
-
-    std::vector<int2> rec;
+    ++g->generation;   // carving, and object id 0 for instance 0, change voxels
+    uint32_t counts[2] = {0, 0};   // records, runs
     if (nb > 0) {
         const float *d_depth = depth_image;
         const int32_t *d_cls = class_image, *d_inst = instance_image;
-        if (g->stage_input("b2v_sgrid_assign_object_ids_to_instance_ids", height, width, false, &d_depth, nullptr,
-                           &d_cls, &d_inst) != B2V_OK)
-            return -1;
+        if (g->stage_input(fn, height, width, false, &d_depth, nullptr, &d_cls, &d_inst) != B2V_OK) return -1;
+        cudaStream_t s = g->stream;
+        cudaError_t e = cudaSuccess;
         if (nv > g->records_cap) {
             g->records_cap = 0;
             e = regrow(&g->d_pend, nv);
             if (e == cudaSuccess) e = regrow(&g->d_records, nv);
-            if (e == cudaSuccess) e = regrow(&g->d_n_records, 1);
+            if (e == cudaSuccess) e = regrow(&g->d_n_records, 2);
             if (e == cudaSuccess) g->records_cap = nv;
         }
-        uint32_t n_rec = 0;
-        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_pend, 0xFF, nv * sizeof(int32_t), g->stream);
-        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_n_records, 0, sizeof(uint32_t), g->stream);
+        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_pend, 0xFF, nv * sizeof(int32_t), s);
+        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_n_records, 0, 2 * sizeof(uint32_t), s);
         if (e == cudaSuccess) {
-            sem_assoc_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(
+            sem_assoc_kernel<<<static_cast<unsigned>(nb), kVox, 0, s>>>(
                 g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_cls, d_inst, d_depth,
                 depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend, g->d_records, g->d_n_records,
                 static_cast<uint32_t>(nv));
             e = cudaGetLastError();
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&n_rec, g->d_n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, g->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
-        if (e == cudaSuccess && n_rec) {
-            rec.resize(n_rec);
-            e = cudaMemcpy(rec.data(), g->d_records, n_rec * sizeof(int2), cudaMemcpyDeviceToHost);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(counts, g->d_n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        const uint32_t n_rec = counts[0];
+        if (e == cudaSuccess && n_rec > g->votes_cap) {   // sort and run buffers sized by the records, not the voxels
+            g->votes_cap = 0;
+            const size_t cap = std::min<size_t>(nv, static_cast<size_t>(n_rec) + n_rec / 4 + 1024);
+            e = regrow(&g->d_sorted, cap);
+            if (e == cudaSuccess) e = regrow(&g->d_runs, cap);
+            if (e == cudaSuccess) e = regrow(&g->d_run_counts, cap);
+            if (e == cudaSuccess) e = regrow(&g->d_triples, 3 * cap);
+            size_t sort_bytes = 0, rle_bytes = 0;
+            cub::DoubleBuffer<unsigned long long> db(g->d_records, g->d_sorted);
+            if (e == cudaSuccess)
+                e = cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, db, static_cast<int>(cap), 0, 64, s);
+            if (e == cudaSuccess)
+                e = cub::DeviceRunLengthEncode::Encode(nullptr, rle_bytes, g->d_records, g->d_runs, g->d_run_counts,
+                                                       g->d_n_records + 1, static_cast<int>(cap), s);
+            if (e == cudaSuccess) e = regrow(&g->d_votes_tmp, std::max(sort_bytes, rle_bytes));
+            if (e == cudaSuccess) {
+                g->votes_tmp_bytes = std::max(sort_bytes, rle_bytes);
+                g->votes_cap = cap;
+            }
         }
-        if (e != cudaSuccess) return fail("device pass", e);
+        if (e == cudaSuccess && n_rec) {
+            // all 64 bits: the triples come out in ascending (instance, object) order, kAssocPending first
+            cub::DoubleBuffer<unsigned long long> db(g->d_records, g->d_sorted);
+            size_t tmp = g->votes_tmp_bytes;
+            e = cub::DeviceRadixSort::SortKeys(g->d_votes_tmp, tmp, db, static_cast<int>(n_rec), 0, 64, s);
+            tmp = g->votes_tmp_bytes;
+            if (e == cudaSuccess)
+                e = cub::DeviceRunLengthEncode::Encode(g->d_votes_tmp, tmp, db.Current(), g->d_runs, g->d_run_counts,
+                                                       g->d_n_records + 1, static_cast<int>(n_rec), s);
+            if (e == cudaSuccess) {
+                sem_assoc_triples_kernel<<<(n_rec + 255) / 256, 256, 0, s>>>(g->d_runs, g->d_run_counts,
+                                                                             g->d_n_records + 1, g->d_triples);
+                e = cudaGetLastError();
+            }
+            if (e == cudaSuccess)
+                e = cudaMemcpyAsync(counts + 1, g->d_n_records + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        }
+        if (e != cudaSuccess) {
+            g->err = std::string(fn) + ": device pass: " + cudaGetErrorString(e);
+            return -1;
+        }
     }
+    g->n_triples = counts[1];
+    g->votes_blocks = static_cast<uint32_t>(nb);
+    g->votes_generation = g->generation;
+    g->votes_ready = true;
+    return g->n_triples;
+}
 
-    // votes: instance id -> (object id -> count); pending voxels vote for their instance's NEW object id, handed
-    // out here in ascending instance-id order (the reference hands them out in block-iteration order, :118-141)
-    std::map<int32_t, std::map<int32_t, int>> votes;
+extern "C" int64_t b2v_sgrid_assoc_votes(b2v_sgrid *g, const float K[4], int32_t width, int32_t height,
+                                         const double Tcw[16], float depth_max, float depth_min,
+                                         const int32_t *class_image, const int32_t *instance_image,
+                                         const float *depth_image, float depth_threshold, int32_t do_carving) {
+    if (!g) return -1;
+    return sgrid_assoc_votes(g, "b2v_sgrid_assoc_votes", K, width, height, Tcw, depth_max, depth_min, class_image,
+                             instance_image, depth_image, depth_threshold, do_carving);
+}
+
+extern "C" int b2v_sgrid_copy_assoc_votes(b2v_sgrid *g, int32_t *triples) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (!g->votes_ready) {
+        g->err = "b2v_sgrid_copy_assoc_votes: no votes (run b2v_sgrid_assoc_votes first)";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    if (g->n_triples == 0) return B2V_OK;
+    if (!triples) {
+        g->err = "b2v_sgrid_copy_assoc_votes: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    B2V_CUDA(g, cudaMemcpyAsync(triples, g->d_triples, static_cast<size_t>(g->n_triples) * 3 * sizeof(int32_t),
+                                cudaMemcpyDefault, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return B2V_OK;
+}
+
+// resolve of the association from the triples of every rank; `fn` names the call in err
+static int64_t sgrid_assoc_resolve(b2v_sgrid *g, const char *fn, const int32_t *triples, int64_t n_triples,
+                                   int32_t width, int32_t height, const int32_t *class_image,
+                                   const int32_t *instance_image, float min_vote_ratio, int32_t min_votes) {
+    if (n_triples < 0 || (n_triples > 0 && !triples) || !class_image || !instance_image || width <= 0 ||
+        height <= 0) {
+        g->err = std::string(fn) + ": bad arguments";
+        return -1;
+    }
+    if (!g->votes_ready || g->votes_generation != g->generation) {
+        g->err = std::string(fn) + ": no votes of the grid's current state (an integrate, edit or clear, or an "
+                                   "earlier resolve, followed the votes)";
+        return -1;
+    }
+    g->votes_ready = false;
+    auto fail = [&](const char *what, cudaError_t e) {
+        g->err = std::string(fn) + ": " + what + ": " + cudaGetErrorString(e);
+        return static_cast<int64_t>(-1);
+    };
+    cudaError_t e = cudaSetDevice(g->device);
+    // host copies of the label images: the map must cover every (instance >= 0, class >= 0) pixel (:322-352)
+    const size_t pixels = static_cast<size_t>(width) * height;
+    std::vector<int32_t> h_cls(pixels), h_inst(pixels), t(static_cast<size_t>(n_triples) * 3);
+    if (e == cudaSuccess) e = cudaMemcpy(h_cls.data(), class_image, pixels * sizeof(int32_t), cudaMemcpyDefault);
+    if (e == cudaSuccess) e = cudaMemcpy(h_inst.data(), instance_image, pixels * sizeof(int32_t), cudaMemcpyDefault);
+    if (e != cudaSuccess) return fail("label images", e);
+    if (n_triples && (e = cudaMemcpy(t.data(), triples, t.size() * sizeof(int32_t), cudaMemcpyDefault)) != cudaSuccess)
+        return fail("votes", e);
+
+    // votes: instance id -> (object id -> count), summed over the triples of every rank; pending voxels vote for
+    // their instance's NEW object id, handed out here in ascending instance-id order (the reference hands them out in
+    // block-iteration order, :118-141).  The counts are integers, so the sums equal the unsharded counts exactly.
+    std::map<int32_t, std::map<int32_t, int64_t>> votes;
     std::map<int32_t, int32_t> new_id;
-    for (const int2 &r : rec)
-        if (r.y == kAssocPending) new_id.emplace(r.x, 0);
+    for (size_t i = 0; i < t.size(); i += 3)
+        if (t[i + 1] == kAssocPending) new_id.emplace(t[i], 0);
     for (auto &kv : new_id) kv.second = g->next_object_id++;
-    for (const int2 &r : rec) votes[r.x][r.y == kAssocPending ? new_id[r.x] : r.y] += 1;
+    for (size_t i = 0; i < t.size(); i += 3)
+        votes[t[i]][t[i + 1] == kAssocPending ? new_id[t[i]] : t[i + 1]] += t[i + 2];
     std::map<int32_t, int32_t> result;
     for (const auto &[inst, ov] : votes) {  // :287-320
-        int max_votes = 0, winner = -1, total = 0;
+        int64_t max_votes = 0, total = 0;
+        int32_t winner = -1;
         for (const auto &[obj, cnt] : ov) {
             total += cnt;
             if (cnt > max_votes) {
@@ -1162,13 +1308,15 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
         else
             result[inst] = winner;
     }
+    int32_t prev = -1;   // labelled pixels come in runs of one instance; repeating an entry changes nothing
     for (size_t i = 0; i < pixels; ++i) {  // :322-352: every labelled instance of the image gets an entry
         const int32_t inst = h_inst[i];
-        if (inst < 0 || h_cls[i] < 0) continue;
+        if (inst < 0 || h_cls[i] < 0 || inst == prev) continue;
+        prev = inst;
         if (inst == 0)
             result[0] = 0;
         else
-            result.emplace(inst, -1);
+            result.try_emplace(inst, -1);   // no node allocated for an instance already present
     }
     for (const auto &[inst, obj] : result) {
         g->map_inst.push_back(inst);
@@ -1185,15 +1333,38 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
         e = cudaMemcpyAsync(g->d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
     if (e == cudaSuccess && m)
         e = cudaMemcpyAsync(g->d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
-    if (e == cudaSuccess && !new_id.empty() && nb > 0) {  // deferred assignment of the pending voxels
-        sem_assoc_apply_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(g->dev(), g->d_pend, g->d_map,
-                                                                                   g->d_map + m, static_cast<int>(m));
+    if (e == cudaSuccess && !new_id.empty() && g->votes_blocks > 0) {  // deferred assignment of this grid's pending voxels
+        ++g->generation;
+        sem_assoc_apply_kernel<<<g->votes_blocks, kVox, 0, g->stream>>>(g->dev(), g->d_pend, g->d_map, g->d_map + m,
+                                                                         static_cast<int>(m));
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
     if (e != cudaSuccess) return fail("instance map", e);
     g->has_instance_map = true;
-    return static_cast<int64_t>(g->map_inst.size());
+    return static_cast<int64_t>(m);
+}
+
+extern "C" int64_t b2v_sgrid_assoc_resolve(b2v_sgrid *g, const int32_t *triples, int64_t n_triples, int32_t width,
+                                           int32_t height, const int32_t *class_image, const int32_t *instance_image,
+                                           float min_vote_ratio, int32_t min_votes) {
+    if (!g) return -1;
+    return sgrid_assoc_resolve(g, "b2v_sgrid_assoc_resolve", triples, n_triples, width, height, class_image,
+                               instance_image, min_vote_ratio, min_votes);
+}
+
+// the unsharded association: the votes, then the resolve of this grid's own triples
+extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
+    b2v_sgrid *g, const float K[4], int32_t width, int32_t height, const double Tcw[16], float depth_max,
+    float depth_min, const int32_t *class_image, const int32_t *instance_image, const float *depth_image,
+    float depth_threshold, int32_t do_carving, float min_vote_ratio, int32_t min_votes) {
+    if (!g) return -1;
+    const char *fn = "b2v_sgrid_assign_object_ids_to_instance_ids";
+    const int64_t n = sgrid_assoc_votes(g, fn, K, width, height, Tcw, depth_max, depth_min, class_image,
+                                        instance_image, depth_image, depth_threshold, do_carving);
+    if (n < 0) return -1;
+    return sgrid_assoc_resolve(g, fn, g->d_triples, n, width, height, class_image, instance_image, min_vote_ratio,
+                               min_votes);
 }
 
 extern "C" int b2v_sgrid_set_rectification(b2v_sgrid *g, const float *map_x, const float *map_y, int32_t height,

@@ -13,6 +13,12 @@ integrates every frame into the blocks it owns (`b2v_config.shard_rank / shard_c
   `mesh_piece`, `point_piece`, `weld`) so that N shards held in one process can run them too.
   `extract_mesh_distributed` is the older route: `gather_blocks_device` collects all shards on one rank GPU-to-GPU over
   NCCL (`gather_blocks` is the host-array variant used with gloo in the CPU tests), which then meshes the union.
+
+The point-average and semantic grids shard the same way (`shard_rank` / `shard_count`; DESIGN.md §7, "Sharded grids"):
+every rank is fed every frame and keeps its own blocks, voxel edits apply per rank, and the read-outs are gathered
+(`get_voxels_sharded`, `get_object_segments_sharded`, ...).  The one step that is not per voxel, the instance -> object
+association, exchanges vote triples: `association_votes` on every rank, then `resolve_association` of all ranks'
+triples on every rank (`assign_object_ids_to_instance_ids_sharded` runs both over a process group).
 """
 
 from __future__ import annotations
@@ -32,7 +38,8 @@ def owner_of(keys, world: int) -> np.ndarray:
 
 
 def merge_dumps(dumps):
-    """Union of per-rank block dumps (dicts with keys/hashes/vox), sorted by key."""
+    """Union of per-rank block dumps, sorted by key: any dicts of per-block arrays with a "keys" entry, such as
+    `B200TsdfVolume.dump_blocks` (keys / hashes / vox) or a grid's `dump_blocks`."""
     keys = np.concatenate([d["keys"] for d in dumps])
     order = np.lexsort((keys[:, 2], keys[:, 1], keys[:, 0]))
     return {name: np.concatenate([d[name] for d in dumps])[order] for name in dumps[0]}
@@ -356,20 +363,26 @@ def _exchange_halo(volume, group):
 
 
 def _gather_rows(arr, dst, group, on_device, device):
-    """Variable-length row arrays of every rank, on dst (list in rank order), None elsewhere."""
+    """Variable-length row arrays (numpy, or torch tensors on any device) of every rank, as numpy arrays in rank order:
+    on dst, or on every rank with dst=None; None elsewhere.  The rows travel as CUDA tensors on `device` with NCCL
+    (on_device), as host tensors otherwise."""
     import torch
     import torch.distributed as dist
     world = dist.get_world_size(group)
     dev = torch.device("cuda", device) if on_device else torch.device("cpu")
-    t = torch.from_numpy(np.ascontiguousarray(arr)).to(dev)
+    t = (arr if torch.is_tensor(arr) else torch.from_numpy(np.ascontiguousarray(arr))).to(dev)
     n = torch.tensor([t.shape[0]], dtype=torch.int64, device=dev)
     sizes = [torch.zeros_like(n) for _ in range(world)]
     dist.all_gather(sizes, n, group=group)
     sizes = [int(s.item()) for s in sizes]
     pad = torch.zeros((max(max(sizes), 1),) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
     pad[:t.shape[0]] = t
-    bufs = [torch.zeros_like(pad) for _ in range(world)] if dist.get_rank(group) == dst else None
-    dist.gather(pad, bufs, dst=dst, group=group)
+    if dst is None:
+        bufs = [torch.zeros_like(pad) for _ in range(world)]
+        dist.all_gather(bufs, pad, group=group)
+    else:
+        bufs = [torch.zeros_like(pad) for _ in range(world)] if dist.get_rank(group) == dst else None
+        dist.gather(pad, bufs, dst=dst, group=group)
     if bufs is None:
         return None
     return [bufs[r][:sizes[r]].cpu().numpy() for r in range(world)]
@@ -408,3 +421,153 @@ def extract_point_cloud_sharded(volume, dst: int = 0, group=None, gather: bool =
     """Point cloud of a hash-sharded volume, like `extract_mesh_sharded`: each rank extracts the zero crossings rooted
     in its own blocks; the disjoint pieces are concatenated in rank order on `dst` (a PointCloud with edge_ids)."""
     return _sharded(volume, dst, group, gather, points=True)
+
+
+# ---- sharded point-average and semantic grids ------------------------------------------------------------------------
+
+def association_votes(grid, camera_frustrum, class_ids_image, semantic_instances_image, depth_image=None,
+                      depth_threshold: float = 0.1, do_carving: bool = False, device: bool = False):
+    """The votes step of `assign_object_ids_to_instance_ids` on one shard of a semantic grid (b2v_sgrid_assoc_votes):
+    the shard's frustum voxels vote, pending voxels are marked and `do_carving` carves, as in the unsharded call.
+    Returns the shard's sorted unique vote triples int32 [n,3] = (instance id, object id or `_lib.B2V_ASSOC_PENDING`,
+    count): numpy, or a CUDA tensor on the grid's device with `device=True` (for NCCL).  None when the label images are
+    empty or wrongly sized (the reference's soft failure, which `resolve_association` repeats)."""
+    import ctypes as C
+    from . import _lib
+    hold = []
+    imgs = grid._assoc_images((camera_frustrum.height, camera_frustrum.width), class_ids_image,
+                              semantic_instances_image, depth_image, hold)
+    if imgs is None:
+        return None
+    K, T = camera_frustrum._args()
+    n = grid._L.b2v_sgrid_assoc_votes(grid._h, K.ctypes.data, camera_frustrum.width, camera_frustrum.height,
+                                      T.ctypes.data, camera_frustrum.depth_max, camera_frustrum.depth_min, *imgs,
+                                      float(depth_threshold), 1 if do_carving else 0)
+    if n < 0:
+        raise RuntimeError(grid._L.b2v_sgrid_last_error(grid._h).decode())
+    if device:
+        import torch
+        out = torch.empty((n, 3), dtype=torch.int32, device=torch.device("cuda", grid.device))
+        torch.cuda.synchronize(out.device)
+        ptr = out.data_ptr()
+    else:
+        out = np.zeros((n, 3), np.int32)
+        ptr = out.ctypes.data
+    grid._check(grid._L.b2v_sgrid_copy_assoc_votes(grid._h, C.c_void_p(ptr) if n else None),
+                "b2v_sgrid_copy_assoc_votes")
+    return out
+
+
+def resolve_association(grid, votes_list, class_ids_image, semantic_instances_image, min_vote_ratio: float = 0.5,
+                        min_votes: int = 3) -> dict:
+    """The resolve step on one shard (b2v_sgrid_assoc_resolve): the triples of every rank (`association_votes`, any
+    order, numpy or tensors) are summed, new object ids go to the instances with a pending triple in ascending
+    instance order, the reference's winner rule picks each instance's object, and the shard's pending voxels take
+    their instance's id.  Every rank that resolves the same triples returns the unsharded map and advances
+    `next_object_id` alike.  No integrate, edit or clear may come between the votes and the resolve."""
+    import torch
+    parts = [v for v in votes_list if v is not None]
+    if len(parts) < len(votes_list):
+        return {}
+    hw = tuple(getattr(class_ids_image, "shape", None) or np.shape(class_ids_image))
+    hold = []
+    imgs = grid._assoc_images(hw, class_ids_image, semantic_instances_image, None, hold) if len(hw) == 2 else None
+    if imgs is None:
+        return {}
+    t = np.ascontiguousarray(np.concatenate([np.asarray(v.cpu() if torch.is_tensor(v) else v, np.int32).reshape(-1, 3)
+                                             for v in parts] or [np.zeros((0, 3), np.int32)]))
+    H, W = hw
+    n = grid._L.b2v_sgrid_assoc_resolve(grid._h, t.ctypes.data, len(t), W, H, imgs[0], imgs[1],
+                                        float(min_vote_ratio), int(min_votes))
+    return grid._instance_map(n)
+
+
+def _on_device(group):
+    import torch.distributed as dist
+    return dist.get_backend(group) == "nccl"
+
+
+def assign_object_ids_to_instance_ids_sharded(grid, camera_frustrum, class_ids_image, semantic_instances_image,
+                                              depth_image=None, depth_threshold: float = 0.1,
+                                              do_carving: bool = False, min_vote_ratio: float = 0.5,
+                                              min_votes: int = 3, group=None) -> dict:
+    """`assign_object_ids_to_instance_ids` of a hash-sharded semantic grid over a process group, called on every rank
+    with the same frame: the votes of every rank, one all-gather of the vote triples (GPU to GPU with NCCL, host
+    tensors with any other backend), then the resolve on every rank.  Every rank returns the map of the unsharded grid
+    and its voxels are those of the unsharded grid it owns."""
+    on_device = _on_device(group)
+    votes = association_votes(grid, camera_frustrum, class_ids_image, semantic_instances_image, depth_image,
+                              depth_threshold, do_carving, device=on_device)
+    if votes is None:   # the same images on every rank: all ranks return here
+        return {}
+    parts = _gather_rows(votes, None, group, on_device, grid.device)
+    return resolve_association(grid, parts, class_ids_image, semantic_instances_image, min_vote_ratio, min_votes)
+
+
+def _gather_voxels(grid, v, dst, group):
+    """A read-out (VoxelGridData) of every rank, concatenated in rank order on dst; None elsewhere."""
+    import torch.distributed as dist
+    from .volume import VoxelGridData
+    names = [k for k in ("points", "colors", "class_ids", "object_ids", "confidences") if getattr(v, k) is not None]
+    parts = {k: _gather_rows(getattr(v, k), dst, group, _on_device(group), grid.device) for k in names}
+    if dist.get_rank(group) != dst:
+        return None
+    out = VoxelGridData(np.concatenate(parts["points"]), np.concatenate(parts["colors"]))
+    for k in names[2:]:
+        setattr(out, k, np.concatenate(parts[k]))
+    return out
+
+
+def get_voxels_sharded(grid, min_count: int = 1, min_confidence: float = 0.0, dst: int = 0, group=None):
+    """`get_voxels` of a hash-sharded grid: every rank's voxels, rank-major on `dst` (the reference leaves the order
+    unspecified); None elsewhere."""
+    return _gather_voxels(grid, grid.get_voxels(min_count, min_confidence), dst, group)
+
+
+def get_voxels_in_bb_sharded(grid, bbox, min_count: int = 1, min_confidence: float = 0.0, dst: int = 0, group=None):
+    """`get_voxels_in_bb` of a hash-sharded grid, gathered like `get_voxels_sharded`."""
+    return _gather_voxels(grid, grid.get_voxels_in_bb(bbox, min_count, min_confidence), dst, group)
+
+
+def get_voxels_in_camera_frustrum_sharded(grid, camera_frustrum, min_count: int = 1, min_confidence: float = 0.0,
+                                          dst: int = 0, group=None):
+    """`get_voxels_in_camera_frustrum` of a hash-sharded grid, gathered like `get_voxels_sharded`."""
+    return _gather_voxels(grid, grid.get_voxels_in_camera_frustrum(camera_frustrum, min_count, min_confidence), dst,
+                          group)
+
+
+def _segments_sharded(grid, by_class, min_count, min_confidence, dst, group):
+    from .volume import segment_min_count, segments
+    v = get_voxels_sharded(grid, segment_min_count(min_count), min_confidence, dst, group)
+    return None if v is None else segments(v, by_class)
+
+
+def get_object_segments_sharded(grid, min_count: int = 1, min_confidence: float = 0.0, dst: int = 0, group=None):
+    """`get_object_segments` of a hash-sharded semantic grid: the voxels gathered on `dst`, then grouped there (same
+    ids, voxels and confidence ranges as the unsharded grid; the voxels of a segment come rank-major).  None
+    elsewhere."""
+    return _segments_sharded(grid, False, min_count, min_confidence, dst, group)
+
+
+def get_class_segments_sharded(grid, min_count: int = 1, min_confidence: float = 0.0, dst: int = 0, group=None):
+    """`get_class_segments` of a hash-sharded semantic grid, like `get_object_segments_sharded`."""
+    return _segments_sharded(grid, True, min_count, min_confidence, dst, group)
+
+
+def _all_sum(grid, x: int, group) -> int:
+    import torch
+    import torch.distributed as dist
+    dev = torch.device("cuda", grid.device) if _on_device(group) else torch.device("cpu")
+    t = torch.tensor([int(x)], dtype=torch.int64, device=dev)
+    dist.all_reduce(t, group=group)
+    return int(t.item())
+
+
+def num_blocks_sharded(grid, group=None) -> int:
+    """Blocks of a hash-sharded grid over all ranks (an all-reduce; the ranks' blocks are disjoint)."""
+    return _all_sum(grid, grid.num_blocks(), group)
+
+
+def size_sharded(grid, group=None) -> int:
+    """`size()` (non-empty voxels) of a hash-sharded grid over all ranks (an all-reduce)."""
+    return _all_sum(grid, grid.size(), group)

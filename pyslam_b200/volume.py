@@ -621,7 +621,8 @@ class _BlockGrid:
 
     _P = ""
 
-    def __init__(self, voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, *kind):
+    def __init__(self, voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count,
+                 *kind):
         self._L = _lib.load()
         self._h = C.c_void_p()
         self.voxel_size = float(voxel_size)
@@ -637,6 +638,8 @@ class _BlockGrid:
                 self._c("destroy")(self._h)
                 self._h = C.c_void_p()
             raise RuntimeError(f"{self._P}create failed (status {rc}): {msg}")
+        self.shard_rank, self.shard_count = 0, 1
+        self.set_shard(shard_rank, shard_count)
 
     def _c(self, name):
         """The grid's entry point `name` (without the prefix)."""
@@ -753,8 +756,17 @@ class _BlockGrid:
     def get_colors(self):
         return self.get_voxels(1).colors
 
+    def set_shard(self, shard_rank: int, shard_count: int):
+        """Hash sharding over `shard_count` ranks, like `B200TsdfVolume(shard_rank=, shard_count=)`: from now on the
+        grid keeps only the blocks with `BlockKeyHash(key) % shard_count == shard_rank` (`sharding.owner_of`).  Feed
+        every rank every frame; each rank then holds, voxel for voxel, the blocks of the unsharded grid it owns, and
+        the edits apply per rank.  `pyslam_b200.sharding` gathers the read-outs and runs the association.  Only on a
+        grid without blocks; raises otherwise, or for a bad rank or count, and changes nothing.  `clear` keeps it."""
+        self._check(self._c("set_shard")(self._h, int(shard_rank), int(shard_count)), self._P + "set_shard")
+        self.shard_rank, self.shard_count = int(shard_rank), int(shard_count)
+
     def clear(self):
-        """Empties the grid; grown storage is kept."""
+        """Empties the grid; grown storage and the shard setting are kept."""
         self._check(self._c("clear")(self._h), self._P + "clear")
 
     reset = clear
@@ -784,12 +796,12 @@ class VoxelBlockGrid(_BlockGrid):
     _P = "b2v_grid_"
 
     def __init__(self, voxel_size: float, block_size: int = 8, capacity_blocks: int = 1 << 17,
-                 device: int = 0, max_capacity_blocks: int | None = None):
+                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1):
         """`max_capacity_blocks`: growth ceiling of the block pool.  Above `capacity_blocks`, the pool starts with
         `capacity_blocks` blocks of storage and grows inside the integrate call that needs more; the grid then holds
         what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the
-        pool fixed."""
-        super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks)
+        pool fixed.  `shard_rank` / `shard_count`: see `set_shard`."""
+        super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count)
 
     def _stage_frame(self, images, labels, shape, filter_shadow_points, out):
         if labels[0] is not None or labels[1] is not None:
@@ -998,6 +1010,34 @@ class ClassDataGroup:
         self.class_ids = [c.class_id for c in classes]
 
 
+def segment_min_count(min_count: int) -> int:
+    """The `get_voxels` min_count of the segments' voxels: the reference keeps voxels with count > min_count (strict,
+    unlike get_voxels' >=) and confidence >= min_confidence; the GPU read-out (count -> scan -> emit) does the scan
+    and the compaction, `segments` the grouping."""
+    return int(min_count) + 1
+
+
+def segments(v: VoxelGridData, by_class: bool):
+    """The voxels of a semantic read-out grouped by object id (ObjectDataGroup) or class id (ClassDataGroup), ids < 0
+    dropped, stable: the read-out's order within a segment is kept (voxel_block_semantic_grid.hpp:204-316)."""
+    ids = np.asarray(v.class_ids if by_class else v.object_ids)
+    keep = ids >= 0                                   # negative = uninitialised label
+    pts, cols = np.asarray(v.points)[keep], np.asarray(v.colors)[keep]
+    cls, conf, ids = np.asarray(v.class_ids)[keep], np.asarray(v.confidences)[keep], ids[keep]
+    order = np.argsort(ids, kind="stable")
+    uniq, start = np.unique(ids[order], return_index=True)
+    bounds = list(start) + [len(order)]
+    out = []
+    for k, seg_id in enumerate(uniq):
+        sel = order[bounds[k]:bounds[k + 1]]
+        cmin, cmax = float(conf[sel].min()), float(conf[sel].max())
+        if by_class:
+            out.append(ClassData(int(seg_id), pts[sel], cols[sel], cmin, cmax))
+        else:
+            out.append(ObjectData(int(seg_id), int(cls[sel[0]]), pts[sel], cols[sel], cmin, cmax))
+    return ClassDataGroup(out) if by_class else ObjectDataGroup(out)
+
+
 class VoxelBlockSemanticGrid(_BlockGrid):
     """GPU drop-in for `volumetric.VoxelBlockSemanticGrid(voxel_size, block_size=8)` — per-voxel label
     *voting* (cpp/volumetric/voxel_block_semantic_grid.h:59-118; voxel_data_semantic.h:106-199).
@@ -1010,12 +1050,14 @@ class VoxelBlockSemanticGrid(_BlockGrid):
     _P = "b2v_sgrid_"
 
     def __init__(self, voxel_size: float = 0.05, block_size: int = 8, capacity_blocks: int = 1 << 14,
-                 device: int = 0, max_capacity_blocks: int | None = None):
+                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1):
         """`max_capacity_blocks`: growth ceiling (at most 2^22 blocks).  Above `capacity_blocks`, the per-voxel storage
         starts with `capacity_blocks` blocks and grows inside the integrate call that needs more; the grid then holds,
         bit for bit, what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or
-        `capacity_blocks`) keeps the storage fixed."""
-        super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, self.KIND)
+        `capacity_blocks`) keeps the storage fixed.  `shard_rank` / `shard_count`: see `set_shard`; the association
+        of a sharded grid runs over all ranks (`sharding.assign_object_ids_to_instance_ids_sharded`)."""
+        super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count,
+                         self.KIND)
 
     def _stage_frame(self, images, labels, shape, filter_shadow_points, out):
         return self._L.b2v_sgrid_set_frame(self._h, *images, *labels, shape[0], shape[1], filter_shadow_points, out)
@@ -1069,38 +1111,16 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         self.integrate(pts, cols, np.full(n, int(class_id), np.int32), np.full(n, int(object_id), np.int32))
 
     # ---- segments (voxel_block_semantic_grid.hpp:204-316) ----
-    def _segments(self, by_class: bool, min_count: int, min_confidence: float):
-        # the reference keeps voxels with count > min_count (strict, unlike get_voxels' >=) and confidence >=
-        # min_confidence: the GPU read-out (count -> scan -> emit) does the scan and the compaction ...
-        v = self.get_voxels(int(min_count) + 1, float(min_confidence))
-        ids = np.asarray(v.class_ids if by_class else v.object_ids)
-        keep = ids >= 0                                   # negative = uninitialised label
-        pts, cols = np.asarray(v.points)[keep], np.asarray(v.colors)[keep]
-        cls, conf, ids = np.asarray(v.class_ids)[keep], np.asarray(v.confidences)[keep], ids[keep]
-        # ... and the host groups the survivors by id (stable: block order within a segment is kept)
-        order = np.argsort(ids, kind="stable")
-        uniq, start = np.unique(ids[order], return_index=True)
-        bounds = list(start) + [len(order)]
-        out = []
-        for k, seg_id in enumerate(uniq):
-            sel = order[bounds[k]:bounds[k + 1]]
-            out.append((int(seg_id), pts[sel], cols[sel], int(cls[sel[0]]), float(conf[sel].min()),
-                        float(conf[sel].max())))
-        return out
-
     def get_object_segments(self, min_count: int = 1, min_confidence: float = 0.0):
         """`get_object_segments(min_count, min_confidence)` -> ObjectDataGroup (voxel_grid_data.h:64-96): voxels grouped
         by object id (ids < 0 dropped), each with its points / colours, the class id of its first voxel, the
         confidence range and a PCA oriented bounding box (bounding_boxes_3d.cpp:373-556, the reference's default
         OBBComputationMethod::PCA)."""
-        objs = [ObjectData(i, c, p, col, cmin, cmax) for i, p, col, c, cmin, cmax in
-                self._segments(False, min_count, min_confidence)]
-        return ObjectDataGroup(objs)
+        return segments(self.get_voxels(segment_min_count(min_count), float(min_confidence)), by_class=False)
 
     def get_class_segments(self, min_count: int = 1, min_confidence: float = 0.0):
         """`get_class_segments(min_count, min_confidence)` -> ClassDataGroup (voxel_grid_data.h:110-140)."""
-        return ClassDataGroup([ClassData(i, p, col, cmin, cmax) for i, p, col, _c, cmin, cmax in
-                               self._segments(True, min_count, min_confidence)])
+        return segments(self.get_voxels(segment_min_count(min_count), float(min_confidence)), by_class=True)
 
     def integrate_rgbd(self, depth, color, K, Twc, class_image=None, object_image=None, max_depth=np.inf,
                        min_depth=0.0, use_depths=True, filter_shadow_points=False):
@@ -1200,16 +1220,28 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         voxel_semantic_data_association.h:69-373): 2-D instance id -> 3-D object id (-1: no confident match).
         Soft failures (empty / wrongly sized label images) return an empty map like the reference (:80-103).  The
         images may be those of a staged frame (`set_frame`)."""
-        hw = (camera_frustrum.height, camera_frustrum.width)
+        hold = []
+        imgs = self._assoc_images((camera_frustrum.height, camera_frustrum.width), class_ids_image,
+                                  semantic_instances_image, depth_image, hold)
+        if imgs is None:
+            return {}
+        K, T = camera_frustrum._args()
+        n = self._L.b2v_sgrid_assign_object_ids_to_instance_ids(
+            self._h, K.ctypes.data, camera_frustrum.width, camera_frustrum.height, T.ctypes.data,
+            camera_frustrum.depth_max, camera_frustrum.depth_min, *imgs,
+            float(depth_threshold), 1 if do_carving else 0, float(min_vote_ratio), int(min_votes))
+        return self._instance_map(n)
 
+    def _assoc_images(self, hw, class_ids_image, semantic_instances_image, depth_image, hold):
+        """(class, instance, depth or None) image pointers of an association of [H,W] = `hw` images, or None (printed)
+        when the label images are empty or wrongly sized, a soft failure like the reference's (:80-103)."""
         def arr(a):
             return a if isinstance(a, DeviceImage) else np.asarray(a)
 
         ci, ii = arr(class_ids_image), arr(semantic_instances_image)
         if not np.prod(ci.shape) or not np.prod(ii.shape) or ci.shape != hw or ii.shape != hw:
             print("volumetric::assign_object_ids_to_instance_ids: label images are empty or have the wrong size")
-            return {}
-        hold = []
+            return None
         cp, _, _ = _image_arg(self, ci, np.int32, hold)
         ip, _, _ = _image_arg(self, ii, np.int32, hold)
         dp = None
@@ -1217,11 +1249,10 @@ class VoxelBlockSemanticGrid(_BlockGrid):
             d = arr(depth_image)
             if np.prod(d.shape) and d.shape == hw:
                 dp, _, _ = _image_arg(self, d, np.float32, hold)
-        K, T = camera_frustrum._args()
-        n = self._L.b2v_sgrid_assign_object_ids_to_instance_ids(
-            self._h, K.ctypes.data, camera_frustrum.width, camera_frustrum.height, T.ctypes.data,
-            camera_frustrum.depth_max, camera_frustrum.depth_min, cp, ip, dp,
-            float(depth_threshold), 1 if do_carving else 0, float(min_vote_ratio), int(min_votes))
+        return cp, ip, dp
+
+    def _instance_map(self, n) -> dict:
+        """The map an association call left (its return value `n`: size or -1) as a dict."""
         if n < 0:
             raise RuntimeError(self._L.b2v_sgrid_last_error(self._h).decode())
         ids, objs = np.zeros(n, np.int32), np.zeros(n, np.int32)
