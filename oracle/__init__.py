@@ -17,11 +17,13 @@ legs may import this package; the product (`pyslam_b200/`) never does.
 * `numpy_tsdf`  - a second, independent numpy restatement of A.3 used to pin the C oracle.
 * `numpy_point_cloud` - numpy restatement of the documented ExtractPointCloud formulas (DESIGN §3) on a block dump.
 * `numpy_grid`  - numpy restatement of the point-average `VoxelBlockGrid` (keys, sums, queries, carve).
+* `numpy_semantic_grid` - plain Python / numpy restatement of both semantic block grids (label voting, Bayesian label
+                  fusion with the kernel's 8-slot eviction, read-outs, edits, carve, instance association).
 * `numpy_shadow_filter` - numpy restatement of the reference's `filter_shadow_points` (median threshold).
 """
 
 from .oracle import (EigenOps, Open3DOrderVolume, have_eigen_ops, open3d_order_inverse4, RefGrid, RefSemanticGrid, TsdfOracle, build, canonical_mesh, have_ref, have_ref_semantic, numpy_grid, numpy_integrate_block,
-                     numpy_point_cloud, numpy_shadow_filter, numpy_touched_blocks, ref_block_key_hash, ref_floor_div, ref_keys)
+                     numpy_point_cloud, numpy_semantic_grid, numpy_shadow_filter, numpy_touched_blocks, ref_block_key_hash, ref_floor_div, ref_keys)
 
 __all__ = ["EigenOps", "have_eigen_ops", "open3d_order_inverse4", "Open3DOrderVolume", "RefGrid", "RefSemanticGrid", "TsdfOracle", "build", "canonical_mesh", "have_ref", "have_ref_semantic", "numpy_grid", "numpy_integrate_block",
-           "numpy_point_cloud", "numpy_shadow_filter", "numpy_touched_blocks", "ref_block_key_hash", "ref_floor_div", "ref_keys"]
+           "numpy_point_cloud", "numpy_semantic_grid", "numpy_shadow_filter", "numpy_touched_blocks", "ref_block_key_hash", "ref_floor_div", "ref_keys"]

@@ -644,9 +644,15 @@ class numpy_grid:
     @staticmethod
     def project(points, K, W, H, Tcw, depth_max, depth_min):
         """CameraFrustrum::contains on float32 points -> (inside, u, v, depth) with u, v, depth float32."""
+        return numpy_grid.project64(np.asarray(points, np.float32).astype(np.float64), K, W, H, Tcw, depth_max,
+                                    depth_min)
+
+    @staticmethod
+    def project64(points, K, W, H, Tcw, depth_max, depth_min):
+        """`project` on float64 points (the semantic grids' float64 means)."""
         fx, fy, cx, cy = [np.float64(np.float32(v)) for v in K]
         T = np.asarray(Tcw, np.float64).reshape(4, 4)
-        p = np.asarray(points, np.float32).astype(np.float64)
+        p = np.asarray(points, np.float64).reshape(-1, 3)
         pc = [((T[a, 0] * p[:, 0] + T[a, 1] * p[:, 1]) + T[a, 2] * p[:, 2]) + T[a, 3] for a in range(3)]
         depth = pc[2].astype(np.float32)
         with np.errstate(divide="ignore", invalid="ignore"):
@@ -678,6 +684,426 @@ class numpy_grid:
         self.pos[gone] = 0
         self.col[gone] = 0
         return gone
+
+
+class numpy_semantic_grid:
+    """The semantic block grids `VoxelBlockSemanticGrid` (kind="voting") and `VoxelBlockSemanticProbabilisticGrid`
+    (kind="probabilistic") of b2v_semantic.cu restated voxel by voxel in plain Python / numpy.  Every float32
+    operation is one np.float32 operation; exp and log are evaluated in float64 and rounded to float32.
+
+    keys       as numpy_grid (voxel_hashing.h:69-75, voxel_block_grid.hpp:473); a block exists once a point lands in it
+               and holds 512 voxels in the cleared state: count 0, sums 0, object = class = -1, counter 0, no label
+               slots, ml_logp = -inf, confidence 0
+    per point  in input order (voxel_block_grid.hpp:12-112, 220-288, 524-614):
+                 labels (below) when the call has class ids AND colours (no colours: positions only, hpp:228-231);
+                 the object id is the instance id, or 0 without instance ids (hpp:259-286)
+                 pos_sum += float64(x) (voxel_data.h:53-57); col_sum += c in float32, c = float32 colour or
+                 float32(u8) * float32(1/255) (voxel_data.h:79-90); count += 1
+    voting     (voxel_data_semantic.h:153-198) an observation with depth >= depth_threshold is ignored; otherwise
+               count == 0: take the label, counter = 1; same label: counter += 1; other label: counter -= 1 and at
+               counter <= 0 take the label with counter = 1.  confidence = min(1, float32(counter) / float32(count))
+               (:117-132), 0 for an empty voxel
+    Bayesian   (voxel_data_semantic.h:312-451) evidence w = -log(0.9) as float32 (:287) for depth <= depth_threshold or
+               no depth, else float32(exp(float32(-(depth - threshold)) * rate)) * -log(0.9).
+               count == 0: slot[label] = w, argmax = label, ml_logp = w.  Known label: slot += w; if it is the argmax
+               ml_logp follows it, else it takes the argmax only when strictly larger than ml_logp (ties keep the
+               earlier label).  New label: slot = w, argmax when w > ml_logp.
+               The reference keeps a std::map; the kernel keeps 8 slots in insertion order.  A ninth distinct label
+               replaces the slot with the least evidence that is not the argmax (the first such slot on ties) and
+               counts one label overflow: the kernel's own rule, not the reference's.
+               confidence (:561-570, 607-624): 0 when the argmax has a -1 id or there is no slot, else
+               exp(ml_logp - logsumexp) with the sum folded over the slots in ascending (object, class) order by
+               log_add_exp(a, b) = m + log(exp(a - m) + exp(b - m)), m = max(a, b) (:626-635); evaluated for every
+               voxel a labelled call touched, at the end of the call
+    read-outs  count >= min_count and confidence >= min_confidence (voxel_block_grid.hpp:797-803); mean position
+               pos_sum / float64(count), mean colour col_sum / float32(count) (voxel_data.h:58-69, 98-109).  Box
+               (hpp:822-1016) and frustum (:1019-1195, 1336-1460): count >= 1, the key bounds and the fine test of
+               numpy_grid on the float64 mean
+    edits      applied to every voxel of every block, empty ones included (voxel_block_grid.hpp:625-647,
+               voxel_block_semantic_grid.hpp:101-183): remove_low_count_voxels(n) resets count < n;
+               remove_low_confidence_segments(int n) resets confidence < float32(n); remove_segment(id) resets
+               object == id; merge_segments(a, b) gives every voxel with object == b the object a, and a Bayesian voxel
+               then holds the single slot (a, class) with evidence 0, ml_logp 0 and confidence 1 when a >= 0 and
+               class >= 0, else no slot, ml_logp -inf and confidence 0 (set_object_id, voxel_data_semantic.h:135,
+               455-460, 589-605).  -1 is also the object id of every empty voxel.  Reset = the cleared state.
+    carve      voxel_grid_carving.h:47-80, as numpy_grid.carve
+    association  assign_object_ids_to_instance_ids (voxel_semantic_data_association.h:69-373): every voxel in the
+               frustum looks up its truncated pixel; skipped when the pixel's class < 0, the voxel's class < 0 or
+               differs, the pixel's instance < 0, or (with a depth image) the image depth is <= 0 or not finite;
+               with carving, depth < image - thr resets the voxel; depth > image + thr is skipped.  A voxel without
+               object id takes object 0 at once for instance 0, else is pending.  Each remaining voxel votes
+               (instance -> its object).  Instances with pending voxels get new object ids in ascending instance
+               order (the reference: block-iteration order), the pending votes count for them.  Winner per instance:
+               the most votes, the lowest object id on ties (:287-320); -1 when total < min_votes or
+               float32(max) / float32(total) < min_vote_ratio.  Every pixel with instance >= 0 and class >= 0 adds
+               its instance with -1 if absent, and instance 0 maps to 0 (:322-352).  Pending voxels whose instance
+               won an id >= 0 take it (:354-370).
+    `dump()` has the layout of `sort_dump(grid.dump_blocks(8))` without the hashes: `aux` is the voting counter or the
+    number of slots, `lab_*` the slots in ascending (object, class) order padded with (-1, -1, -inf); dump_blocks never
+    shows the kernel's stale slots past `aux`.  The class neither loads nor calls the CUDA library."""
+
+    MAX_LABELS = 8
+    BASE_LOG = np.float32(0.10536051565782628)   # voxel_data_semantic.h:287
+
+    def __init__(self, voxel_size, kind="voting"):
+        assert kind in ("voting", "probabilistic")
+        self.bayes = kind == "probabilistic"
+        self.inv_vs = np.float32(1.0) / np.float32(voxel_size)
+        self.depth_threshold = np.float32(5.0 if self.bayes else 10.0)   # voxel_data_semantic.h:107-108, 251-254
+        self.depth_decay_rate = np.float32(0.07)
+        self.next_object_id = 1
+        self.clear()
+
+    def set_depth_threshold(self, v):
+        self.depth_threshold = np.float32(v)
+
+    def set_depth_decay_rate(self, v):
+        if self.bayes:
+            self.depth_decay_rate = np.float32(v)
+
+    def set_next_object_id(self, v):
+        self.next_object_id = int(v)
+
+    def clear(self):
+        self.block_of = {}                      # block key -> row of the arrays below
+        self.keys = np.zeros((0, 3), np.int64)
+        self.count = np.zeros((0, 512), np.int64)
+        self.pos = np.zeros((0, 512, 3), np.float64)
+        self.col = np.zeros((0, 512, 3), np.float32)
+        self.obj = np.zeros((0, 512), np.int32)
+        self.cls = np.zeros((0, 512), np.int32)
+        self.counter = np.zeros((0, 512), np.int32)
+        self.ml_logp = np.zeros((0, 512), np.float32)
+        self.conf = np.zeros((0, 512), np.float32)
+        self.slots = {}                         # (row, voxel) -> [[object, class, float32 evidence], ...]
+        self.label_overflows = 0
+
+    def _add_blocks(self, block_keys):
+        new = [k for k in dict.fromkeys(map(tuple, block_keys.tolist())) if k not in self.block_of]
+        if not new:
+            return
+        for k in new:
+            self.block_of[k] = len(self.block_of)
+        m = len(new)
+        self.keys = np.concatenate([self.keys, np.array(new, np.int64).reshape(m, 3)])
+        self.count = np.concatenate([self.count, np.zeros((m, 512), np.int64)])
+        self.pos = np.concatenate([self.pos, np.zeros((m, 512, 3), np.float64)])
+        self.col = np.concatenate([self.col, np.zeros((m, 512, 3), np.float32)])
+        self.obj = np.concatenate([self.obj, np.full((m, 512), -1, np.int32)])
+        self.cls = np.concatenate([self.cls, np.full((m, 512), -1, np.int32)])
+        self.counter = np.concatenate([self.counter, np.zeros((m, 512), np.int32)])
+        self.ml_logp = np.concatenate([self.ml_logp, np.full((m, 512), -np.inf, np.float32)])
+        self.conf = np.concatenate([self.conf, np.zeros((m, 512), np.float32)])
+
+    # ---- float32 helpers ----
+    @staticmethod
+    def _exp(x):
+        return np.float32(np.exp(np.float64(x)))
+
+    @staticmethod
+    def _log(x):
+        return np.float32(np.log(np.float64(x)))
+
+    @classmethod
+    def _log_add_exp(cls, a, b):
+        if a == -np.inf:
+            return b
+        if b == -np.inf:
+            return a
+        m = max(a, b)
+        return np.float32(m + cls._log(np.float32(cls._exp(np.float32(a - m)) + cls._exp(np.float32(b - m)))))
+
+    def _confidence_of(self, slots, obj, cls, ml):
+        if obj == -1 or cls == -1 or not slots:
+            return np.float32(0.0)
+        total = np.float32(-np.inf)
+        for _, _, lp in sorted(slots, key=lambda s: (s[0], s[1])):
+            total = self._log_add_exp(total, lp)
+        return self._exp(np.float32(ml - total))
+
+    def _weight(self, depth):
+        if depth is None or depth <= self.depth_threshold:
+            return self.BASE_LOG
+        e = self._exp(np.float32(np.float32(-np.float32(depth - self.depth_threshold)) * self.depth_decay_rate))
+        return np.float32(e * self.BASE_LOG)
+
+    # ---- integrate ----
+    def integrate(self, points, colors=None, class_ids=None, instance_ids=None, depths=None):
+        p = np.asarray(points)
+        assert p.dtype in (np.float32, np.float64) and p.ndim == 2 and p.shape[1] == 3
+        n = len(p)
+        if n == 0:
+            return
+        inv = np.float64(self.inv_vs) if p.dtype == np.float64 else self.inv_vs
+        vk = np.floor(p * inv).astype(np.int64)
+        bk = vk // 8
+        self._add_blocks(bk)
+        lk = vk - bk * 8
+        local = (lk[:, 0] + 8 * lk[:, 1] + 64 * lk[:, 2]).tolist()
+        rows = [self.block_of[k] for k in map(tuple, bk.tolist())]
+        c = None
+        if colors is not None:
+            c = np.asarray(colors)
+            c = c.astype(np.float32) * (np.float32(1.0) / np.float32(255.0)) if c.dtype == np.uint8 else \
+                c.astype(np.float32)
+        semantics = class_ids is not None and c is not None
+        assert instance_ids is None or class_ids is not None
+        oc = None if class_ids is None else np.asarray(class_ids, np.int32).tolist()
+        oo = None if instance_ids is None else np.asarray(instance_ids, np.int32).tolist()
+        dep = None if depths is None else np.asarray(depths, np.float32)
+        p64 = p.astype(np.float64)
+        touched = set()
+        for i in range(n):
+            b, l = rows[i], local[i]
+            if semantics:
+                label = (oo[i] if oo is not None else 0, oc[i])
+                d = None if dep is None else dep[i]
+                if self.bayes:
+                    self._observe_bayes(b, l, label, d)
+                    touched.add((b, l))
+                else:
+                    self._observe_vote(b, l, label, d)
+            self.pos[b, l] += p64[i]
+            if c is not None:
+                self.col[b, l] += c[i]
+            self.count[b, l] += 1
+        for b, l in touched:
+            self.conf[b, l] = self._confidence_of(self.slots.get((b, l), []), self.obj[b, l], self.cls[b, l],
+                                                  self.ml_logp[b, l])
+
+    def integrate_segment(self, points, colors, class_id, object_id):
+        """voxel_block_semantic_grid.hpp:52-99: one label for every point; a negative id skips the segment."""
+        n = len(points)
+        if class_id < 0 or object_id < 0 or n == 0:
+            return
+        self.integrate(points, colors, np.full(n, class_id, np.int32), np.full(n, object_id, np.int32))
+
+    def _observe_vote(self, b, l, label, depth):
+        if depth is not None and not depth < self.depth_threshold:
+            return
+        if self.count[b, l] == 0:
+            self.obj[b, l], self.cls[b, l], self.counter[b, l] = label[0], label[1], 1
+        elif (self.obj[b, l], self.cls[b, l]) == label:
+            self.counter[b, l] += 1
+        else:
+            self.counter[b, l] -= 1
+            if self.counter[b, l] <= 0:
+                self.obj[b, l], self.cls[b, l], self.counter[b, l] = label[0], label[1], 1
+
+    def _observe_bayes(self, b, l, label, depth):
+        w = self._weight(depth)
+        slots = self.slots.setdefault((b, l), [])
+        arg = (int(self.obj[b, l]), int(self.cls[b, l]))
+        k = next((q for q, s in enumerate(slots) if (s[0], s[1]) == label), None)
+        if self.count[b, l] == 0:
+            if k is None:
+                slots.append([label[0], label[1], w])
+            else:
+                slots[k][2] = w
+            self.obj[b, l], self.cls[b, l], self.ml_logp[b, l] = label[0], label[1], w
+        elif k is not None:
+            slots[k][2] = np.float32(slots[k][2] + w)
+            if label == arg:
+                self.ml_logp[b, l] = slots[k][2]
+            elif slots[k][2] > self.ml_logp[b, l]:
+                self.obj[b, l], self.cls[b, l], self.ml_logp[b, l] = label[0], label[1], slots[k][2]
+        else:
+            if len(slots) < self.MAX_LABELS:
+                slots.append([label[0], label[1], w])
+            else:
+                weakest = None
+                for q, s in enumerate(slots):
+                    if (s[0], s[1]) != arg and (weakest is None or s[2] < slots[weakest][2]):
+                        weakest = q
+                slots[weakest] = [label[0], label[1], w]
+                self.label_overflows += 1
+            if w > self.ml_logp[b, l]:
+                self.obj[b, l], self.cls[b, l], self.ml_logp[b, l] = label[0], label[1], w
+
+    # ---- read-outs ----
+    def confidence(self):
+        """[nb, 512] float32: the read-out confidence of every voxel."""
+        if self.bayes:
+            return np.where(self.count > 0, self.conf, np.float32(0.0)).astype(np.float32)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            q = self.counter.astype(np.float32) / self.count.astype(np.float32)
+        return np.where(self.count > 0, np.minimum(np.float32(1.0), q), np.float32(0.0)).astype(np.float32)
+
+    def _voxel_keys(self):
+        l = np.arange(512)
+        return self.keys[:, None, :] * 8 + np.stack([l % 8, (l // 8) % 8, l // 64], 1)[None]
+
+    def _means(self):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            return self.pos / self.count.astype(np.float64)[..., None]
+
+    def _collect(self, sel):
+        c = self.count[sel]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            pts = np.where(c[:, None] > 0, self.pos[sel] / c.astype(np.float64)[:, None], 0.0)
+            cols = np.where(c[:, None] > 0, self.col[sel] / c.astype(np.float32)[:, None], np.float32(0.0))
+        return dict(points=pts, colors=cols.astype(np.float32), class_ids=self.cls[sel], object_ids=self.obj[sel],
+                    confidences=self.confidence()[sel])
+
+    def _keep(self, min_count, min_confidence):
+        return (self.count >= min_count) & (self.confidence() >= np.float32(min_confidence))
+
+    def get_voxels(self, min_count=1, min_confidence=0.0):
+        return self._collect(self._keep(min_count, min_confidence))
+
+    def _in_bounds(self, bb):
+        bb = np.asarray(bb, np.float64)
+        lo = np.floor(bb[:3] * np.float64(self.inv_vs)).astype(np.int64)
+        hi = np.floor(bb[3:] * np.float64(self.inv_vs)).astype(np.int64)
+        vk = self._voxel_keys()
+        return (self.count >= 1) & np.all((vk >= lo) & (vk <= hi), axis=-1)
+
+    def _in_box(self, bbox):
+        bb = np.asarray(bbox, np.float64).reshape(6)
+        m = self._means()
+        with np.errstate(invalid="ignore"):
+            return self._in_bounds(bb) & np.all((m >= bb[:3]) & (m <= bb[3:]), axis=-1)
+
+    def _in_frustum(self, K, W, H, Tcw, depth_max, depth_min):
+        """(inside [nb,512], u, v, depth [nb,512] float32)."""
+        sel = self._in_bounds(numpy_grid.frustum_bounds(K, W, H, Tcw, depth_max, depth_min))
+        ok, u, v, depth = numpy_grid.project64(self._means().reshape(-1, 3), K, W, H, Tcw, depth_max, depth_min)
+        shape = self.count.shape
+        return sel & ok.reshape(shape), u.reshape(shape), v.reshape(shape), depth.reshape(shape)
+
+    def get_voxels_in_bb(self, bbox, min_count=1, min_confidence=0.0):
+        return self._collect(self._keep(min_count, min_confidence) & self._in_box(bbox))
+
+    def get_voxels_in_camera_frustrum(self, K, W, H, Tcw, depth_max, depth_min, min_count=1, min_confidence=0.0):
+        return self._collect(self._keep(min_count, min_confidence) &
+                             self._in_frustum(K, W, H, Tcw, depth_max, depth_min)[0])
+
+    # ---- edits ----
+    def _reset(self, sel):
+        self.count[sel] = 0
+        self.pos[sel] = 0
+        self.col[sel] = 0
+        self.obj[sel] = -1
+        self.cls[sel] = -1
+        self.counter[sel] = 0
+        self.ml_logp[sel] = -np.inf
+        self.conf[sel] = 0
+        for b, l in zip(*np.nonzero(sel)):
+            self.slots.pop((int(b), int(l)), None)
+
+    def remove_low_count_voxels(self, min_count):
+        self._reset(self.count < int(min_count))
+
+    def remove_low_confidence_segments(self, min_confidence):
+        self._reset(self.confidence() < np.float32(int(min_confidence)))
+
+    def remove_segment(self, object_id):
+        self._reset(self.obj == int(object_id))
+
+    def _set_object_id(self, sel, object_id):
+        self.obj[sel] = object_id
+        if not self.bayes:
+            return
+        for b, l in zip(*np.nonzero(sel)):
+            b, l = int(b), int(l)
+            if object_id >= 0 and self.cls[b, l] >= 0:
+                self.slots[(b, l)] = [[object_id, int(self.cls[b, l]), np.float32(0.0)]]
+                self.ml_logp[b, l], self.conf[b, l] = 0.0, 1.0
+            else:
+                self.slots.pop((b, l), None)
+                self.ml_logp[b, l], self.conf[b, l] = -np.inf, 0.0
+
+    def merge_segments(self, a, b):
+        self._set_object_id(self.obj == int(b), int(a))
+
+    def carve(self, K, W, H, Tcw, depth_max, depth_min, depth_image, depth_threshold):
+        ok, u, v, depth = self._in_frustum(K, W, H, Tcw, depth_max, depth_min)
+        img = np.zeros(ok.shape, np.float32)
+        img[ok] = np.asarray(depth_image, np.float32)[v[ok].astype(np.int64), u[ok].astype(np.int64)]
+        with np.errstate(invalid="ignore"):
+            self._reset(ok & (img > 0) & np.isfinite(img) & (depth < img - np.float32(depth_threshold)))
+
+    def assign_object_ids_to_instance_ids(self, K, W, H, Tcw, depth_max, depth_min, class_image, instance_image,
+                                          depth_image=None, depth_threshold=0.1, do_carving=False, min_vote_ratio=0.5,
+                                          min_votes=3):
+        ci, ii = np.asarray(class_image, np.int32), np.asarray(instance_image, np.int32)
+        di = None if depth_image is None else np.asarray(depth_image, np.float32)
+        thr = np.float32(depth_threshold)
+        ok, u, v, depth = self._in_frustum(K, W, H, Tcw, depth_max, depth_min)
+        votes, pending, carved = {}, [], np.zeros(ok.shape, bool)
+        for b, l in zip(*np.nonzero(ok)):
+            r, c = int(v[b, l]), int(u[b, l])
+            if ci[r, c] < 0 or self.cls[b, l] < 0 or self.cls[b, l] != ci[r, c] or ii[r, c] < 0:
+                continue
+            inst, obj = int(ii[r, c]), int(self.obj[b, l])
+            if di is not None:
+                d = di[r, c]
+                if not (d > 0 and np.isfinite(d)):
+                    continue
+                if do_carving and depth[b, l] < np.float32(d - thr):
+                    carved[b, l] = True
+                    continue
+                if depth[b, l] > np.float32(d + thr):
+                    continue
+            if obj < 0:
+                if inst == 0:
+                    one = np.zeros(ok.shape, bool)
+                    one[b, l] = True
+                    self._set_object_id(one, 0)
+                    obj = 0
+                else:
+                    pending.append((b, l, inst))
+                    obj = None
+            per = votes.setdefault(inst, {})
+            per[obj] = per.get(obj, 0) + 1
+        self._reset(carved)
+        new_id = {}
+        for inst in sorted({inst for _, _, inst in pending}):
+            new_id[inst] = self.next_object_id
+            self.next_object_id += 1
+        result = {}
+        for inst in sorted(votes):
+            per = {}
+            for obj, cnt in votes[inst].items():
+                o = new_id[inst] if obj is None else obj
+                per[o] = per.get(o, 0) + cnt
+            best, winner, total = 0, -1, 0
+            for o in sorted(per):
+                total += per[o]
+                if per[o] > best:
+                    best, winner = per[o], o
+            low = total < int(min_votes) or np.float32(best) / np.float32(total) < np.float32(min_vote_ratio)
+            result[inst] = -1 if low else winner
+        for inst in np.unique(ii[(ii >= 0) & (ci >= 0)]).tolist():
+            if inst == 0:
+                result[0] = 0
+            else:
+                result.setdefault(inst, -1)
+        for b, l, inst in pending:
+            if result[inst] >= 0:
+                one = np.zeros(ok.shape, bool)
+                one[b, l] = True
+                self._set_object_id(one, result[inst])
+        return dict(sorted(result.items()))
+
+    def dump(self):
+        order = np.lexsort((self.keys[:, 2], self.keys[:, 1], self.keys[:, 0]))
+        nb, K = len(order), self.MAX_LABELS
+        lab_obj = np.full((nb, 512, K), -1, np.int32)
+        lab_cls = np.full((nb, 512, K), -1, np.int32)
+        lab_logp = np.full((nb, 512, K), -np.inf, np.float32)
+        aux = self.counter.copy()
+        if self.bayes:
+            aux[:] = 0
+            for (b, l), slots in self.slots.items():
+                aux[b, l] = len(slots)
+                for k, (o, c, lp) in enumerate(sorted(slots, key=lambda s: (s[0], s[1]))):
+                    lab_obj[b, l, k], lab_cls[b, l, k], lab_logp[b, l, k] = o, c, lp
+        conf = self.conf if self.bayes else self.confidence()
+        d = dict(keys=self.keys.astype(np.int32), count=self.count.astype(np.int32), pos_sum=self.pos,
+                 col_sum=self.col, object_id=self.obj, class_id=self.cls, confidence=conf, aux=aux,
+                 lab_obj=lab_obj, lab_cls=lab_cls, lab_logp=lab_logp)
+        return {k: a[order].copy() for k, a in d.items()}
 
 
 def numpy_shadow_filter(depth, delta_x=2, delta_y=2, fill_value=-1.0):

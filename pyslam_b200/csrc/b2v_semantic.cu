@@ -20,8 +20,8 @@
 //
 // Bayesian labels: the reference keeps a std::map<(object, class), float> per voxel (typically 1-5 entries);
 // here a voxel has kSemLabels = 8 fixed slots.  A ninth distinct pair evicts the slot with the least evidence
-// that is not the current argmax and bumps the overflow counter (b2v_sgrid_label_overflows) - a documented
-// deviation that no test or reference KAT reaches.
+// that is not the current argmax (the first on ties) and bumps the overflow counter (b2v_sgrid_label_overflows) - a
+// documented deviation no reference KAT reaches; tests/test_gpu_semantic_edges.py checks the evicted slot.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 
