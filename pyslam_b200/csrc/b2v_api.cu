@@ -101,6 +101,17 @@ bool b2v::is_device_pointer(const void *p) {
 namespace {
 // staging and texel slots: slot buf * kMaxGroup + k holds frame k of the group in group buffer buf
 constexpr int kStage = kGroupBufs * kMaxGroup;
+
+// Slot s of a staging buffer, `per_frame` elements per slot at the pitch of the current frame; the buffers are
+// reserved for kStage slots of the largest frame so far.  A slot's address thus moves with the frame size.  That is
+// safe because enqueue_frames drains the device whenever H x W changes (cudaDeviceSynchronize, then resolve_skipped,
+// before it rewrites the lambda image), so no kernel in flight and no pending replay holds a slot address at the old
+// pitch.
+template <typename T> T *stage_slot(const DeviceBuffer<T> &b, size_t per_frame, int s) {
+    return b.get() + per_frame * static_cast<size_t>(s);
+}
+// texels per slot: the image + the out-of-image texel at index H * W, rounded up to 256 bytes
+size_t texel_pitch(size_t pixels) { return (pixels + 32) & ~static_cast<size_t>(31); }
 }  // namespace
 
 struct b2v_volume {
@@ -119,27 +130,28 @@ struct b2v_volume {
     cudaEvent_t ev_ready[kGroupBufs] = {}, ev_galloc[kGroupBufs] = {}, ev_group_done[kGroupBufs] = {};
     int64_t prof_frames = 0, prof_int_launches = 0;
     // optional rectification stage (b2v_set_rectification)
-    float *d_mapx = nullptr, *d_mapy = nullptr;
+    DeviceBuffer<float> d_mapx, d_mapy;
     int rect_H = 0, rect_W = 0, rect_swap = 0;
-    float *d_rdepth[kStage] = {};    // rectified frames (same slot layout as the raw staging)
-    uint8_t *d_rcolor[kStage] = {};
+    DeviceBuffer<float> d_rdepth;    // rectified frames (same slots as the raw staging)
+    DeviceBuffer<uint8_t> d_rcolor;
     // TMA descriptors are cached per image address (encoding costs ~1 us of host time each)
     std::unordered_map<uintptr_t, FrameMaps> map_cache;
     int map_H = 0, map_W = 0;
     // raw 16-bit depth input (b2v_integrate_u16 / b2v_integrate_batch_u16): uploaded as is, widened on the device
-    uint16_t *d_depth16[kStage] = {};   // same slot layout as d_depth; allocated on first use
-    size_t stage16_pixels = 0;
+    DeviceBuffer<uint16_t> d_depth16;   // same slots as d_depth; allocated on first use
     float in_u16_scale = 0.0f;          // > 0 while a *_u16 entry point runs: `depth` pointers are uint16_t
-    float *d_depth[kStage] = {};
-    uint8_t *d_color[kStage] = {};
-    Texel *d_tex[kStage] = {};      // texel images, written by the allocate kernels and read by the update kernels
-    float *d_lambda = nullptr;      // lambda image of the cached intrinsics, read by the update kernels
+    DeviceBuffer<float> d_depth;        // staging of host frames (and of widened uint16 depth), see stage_slot
+    DeviceBuffer<uint8_t> d_color;
+    DeviceBuffer<Texel> d_tex;      // texel images, written by the allocate kernels and read by the update kernels
+    DeviceBuffer<float> d_lambda;   // lambda image of the cached intrinsics, read by the update kernels
     double lam_K[4] = {0, 0, 0, 0};
     int lam_H = 0, lam_W = 0;
-    size_t stage_pixels = 0;
-    HashTable table{};
+    HashTable table{};                   // the kernels' views of the buffers below
     PoolMeta meta{};
     UnitSet units{};                     // group unit sets of the fused allocation, one per group buffer
+    DeviceBuffer<uint4> table_mem, unit_entries;
+    DeviceBuffer<int4> block_keys;
+    DeviceBuffer<uint32_t> counters, group_mask, union_slots, block_flags, unit_list;
     // The pool is one virtual-address reservation for meta.capacity blocks; physical chunks are mapped as it grows
     // (fixed volumes map it whole at create), so the pool address the kernels see never changes.
     bool growable = false;               // max_capacity_blocks > capacity_blocks
@@ -154,10 +166,14 @@ struct b2v_volume {
     int64_t launches = 0;
     uint32_t *h_counters = nullptr;  // pinned mirror
     std::string err;
-    // mesh / point-cloud extraction
+    // mesh / point-cloud extraction: mb is the kernels' view of the buffers in `mesh`
     MeshBuffers mb{};
-    uint32_t mesh_blocks_cap = 0;
-    size_t mesh_v_cap = 0, mesh_t_cap = 0;
+    struct {
+        DeviceBuffer<int32_t> nbr, edge_ids, triangles;
+        DeviceBuffer<uint8_t> cube;
+        DeviceBuffer<uint32_t> edge_mask, local, sums, offs, partials, totals, work;
+        DeviceBuffer<double> vertices, colors;
+    } mesh;
     int64_t last_nv = 0, last_nt = 0;
     uint32_t *h_totals = nullptr;
     // sharded extraction (b2v_extract_*_with_halo): an unsharded scratch volume holding this volume's blocks at the
@@ -266,6 +282,8 @@ bool b2v::vmm_map(VmmRange *r, size_t bytes, cudaStream_t stream, std::string *e
     return true;
 }
 
+b2v::VmmRange::~VmmRange() { vmm_release(this); }
+
 void b2v::vmm_release(VmmRange *r) {
     const VmmApi *api = vmm_api();
     if (!api || !r->va) return;
@@ -292,8 +310,6 @@ static int pool_map(b2v_volume *v, uint64_t blocks) {
     return B2V_OK;
 }
 
-static void pool_release(b2v_volume *v) { vmm_release(&v->pool); }
-
 // growth policy: at least double, at least `need` blocks, at most the maximum
 static int pool_grow(b2v_volume *v, uint64_t need) {
     const uint32_t old = v->meta.pool_capacity;
@@ -317,12 +333,12 @@ extern "C" int b2v_version(void) { return 104; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
-    unsigned long long *d = nullptr, h[2] = {0, 0};
-    if (cudaMalloc(&d, sizeof(h)) != cudaSuccess) return B2V_ERR_CUDA;
-    cudaError_t e = cudaMemset(d, 0, sizeof(h));
-    if (e == cudaSuccess) e = launch_selftest_division(d, pairs, nullptr);
-    if (e == cudaSuccess) e = cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(d);
+    DeviceBuffer<unsigned long long> d;
+    unsigned long long h[2] = {0, 0};
+    cudaError_t e = d.reserve(2);
+    if (e == cudaSuccess) e = cudaMemset(d.get(), 0, sizeof(h));
+    if (e == cudaSuccess) e = launch_selftest_division(d.get(), pairs, nullptr);
+    if (e == cudaSuccess) e = cudaMemcpy(h, d.get(), sizeof(h), cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) return B2V_ERR_CUDA;
     if (bad_reciprocals) *bad_reciprocals = h[0];
     if (bad_quotients) *bad_quotients = h[1];
@@ -392,7 +408,8 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     const uint32_t tcap = next_pow2(static_cast<uint64_t>(cap) * 2);
     v->table.mask = tcap - 1;
     v->meta.capacity = cap;
-    B2V_CUDA(v, cudaMalloc(&v->table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
+    B2V_CUDA(v, v->table_mem.reserve(tcap));
+    v->table.entries = v->table_mem.get();
     {
         int rc = pool_reserve(v);
         if (rc == B2V_OK) rc = pool_map(v, cfg->capacity_blocks);
@@ -401,11 +418,16 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     }
     B2V_CUDA(v, cudaMallocHost(&v->h_skip, kGroupBufs * sizeof(uint32_t)));
     std::memset(v->h_skip, 0, kGroupBufs * sizeof(uint32_t));
-    B2V_CUDA(v, cudaMalloc(&v->meta.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.counters, kNumCounters * sizeof(uint32_t)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.group_mask, static_cast<size_t>(tcap) * kGroupBufs * sizeof(uint32_t)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.union_slots, static_cast<size_t>(cap) * kGroupBufs * sizeof(uint32_t)));
-    B2V_CUDA(v, cudaMalloc(&v->meta.block_flags, static_cast<size_t>(cap) * sizeof(uint32_t)));
+    B2V_CUDA(v, v->block_keys.reserve(cap));
+    B2V_CUDA(v, v->counters.reserve(kNumCounters));
+    B2V_CUDA(v, v->group_mask.reserve(static_cast<size_t>(tcap) * kGroupBufs));
+    B2V_CUDA(v, v->union_slots.reserve(static_cast<size_t>(cap) * kGroupBufs));
+    B2V_CUDA(v, v->block_flags.reserve(cap));
+    v->meta.block_keys = v->block_keys.get();
+    v->meta.counters = v->counters.get();
+    v->meta.group_mask = v->group_mask.get();
+    v->meta.union_slots = v->union_slots.get();
+    v->meta.block_flags = v->block_flags.get();
     {
         // Group unit sets: 2^16 entries (1 MB) per group buffer, L2-resident.  The largest union of 32-frame groups
         // on the bench configs is ~2.6 k 16^3 units on C2 (~21 k under decision D1's 8^3 units); units that find no
@@ -417,8 +439,10 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
             if (n >= 1 && n <= (1l << 24) && (n & (n - 1)) == 0) entries = static_cast<uint32_t>(n);
         }
         v->units.mask = entries - 1;
-        B2V_CUDA(v, cudaMalloc(&v->units.entries, static_cast<size_t>(entries) * kGroupBufs * sizeof(uint4)));
-        B2V_CUDA(v, cudaMalloc(&v->units.list, static_cast<size_t>(entries) * kGroupBufs * sizeof(uint32_t)));
+        B2V_CUDA(v, v->unit_entries.reserve(static_cast<size_t>(entries) * kGroupBufs));
+        B2V_CUDA(v, v->unit_list.reserve(static_cast<size_t>(entries) * kGroupBufs));
+        v->units.entries = v->unit_entries.get();
+        v->units.list = v->unit_list.get();
     }
     B2V_CUDA(v, cudaMemsetAsync(v->meta.block_flags, 0, static_cast<size_t>(cap) * sizeof(uint32_t), v->compute));
     B2V_CUDA(v, cudaMallocHost(&v->h_counters, kNumCounters * sizeof(uint32_t)));
@@ -446,43 +470,12 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     cudaSetDevice(v->cfg.device);
     cudaDeviceSynchronize();
     if (v->ev_in) cudaEventDestroy(v->ev_in);
-    cudaFree(v->d_depth[0]);  // slots 1.. point into the same three allocations
-    cudaFree(v->d_color[0]);
-    cudaFree(v->d_tex[0]);
-    cudaFree(v->d_lambda);
-    cudaFree(v->d_mapx);
-    cudaFree(v->d_mapy);
-    cudaFree(v->d_rdepth[0]);
-    cudaFree(v->d_rcolor[0]);
-    cudaFree(v->d_depth16[0]);
     for (int b = 0; b < kGroupBufs; ++b) {
         if (v->ev_ready[b]) cudaEventDestroy(v->ev_ready[b]);
         if (v->ev_galloc[b]) cudaEventDestroy(v->ev_galloc[b]);
         if (v->ev_group_done[b]) cudaEventDestroy(v->ev_group_done[b]);
     }
-    cudaFree(v->meta.group_mask);
-    cudaFree(v->meta.union_slots);
-    cudaFree(v->meta.block_flags);
-    cudaFree(v->units.entries);
-    cudaFree(v->units.list);
-    cudaFree(v->table.entries);
-    pool_release(v);
     cudaFreeHost(v->h_skip);
-    cudaFree(v->meta.block_keys);
-    cudaFree(v->meta.counters);
-    cudaFree(v->mb.nbr);
-    cudaFree(v->mb.cube);
-    cudaFree(v->mb.edge_mask);
-    cudaFree(v->mb.local);
-    cudaFree(v->mb.sums);
-    cudaFree(v->mb.offs);
-    cudaFree(v->mb.work);
-    cudaFree(v->mb.totals);
-    cudaFree(v->mb.partials);
-    cudaFree(v->mb.vertices);
-    cudaFree(v->mb.colors);
-    cudaFree(v->mb.edge_ids);
-    cudaFree(v->mb.triangles);
     cudaFreeHost(v->h_counters);
     cudaFreeHost(v->h_totals);
     for (cudaEvent_t e : v->prof_events)
@@ -582,48 +575,28 @@ extern "C" int b2v_reset(b2v_volume *v) {
 
 // Raw staging, texel images and the lambda image for frames of up to `pixels` pixels.
 static int ensure_staging(b2v_volume *v, size_t pixels) {
-    if (pixels <= v->stage_pixels) return B2V_OK;
-    // the texel and lambda images freed below are read by update kernels on the library's streams and on callers'
-    B2V_CUDA(v, cudaDeviceSynchronize());
-    if (v->growable) {  // and by the replay of skipped groups
-        const int rc = resolve_skipped(v);
-        if (rc == B2V_ERR_CUDA) return rc;
+    // the lambda image is reserved last, so it is short whenever a buffer below that holds memory is reallocated
+    if (v->d_lambda.size() <= pixels) {
+        // the texel and lambda images are read by update kernels on the library's streams and on callers'
+        B2V_CUDA(v, cudaDeviceSynchronize());
+        if (v->growable) {  // and by the replay of skipped groups
+            const int rc = resolve_skipped(v);
+            if (rc == B2V_ERR_CUDA) return rc;
+        }
+        v->lam_H = v->lam_W = 0;
     }
-    // slots are carved out of contiguous allocations, so the frames of a group (which are contiguous in the caller's
-    // arrays) upload with ONE copy per image type
-    cudaFree(v->d_depth[0]);
-    cudaFree(v->d_color[0]);
-    cudaFree(v->d_tex[0]);
-    for (int s = 0; s < kStage; ++s) {
-        v->d_depth[s] = nullptr;
-        v->d_color[s] = nullptr;
-        v->d_tex[s] = nullptr;
+    // the slots of a buffer are contiguous, so the frames of a group (which are contiguous in the caller's arrays)
+    // upload with ONE copy per image type
+    B2V_CUDA(v, v->d_depth.reserve(pixels * kStage));
+    B2V_CUDA(v, v->d_color.reserve(pixels * 3 * kStage));
+    const size_t texels = texel_pitch(pixels) * kStage;
+    if (texels > v->d_tex.size()) {   // zeroed once, here
+        B2V_CUDA(v, v->d_tex.reserve(texels));
+        B2V_CUDA(v, cudaMemsetAsync(v->d_tex.get(), 0, texels * sizeof(Texel), v->compute));
+        B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     }
-    v->stage_pixels = 0;  // stays 0 if an allocation below fails
-    float *dbase = nullptr;
-    uint8_t *cbase = nullptr;
-    Texel *tbase = nullptr;
-    B2V_CUDA(v, cudaMalloc(&dbase, pixels * sizeof(float) * kStage));
-    v->d_depth[0] = dbase;
-    B2V_CUDA(v, cudaMalloc(&cbase, pixels * 3 * kStage));
-    v->d_color[0] = cbase;
-    // a texel slot holds the image + the out-of-image texel (zeroed once, here), rounded up to 256 bytes
-    const size_t tex_pitch = (pixels + 32) & ~static_cast<size_t>(31);
-    B2V_CUDA(v, cudaMalloc(&tbase, tex_pitch * sizeof(Texel) * kStage));
-    v->d_tex[0] = tbase;
-    B2V_CUDA(v, cudaMemsetAsync(tbase, 0, tex_pitch * sizeof(Texel) * kStage, v->compute));
-    for (int s = 0; s < kStage; ++s) {
-        v->d_depth[s] = dbase + pixels * s;
-        v->d_color[s] = cbase + pixels * 3 * s;
-        v->d_tex[s] = tbase + tex_pitch * s;
-    }
-    cudaFree(v->d_lambda);
-    v->d_lambda = nullptr;
     // + the out-of-image element, which launch_lambda sets to kLambdaSentinel at index W * H of each image it writes
-    B2V_CUDA(v, cudaMalloc(&v->d_lambda, (pixels + 1) * sizeof(float)));
-    B2V_CUDA(v, cudaStreamSynchronize(v->compute));
-    v->lam_H = v->lam_W = 0;
-    v->stage_pixels = pixels;
+    B2V_CUDA(v, v->d_lambda.reserve(pixels + 1));
     return B2V_OK;
 }
 
@@ -655,18 +628,12 @@ static const FrameMaps *frame_maps(b2v_volume *v, const float *d_depth, const ui
 
 // raw uint16 staging, one contiguous allocation carved into the same slots as the float staging
 static int ensure_staging16(b2v_volume *v, size_t pixels) {
-    if (pixels <= v->stage16_pixels) return B2V_OK;
+    if (pixels * kStage <= v->d_depth16.size()) return B2V_OK;
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     B2V_CUDA(v, cudaStreamSynchronize(v->copy));
     B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
     if (v->last_stream) B2V_CUDA(v, cudaStreamSynchronize(v->last_stream));
-    cudaFree(v->d_depth16[0]);
-    for (int s = 0; s < kStage; ++s) v->d_depth16[s] = nullptr;
-    v->stage16_pixels = 0;
-    uint16_t *base = nullptr;
-    B2V_CUDA(v, cudaMalloc(&base, pixels * sizeof(uint16_t) * kStage));
-    for (int s = 0; s < kStage; ++s) v->d_depth16[s] = base + pixels * s;
-    v->stage16_pixels = pixels;
+    B2V_CUDA(v, v->d_depth16.reserve(pixels * kStage));
     return B2V_OK;
 }
 
@@ -675,15 +642,10 @@ extern "C" int b2v_set_rectification(b2v_volume *v, const float *map_x, const fl
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
     const int rc = read_counters(v);  // drains every stream
     if (rc == B2V_ERR_CUDA) return rc;
-    cudaFree(v->d_mapx);
-    cudaFree(v->d_mapy);
-    cudaFree(v->d_rdepth[0]);
-    cudaFree(v->d_rcolor[0]);
-    v->d_mapx = v->d_mapy = nullptr;
-    for (int s = 0; s < kStage; ++s) {
-        v->d_rdepth[s] = nullptr;
-        v->d_rcolor[s] = nullptr;
-    }
+    v->d_mapx = {};
+    v->d_mapy = {};
+    v->d_rdepth = {};
+    v->d_rcolor = {};
     v->rect_H = v->rect_W = 0;
     v->rect_swap = swap_rb;
     v->map_cache.clear();
@@ -693,18 +655,12 @@ extern "C" int b2v_set_rectification(b2v_volume *v, const float *map_x, const fl
         return B2V_ERR_INVALID_ARGUMENT;
     }
     const size_t pixels = static_cast<size_t>(height) * width;
-    B2V_CUDA(v, cudaMalloc(&v->d_mapx, pixels * sizeof(float)));
-    B2V_CUDA(v, cudaMalloc(&v->d_mapy, pixels * sizeof(float)));
-    B2V_CUDA(v, cudaMemcpy(v->d_mapx, map_x, pixels * sizeof(float), cudaMemcpyHostToDevice));
-    B2V_CUDA(v, cudaMemcpy(v->d_mapy, map_y, pixels * sizeof(float), cudaMemcpyHostToDevice));
-    float *dbase = nullptr;
-    uint8_t *cbase = nullptr;
-    B2V_CUDA(v, cudaMalloc(&dbase, pixels * sizeof(float) * kStage));
-    B2V_CUDA(v, cudaMalloc(&cbase, pixels * 3 * kStage));
-    for (int s = 0; s < kStage; ++s) {
-        v->d_rdepth[s] = dbase + pixels * s;
-        v->d_rcolor[s] = cbase + pixels * 3 * s;
-    }
+    B2V_CUDA(v, v->d_mapx.reserve(pixels));
+    B2V_CUDA(v, v->d_mapy.reserve(pixels));
+    B2V_CUDA(v, cudaMemcpy(v->d_mapx.get(), map_x, pixels * sizeof(float), cudaMemcpyHostToDevice));
+    B2V_CUDA(v, cudaMemcpy(v->d_mapy.get(), map_y, pixels * sizeof(float), cudaMemcpyHostToDevice));
+    B2V_CUDA(v, v->d_rdepth.reserve(pixels * kStage));
+    B2V_CUDA(v, v->d_rcolor.reserve(pixels * 3 * kStage));
     v->rect_H = height;
     v->rect_W = width;
     return B2V_OK;
@@ -717,40 +673,40 @@ extern "C" int b2v_remap(const void *src, int32_t kind, int32_t height, int32_t 
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
     const size_t pixels = static_cast<size_t>(height) * width;
     const size_t bytes = pixels * (kind == 0 ? 3 : 4);
-    void *d_src = nullptr, *d_dst = nullptr;
-    float *d_mx = nullptr, *d_my = nullptr;
-    cudaError_t e = cudaMalloc(&d_src, bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_dst, bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_mx, pixels * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&d_my, pixels * sizeof(float));
-    if (e == cudaSuccess) e = cudaMemcpy(d_src, src, bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d_mx, map_x, pixels * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d_my, map_y, pixels * sizeof(float), cudaMemcpyHostToDevice);
+    DeviceBuffer<uint8_t> d_src, d_dst;
+    DeviceBuffer<float> d_mx, d_my;
+    cudaError_t e = d_src.reserve(bytes);
+    if (e == cudaSuccess) e = d_dst.reserve(bytes);
+    if (e == cudaSuccess) e = d_mx.reserve(pixels);
+    if (e == cudaSuccess) e = d_my.reserve(pixels);
+    if (e == cudaSuccess) e = cudaMemcpy(d_src.get(), src, bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_mx.get(), map_x, pixels * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d_my.get(), map_y, pixels * sizeof(float), cudaMemcpyHostToDevice);
     if (e == cudaSuccess)
-        e = kind == 0 ? launch_remap_u8c3_linear(static_cast<const uint8_t *>(d_src), height, width, d_mx, d_my,
-                                                 static_cast<uint8_t *>(d_dst), swap_rb, nullptr)
-                      : launch_remap_b32_nearest(d_src, height, width, d_mx, d_my, d_dst, nullptr);
+        e = kind == 0 ? launch_remap_u8c3_linear(d_src.get(), height, width, d_mx.get(), d_my.get(), d_dst.get(),
+                                                 swap_rb, nullptr)
+                      : launch_remap_b32_nearest(d_src.get(), height, width, d_mx.get(), d_my.get(), d_dst.get(),
+                                                 nullptr);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(dst, d_dst, bytes, cudaMemcpyDeviceToHost);
-    cudaFree(d_src);
-    cudaFree(d_dst);
-    cudaFree(d_mx);
-    cudaFree(d_my);
+    if (e == cudaSuccess) e = cudaMemcpy(dst, d_dst.get(), bytes, cudaMemcpyDeviceToHost);
     return e == cudaSuccess ? B2V_OK : B2V_ERR_CUDA;
 }
 
 // rectify one frame (raw staging or caller device buffers -> rectified slot), on the allocate stream
 static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d_color, int H, int W, int slot,
                          cudaStream_t as) {
-    if (!v->d_mapx) return B2V_OK;
+    if (!v->d_mapx.get()) return B2V_OK;
     if (H != v->rect_H || W != v->rect_W) {
         v->err = "rectification maps were installed for a different image size";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    B2V_CUDA(v, launch_remap_b32_nearest(*d_depth, H, W, v->d_mapx, v->d_mapy, v->d_rdepth[slot], as));
-    B2V_CUDA(v, launch_remap_u8c3_linear(*d_color, H, W, v->d_mapx, v->d_mapy, v->d_rcolor[slot], v->rect_swap, as));
-    *d_depth = v->d_rdepth[slot];
-    *d_color = v->d_rcolor[slot];
+    const size_t pixels = static_cast<size_t>(H) * W;
+    float *depth = stage_slot(v->d_rdepth, pixels, slot);
+    uint8_t *color = stage_slot(v->d_rcolor, pixels * 3, slot);
+    B2V_CUDA(v, launch_remap_b32_nearest(*d_depth, H, W, v->d_mapx.get(), v->d_mapy.get(), depth, as));
+    B2V_CUDA(v, launch_remap_u8c3_linear(*d_color, H, W, v->d_mapx.get(), v->d_mapy.get(), color, v->rect_swap, as));
+    *d_depth = depth;
+    *d_color = color;
     v->launches += 2;
     return B2V_OK;
 }
@@ -797,7 +753,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             const int rc = resolve_skipped(v);
             if (rc == B2V_ERR_CUDA) return rc;
         }
-        B2V_CUDA(v, launch_lambda(P, v->d_lambda, as));
+        B2V_CUDA(v, launch_lambda(P, v->d_lambda.get(), as));
         std::memcpy(v->lam_K, K, sizeof(v->lam_K));
         v->lam_H = height;
         v->lam_W = width;
@@ -840,20 +796,21 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             // the group's frames are contiguous on both sides: one H2D copy per image type
             B2V_CUDA(v, cudaStreamWaitEvent(v->copy, v->ev_galloc[buf], 0));
             if (!dev_depth && u16)
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth16[s0], depth16 + pixels * g0, pixels * sizeof(uint16_t) * count,
-                                            cudaMemcpyHostToDevice, v->copy));
+                B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_depth16, pixels, s0), depth16 + pixels * g0,
+                                            pixels * sizeof(uint16_t) * count, cudaMemcpyHostToDevice, v->copy));
             else if (!dev_depth)
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_depth[s0], depth + pixels * g0, pixels * sizeof(float) * count,
-                                            cudaMemcpyHostToDevice, v->copy));
+                B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_depth, pixels, s0), depth + pixels * g0,
+                                            pixels * sizeof(float) * count, cudaMemcpyHostToDevice, v->copy));
             if (!dev_color)
-                B2V_CUDA(v, cudaMemcpyAsync(v->d_color[s0], color + pixels * 3 * g0, pixels * 3 * count,
-                                            cudaMemcpyHostToDevice, v->copy));
+                B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_color, pixels * 3, s0), color + pixels * 3 * g0,
+                                            pixels * 3 * count, cudaMemcpyHostToDevice, v->copy));
             B2V_CUDA(v, cudaEventRecord(v->ev_ready[buf], v->copy));
             B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_ready[buf], 0));
         }
         if (u16) {  // widen the group's raw depth into its (contiguous) float staging slots in one launch
-            const uint16_t *src = dev_depth ? depth16 + pixels * g0 : v->d_depth16[s0];
-            B2V_CUDA(v, launch_depth_u16_to_f32(src, v->d_depth[s0], pixels * count, v->in_u16_scale, as));
+            const uint16_t *src = dev_depth ? depth16 + pixels * g0 : stage_slot(v->d_depth16, pixels, s0);
+            B2V_CUDA(v, launch_depth_u16_to_f32(src, stage_slot(v->d_depth, pixels, s0), pixels * count,
+                                                v->in_u16_scale, as));
             v->launches += 1;
         }
         static thread_local GroupAllocArgs aargs;  // ~15 KB: keep it off the stack
@@ -865,20 +822,22 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         aargs.use_tma = 1;
         for (int k = 0; k < count; ++k) {
             const size_t f = static_cast<size_t>(g0 + k);
-            const float *d_depth = dev_depth && !u16 ? depth + pixels * f : v->d_depth[s0 + k];  // (widened) staging
-            const uint8_t *d_color = dev_color ? color + pixels * 3 * f : v->d_color[s0 + k];
+            // (widened) staging
+            const float *d_depth = dev_depth && !u16 ? depth + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
+            const uint8_t *d_color = dev_color ? color + pixels * 3 * f : stage_slot(v->d_color, pixels * 3, s0 + k);
+            Texel *tex = stage_slot(v->d_tex, texel_pitch(pixels), s0 + k);
             const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s0 + k, as);
             if (rc != B2V_OK) return rc;
             FrameParams P;
             fill_frame_params(&P, K, Tcw + 16 * f, height, width, v->geo);
             P.group_buf = buf;
-            P.I.tex = v->d_tex[s0 + k];
-            P.I.lam = v->d_lambda;
+            P.I.tex = tex;
+            P.I.lam = v->d_lambda.get();
             if (k == 0) aargs.P = P;
             aargs.pose[k] = P.pose;
             aargs.depth[k] = d_depth;
             aargs.color[k] = d_color;
-            aargs.tex[k] = v->d_tex[s0 + k];
+            aargs.tex[k] = tex;
             const FrameMaps *fm = frame_maps(v, d_depth, d_color, height, width);
             if (fm) aargs.maps[k] = *fm; else aargs.use_tma = 0;
             args.f[k] = P.I;
@@ -1111,12 +1070,11 @@ extern "C" int64_t b2v_dump_blocks(b2v_volume *v, int32_t *keys, uint64_t *hashe
         }
     }
     if (hashes) {
-        uint64_t *d_h = nullptr;
-        if (cudaMalloc(&d_h, nb * sizeof(uint64_t)) != cudaSuccess) return -1;
-        cudaError_t e = launch_block_hashes(v->meta.block_keys, d_h, nb, v->compute);
+        DeviceBuffer<uint64_t> d_h;
+        if (d_h.reserve(nb) != cudaSuccess) return -1;
+        cudaError_t e = launch_block_hashes(v->meta.block_keys, d_h.get(), nb, v->compute);
         if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-        if (e == cudaSuccess) e = cudaMemcpy(hashes, d_h, nb * sizeof(uint64_t), cudaMemcpyDeviceToHost);
-        cudaFree(d_h);
+        if (e == cudaSuccess) e = cudaMemcpy(hashes, d_h.get(), nb * sizeof(uint64_t), cudaMemcpyDeviceToHost);
         v->launches += 1;
         if (e != cudaSuccess) return -1;
     }
@@ -1151,21 +1109,20 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
     const size_t n = static_cast<size_t>(n_blocks);
     std::vector<int4> k4(n);
     for (size_t i = 0; i < n; ++i) k4[i] = make_int4(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2], 0);
-    int4 *d_k = nullptr;
-    float *d_v = nullptr;
-    uint32_t *d_i = nullptr;
-    cudaError_t e = cudaMalloc(&d_k, n * sizeof(int4));
-    if (e == cudaSuccess) e = cudaMalloc(&d_v, n * kBlockFloats * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&d_i, n * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_k, k4.data(), n * sizeof(int4), cudaMemcpyHostToDevice, v->compute);
+    DeviceBuffer<int4> d_k;
+    DeviceBuffer<float> d_v;
+    DeviceBuffer<uint32_t> d_i;
+    cudaError_t e = d_k.reserve(n);
+    if (e == cudaSuccess) e = d_v.reserve(n * kBlockFloats);
+    if (e == cudaSuccess) e = d_i.reserve(n);
     if (e == cudaSuccess)
-        e = cudaMemcpyAsync(d_v, voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice, v->compute);
+        e = cudaMemcpyAsync(d_k.get(), k4.data(), n * sizeof(int4), cudaMemcpyHostToDevice, v->compute);
     if (e == cudaSuccess)
-        e = launch_upload_blocks(d_k, d_v, static_cast<uint32_t>(n), d_i, v->table, v->meta, v->compute);
+        e = cudaMemcpyAsync(d_v.get(), voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice, v->compute);
+    if (e == cudaSuccess)
+        e = launch_upload_blocks(d_k.get(), d_v.get(), static_cast<uint32_t>(n), d_i.get(), v->table, v->meta,
+                                 v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    cudaFree(d_k);
-    cudaFree(d_v);
-    cudaFree(d_i);
     v->launches += 2;
     if (e != cudaSuccess) {
         v->err = std::string("b2v_upload_blocks: ") + cudaGetErrorString(e);
@@ -1210,13 +1167,12 @@ extern "C" int b2v_import_blocks_device(b2v_volume *v, int64_t n_blocks, const i
         const int rc = grow_for_blocks(v, n_blocks);
         if (rc == B2V_ERR_CUDA) return rc;
     }
-    uint32_t *d_i = nullptr;
-    cudaError_t e = cudaMalloc(&d_i, static_cast<size_t>(n_blocks) * sizeof(uint32_t));
+    DeviceBuffer<uint32_t> d_i;
+    cudaError_t e = d_i.reserve(static_cast<size_t>(n_blocks));
     if (e == cudaSuccess)
-        e = launch_upload_blocks(reinterpret_cast<const int4 *>(d_keys4), d_voxels, static_cast<uint32_t>(n_blocks), d_i,
-                                 v->table, v->meta, v->compute);
+        e = launch_upload_blocks(reinterpret_cast<const int4 *>(d_keys4), d_voxels, static_cast<uint32_t>(n_blocks),
+                                 d_i.get(), v->table, v->meta, v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    cudaFree(d_i);
     v->launches += 2;
     if (e != cudaSuccess) {
         v->err = std::string("b2v_import_blocks_device: ") + cudaGetErrorString(e);
@@ -1235,14 +1191,13 @@ extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys, int64_t m
     if (!keys) return n;
     if (static_cast<int64_t>(n) > max_keys) n = static_cast<uint32_t>(max_keys);
     if (n == 0) return 0;
-    int4 *d_k = nullptr;
-    if (cudaMalloc(&d_k, n * sizeof(int4)) != cudaSuccess) return -1;
+    DeviceBuffer<int4> d_k;
+    if (d_k.reserve(n) != cudaSuccess) return -1;
     std::vector<int4> tmp(n);
     const uint32_t *list = v->meta.union_slots + static_cast<size_t>(buf) * v->meta.capacity;
-    cudaError_t e = launch_gather_active_keys(v->table, list, n, d_k, v->compute);
+    cudaError_t e = launch_gather_active_keys(v->table, list, n, d_k.get(), v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    if (e == cudaSuccess) e = cudaMemcpy(tmp.data(), d_k, n * sizeof(int4), cudaMemcpyDeviceToHost);
-    cudaFree(d_k);
+    if (e == cudaSuccess) e = cudaMemcpy(tmp.data(), d_k.get(), n * sizeof(int4), cudaMemcpyDeviceToHost);
     v->launches += 1;
     if (e != cudaSuccess) return -1;
     for (uint32_t i = 0; i < n; ++i) {
@@ -1255,20 +1210,28 @@ extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys, int64_t m
 
 // ---- mesh / point cloud ---------------------------------------------------------------------
 
+// per-block scratch of the extraction for nb blocks
 static int ensure_mesh_scratch(b2v_volume *v, uint32_t nb) {
-    if (!v->mb.totals) B2V_CUDA(v, cudaMalloc(&v->mb.totals, kNumMeshTotals * sizeof(uint32_t)));
-    if (nb <= v->mesh_blocks_cap) return B2V_OK;
     const size_t n = nb;
-    B2V_CUDA(v, regrow(&v->mb.nbr, n * 8));
-    B2V_CUDA(v, regrow(&v->mb.cube, n * kVox));
-    B2V_CUDA(v, regrow(&v->mb.edge_mask, n * (kVox / 4)));
-    B2V_CUDA(v, regrow(&v->mb.local, n * kVox));
-    B2V_CUDA(v, regrow(&v->mb.sums, n * 2));
-    B2V_CUDA(v, regrow(&v->mb.offs, n * 2));
-    B2V_CUDA(v, regrow(&v->mb.partials, 2 * ((n + 1023) / 1024)));
-    B2V_CUDA(v, regrow(&v->mb.work, n * 4));
-    v->mesh_blocks_cap = nb;
+    auto &m = v->mesh;
+    B2V_CUDA(v, m.totals.reserve(kNumMeshTotals));
+    B2V_CUDA(v, m.nbr.reserve(n * 8));
+    B2V_CUDA(v, m.cube.reserve(n * kVox));
+    B2V_CUDA(v, m.edge_mask.reserve(n * (kVox / 4)));
+    B2V_CUDA(v, m.local.reserve(n * kVox));
+    B2V_CUDA(v, m.sums.reserve(n * 2));
+    B2V_CUDA(v, m.offs.reserve(n * 2));
+    B2V_CUDA(v, m.partials.reserve(2 * ((n + 1023) / 1024)));
+    B2V_CUDA(v, m.work.reserve(n * 4));
     return B2V_OK;
+}
+
+// the kernels' view of v->mesh for nb blocks
+static MeshBuffers mesh_view(const b2v_volume *v, uint32_t nb) {
+    const auto &m = v->mesh;
+    return MeshBuffers{nb, m.nbr.get(), m.cube.get(), m.edge_mask.get(), m.local.get(), m.sums.get(),
+                       m.offs.get(), m.partials.get(), m.totals.get(), m.work.get(), m.vertices.get(),
+                       m.colors.get(), m.edge_ids.get(), m.triangles.get()};
 }
 
 static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t *n_triangles) {
@@ -1277,7 +1240,7 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     const uint32_t nb = block_count(v);
     rc = ensure_mesh_scratch(v, nb);
     if (rc != B2V_OK) return rc;
-    v->mb.n_blocks = nb;
+    v->mb = mesh_view(v, nb);
     v->last_from_halo = false;
     cudaStream_t cs = v->compute;
     const int sms = v->sm_count;
@@ -1290,16 +1253,11 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     B2V_CUDA(v, cudaMemcpyAsync(v->h_totals, v->mb.totals, kNumMeshTotals * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs));
     B2V_CUDA(v, cudaStreamSynchronize(cs));
     const size_t nv = v->h_totals[kMtVertices], nt = v->h_totals[kMtTriangles];
-    if (nv > v->mesh_v_cap) {
-        B2V_CUDA(v, regrow(&v->mb.vertices, nv * 3));
-        B2V_CUDA(v, regrow(&v->mb.colors, nv * 3));
-        B2V_CUDA(v, regrow(&v->mb.edge_ids, nv * 4));
-        v->mesh_v_cap = nv;
-    }
-    if (nt > v->mesh_t_cap) {
-        B2V_CUDA(v, regrow(&v->mb.triangles, nt * 3));
-        v->mesh_t_cap = nt;
-    }
+    B2V_CUDA(v, v->mesh.vertices.reserve(nv * 3));
+    B2V_CUDA(v, v->mesh.colors.reserve(nv * 3));
+    B2V_CUDA(v, v->mesh.edge_ids.reserve(nv * 4));
+    B2V_CUDA(v, v->mesh.triangles.reserve(nt * 3));
+    v->mb = mesh_view(v, nb);
     B2V_CUDA(v, launch_mesh_vertices(v->meta, v->mb, v->geo.voxel_length, v->geo.unit_shift, !mesh, v->h_totals[kMtVertexBlocks], cs));
     if (mesh) B2V_CUDA(v, launch_mesh_triangles(v->mb, v->h_totals[kMtTriangleBlocks], cs));
     B2V_CUDA(v, cudaStreamSynchronize(cs));
@@ -1374,16 +1332,19 @@ extern "C" int b2v_export_halo_device(b2v_volume *v, int32_t world, int64_t *rec
         return B2V_ERR_UNSUPPORTED;
     }
     const uint64_t chunks = (n + 1023) / 1024;
-    uint32_t *d_counts = nullptr, *d_offs = nullptr, *d_part = nullptr, *d_tot = nullptr, *d_dest = nullptr;
+    DeviceBuffer<uint32_t> d_counts, d_offs, d_part, d_tot, d_dest;
     std::vector<uint32_t> dest(2 * (static_cast<size_t>(world) + 1));
     cudaStream_t cs = v->compute;
-    cudaError_t e = cudaMalloc(&d_counts, 2 * n * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_offs, 2 * n * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_part, 2 * chunks * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_tot, 2 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_dest, dest.size() * sizeof(uint32_t));
-    if (e == cudaSuccess) e = launch_halo_count(v->meta, nb, world, d_counts, d_offs, d_part, d_tot, d_dest, cs);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dest.data(), d_dest, dest.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
+    cudaError_t e = d_counts.reserve(2 * n);
+    if (e == cudaSuccess) e = d_offs.reserve(2 * n);
+    if (e == cudaSuccess) e = d_part.reserve(2 * chunks);
+    if (e == cudaSuccess) e = d_tot.reserve(2);
+    if (e == cudaSuccess) e = d_dest.reserve(dest.size());
+    if (e == cudaSuccess)
+        e = launch_halo_count(v->meta, nb, world, d_counts.get(), d_offs.get(), d_part.get(), d_tot.get(),
+                              d_dest.get(), cs);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(dest.data(), d_dest.get(), dest.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
     int out = B2V_OK;
     if (e == cudaSuccess) {
@@ -1397,16 +1358,11 @@ extern "C" int b2v_export_halo_device(b2v_volume *v, int32_t world, int64_t *rec
                 v->err = "b2v_export_halo_device: destination too small";
                 out = B2V_ERR_INVALID_ARGUMENT;
             } else {
-                e = launch_halo_emit(v->meta, nb, world, d_offs, d_headers, d_payload, cs);
+                e = launch_halo_emit(v->meta, nb, world, d_offs.get(), d_headers, d_payload, cs);
                 if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
             }
         }
     }
-    cudaFree(d_counts);
-    cudaFree(d_offs);
-    cudaFree(d_part);
-    cudaFree(d_tot);
-    cudaFree(d_dest);
     if (e != cudaSuccess) {
         v->err = std::string("b2v_export_halo_device: ") + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
@@ -1455,24 +1411,21 @@ static int extract_with_halo(b2v_volume *v, bool mesh, int64_t n_records, const 
     b2v_volume *h = v->halo;
     const uint32_t nr = static_cast<uint32_t>(n_records);
     cudaStream_t cs = h->compute;
-    uint32_t *d_sizes = nullptr, *d_offs = nullptr, *d_part = nullptr, *d_tot = nullptr;
+    DeviceBuffer<uint32_t> d_sizes, d_offs, d_part, d_tot;
     uint32_t head[2] = {nb + nr, 0u};   // the scratch's block count; its error flag after the import
-    cudaError_t e = cudaMalloc(&d_sizes, (nr ? nr : 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_offs, (nr ? nr : 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_part, ((nr + 1023) / 1024 + 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_tot, sizeof(uint32_t));
+    cudaError_t e = d_sizes.reserve(nr);
+    if (e == cudaSuccess) e = d_offs.reserve(nr);
+    if (e == cudaSuccess) e = d_part.reserve((nr + 1023) / 1024 + 1);
+    if (e == cudaSuccess) e = d_tot.reserve(1);
     if (e == cudaSuccess)
         e = cudaMemsetAsync(h->table.entries, 0xFF, (static_cast<size_t>(h->table.mask) + 1) * sizeof(uint4), cs);
     if (e == cudaSuccess) e = cudaMemsetAsync(h->meta.counters, 0, kNumCounters * sizeof(uint32_t), cs);
     if (e == cudaSuccess)
-        e = launch_halo_import(v->meta, nb, d_headers, d_payload, nr, d_sizes, d_offs, d_part, d_tot, h->table, h->meta, cs);
+        e = launch_halo_import(v->meta, nb, d_headers, d_payload, nr, d_sizes.get(), d_offs.get(), d_part.get(),
+                               d_tot.get(), h->table, h->meta, cs);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h->meta.counters + kCtrPool, &head[0], sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
     if (e == cudaSuccess) e = cudaMemcpyAsync(&head[1], h->meta.counters + kCtrError, sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-    cudaFree(d_sizes);
-    cudaFree(d_offs);
-    cudaFree(d_part);
-    cudaFree(d_tot);
     if (e != cudaSuccess) {
         v->err = std::string("halo import: ") + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
@@ -1567,34 +1520,34 @@ extern "C" int b2v_weld_mesh_device(int32_t device, int32_t n_pieces, const int6
     a.out_triangles = d_out_triangles;
     const uint32_t scap = next_pow2(std::max<uint64_t>(1024, 2 * nv));
     a.set.mask = scap - 1;
-    uint32_t *d_base = nullptr;
+    DeviceBuffer<uint4> set;
+    DeviceBuffer<uint32_t> first, slot_of, keep, newidx, partials, totals, d_base;
     uint32_t host_tot[2] = {0u, 0u};
     cudaStream_t cs = nullptr;
     const size_t n1 = nv ? nv : 1;
     cudaError_t e = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMalloc(&a.set.entries, static_cast<size_t>(scap) * sizeof(uint4));
-    if (e == cudaSuccess) e = cudaMalloc(&a.first, static_cast<size_t>(scap) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&a.slot_of, n1 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&a.keep, n1 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&a.newidx, n1 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&a.partials, ((n1 + 1023) / 1024) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&a.totals, 2 * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaMalloc(&d_base, base.size() * sizeof(uint32_t));
+    if (e == cudaSuccess) e = set.reserve(scap);
+    if (e == cudaSuccess) e = first.reserve(scap);
+    if (e == cudaSuccess) e = slot_of.reserve(n1);
+    if (e == cudaSuccess) e = keep.reserve(n1);
+    if (e == cudaSuccess) e = newidx.reserve(n1);
+    if (e == cudaSuccess) e = partials.reserve((n1 + 1023) / 1024);
+    if (e == cudaSuccess) e = totals.reserve(2);
+    if (e == cudaSuccess) e = d_base.reserve(base.size());
     if (e == cudaSuccess)
-        e = cudaMemcpyAsync(d_base, base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
-    a.vbase = d_base;
-    a.tbase = d_base + n_pieces + 1;
+        e = cudaMemcpyAsync(d_base.get(), base.data(), base.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
+    a.set.entries = set.get();
+    a.first = first.get();
+    a.slot_of = slot_of.get();
+    a.keep = keep.get();
+    a.newidx = newidx.get();
+    a.partials = partials.get();
+    a.totals = totals.get();
+    a.vbase = d_base.get();
+    a.tbase = d_base.get() + n_pieces + 1;
     if (e == cudaSuccess) e = launch_weld(a, cs);
     if (e == cudaSuccess) e = cudaMemcpyAsync(host_tot, a.totals, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-    cudaFree(a.set.entries);
-    cudaFree(a.first);
-    cudaFree(a.slot_of);
-    cudaFree(a.keep);
-    cudaFree(a.newidx);
-    cudaFree(a.partials);
-    cudaFree(a.totals);
-    cudaFree(d_base);
     if (cs) cudaStreamDestroy(cs);
     if (e != cudaSuccess) {
         g_weld_err = std::string("b2v_weld_mesh_device: ") + cudaGetErrorString(e);
@@ -1618,21 +1571,18 @@ extern "C" int b2v_filter_shadow_points(const float *depth, int32_t height, int3
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
     const size_t pixels = static_cast<size_t>(height) * width;
     const bool din = is_device_pointer(depth), dout = is_device_pointer(out);
-    float *d_in = nullptr, *d_out = nullptr;
-    void *scratch = nullptr;
-    cudaError_t e = cudaMalloc(&scratch, kShadowScratchBytes);
+    DeviceBuffer<float> d_in, d_out;
+    DeviceBuffer<uint8_t> scratch;
+    cudaError_t e = scratch.reserve(kShadowScratchBytes);
     if (e == cudaSuccess && !din) {
-        e = cudaMalloc(&d_in, pixels * sizeof(float));
-        if (e == cudaSuccess) e = cudaMemcpy(d_in, depth, pixels * sizeof(float), cudaMemcpyHostToDevice);
+        e = d_in.reserve(pixels);
+        if (e == cudaSuccess) e = cudaMemcpy(d_in.get(), depth, pixels * sizeof(float), cudaMemcpyHostToDevice);
     }
-    if (e == cudaSuccess && !dout) e = cudaMalloc(&d_out, pixels * sizeof(float));
+    if (e == cudaSuccess && !dout) e = d_out.reserve(pixels);
     if (e == cudaSuccess)
-        e = launch_filter_shadow_points(din ? depth : d_in, height, width, delta_x, delta_y, fill_value,
-                                        dout ? out : d_out, scratch, nullptr);
+        e = launch_filter_shadow_points(din ? depth : d_in.get(), height, width, delta_x, delta_y, fill_value,
+                                        dout ? out : d_out.get(), scratch.get(), nullptr);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e == cudaSuccess && !dout) e = cudaMemcpy(out, d_out, pixels * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(scratch);
-    cudaFree(d_in);
-    cudaFree(d_out);
+    if (e == cudaSuccess && !dout) e = cudaMemcpy(out, d_out.get(), pixels * sizeof(float), cudaMemcpyDeviceToHost);
     return e == cudaSuccess ? B2V_OK : B2V_ERR_CUDA;
 }

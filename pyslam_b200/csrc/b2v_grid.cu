@@ -309,10 +309,13 @@ int BlockGridCore::create(double voxel_size, uint32_t capacity_blocks, uint32_t 
     B2V_CUDA(this, cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     const uint32_t tcap = next_pow2(static_cast<uint64_t>(cap) * 2);
     table.mask = tcap - 1;
-    B2V_CUDA(this, cudaMalloc(&table.entries, static_cast<size_t>(tcap) * sizeof(uint4)));
-    B2V_CUDA(this, cudaMalloc(&index.block_keys, static_cast<size_t>(cap) * sizeof(int4)));
-    B2V_CUDA(this, cudaMalloc(&index.counters, kBgNumCounters * sizeof(uint32_t)));
-    B2V_CUDA(this, cudaMalloc(&d_total, sizeof(uint32_t)));
+    B2V_CUDA(this, table_mem.reserve(tcap));
+    B2V_CUDA(this, block_keys.reserve(cap));
+    B2V_CUDA(this, counters.reserve(kBgNumCounters));
+    B2V_CUDA(this, d_total.reserve(1));
+    table.entries = table_mem.get();
+    index.block_keys = block_keys.get();
+    index.counters = counters.get();
     B2V_CUDA(this, cudaMallocHost(&h_counters, kBgNumCounters * sizeof(uint32_t)));
     return B2V_OK;
 }
@@ -320,9 +323,6 @@ int BlockGridCore::create(double voxel_size, uint32_t capacity_blocks, uint32_t 
 void BlockGridCore::destroy() {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
-    void *ptrs[] = {table.entries, index.block_keys, index.counters, d_sums, d_offs, d_total};
-    for (void *p : ptrs) cudaFree(p);
-    free_frame();
     cudaFreeHost(h_counters);
     if (stream) cudaStreamDestroy(stream);
 }
@@ -377,19 +377,18 @@ int BlockGridCore::clear_index() {
 }
 
 int BlockGridCore::ensure_scan(uint32_t n_blocks) {
-    if (n_blocks <= scan_cap) return B2V_OK;
-    B2V_CUDA(this, regrow(&d_sums, static_cast<size_t>(n_blocks) * 2));
-    B2V_CUDA(this, regrow(&d_offs, static_cast<size_t>(n_blocks) * 2));
-    scan_cap = n_blocks * 2;
+    // room for twice the blocks, so a growing map rarely reallocates
+    if (n_blocks > d_sums.size()) B2V_CUDA(this, d_sums.reserve(static_cast<size_t>(n_blocks) * 2));
+    if (n_blocks > d_offs.size()) B2V_CUDA(this, d_offs.reserve(static_cast<size_t>(n_blocks) * 2));
     return B2V_OK;
 }
 
 cudaError_t BlockGridCore::scan_total(uint32_t n_blocks, uint32_t *total) {
     *total = 0;
     if (n_blocks == 0) return cudaSuccess;
-    exclusive_scan_kernel<<<1, 1024, 0, stream>>>(d_sums, d_offs, d_total, n_blocks);
+    exclusive_scan_kernel<<<1, 1024, 0, stream>>>(d_sums.get(), d_offs.get(), d_total.get(), n_blocks);
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(total, d_total, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(total, d_total.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
     return e;
 }
@@ -470,31 +469,19 @@ int BlockGridCore::stage_input(const char *fn, int H, int W, bool filter_shadow_
     B2V_CUDA(this, cudaSetDevice(device));
     const size_t pixels = static_cast<size_t>(H) * W;
     auto on_host = [](auto **p) { return p && *p && !is_device_pointer(*p); };
-    if ((filter_shadow_points || on_host(depth) || on_host(rgb)) && pixels > input.pixels) {
-        B2V_CUDA(this, cudaStreamSynchronize(stream));
-        void **bufs[] = {reinterpret_cast<void **>(&input.depth), reinterpret_cast<void **>(&input.filtered),
-                         reinterpret_cast<void **>(&input.rgb), &input.shadow_scratch};
-        for (void **b : bufs) {
-            cudaFree(*b);
-            *b = nullptr;
-        }
-        input.pixels = 0;   // stays 0 if an allocation below fails
-        B2V_CUDA(this, cudaMalloc(&input.depth, pixels * sizeof(float)));
-        B2V_CUDA(this, cudaMalloc(&input.filtered, pixels * sizeof(float)));
-        B2V_CUDA(this, cudaMalloc(&input.rgb, pixels * 3));
-        B2V_CUDA(this, cudaMalloc(&input.shadow_scratch, kShadowScratchBytes));
-        input.pixels = pixels;
+    // Each group below synchronises when the last buffer it reserves is short: that buffer only ever held what
+    // the ones before it were reserved for, so no buffer that holds memory is reallocated without the wait.
+    if (filter_shadow_points || on_host(depth) || on_host(rgb)) {
+        if (pixels * 3 > input.rgb.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+        B2V_CUDA(this, input.depth.reserve(pixels));
+        B2V_CUDA(this, input.filtered.reserve(pixels));
+        B2V_CUDA(this, input.shadow_scratch.reserve(kShadowScratchBytes));
+        B2V_CUDA(this, input.rgb.reserve(pixels * 3));
     }
-    if ((on_host(cls) || on_host(obj)) && pixels > input.label_pixels) {
-        B2V_CUDA(this, cudaStreamSynchronize(stream));
-        int32_t **bufs[] = {&input.cls, &input.obj};
-        for (int32_t **b : bufs) {
-            cudaFree(*b);
-            *b = nullptr;
-        }
-        input.label_pixels = 0;
-        for (int32_t **b : bufs) B2V_CUDA(this, cudaMalloc(b, pixels * sizeof(int32_t)));
-        input.label_pixels = pixels;
+    if (on_host(cls) || on_host(obj)) {
+        if (pixels > input.obj.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+        B2V_CUDA(this, input.cls.reserve(pixels));
+        B2V_CUDA(this, input.obj.reserve(pixels));
     }
     cudaError_t e = cudaSuccess;
     auto upload = [&](auto **p, void *buf, size_t bytes) {
@@ -502,28 +489,20 @@ int BlockGridCore::stage_input(const char *fn, int H, int W, bool filter_shadow_
         e = cudaMemcpyAsync(buf, *p, bytes, cudaMemcpyHostToDevice, stream);
         *p = static_cast<std::remove_reference_t<decltype(*p)>>(buf);
     };
-    upload(depth, input.depth, pixels * sizeof(float));
-    upload(rgb, input.rgb, pixels * 3);
-    upload(cls, input.cls, pixels * sizeof(int32_t));
-    upload(obj, input.obj, pixels * sizeof(int32_t));
+    upload(depth, input.depth.get(), pixels * sizeof(float));
+    upload(rgb, input.rgb.get(), pixels * 3);
+    upload(cls, input.cls.get(), pixels * sizeof(int32_t));
+    upload(obj, input.obj.get(), pixels * sizeof(int32_t));
     if (e == cudaSuccess && filter_shadow_points) {
-        e = launch_filter_shadow_points(*depth, H, W, 2, 2, -1.0f, input.filtered, input.shadow_scratch, stream);
-        *depth = input.filtered;
+        e = launch_filter_shadow_points(*depth, H, W, 2, 2, -1.0f, input.filtered.get(), input.shadow_scratch.get(),
+                                        stream);
+        *depth = input.filtered.get();
     }
     if (e != cudaSuccess) {
         err = std::string(fn) + ": " + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
     }
     return B2V_OK;
-}
-
-void BlockGridCore::free_frame() {
-    void *ptrs[] = {frame.mapx, frame.mapy, frame.raw, frame.depth, frame.filtered, frame.rgb, frame.shadow_scratch,
-                    frame.cls, frame.inst, frame.obj, input.depth, input.filtered, input.rgb, input.shadow_scratch,
-                    input.cls, input.obj};
-    for (void *p : ptrs) cudaFree(p);
-    frame = FrameStage{};
-    input = InputStage{};
 }
 
 int BlockGridCore::set_rectification(const float *map_x, const float *map_y, int H, int W, int swap_rb) {
@@ -533,17 +512,16 @@ int BlockGridCore::set_rectification(const float *map_x, const float *map_y, int
     }
     B2V_CUDA(this, cudaSetDevice(device));
     B2V_CUDA(this, cudaStreamSynchronize(stream));
-    cudaFree(frame.mapx);
-    cudaFree(frame.mapy);
-    frame.mapx = frame.mapy = nullptr;
+    frame.mapx = {};
+    frame.mapy = {};
     frame.map_h = frame.map_w = 0;
     frame.swap_rb = swap_rb;
     if (!map_x || !map_y) return B2V_OK;
-    const size_t bytes = static_cast<size_t>(H) * W * sizeof(float);
-    B2V_CUDA(this, cudaMalloc(&frame.mapx, bytes));
-    B2V_CUDA(this, cudaMalloc(&frame.mapy, bytes));
-    B2V_CUDA(this, cudaMemcpy(frame.mapx, map_x, bytes, cudaMemcpyDefault));
-    B2V_CUDA(this, cudaMemcpy(frame.mapy, map_y, bytes, cudaMemcpyDefault));
+    const size_t pixels = static_cast<size_t>(H) * W;
+    B2V_CUDA(this, frame.mapx.reserve(pixels));
+    B2V_CUDA(this, frame.mapy.reserve(pixels));
+    B2V_CUDA(this, cudaMemcpy(frame.mapx.get(), map_x, pixels * sizeof(float), cudaMemcpyDefault));
+    B2V_CUDA(this, cudaMemcpy(frame.mapy.get(), map_y, pixels * sizeof(float), cudaMemcpyDefault));
     frame.map_h = H;
     frame.map_w = W;
     return B2V_OK;
@@ -556,7 +534,7 @@ int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scal
     if (!depth || !color || !out || H <= 0 || W <= 0) bad = "set_frame: bad arguments";
     else if (depth_u16 && !(depth_scale > 0.0f)) bad = "set_frame: uint16 depth needs a positive depth_scale";
     else if (inst && !cls) bad = "set_frame: an instance image needs a class image";
-    else if (frame.mapx && (H != frame.map_h || W != frame.map_w))
+    else if (frame.mapx.get() && (H != frame.map_h || W != frame.map_w))
         bad = "set_frame: rectification maps were installed for a different image size";
     else if (filter_shadow_points && (H <= 2 || W <= 2)) bad = "set_frame: image too small for the shadow filter";
     if (bad) {
@@ -566,35 +544,22 @@ int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scal
     B2V_CUDA(this, cudaSetDevice(device));
     frame.staged = b2v_frame{};
     const size_t pixels = static_cast<size_t>(H) * W;
-    if (pixels > frame.pixels) {
-        B2V_CUDA(this, cudaStreamSynchronize(stream));
-        void **bufs[] = {&frame.raw, reinterpret_cast<void **>(&frame.depth), reinterpret_cast<void **>(&frame.filtered),
-                         reinterpret_cast<void **>(&frame.rgb), &frame.shadow_scratch};
-        for (void **b : bufs) {
-            cudaFree(*b);
-            *b = nullptr;
-        }
-        frame.pixels = 0;   // stays 0 if an allocation below fails
-        B2V_CUDA(this, cudaMalloc(&frame.raw, pixels * sizeof(float)));
-        B2V_CUDA(this, cudaMalloc(&frame.depth, pixels * sizeof(float)));
-        B2V_CUDA(this, cudaMalloc(&frame.filtered, pixels * sizeof(float)));
-        B2V_CUDA(this, cudaMalloc(&frame.rgb, pixels * 3));
-        B2V_CUDA(this, cudaMalloc(&frame.shadow_scratch, kShadowScratchBytes));
-        frame.pixels = pixels;
-    }
-    if (cls && pixels > frame.label_pixels) {
-        B2V_CUDA(this, cudaStreamSynchronize(stream));
-        int32_t **bufs[] = {&frame.cls, &frame.inst, &frame.obj};
-        for (int32_t **b : bufs) {
-            cudaFree(*b);
-            *b = nullptr;
-        }
-        frame.label_pixels = 0;
-        for (int32_t **b : bufs) B2V_CUDA(this, cudaMalloc(b, pixels * sizeof(int32_t)));
-        frame.label_pixels = pixels;
+    // synchronise when the last buffer of a group is short, as stage_input does
+    if (pixels * 3 > frame.rgb.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+    B2V_CUDA(this, frame.raw.reserve(pixels));
+    B2V_CUDA(this, frame.depth.reserve(pixels));
+    B2V_CUDA(this, frame.filtered.reserve(pixels));
+    B2V_CUDA(this, frame.shadow_scratch.reserve(kShadowScratchBytes));
+    B2V_CUDA(this, frame.rgb.reserve(pixels * 3));
+    if (cls) {
+        if (pixels > frame.obj.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+        B2V_CUDA(this, frame.cls.reserve(pixels));
+        B2V_CUDA(this, frame.inst.reserve(pixels));
+        B2V_CUDA(this, frame.obj.reserve(pixels));
     }
     cudaStream_t s = stream;
-    const bool rect = frame.mapx != nullptr;
+    const bool rect = frame.mapx.get() != nullptr;
+    void *const raw = frame.raw.get();
     cudaError_t e = cudaSuccess;
     // a host image is uploaded into `dst`, a device image is read in place.  Uploads through frame.raw are ordered
     // after the kernels that read the previous one (one stream).
@@ -607,40 +572,41 @@ int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scal
     auto place_b32 = [&](const void *src, void *dst) {
         if (e != cudaSuccess) return;
         if (rect)
-            e = launch_remap_b32_nearest(src, H, W, frame.mapx, frame.mapy, dst, s);
+            e = launch_remap_b32_nearest(src, H, W, frame.mapx.get(), frame.mapy.get(), dst, s);
         else if (src != dst)
             e = cudaMemcpyAsync(dst, src, pixels * 4, cudaMemcpyDeviceToDevice, s);
     };
     // depth: upload -> widen (uint16; into `filtered`, free until the filter runs, when the remap follows) -> remap
-    const void *d = input(depth, pixels * (depth_u16 ? 2 : 4), (depth_u16 || rect) ? frame.raw : frame.depth);
+    const void *d = input(depth, pixels * (depth_u16 ? 2 : 4), (depth_u16 || rect) ? raw : frame.depth.get());
     if (depth_u16 && e == cudaSuccess) {
-        float *wide = rect ? frame.filtered : frame.depth;
+        float *wide = rect ? frame.filtered.get() : frame.depth.get();
         e = launch_depth_u16_to_f32(static_cast<const uint16_t *>(d), wide, pixels, depth_scale, s);
         d = wide;
     }
-    place_b32(d, frame.depth);
-    const void *c = input(color, pixels * 3, rect ? frame.raw : frame.rgb);
+    place_b32(d, frame.depth.get());
+    const void *c = input(color, pixels * 3, rect ? raw : frame.rgb.get());
     if (e == cudaSuccess) {
         if (rect)
-            e = launch_remap_u8c3_linear(static_cast<const uint8_t *>(c), H, W, frame.mapx, frame.mapy, frame.rgb,
-                                         frame.swap_rb, s);
-        else if (c != frame.rgb)
-            e = cudaMemcpyAsync(frame.rgb, c, pixels * 3, cudaMemcpyDeviceToDevice, s);
+            e = launch_remap_u8c3_linear(static_cast<const uint8_t *>(c), H, W, frame.mapx.get(), frame.mapy.get(),
+                                         frame.rgb.get(), frame.swap_rb, s);
+        else if (c != frame.rgb.get())
+            e = cudaMemcpyAsync(frame.rgb.get(), c, pixels * 3, cudaMemcpyDeviceToDevice, s);
     }
-    if (cls) place_b32(input(cls, pixels * 4, rect ? frame.raw : frame.cls), frame.cls);
-    if (inst) place_b32(input(inst, pixels * 4, rect ? frame.raw : frame.inst), frame.inst);
+    if (cls) place_b32(input(cls, pixels * 4, rect ? raw : frame.cls.get()), frame.cls.get());
+    if (inst) place_b32(input(inst, pixels * 4, rect ? raw : frame.inst.get()), frame.inst.get());
     if (e == cudaSuccess && filter_shadow_points)
-        e = launch_filter_shadow_points(frame.depth, H, W, 2, 2, -1.0f, frame.filtered, frame.shadow_scratch, s);
+        e = launch_filter_shadow_points(frame.depth.get(), H, W, 2, 2, -1.0f, frame.filtered.get(),
+                                        frame.shadow_scratch.get(), s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) {
         err = std::string("set_frame: ") + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
     }
-    frame.staged.depth = frame.depth;
-    frame.staged.filtered_depth = filter_shadow_points ? frame.filtered : frame.depth;
-    frame.staged.color = frame.rgb;
-    frame.staged.class_image = cls ? frame.cls : nullptr;
-    frame.staged.instance_image = inst ? frame.inst : nullptr;
+    frame.staged.depth = frame.depth.get();
+    frame.staged.filtered_depth = filter_shadow_points ? frame.filtered.get() : frame.depth.get();
+    frame.staged.color = frame.rgb.get();
+    frame.staged.class_image = cls ? frame.cls.get() : nullptr;
+    frame.staged.instance_image = inst ? frame.inst.get() : nullptr;
     frame.staged.height = H;
     frame.staged.width = W;
     *out = frame.staged;
@@ -658,10 +624,7 @@ struct b2v_grid : BlockGridCore {
     // the pool is a reservation for index.capacity blocks with storage mapped for index.pool_capacity (a fixed grid
     // maps it whole at create); a growable grid maps more inside the integrate call that needs it
     VmmRange pool;
-    float *d_pts = nullptr, *d_cols = nullptr;
-    size_t stage_points = 0;
-    float *d_out_pts = nullptr, *d_out_cols = nullptr;
-    size_t out_cap = 0;
+    DeviceBuffer<float> d_pts, d_cols, d_out_pts, d_out_cols;   // staging of host points, read-out
     int64_t last_n = 0;
 
     GridMeta meta() const { return GridMeta{reinterpret_cast<uint32_t *>(pool.va), index}; }
@@ -716,9 +679,6 @@ extern "C" int b2v_grid_create_ex(float voxel_size, int32_t block_size, uint32_t
 extern "C" int b2v_grid_destroy(b2v_grid *g) {
     if (!g) return B2V_OK;
     g->destroy();
-    vmm_release(&g->pool);
-    void *ptrs[] = {g->d_pts, g->d_cols, g->d_out_pts, g->d_out_cols};
-    for (void *p : ptrs) cudaFree(p);
     delete g;
     return B2V_OK;
 }
@@ -777,21 +737,19 @@ static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const v
     const bool dev_p = is_device_pointer(points);
     const bool dev_c = colors ? is_device_pointer(colors) : true;
     if (!dev_p || !dev_c) {
-        if (static_cast<size_t>(n_points) > g->stage_points) {
-            B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-            B2V_CUDA(g, regrow(&g->d_pts, static_cast<size_t>(n_points) * 3 * 2));  // room for float64 points
-            B2V_CUDA(g, regrow(&g->d_cols, static_cast<size_t>(n_points) * 3));
-            g->stage_points = static_cast<size_t>(n_points);
-        }
+        const size_t n = static_cast<size_t>(n_points);
+        if (n * 3 > g->d_cols.size()) B2V_CUDA(g, cudaStreamSynchronize(g->stream));   // reserved last
+        B2V_CUDA(g, g->d_pts.reserve(n * 3 * 2));  // room for float64 points
+        B2V_CUDA(g, g->d_cols.reserve(n * 3));
         if (!dev_p) {
-            B2V_CUDA(g, cudaMemcpyAsync(g->d_pts, points, static_cast<size_t>(n_points) * 3 * (f64 ? sizeof(double) : sizeof(float)),
+            B2V_CUDA(g, cudaMemcpyAsync(g->d_pts.get(), points, static_cast<size_t>(n_points) * 3 * (f64 ? sizeof(double) : sizeof(float)),
                                         cudaMemcpyHostToDevice, g->stream));
-            d_p = g->d_pts;
+            d_p = g->d_pts.get();
         }
         if (colors && !dev_c) {
-            B2V_CUDA(g, cudaMemcpyAsync(g->d_cols, colors, static_cast<size_t>(n_points) * 3 * (u8 ? 1 : sizeof(float)),
+            B2V_CUDA(g, cudaMemcpyAsync(g->d_cols.get(), colors, static_cast<size_t>(n_points) * 3 * (u8 ? 1 : sizeof(float)),
                                         cudaMemcpyHostToDevice, g->stream));
-            d_c = g->d_cols;
+            d_c = g->d_cols.get();
         }
     }
     B2V_CUDA(g, launch_point_insert(d_p, f64, nullptr, n_points, g->inv_voxel_size, g->table, g->index, g->stream));
@@ -885,16 +843,16 @@ static int64_t grid_run_query(b2v_grid *g, const GridQuery &q, bool count_only =
     if (g->read_counters() == B2V_ERR_CUDA) return -1;
     const uint32_t nb = g->block_count();
     if (g->ensure_scan(nb) != B2V_OK) return -1;
-    if (nb) grid_query_count_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), q, g->d_sums);
+    if (nb) grid_query_count_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), q, g->d_sums.get());
     uint32_t total = 0;
     if (cudaGetLastError() != cudaSuccess || g->scan_total(nb, &total) != cudaSuccess) return -1;
     if (count_only) return total;
-    if (static_cast<size_t>(total) > g->out_cap) {
-        if (regrow(&g->d_out_pts, static_cast<size_t>(total) * 3) != cudaSuccess) return -1;
-        if (regrow(&g->d_out_cols, static_cast<size_t>(total) * 3) != cudaSuccess) return -1;
-        g->out_cap = total;
-    }
-    if (nb) grid_query_emit_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), q, g->d_offs, g->d_out_pts, g->d_out_cols);
+    if (g->d_out_pts.reserve(static_cast<size_t>(total) * 3) != cudaSuccess ||
+        g->d_out_cols.reserve(static_cast<size_t>(total) * 3) != cudaSuccess)
+        return -1;
+    if (nb)
+        grid_query_emit_kernel<<<nb, kVox, 0, g->stream>>>(g->meta(), q, g->d_offs.get(), g->d_out_pts.get(),
+                                                           g->d_out_cols.get());
     if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(g->stream) != cudaSuccess) return -1;
     g->last_n = total;
     return total;
@@ -925,8 +883,8 @@ extern "C" int64_t b2v_grid_get_voxels_in_bb(b2v_grid *g, const double bbox[6], 
 extern "C" int b2v_grid_copy_voxels(b2v_grid *g, float *points, float *colors) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     const size_t n = static_cast<size_t>(g->last_n);
-    if (points && n) B2V_CUDA(g, cudaMemcpy(points, g->d_out_pts, n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-    if (colors && n) B2V_CUDA(g, cudaMemcpy(colors, g->d_out_cols, n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    if (points && n) B2V_CUDA(g, cudaMemcpy(points, g->d_out_pts.get(), n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    if (colors && n) B2V_CUDA(g, cudaMemcpy(colors, g->d_out_cols.get(), n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
     return B2V_OK;
 }
 

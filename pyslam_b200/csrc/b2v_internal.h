@@ -27,22 +27,55 @@ namespace b2v {
 // ---- small host utilities (b2v_api.cu) ----
 uint32_t next_pow2(uint64_t v);
 bool is_device_pointer(const void *p);   // device or managed memory
-// replace *p by a fresh allocation of n (at least 1) elements; the contents are not kept
-template <typename T> cudaError_t regrow(T **p, size_t n) {
-    cudaFree(*p);
-    *p = nullptr;
-    return cudaMalloc(p, (n ? n : 1) * sizeof(T));
-}
+
+// One cudaMalloc allocation of T, freed with its owner.  reserve(n) grows it to at least n elements; the contents are
+// not kept across a growth and nothing is synchronised beyond what cudaFree does, so a caller whose kernels may
+// still read the old allocation synchronises first.
+template <typename T> class DeviceBuffer {
+  public:
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer &) = delete;
+    DeviceBuffer &operator=(const DeviceBuffer &) = delete;
+    DeviceBuffer(DeviceBuffer &&o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    DeviceBuffer &operator=(DeviceBuffer &&o) noexcept {
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        return *this;
+    }
+    ~DeviceBuffer() { cudaFree(p_); }
+    T *get() const { return p_; }
+    size_t size() const { return n_; }   // elements
+    // nothing if n <= size(); else a fresh allocation of max(n, 1) elements.  On failure it holds nothing (size 0).
+    cudaError_t reserve(size_t n) {
+        if (n <= n_) return cudaSuccess;
+        cudaFree(p_);
+        p_ = nullptr;
+        n_ = 0;
+        const cudaError_t e = cudaMalloc(&p_, std::max<size_t>(n, 1) * sizeof(T));
+        if (e == cudaSuccess) n_ = std::max<size_t>(n, 1);
+        else p_ = nullptr;
+        return e;
+    }
+
+  private:
+    T *p_ = nullptr;
+    size_t n_ = 0;
+};
 
 // ---- device storage that grows in place (b2v_api.cu) ----
 // One virtual-address range reserved for the maximum size; physical memory is mapped into it in whole granules with
 // the driver's virtual memory management entry points, so the address the kernels see never changes and a growth
-// copies nothing.  Fixed-size storage takes the same path with the whole reservation mapped at create.
+// copies nothing.  Fixed-size storage takes the same path with the whole reservation mapped at create.  The range
+// is released with its owner.
 struct VmmRange {
     CUdeviceptr va = 0;
     size_t reserved = 0, mapped = 0, gran = 0;      // bytes
     int device = 0;
     std::vector<std::pair<size_t, size_t>> chunks;  // (offset, bytes) of each mapping
+    VmmRange() = default;
+    VmmRange(const VmmRange &) = delete;
+    VmmRange &operator=(const VmmRange &) = delete;
+    ~VmmRange();
 };
 // reserve at least `bytes`, rounded up to the granularity; false (and *err) on failure
 bool vmm_reserve(VmmRange *r, size_t bytes, int device, std::string *err);
@@ -384,14 +417,16 @@ struct BlockGridCore {
     cudaStream_t stream = nullptr;
     // the reference stores the voxel size as float and inverts it in float (voxel_block_grid.h:225-226, .hpp:6)
     float inv_voxel_size = 0.0f;
-    HashTable table{};
+    HashTable table{};   // views of table_mem, block_keys, counters
     BlockIndex index{};
     // the table and block_keys are sized for index.capacity; a growable grid maps its storage on demand
+    DeviceBuffer<uint4> table_mem;
+    DeviceBuffer<int4> block_keys;
+    DeviceBuffer<uint32_t> counters;
     bool growable = false;
     int64_t growths = 0;
     uint32_t *h_counters = nullptr;   // pinned mirror of index.counters
-    uint32_t *d_sums = nullptr, *d_offs = nullptr, *d_total = nullptr;   // count -> scan of the read-outs
-    uint32_t scan_cap = 0;
+    DeviceBuffer<uint32_t> d_sums, d_offs, d_total;   // count -> scan of the read-outs
     std::string err;
 
     // the arguments both grids accept (max_capacity_blocks 0: a fixed grid)
@@ -400,7 +435,7 @@ struct BlockGridCore {
     // stream, table, block index and counters for max(capacity_blocks, max_capacity_blocks) blocks; the grid then
     // maps its storage, sets index.pool_capacity and clears the index (clear_index) with its storage
     int create(double voxel_size, uint32_t capacity_blocks, uint32_t max_capacity_blocks, int32_t device);
-    void destroy();         // waits for the stream, frees everything above
+    void destroy();         // waits for the stream, destroys it and frees the pinned mirror
     int fetch_counters();   // h_counters := index.counters (synchronises)
     int read_counters();    // fetch_counters + B2V_ERR_CAPACITY ("hash table full" / "block pool full") on an error bit
     uint32_t block_count() const {   // blocks with storage, as of the last fetch_counters
@@ -432,12 +467,9 @@ struct BlockGridCore {
     // Kept apart from `frame`, so a staged frame stays valid across calls made with host images.  A call's buffers
     // are next written by a later call on the same stream, so the growth replay of the call may read them.
     struct InputStage {
-        float *depth = nullptr, *filtered = nullptr;
-        uint8_t *rgb = nullptr;
-        void *shadow_scratch = nullptr;
-        size_t pixels = 0;                        // capacity of the buffers above
-        int32_t *cls = nullptr, *obj = nullptr;   // class and object (or instance) images (semantic grids)
-        size_t label_pixels = 0;
+        DeviceBuffer<float> depth, filtered;
+        DeviceBuffer<uint8_t> rgb, shadow_scratch;
+        DeviceBuffer<int32_t> cls, obj;   // class and object (or instance) images (semantic grids)
     } input;
     // The [H][W] images of one call on the device: each non-NULL pointer is read in place if it is device memory, else
     // replaced by its upload into `input` on the stream.  filter_shadow_points: *depth is then replaced by its
@@ -449,15 +481,12 @@ struct BlockGridCore {
     // Per-frame preparation (b2v_grid_set_frame / b2v_sgrid_set_frame): the rectification maps and the staged images
     // of the last frame, in buffers sized for the largest frame so far.
     struct FrameStage {
-        float *mapx = nullptr, *mapy = nullptr;   // NULL: no rectification
+        DeviceBuffer<float> mapx, mapy;           // empty: no rectification
         int32_t map_h = 0, map_w = 0, swap_rb = 0;
-        void *raw = nullptr;                      // upload of one host image at a time (4 bytes per pixel)
-        float *depth = nullptr, *filtered = nullptr;
-        uint8_t *rgb = nullptr;
-        void *shadow_scratch = nullptr;
-        size_t pixels = 0;                        // capacity of the buffers above
-        int32_t *cls = nullptr, *inst = nullptr, *obj = nullptr;   // label images (semantic grids)
-        size_t label_pixels = 0;
+        DeviceBuffer<uint32_t> raw;               // upload of one host image at a time (4 bytes per pixel)
+        DeviceBuffer<float> depth, filtered;
+        DeviceBuffer<uint8_t> rgb, shadow_scratch;
+        DeviceBuffer<int32_t> cls, inst, obj;     // label images (semantic grids)
         b2v_frame staged{};                       // the last staged frame (all NULL: none)
     } frame;
     int set_rectification(const float *map_x, const float *map_y, int H, int W, int swap_rb);   // synchronises
@@ -465,7 +494,6 @@ struct BlockGridCore {
     // are checked before anything is touched.
     int set_frame(const void *depth, bool depth_u16, float depth_scale, const uint8_t *color, const int32_t *cls,
                   const int32_t *inst, int H, int W, bool filter_shadow_points, b2v_frame *out);
-    void free_frame();      // frees `frame` and `input`
 };
 
 template <typename MapStorage, typename Replay> int BlockGridCore::resolve(MapStorage map_storage, Replay replay) {

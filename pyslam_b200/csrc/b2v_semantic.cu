@@ -562,24 +562,22 @@ struct b2v_sgrid : BlockGridCore {
     // each per-voxel array of G is a reservation for index.capacity blocks with storage mapped on demand (a fixed grid
     // maps it whole at create); index.pool_capacity is the least any array holds
     VmmRange store[kSemArrays];
-    // staging
-    void *d_pts = nullptr, *d_cols = nullptr;
-    int32_t *d_cls = nullptr, *d_inst = nullptr;
-    float *d_depths = nullptr;
-    uint32_t *d_vid[2] = {nullptr, nullptr}, *d_ord[2] = {nullptr, nullptr};
-    uint8_t *d_valid = nullptr;   // per-point mask of the fused RGBD front-end
-    void *d_sort_tmp = nullptr;
-    size_t sort_tmp_bytes = 0, stage_points = 0;
+    // staging of the points of one call (float or double points, float or uint8 colours)
+    DeviceBuffer<double> d_pts;
+    DeviceBuffer<float> d_cols, d_depths;
+    DeviceBuffer<int32_t> d_cls, d_inst;
+    DeviceBuffer<uint32_t> d_vid[2], d_ord[2];
+    DeviceBuffer<uint8_t> d_sort_tmp;
+    DeviceBuffer<uint8_t> d_valid;   // per-point mask of the fused RGBD front-end; its size is the staging capacity
     // instance -> object association: votes (records -> sort -> runs -> triples), then resolve
-    int32_t *d_pend = nullptr;                       // [voxels] instance id of a pending voxel, else -1
-    unsigned long long *d_records = nullptr;         // [voxels] vote records (sort keys)
-    uint32_t *d_n_records = nullptr;                 // [2] records, runs
-    size_t records_cap = 0;
-    unsigned long long *d_sorted = nullptr, *d_runs = nullptr;   // [votes_cap] sort buffer, run keys
-    uint32_t *d_run_counts = nullptr;                // [votes_cap]
-    int32_t *d_triples = nullptr;                    // [votes_cap][3]
-    uint8_t *d_votes_tmp = nullptr;
-    size_t votes_cap = 0, votes_tmp_bytes = 0;
+    DeviceBuffer<int32_t> d_pend;                  // [voxels] instance id of a pending voxel, else -1
+    DeviceBuffer<unsigned long long> d_records;    // [voxels] vote records (sort keys)
+    DeviceBuffer<uint32_t> d_n_records;            // [2] records, runs
+    DeviceBuffer<unsigned long long> d_runs;       // [votes capacity] run keys
+    DeviceBuffer<uint32_t> d_run_counts;           // [votes capacity]
+    DeviceBuffer<int32_t> d_triples;               // [votes capacity][3]
+    DeviceBuffer<uint8_t> d_votes_tmp;
+    DeviceBuffer<unsigned long long> d_sorted;     // [votes capacity] sort buffer; its size is the votes capacity
     int64_t n_triples = 0;
     // every call that may change a voxel bumps `generation`; resolve needs the votes of the current state
     uint64_t generation = 0, votes_generation = 0;
@@ -588,13 +586,12 @@ struct b2v_sgrid : BlockGridCore {
     int32_t next_object_id = 1;  // VoxelSemanticSharedData::next_object_id (process-wide in the reference)
     std::vector<int32_t> map_inst, map_obj;
     bool has_instance_map = false;   // the last association succeeded (map_inst / map_obj are its map)
-    int32_t *d_map = nullptr;        // its map_inst then map_obj on the device, room for 2 * map_cap
-    size_t map_cap = 0;
+    DeviceBuffer<int32_t> d_map;     // its map_inst then map_obj on the device
     // read-out
-    double *d_out_pts = nullptr;
-    float *d_out_cols = nullptr, *d_out_conf = nullptr;
-    int32_t *d_out_cls = nullptr, *d_out_obj = nullptr;
-    size_t out_cap = 0;
+    DeviceBuffer<double> d_out_pts;
+    DeviceBuffer<float> d_out_cols, d_out_conf;
+    DeviceBuffer<int32_t> d_out_cls;
+    DeviceBuffer<int32_t> d_out_obj;   // its size is the read-out capacity
     int64_t last_n = 0;
 
     SemGrid dev() const {   // the kernels' view
@@ -703,12 +700,6 @@ extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32
 extern "C" int b2v_sgrid_destroy(b2v_sgrid *g) {
     if (!g) return B2V_OK;
     g->destroy();
-    for (VmmRange &r : g->store) vmm_release(&r);
-    void *ptrs[] = {g->d_pts, g->d_cols, g->d_cls, g->d_inst, g->d_depths, g->d_vid[0], g->d_vid[1], g->d_ord[0],
-                    g->d_ord[1], g->d_sort_tmp, g->d_out_pts, g->d_out_cols, g->d_out_conf, g->d_out_cls,
-                    g->d_out_obj, g->d_valid, g->d_pend, g->d_records, g->d_n_records, g->d_map,
-                    g->d_sorted, g->d_runs, g->d_run_counts, g->d_triples, g->d_votes_tmp};
-    for (void *p : ptrs) cudaFree(p);
     delete g;
     return B2V_OK;
 }
@@ -742,34 +733,24 @@ extern "C" int b2v_sgrid_set_depth_decay_rate(b2v_sgrid *g, float depth_decay_ra
 }
 
 static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
-    if (n <= g->stage_points) return B2V_OK;
+    if (n <= g->d_valid.size()) return B2V_OK;
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-    void **bufs[] = {&g->d_pts, &g->d_cols, reinterpret_cast<void **>(&g->d_cls), reinterpret_cast<void **>(&g->d_inst),
-                     reinterpret_cast<void **>(&g->d_depths), reinterpret_cast<void **>(&g->d_vid[0]),
-                     reinterpret_cast<void **>(&g->d_vid[1]), reinterpret_cast<void **>(&g->d_ord[0]),
-                     reinterpret_cast<void **>(&g->d_ord[1]), reinterpret_cast<void **>(&g->d_valid), &g->d_sort_tmp};
-    for (void **b : bufs) {
-        cudaFree(*b);
-        *b = nullptr;
-    }
-    g->stage_points = 0;  // stays 0 if an allocation below fails
+    g->d_valid = {};   // reserved last: it holds the capacity only once every staging buffer does
     const size_t cap = n + n / 4 + 1024;
-    B2V_CUDA(g, cudaMalloc(&g->d_pts, cap * 3 * sizeof(double)));
-    B2V_CUDA(g, cudaMalloc(&g->d_cols, cap * 3 * sizeof(float)));
-    B2V_CUDA(g, cudaMalloc(&g->d_cls, cap * sizeof(int32_t)));
-    B2V_CUDA(g, cudaMalloc(&g->d_inst, cap * sizeof(int32_t)));
-    B2V_CUDA(g, cudaMalloc(&g->d_depths, cap * sizeof(float)));
-    B2V_CUDA(g, cudaMalloc(&g->d_valid, cap));
+    B2V_CUDA(g, g->d_pts.reserve(cap * 3));
+    B2V_CUDA(g, g->d_cols.reserve(cap * 3));
+    B2V_CUDA(g, g->d_cls.reserve(cap));
+    B2V_CUDA(g, g->d_inst.reserve(cap));
+    B2V_CUDA(g, g->d_depths.reserve(cap));
     for (int k = 0; k < 2; ++k) {
-        B2V_CUDA(g, cudaMalloc(&g->d_vid[k], cap * sizeof(uint32_t)));
-        B2V_CUDA(g, cudaMalloc(&g->d_ord[k], cap * sizeof(uint32_t)));
+        B2V_CUDA(g, g->d_vid[k].reserve(cap));
+        B2V_CUDA(g, g->d_ord[k].reserve(cap));
     }
     size_t tmp = 0;
-    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(nullptr, tmp, g->d_vid[0], g->d_vid[1], g->d_ord[0], g->d_ord[1],
-                                               static_cast<int64_t>(cap), 0, 32, g->stream));
-    B2V_CUDA(g, cudaMalloc(&g->d_sort_tmp, tmp));
-    g->sort_tmp_bytes = tmp;
-    g->stage_points = cap;
+    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(nullptr, tmp, g->d_vid[0].get(), g->d_vid[1].get(), g->d_ord[0].get(),
+                                               g->d_ord[1].get(), static_cast<int64_t>(cap), 0, 32, g->stream));
+    B2V_CUDA(g, g->d_sort_tmp.reserve(tmp));
+    B2V_CUDA(g, g->d_valid.reserve(cap));
     return B2V_OK;
 }
 
@@ -779,15 +760,16 @@ static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
     if (in.pts_f64)
         sem_keys_kernel<double><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n, g->inv_voxel_size,
-                                                     g->table, g->dev(), lo, hi, g->d_vid[0], g->d_ord[0]);
+                                                     g->table, g->dev(), lo, hi, g->d_vid[0].get(), g->d_ord[0].get());
     else
         sem_keys_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n, g->inv_voxel_size,
-                                                    g->table, g->dev(), lo, hi, g->d_vid[0], g->d_ord[0]);
+                                                    g->table, g->dev(), lo, hi, g->d_vid[0].get(), g->d_ord[0].get());
     B2V_CUDA(g, cudaGetLastError());
-    size_t tmp = g->sort_tmp_bytes;  // all 32 key bits: kBadVid (points without storage) must sort last
-    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp, tmp, g->d_vid[0], g->d_vid[1], g->d_ord[0], g->d_ord[1],
-                                               n, 0, 32, s));
-    sem_runs_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1], g->d_ord[1], n, in, g->dev());
+    size_t tmp = g->d_sort_tmp.size();  // all 32 key bits: kBadVid (points without storage) must sort last
+    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp.get(), tmp, g->d_vid[0].get(), g->d_vid[1].get(),
+                                               g->d_ord[0].get(), g->d_ord[1].get(), n, 0, 32, s));
+    sem_runs_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(), n,
+                                                                          in, g->dev());
     B2V_CUDA(g, cudaGetLastError());
     return B2V_OK;
 }
@@ -834,19 +816,19 @@ extern "C" int b2v_sgrid_integrate(b2v_sgrid *g, int64_t n, const void *points, 
     if (rc != B2V_OK) return rc;
     const size_t m = static_cast<size_t>(n);
     cudaStream_t s = g->stream;
-    B2V_CUDA(g, cudaMemcpyAsync(g->d_pts, points, m * 3 * (points_f64 ? sizeof(double) : sizeof(float)),
+    B2V_CUDA(g, cudaMemcpyAsync(g->d_pts.get(), points, m * 3 * (points_f64 ? sizeof(double) : sizeof(float)),
                                cudaMemcpyDefault, s));
     if (colors)
-        B2V_CUDA(g, cudaMemcpyAsync(g->d_cols, colors, m * 3 * (colors_u8 ? 1 : sizeof(float)), cudaMemcpyDefault, s));
-    if (class_ids) B2V_CUDA(g, cudaMemcpyAsync(g->d_cls, class_ids, m * sizeof(int32_t), cudaMemcpyDefault, s));
-    if (instance_ids) B2V_CUDA(g, cudaMemcpyAsync(g->d_inst, instance_ids, m * sizeof(int32_t), cudaMemcpyDefault, s));
-    if (depths) B2V_CUDA(g, cudaMemcpyAsync(g->d_depths, depths, m * sizeof(float), cudaMemcpyDefault, s));
+        B2V_CUDA(g, cudaMemcpyAsync(g->d_cols.get(), colors, m * 3 * (colors_u8 ? 1 : sizeof(float)), cudaMemcpyDefault, s));
+    if (class_ids) B2V_CUDA(g, cudaMemcpyAsync(g->d_cls.get(), class_ids, m * sizeof(int32_t), cudaMemcpyDefault, s));
+    if (instance_ids) B2V_CUDA(g, cudaMemcpyAsync(g->d_inst.get(), instance_ids, m * sizeof(int32_t), cudaMemcpyDefault, s));
+    if (depths) B2V_CUDA(g, cudaMemcpyAsync(g->d_depths.get(), depths, m * sizeof(float), cudaMemcpyDefault, s));
     SemInputs in{};
-    in.pts = g->d_pts;
-    in.cols = colors ? g->d_cols : nullptr;
-    in.cls = class_ids ? g->d_cls : nullptr;
-    in.inst = instance_ids ? g->d_inst : nullptr;
-    in.depths = depths ? g->d_depths : nullptr;
+    in.pts = g->d_pts.get();
+    in.cols = colors ? g->d_cols.get() : nullptr;
+    in.cls = class_ids ? g->d_cls.get() : nullptr;
+    in.inst = instance_ids ? g->d_inst.get() : nullptr;
+    in.depths = depths ? g->d_depths.get() : nullptr;
     in.pts_f64 = points_f64 ? 1 : 0;
     in.cols_u8 = colors_u8 ? 1 : 0;
     rc = sgrid_fuse_staged(g, n, in, nullptr);
@@ -875,16 +857,16 @@ extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const 
     if (rc != B2V_OK) return rc;
     const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
     sem_rgbd_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, g->stream>>>(
-        P, d_depth, d_rgb, d_cls, d_obj, static_cast<float *>(g->d_pts), static_cast<float *>(g->d_cols), g->d_cls,
-        g->d_inst, g->d_depths, g->d_valid);
+        P, d_depth, d_rgb, d_cls, d_obj, reinterpret_cast<float *>(g->d_pts.get()), g->d_cols.get(), g->d_cls.get(),
+        g->d_inst.get(), g->d_depths.get(), g->d_valid.get());
     B2V_CUDA(g, cudaGetLastError());
     SemInputs in{};
-    in.pts = g->d_pts;
-    in.cols = g->d_cols;
-    in.cls = class_image ? g->d_cls : nullptr;
-    in.inst = object_image ? g->d_inst : nullptr;
-    in.depths = use_depths ? g->d_depths : nullptr;
-    rc = sgrid_fuse_staged(g, n, in, g->d_valid);
+    in.pts = g->d_pts.get();
+    in.cols = g->d_cols.get();
+    in.cls = class_image ? g->d_cls.get() : nullptr;
+    in.inst = object_image ? g->d_inst.get() : nullptr;
+    in.depths = use_depths ? g->d_depths.get() : nullptr;
+    rc = sgrid_fuse_staged(g, n, in, g->d_valid.get());
     if (rc != B2V_OK) return rc;
     return g->read_counters();
 }
@@ -921,29 +903,24 @@ static int64_t sgrid_run_readout(b2v_sgrid *g, const GridQuery &q, float min_con
         return static_cast<int64_t>(-1);
     };
     if (g->ensure_scan(nb) != B2V_OK) return -1;
-    sem_count_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_sums);
+    sem_count_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_sums.get());
     uint32_t total = 0;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = g->scan_total(nb, &total);
     if (e != cudaSuccess) return fail(e);
-    if (total > g->out_cap) {
-        void *old[] = {g->d_out_pts, g->d_out_cols, g->d_out_conf, g->d_out_cls, g->d_out_obj};
-        for (void *p : old) cudaFree(p);
-        g->d_out_pts = nullptr;
-        g->d_out_cols = g->d_out_conf = nullptr;
-        g->d_out_cls = g->d_out_obj = nullptr;
-        g->out_cap = 0;
+    if (total > g->d_out_obj.size()) {
+        g->d_out_obj = {};   // reserved last: it holds the capacity only once every read-out buffer does
         const size_t cap = static_cast<size_t>(total) + total / 4 + 1024;
-        if ((e = cudaMalloc(&g->d_out_pts, cap * 3 * sizeof(double))) != cudaSuccess) return fail(e);
-        if ((e = cudaMalloc(&g->d_out_cols, cap * 3 * sizeof(float))) != cudaSuccess) return fail(e);
-        if ((e = cudaMalloc(&g->d_out_conf, cap * sizeof(float))) != cudaSuccess) return fail(e);
-        if ((e = cudaMalloc(&g->d_out_cls, cap * sizeof(int32_t))) != cudaSuccess) return fail(e);
-        if ((e = cudaMalloc(&g->d_out_obj, cap * sizeof(int32_t))) != cudaSuccess) return fail(e);
-        g->out_cap = cap;
+        if ((e = g->d_out_pts.reserve(cap * 3)) != cudaSuccess) return fail(e);
+        if ((e = g->d_out_cols.reserve(cap * 3)) != cudaSuccess) return fail(e);
+        if ((e = g->d_out_conf.reserve(cap)) != cudaSuccess) return fail(e);
+        if ((e = g->d_out_cls.reserve(cap)) != cudaSuccess) return fail(e);
+        if ((e = g->d_out_obj.reserve(cap)) != cudaSuccess) return fail(e);
     }
     if (total) {
-        sem_emit_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_offs, g->d_out_pts,
-                                                    g->d_out_cols, g->d_out_cls, g->d_out_obj, g->d_out_conf);
+        sem_emit_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_offs.get(), g->d_out_pts.get(),
+                                                    g->d_out_cols.get(), g->d_out_cls.get(), g->d_out_obj.get(),
+                                                    g->d_out_conf.get());
         if ((e = cudaGetLastError()) != cudaSuccess) return fail(e);
     }
     g->last_n = total;
@@ -975,11 +952,11 @@ extern "C" int b2v_sgrid_copy_voxels(b2v_sgrid *g, double *points, float *colors
     const size_t n = static_cast<size_t>(g->last_n);
     B2V_CUDA(g, cudaSetDevice(g->device));
     if (n) {
-        if (points) B2V_CUDA(g, cudaMemcpyAsync(points, g->d_out_pts, n * 3 * sizeof(double), cudaMemcpyDefault, g->stream));
-        if (colors) B2V_CUDA(g, cudaMemcpyAsync(colors, g->d_out_cols, n * 3 * sizeof(float), cudaMemcpyDefault, g->stream));
-        if (class_ids) B2V_CUDA(g, cudaMemcpyAsync(class_ids, g->d_out_cls, n * sizeof(int32_t), cudaMemcpyDefault, g->stream));
-        if (object_ids) B2V_CUDA(g, cudaMemcpyAsync(object_ids, g->d_out_obj, n * sizeof(int32_t), cudaMemcpyDefault, g->stream));
-        if (confidences) B2V_CUDA(g, cudaMemcpyAsync(confidences, g->d_out_conf, n * sizeof(float), cudaMemcpyDefault, g->stream));
+        if (points) B2V_CUDA(g, cudaMemcpyAsync(points, g->d_out_pts.get(), n * 3 * sizeof(double), cudaMemcpyDefault, g->stream));
+        if (colors) B2V_CUDA(g, cudaMemcpyAsync(colors, g->d_out_cols.get(), n * 3 * sizeof(float), cudaMemcpyDefault, g->stream));
+        if (class_ids) B2V_CUDA(g, cudaMemcpyAsync(class_ids, g->d_out_cls.get(), n * sizeof(int32_t), cudaMemcpyDefault, g->stream));
+        if (object_ids) B2V_CUDA(g, cudaMemcpyAsync(object_ids, g->d_out_obj.get(), n * sizeof(int32_t), cudaMemcpyDefault, g->stream));
+        if (confidences) B2V_CUDA(g, cudaMemcpyAsync(confidences, g->d_out_conf.get(), n * sizeof(float), cudaMemcpyDefault, g->stream));
     }
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
@@ -1156,62 +1133,54 @@ static int64_t sgrid_assoc_votes(b2v_sgrid *g, const char *fn, const float K[4],
         const int32_t *d_cls = class_image, *d_inst = instance_image;
         if (g->stage_input(fn, height, width, false, &d_depth, nullptr, &d_cls, &d_inst) != B2V_OK) return -1;
         cudaStream_t s = g->stream;
-        cudaError_t e = cudaSuccess;
-        if (nv > g->records_cap) {
-            g->records_cap = 0;
-            e = regrow(&g->d_pend, nv);
-            if (e == cudaSuccess) e = regrow(&g->d_records, nv);
-            if (e == cudaSuccess) e = regrow(&g->d_n_records, 2);
-            if (e == cudaSuccess) g->records_cap = nv;
-        }
-        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_pend, 0xFF, nv * sizeof(int32_t), s);
-        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_n_records, 0, 2 * sizeof(uint32_t), s);
+        cudaError_t e = g->d_pend.reserve(nv);
+        if (e == cudaSuccess) e = g->d_records.reserve(nv);
+        if (e == cudaSuccess) e = g->d_n_records.reserve(2);
+        uint32_t *const n_records = g->d_n_records.get();
+        if (e == cudaSuccess) e = cudaMemsetAsync(g->d_pend.get(), 0xFF, nv * sizeof(int32_t), s);
+        if (e == cudaSuccess) e = cudaMemsetAsync(n_records, 0, 2 * sizeof(uint32_t), s);
         if (e == cudaSuccess) {
             sem_assoc_kernel<<<static_cast<unsigned>(nb), kVox, 0, s>>>(
                 g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_cls, d_inst, d_depth,
-                depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend, g->d_records, g->d_n_records,
-                static_cast<uint32_t>(nv));
+                depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend.get(), g->d_records.get(),
+                n_records, static_cast<uint32_t>(nv));
             e = cudaGetLastError();
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(counts, g->d_n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(counts, n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         const uint32_t n_rec = counts[0];
-        if (e == cudaSuccess && n_rec > g->votes_cap) {   // sort and run buffers sized by the records, not the voxels
-            g->votes_cap = 0;
+        if (e == cudaSuccess && n_rec > g->d_sorted.size()) {   // sort and run buffers sized by the records, not the voxels
+            g->d_sorted = {};   // reserved last: it holds the capacity only once every buffer of the votes does
             const size_t cap = std::min<size_t>(nv, static_cast<size_t>(n_rec) + n_rec / 4 + 1024);
-            e = regrow(&g->d_sorted, cap);
-            if (e == cudaSuccess) e = regrow(&g->d_runs, cap);
-            if (e == cudaSuccess) e = regrow(&g->d_run_counts, cap);
-            if (e == cudaSuccess) e = regrow(&g->d_triples, 3 * cap);
+            e = g->d_runs.reserve(cap);
+            if (e == cudaSuccess) e = g->d_run_counts.reserve(cap);
+            if (e == cudaSuccess) e = g->d_triples.reserve(3 * cap);
             size_t sort_bytes = 0, rle_bytes = 0;
-            cub::DoubleBuffer<unsigned long long> db(g->d_records, g->d_sorted);
+            cub::DoubleBuffer<unsigned long long> db(g->d_records.get(), g->d_sorted.get());
             if (e == cudaSuccess)
                 e = cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, db, static_cast<int>(cap), 0, 64, s);
             if (e == cudaSuccess)
-                e = cub::DeviceRunLengthEncode::Encode(nullptr, rle_bytes, g->d_records, g->d_runs, g->d_run_counts,
-                                                       g->d_n_records + 1, static_cast<int>(cap), s);
-            if (e == cudaSuccess) e = regrow(&g->d_votes_tmp, std::max(sort_bytes, rle_bytes));
-            if (e == cudaSuccess) {
-                g->votes_tmp_bytes = std::max(sort_bytes, rle_bytes);
-                g->votes_cap = cap;
-            }
+                e = cub::DeviceRunLengthEncode::Encode(nullptr, rle_bytes, g->d_records.get(), g->d_runs.get(),
+                                                       g->d_run_counts.get(), n_records + 1, static_cast<int>(cap), s);
+            if (e == cudaSuccess) e = g->d_votes_tmp.reserve(std::max(sort_bytes, rle_bytes));
+            if (e == cudaSuccess) e = g->d_sorted.reserve(cap);
         }
         if (e == cudaSuccess && n_rec) {
             // all 64 bits: the triples come out in ascending (instance, object) order, kAssocPending first
-            cub::DoubleBuffer<unsigned long long> db(g->d_records, g->d_sorted);
-            size_t tmp = g->votes_tmp_bytes;
-            e = cub::DeviceRadixSort::SortKeys(g->d_votes_tmp, tmp, db, static_cast<int>(n_rec), 0, 64, s);
-            tmp = g->votes_tmp_bytes;
+            cub::DoubleBuffer<unsigned long long> db(g->d_records.get(), g->d_sorted.get());
+            size_t tmp = g->d_votes_tmp.size();
+            e = cub::DeviceRadixSort::SortKeys(g->d_votes_tmp.get(), tmp, db, static_cast<int>(n_rec), 0, 64, s);
+            tmp = g->d_votes_tmp.size();
             if (e == cudaSuccess)
-                e = cub::DeviceRunLengthEncode::Encode(g->d_votes_tmp, tmp, db.Current(), g->d_runs, g->d_run_counts,
-                                                       g->d_n_records + 1, static_cast<int>(n_rec), s);
+                e = cub::DeviceRunLengthEncode::Encode(g->d_votes_tmp.get(), tmp, db.Current(), g->d_runs.get(),
+                                                       g->d_run_counts.get(), n_records + 1, static_cast<int>(n_rec), s);
             if (e == cudaSuccess) {
-                sem_assoc_triples_kernel<<<(n_rec + 255) / 256, 256, 0, s>>>(g->d_runs, g->d_run_counts,
-                                                                             g->d_n_records + 1, g->d_triples);
+                sem_assoc_triples_kernel<<<(n_rec + 255) / 256, 256, 0, s>>>(g->d_runs.get(), g->d_run_counts.get(),
+                                                                             n_records + 1, g->d_triples.get());
                 e = cudaGetLastError();
             }
             if (e == cudaSuccess)
-                e = cudaMemcpyAsync(counts + 1, g->d_n_records + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
+                e = cudaMemcpyAsync(counts + 1, n_records + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
             if (e == cudaSuccess) e = cudaStreamSynchronize(s);
         }
         if (e != cudaSuccess) {
@@ -1247,7 +1216,7 @@ extern "C" int b2v_sgrid_copy_assoc_votes(b2v_sgrid *g, int32_t *triples) {
         return B2V_ERR_INVALID_ARGUMENT;
     }
     B2V_CUDA(g, cudaSetDevice(g->device));
-    B2V_CUDA(g, cudaMemcpyAsync(triples, g->d_triples, static_cast<size_t>(g->n_triples) * 3 * sizeof(int32_t),
+    B2V_CUDA(g, cudaMemcpyAsync(triples, g->d_triples.get(), static_cast<size_t>(g->n_triples) * 3 * sizeof(int32_t),
                                 cudaMemcpyDefault, g->stream));
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
@@ -1324,18 +1293,18 @@ static int64_t sgrid_assoc_resolve(b2v_sgrid *g, const char *fn, const int32_t *
     }
     // the map on the device, for the deferred assignment below and for b2v_sgrid_remap_instance_ids
     const size_t m = g->map_inst.size();
-    if (m > g->map_cap) {
+    if (2 * m > g->d_map.size()) {
         e = cudaStreamSynchronize(g->stream);
-        if (e == cudaSuccess) e = regrow(&g->d_map, 2 * m);
-        g->map_cap = e == cudaSuccess ? m : 0;
+        if (e == cudaSuccess) e = g->d_map.reserve(2 * m);
     }
+    int32_t *const d_map = g->d_map.get();
     if (e == cudaSuccess && m)
-        e = cudaMemcpyAsync(g->d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
+        e = cudaMemcpyAsync(d_map, g->map_inst.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
     if (e == cudaSuccess && m)
-        e = cudaMemcpyAsync(g->d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
+        e = cudaMemcpyAsync(d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
     if (e == cudaSuccess && !new_id.empty() && g->votes_blocks > 0) {  // deferred assignment of this grid's pending voxels
         ++g->generation;
-        sem_assoc_apply_kernel<<<g->votes_blocks, kVox, 0, g->stream>>>(g->dev(), g->d_pend, g->d_map, g->d_map + m,
+        sem_assoc_apply_kernel<<<g->votes_blocks, kVox, 0, g->stream>>>(g->dev(), g->d_pend.get(), d_map, d_map + m,
                                                                          static_cast<int>(m));
         e = cudaGetLastError();
     }
@@ -1363,7 +1332,7 @@ extern "C" int64_t b2v_sgrid_assign_object_ids_to_instance_ids(
     const int64_t n = sgrid_assoc_votes(g, fn, K, width, height, Tcw, depth_max, depth_min, class_image,
                                         instance_image, depth_image, depth_threshold, do_carving);
     if (n < 0) return -1;
-    return sgrid_assoc_resolve(g, fn, g->d_triples, n, width, height, class_image, instance_image, min_vote_ratio,
+    return sgrid_assoc_resolve(g, fn, g->d_triples.get(), n, width, height, class_image, instance_image, min_vote_ratio,
                                min_votes);
 }
 
@@ -1391,10 +1360,10 @@ extern "C" int b2v_sgrid_remap_instance_ids(b2v_sgrid *g, const int32_t **object
     }
     B2V_CUDA(g, cudaSetDevice(g->device));
     const size_t m = g->map_inst.size();   // the association left its map in d_map
-    B2V_CUDA(g, launch_remap_instance_ids(f.instance_image, static_cast<size_t>(f.height) * f.width, g->d_map,
-                                          g->d_map + m, static_cast<int>(m), g->frame.obj, g->stream));
+    B2V_CUDA(g, launch_remap_instance_ids(f.instance_image, static_cast<size_t>(f.height) * f.width, g->d_map.get(),
+                                          g->d_map.get() + m, static_cast<int>(m), g->frame.obj.get(), g->stream));
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-    *object_image = g->frame.obj;
+    *object_image = g->frame.obj.get();
     return B2V_OK;
 }
 

@@ -6,7 +6,8 @@ cloud's values.
   new / first-touched lists), put units beyond rel_key's reach or boxes beyond the box offsets, or boxes wider than 15
   units (tests/test_tsdf_edges_cpu.py proves each scene reaches its path).
 - §2 boundary inputs: special depths, voxels behind / on the camera plane, a principal point off the image, images
-  smaller than one allocation tile at every stride, sparse group masks, the pool capacity boundary.
+  smaller than one allocation tile at every stride, sparse group masks, the pool capacity boundary, fused groups of
+  frames smaller than an earlier frame.
 - §3 extraction on uploaded adversarial blocks: every marching-cubes case, a block at the emit kernels' maximum
   output, and the point cloud's positions and colours against oracle.numpy_point_cloud."""
 
@@ -269,6 +270,37 @@ def test_pool_capacity_boundary():
                     short.integrate(d, c, cfg.K, t)
             short.synchronize()
         short.close()
+
+
+@pytest.mark.parametrize("group", [8, 3])
+@pytest.mark.parametrize("depth_kind", ["f32_host", "u16_host", "u16_cuda"])
+def test_smaller_frames_after_larger_ones(depth_kind, group):
+    """Fused groups of frames smaller than an earlier frame of the volume: the staging slots of a group follow the
+    current frame size, so every frame of a group reads its own upload (or widened uint16 depth)."""
+    cfg, big = S.CONFIGS["T0"], S.CONFIGS["C1"]
+    scale = np.float32(1.0 / 5000.0)
+    vol = _volume(cfg.voxel_size, cfg.sdf_trunc, cfg.depth_trunc, 16)
+    vol.set_group_size(group)
+    tw = oracle.TsdfOracle(cfg.voxel_size, cfg.sdf_trunc, cfg.depth_trunc)
+    for c, n in ((big, 4), (cfg, 8)):
+        fr = [S.render_frame(c, i) for i in range(n)]
+        D, Cc, T = (np.stack([f[k] for f in fr]) for k in range(3))
+        if depth_kind == "f32_host":
+            vol.integrate_batch(D, Cc, c.K, T)
+        else:
+            raw = np.round(D * 5000.0).astype(np.uint16)
+            D = raw.astype(np.float32) * scale
+            if depth_kind == "u16_cuda":
+                import torch
+                vol.integrate_batch(torch.from_numpy(raw).cuda(), torch.from_numpy(Cc).cuda(), c.K, T,
+                                    depth_scale=scale)
+                vol.synchronize()   # before the tensors are released
+            else:
+                vol.integrate_batch(raw, Cc, c.K, T, depth_scale=scale)
+        for i in range(n):
+            tw.integrate(D[i], Cc[i], c.K, T[i])
+    _same(vol.dump_blocks(), tw.dump_blocks())
+    vol.close()
 
 
 # ---------------------------------------------------------------------------------------------------------------------
