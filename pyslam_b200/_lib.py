@@ -48,6 +48,7 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_get_next_object_id", "b2v_grid_set_rectification", "b2v_grid_set_frame", "b2v_sgrid_set_rectification",
     "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids", "b2v_grid_set_shard", "b2v_sgrid_set_shard",
     "b2v_sgrid_assoc_votes", "b2v_sgrid_copy_assoc_votes", "b2v_sgrid_assoc_resolve",
+    "b2v_grid_upload_blocks", "b2v_sgrid_export_blocks", "b2v_sgrid_upload_blocks",
 ]
 
 
@@ -266,6 +267,12 @@ def load() -> C.CDLL:
     L.b2v_grid_get_voxels_in_bb.argtypes = [vp, vp, i32]
     L.b2v_grid_dump_blocks.restype = i64
     L.b2v_grid_dump_blocks.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.b2v_grid_upload_blocks.restype = C.c_int
+    L.b2v_grid_upload_blocks.argtypes = [vp, i64, vp, vp, vp, vp]
+    L.b2v_sgrid_export_blocks.restype = i64
+    L.b2v_sgrid_export_blocks.argtypes = [vp] * 13
+    L.b2v_sgrid_upload_blocks.restype = C.c_int
+    L.b2v_sgrid_upload_blocks.argtypes = [vp, i64] + [vp] * 12
     for prefix in ("b2v_grid", "b2v_sgrid"):
         fn = getattr(L, prefix + "_set_rectification")
         fn.restype = C.c_int

@@ -91,4 +91,19 @@ __device__ __forceinline__ bool region_contains(const GridQuery &Q, const double
     return frustum_contains(Q, p, ip);
 }
 
+// ---- block upload (b2v_grid_upload_blocks, b2v_sgrid_upload_blocks) -------------------------------------------
+// Pool index of the uploaded block `key` that this CTA scatters, for every thread of the CTA: kNoBlock when the block
+// has no table entry (another shard owns it) or no storage (the pool is full).  The keys went through
+// block_import_kernel in an earlier launch, so the table holds their final entries.
+__device__ __forceinline__ uint32_t uploaded_block_index(const HashTable &T, const int4 key, const uint32_t pool_capacity) {
+    __shared__ uint32_t s_idx;
+    if (threadIdx.x == 0) {
+        const uint32_t slot = table_find(T, key.x, key.y, key.z);
+        const uint32_t idx = slot == kEmpty ? kNoBlock : T.entries[slot].w;
+        s_idx = idx < pool_capacity ? idx : kNoBlock;
+    }
+    __syncthreads();
+    return s_idx;
+}
+
 }  // namespace b2v

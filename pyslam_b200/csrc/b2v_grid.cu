@@ -83,6 +83,15 @@ point_insert_kernel(const Tp *__restrict__ pts, const uint8_t *__restrict__ vali
     block_insert(have, bx, by, bz, T, B);
 }
 
+// block upload: one thread per uploaded key, through the same insert (and owner test) as the points' blocks
+__global__ void __launch_bounds__(256)
+block_import_kernel(const int4 *__restrict__ keys, const uint32_t n, const HashTable T, const BlockIndex B) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool have = i < n;
+    const int4 k = have ? keys[i] : make_int4(0, 0, 0, 0);
+    block_insert(have, k.x, k.y, k.z, T, B);
+}
+
 cudaError_t launch_point_insert(const void *pts, bool pts_f64, const uint8_t *valid, int64_t n, float inv_vs,
                                 const HashTable &table, const BlockIndex &index, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
@@ -272,6 +281,26 @@ grid_carve_kernel(const GridMeta G, const GridQuery Q, const float *__restrict__
     }
 }
 
+// block upload: one CTA per uploaded block b copies its voxels, in the layout of b2v_grid_dump_blocks (count [512],
+// pos_sum / col_sum [512][3]), into the planes of its pool block, replacing what the block held
+__global__ void __launch_bounds__(kVox)
+grid_scatter_kernel(const int4 *__restrict__ keys, const int32_t *__restrict__ count, const float *__restrict__ pos,
+                    const float *__restrict__ col, const HashTable T, const GridMeta G) {
+    const uint32_t b = blockIdx.x;
+    const uint32_t idx = uploaded_block_index(T, keys[b], G.index.pool_capacity);
+    if (idx == kNoBlock) return;
+    const int t = threadIdx.x;
+    const size_t v = static_cast<size_t>(b) * kVox + t;
+    uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords;
+    float *fb = reinterpret_cast<float *>(blk);
+    reinterpret_cast<int32_t *>(blk)[t] = count[v];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        fb[(1 + c) * kVox + t] = pos[3 * v + c];
+        fb[(4 + c) * kVox + t] = col[3 * v + c];
+    }
+}
+
 // ====================================================================================================================
 // host side: the block grid core (both grids)
 // ====================================================================================================================
@@ -373,6 +402,18 @@ int BlockGridCore::set_shard(int32_t rank, int32_t count) {
 int BlockGridCore::clear_index() {
     B2V_CUDA(this, cudaMemsetAsync(table.entries, 0xFF, (static_cast<size_t>(table.mask) + 1) * sizeof(uint4), stream));
     B2V_CUDA(this, cudaMemsetAsync(index.counters, 0, kBgNumCounters * sizeof(uint32_t), stream));
+    return B2V_OK;
+}
+
+int BlockGridCore::insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys) {
+    std::vector<int4> k4(static_cast<size_t>(n));
+    for (size_t i = 0; i < k4.size(); ++i) k4[i] = make_int4(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2], 0);
+    B2V_CUDA(this, d_keys->reserve(k4.size()));
+    // a pageable source is staged before the call returns, so k4 may go
+    B2V_CUDA(this, cudaMemcpyAsync(d_keys->get(), k4.data(), k4.size() * sizeof(int4), cudaMemcpyHostToDevice, stream));
+    block_import_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+        d_keys->get(), static_cast<uint32_t>(n), table, index);
+    B2V_CUDA(this, cudaGetLastError());
     return B2V_OK;
 }
 
@@ -954,4 +995,42 @@ extern "C" int64_t b2v_grid_dump_blocks(b2v_grid *g, int32_t *keys, uint64_t *ha
         }
     }
     return nb;
+}
+
+extern "C" int b2v_grid_upload_blocks(b2v_grid *g, int64_t n_blocks, const int32_t *keys, const int32_t *count,
+                                      const float *pos_sum, const float *col_sum) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && (!keys || !count || !pos_sum || !col_sum))) {
+        g->err = "b2v_grid_upload_blocks: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    if (n_blocks == 0) return B2V_OK;
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    DeviceBuffer<int4> d_keys;
+    int rc = g->insert_keys(n_blocks, keys, &d_keys);
+    if (rc != B2V_OK) return rc;
+    if (g->growable) {   // new storage is mapped zeroed: the cleared state of a voxel
+        rc = g->resolve(
+            [&](uint64_t blocks) {
+                std::string map_err;   // a failed mapping surfaces as "block pool full"
+                grid_map_storage(g, blocks, &map_err);
+            },
+            [](uint32_t, uint32_t) { return B2V_OK; });
+        if (rc != B2V_OK) return rc;
+    }
+    const size_t nv = static_cast<size_t>(n_blocks) * kVox;
+    DeviceBuffer<int32_t> d_count;
+    DeviceBuffer<float> d_pos, d_col;
+    B2V_CUDA(g, d_count.reserve(nv));
+    B2V_CUDA(g, d_pos.reserve(nv * 3));
+    B2V_CUDA(g, d_col.reserve(nv * 3));
+    B2V_CUDA(g, cudaMemcpyAsync(d_count.get(), count, nv * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream));
+    B2V_CUDA(g, cudaMemcpyAsync(d_pos.get(), pos_sum, nv * 3 * sizeof(float), cudaMemcpyHostToDevice, g->stream));
+    B2V_CUDA(g, cudaMemcpyAsync(d_col.get(), col_sum, nv * 3 * sizeof(float), cudaMemcpyHostToDevice, g->stream));
+    grid_scatter_kernel<<<static_cast<unsigned>(n_blocks), kVox, 0, g->stream>>>(d_keys.get(), d_count.get(),
+                                                                                 d_pos.get(), d_col.get(), g->table,
+                                                                                 g->meta());
+    B2V_CUDA(g, cudaGetLastError());
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return g->read_counters();
 }

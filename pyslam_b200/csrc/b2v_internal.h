@@ -453,6 +453,11 @@ struct BlockGridCore {
     // in one call belong to one block and a block's index never changes, so every voxel is updated by exactly one of
     // the passes.  If the storage cannot grow, the blocks past it are dropped ("block pool full").  Synchronises.
     template <typename MapStorage, typename Replay> int resolve(MapStorage map_storage, Replay replay);
+    // First half of a block upload: the HOST keys int32 [n][3] as int4 in *d_keys, and each inserted into the table
+    // with a pool index (block_insert: a sharded grid skips the blocks it does not own; past index.capacity the
+    // index is kNoBlock and the error flag says "block pool full").  Asynchronous.  A growable grid then maps storage
+    // for the new pool count (resolve) before the grid's scatter kernel copies the voxels in.
+    int insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys);
     // room for n_blocks per-block counts in d_sums / offsets in d_offs
     int ensure_scan(uint32_t n_blocks);
     // exclusive scan of the per-block counts d_sums -> d_offs, and their total (synchronises)

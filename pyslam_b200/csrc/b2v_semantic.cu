@@ -44,6 +44,7 @@ namespace b2v {
 constexpr int kSemLabels = B2V_SEM_MAX_LABELS;
 constexpr uint32_t kBadVid = 0xFFFFFFFFu;
 constexpr float kBaseLogProb = 0.10536051565782628f;  // voxel_data_semantic.h:287, -log(0.9)
+constexpr int kSemArrays = 11;   // per-voxel arrays of a Bayesian grid (a voting grid has the first 6)
 
 // the block index as the semantic kernels read it: BlockIndex without the shard fields, which only the block insert
 // reads (the 24-byte layout keeps sem_runs_kernel's label slots in a local-memory frame, as before the shard fields)
@@ -548,14 +549,37 @@ __global__ void sem_fill_kernel(const SemGrid G, const size_t v0, const size_t v
     }
 }
 
+// ---- block upload (b2v_sgrid_upload_blocks) ------------------------------------------------------------------
+// The grid's per-voxel arrays (sgrid_arrays order): each uploaded block is a contiguous run of block_bytes[k] bytes in
+// src[k] (the layout of b2v_sgrid_export_blocks) and goes to its pool block's run in dst[k].
+struct SemUpload {
+    void *dst[kSemArrays];
+    const void *src[kSemArrays];
+    uint32_t block_bytes[kSemArrays];   // multiples of 16
+    int32_t n_arrays;
+};
+
+// one CTA per uploaded block: every array's run of the block, 16 bytes per thread and step, replacing what the pool
+// block held
+__global__ void __launch_bounds__(256)
+sem_scatter_kernel(const int4 *__restrict__ keys, const SemUpload U, const HashTable T, const uint32_t pool_capacity) {
+    const uint32_t b = blockIdx.x;
+    const uint32_t idx = uploaded_block_index(T, keys[b], pool_capacity);
+    if (idx == kNoBlock) return;
+    for (int k = 0; k < U.n_arrays; ++k) {
+        const uint32_t words = U.block_bytes[k] / 16u;
+        const uint4 *src = static_cast<const uint4 *>(U.src[k]) + static_cast<size_t>(b) * words;
+        uint4 *dst = static_cast<uint4 *>(U.dst[k]) + static_cast<size_t>(idx) * words;
+        for (uint32_t w = threadIdx.x; w < words; w += blockDim.x) dst[w] = src[w];
+    }
+}
+
 }  // namespace b2v
 
 // ====================================================================================================================
 // host side: the C ABI of include/b2v.h (b2v_sgrid_*)
 // ====================================================================================================================
 using namespace b2v;
-
-constexpr int kSemArrays = 11;   // per-voxel arrays of a Bayesian grid (a voting grid has the first 6)
 
 struct b2v_sgrid : BlockGridCore {
     SemGrid G{};   // G.index is not kept: dev() fills it in
@@ -1374,4 +1398,96 @@ extern "C" int b2v_sgrid_copy_instance_map(b2v_sgrid *g, int32_t *instance_ids, 
         if (object_ids) object_ids[i] = g->map_obj[i];
     }
     return B2V_OK;
+}
+
+// ---- raw block export / upload (map state) --------------------------------------------------------------------------
+extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys, int32_t *count, double *pos_sum, float *col_sum,
+                                           int32_t *object_id, int32_t *class_id, int32_t *counter, float *ml_logp,
+                                           float *conf, int32_t *lab_obj, int32_t *lab_cls, float *lab_logp) {
+    if (!g) return -1;
+    const int64_t nb = b2v_sgrid_num_blocks(g);
+    if (nb <= 0) return nb;
+    void *const out[kSemArrays] = {count, pos_sum, col_sum, object_id, class_id, counter, ml_logp, conf,
+                                   lab_obj, lab_cls, lab_logp};
+    SemArray arr[kSemArrays];
+    const int na = sgrid_arrays(g, arr);
+    std::vector<int4> hk(static_cast<size_t>(nb));
+    cudaError_t e = cudaMemcpyAsync(hk.data(), g->index.block_keys, hk.size() * sizeof(int4), cudaMemcpyDeviceToHost,
+                                    g->stream);
+    for (int k = 0; k < na && e == cudaSuccess; ++k)
+        if (out[k])
+            e = cudaMemcpyAsync(out[k], *arr[k].ptr, static_cast<size_t>(nb) * kVox * arr[k].voxel_bytes,
+                                cudaMemcpyDeviceToHost, g->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
+    if (e != cudaSuccess) {
+        g->err = std::string("b2v_sgrid_export_blocks: ") + cudaGetErrorString(e);
+        return -1;
+    }
+    if (keys)
+        for (int64_t b = 0; b < nb; ++b) {
+            keys[3 * b + 0] = hk[b].x;
+            keys[3 * b + 1] = hk[b].y;
+            keys[3 * b + 2] = hk[b].z;
+        }
+    return nb;
+}
+
+extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys, const int32_t *count,
+                                       const double *pos_sum, const float *col_sum, const int32_t *object_id,
+                                       const int32_t *class_id, const int32_t *counter, const float *ml_logp,
+                                       const float *conf, const int32_t *lab_obj, const int32_t *lab_cls,
+                                       const float *lab_logp) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    const void *const in[kSemArrays] = {count, pos_sum, col_sum, object_id, class_id, counter, ml_logp, conf,
+                                        lab_obj, lab_cls, lab_logp};
+    SemArray arr[kSemArrays];
+    const int na = sgrid_arrays(g, arr);
+    bool bad = n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && !keys);
+    for (int k = 0; k < na; ++k) bad = bad || (n_blocks > 0 && !in[k]);
+    if (bad) {
+        g->err = "b2v_sgrid_upload_blocks: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    // the uploaded voxels are a new state: votes taken before are stale and remap_instance_ids needs a new association
+    ++g->generation;
+    g->has_instance_map = false;
+    if (n_blocks == 0) return B2V_OK;
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    DeviceBuffer<int4> d_keys;
+    int rc = g->insert_keys(n_blocks, keys, &d_keys);
+    if (rc != B2V_OK) return rc;
+    if (g->growable) {
+        rc = g->resolve(
+            [&](uint64_t blocks) {
+                std::string map_err;   // a failed mapping surfaces as "block pool full"
+                sgrid_map_storage(g, blocks, &map_err);
+            },
+            [&](uint32_t lo, uint32_t hi) {   // the cleared state for the voxels that just got storage
+                sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * kVox,
+                                                            static_cast<size_t>(hi) * kVox);
+                B2V_CUDA(g, cudaGetLastError());
+                return B2V_OK;
+            });
+        if (rc != B2V_OK) return rc;
+    }
+    SemUpload U{};
+    U.n_arrays = na;
+    size_t block_bytes = 0;
+    for (int k = 0; k < na; ++k) block_bytes += arr[k].voxel_bytes * kVox;
+    DeviceBuffer<uint8_t> d_src;
+    B2V_CUDA(g, d_src.reserve(static_cast<size_t>(n_blocks) * block_bytes));
+    size_t off = 0;
+    for (int k = 0; k < na; ++k) {
+        const size_t bytes = static_cast<size_t>(n_blocks) * kVox * arr[k].voxel_bytes;
+        B2V_CUDA(g, cudaMemcpyAsync(d_src.get() + off, in[k], bytes, cudaMemcpyHostToDevice, g->stream));
+        U.dst[k] = *arr[k].ptr;
+        U.src[k] = d_src.get() + off;
+        U.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * kVox);
+        off += bytes;
+    }
+    sem_scatter_kernel<<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(d_keys.get(), U, g->table,
+                                                                              g->index.pool_capacity);
+    B2V_CUDA(g, cudaGetLastError());
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return g->read_counters();
 }

@@ -20,6 +20,7 @@ from types import SimpleNamespace
 
 import numpy as np
 
+from . import map_state
 from .volume import B200TsdfVolume
 
 # defaults copied by value from the reference's parameter table (pyslam/config_parameters.py:311,
@@ -44,6 +45,9 @@ DEFAULT_PARAMETERS = {
     "kVolumetricIntegrationB200MaxBatch": 32,
     # Open3D volume_unit_resolution (tsdf.py:104-108 uses 16); 8 = SURVEY decision D1
     "kVolumetricIntegrationB200UnitResolution": 16,
+    # SAVE also writes the map's state beside dense_map.ply (dense_map.state.npz), which LOAD restores; off by default:
+    # the file is as large as the map (10 KiB per TSDF block)
+    "kVolumetricIntegrationB200SaveMapState": False,
 }
 
 
@@ -114,6 +118,38 @@ class B200PluginSetup:
             self.volume.set_rectification(m1, m2, swap_rb=True)
             self._gpu_rectify = True
 
+    def load(self, path):
+        """The LOAD task of the map saved in directory `path`, the mirror of the base class's `save(path)`: it reads
+        `path/dense_map.state.npz` (written by SAVE with kVolumetricIntegrationB200SaveMapState).  The integrator then
+        sets `load_request_completed` to 1 and notifies `load_request_condition`; on failure the flag stays 0."""
+        TaskType = self._api.VolumetricIntegrationTaskType
+        task_t = getattr(self._api, "VolumetricIntegrationTask", SimpleNamespace)
+        self.load_request_completed.value = 0
+        self.q_in.put(task_t(keyframe_data=None, task_type=TaskType.LOAD, load_save_path=path + "/dense_map.ply"))
+
+    def _save_map_state(self, ply_path):
+        """The part of SAVE that writes the map's state beside the .ply, when kVolumetricIntegrationB200SaveMapState."""
+        if self.b200_parameters["kVolumetricIntegrationB200SaveMapState"]:
+            self.volume.save_state(map_state.state_path(ply_path))
+
+    def _load_map_state(self, task, completed, condition):
+        """LOAD: replace the map with the state file beside `task.load_save_path`; the next output shows it.  The
+        waiter is notified either way; `completed` becomes 1 only on success (a failure raises, leaving the map as it
+        was, and the task loop logs it)."""
+        loaded = False
+        try:
+            self.volume.load_state(map_state.state_path(task.load_save_path))
+            self._after_load()
+            loaded = True
+        finally:
+            with condition:
+                if loaded:
+                    completed.value = 1
+                condition.notify_all()
+
+    def _after_load(self):
+        pass
+
     def _intrinsics(self):
         if hasattr(self, "get_camera_intrinsics_for_depth"):
             return self.get_camera_intrinsics_for_depth()
@@ -124,12 +160,15 @@ class B200PluginSetup:
 def make_integrator_class(Base, api):
     """Build the plugin class against a base class and an `api` namespace providing
     `VolumetricIntegrationTaskType`, `VolumetricIntegrationOutput`, `VolumetricIntegrationMesh`,
-    `VolumetricIntegrationPointCloud`, `DatasetEnvironmentType` (or None) and `Parameters` (or None)."""
+    `VolumetricIntegrationPointCloud`, `DatasetEnvironmentType` (or None) and `Parameters` (or None); optionally
+    `VolumetricIntegrationTask`, the task type `load` enqueues (else a namespace with the task's fields)."""
 
     TaskType = api.VolumetricIntegrationTaskType
 
     class VolumetricIntegratorB200(B200PluginSetup, Base):
         """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
+
+        _api = api
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
@@ -257,7 +296,10 @@ def make_integrator_class(Base, api):
                             else:
                                 pc = self.volume.extract_point_cloud()
                                 write_ply_points(path, pc.points, pc.colors)
+                            self._save_map_state(path)
                             last_output = api.VolumetricIntegrationOutput(ttype)
+                        elif ttype == TaskType.LOAD:
+                            self._load_map_state(self.last_input_task, load_request_completed, load_request_condition)
                         elif ttype == TaskType.UPDATE_OUTPUT:
                             do_output = True
                         if do_output:
@@ -297,6 +339,7 @@ def load_pyslam_plugin():
     api = SimpleNamespace(
         USE_CPP=bool(USE_CPP),
         VolumetricIntegrationTaskType=B.VolumetricIntegrationTaskType,
+        VolumetricIntegrationTask=B.VolumetricIntegrationTask,
         VolumetricIntegrationOutput=B.VolumetricIntegrationOutput,
         VolumetricIntegrationMesh=B.VolumetricIntegrationMesh,
         VolumetricIntegrationPointCloud=B.VolumetricIntegrationPointCloud,

@@ -66,6 +66,9 @@ DEFAULT_PARAMETERS = {
     # raw keyframe images to the grid (set_frame): upload once, undistort + BGR->RGB + depth widening + shadow filter
     # on the GPU instead of the base class's cv2.remap / cvtColor (integrator.py has the same switch)
     "kVolumetricIntegrationB200GpuRectify": True,
+    # SAVE also writes the grid's state beside dense_map.ply (dense_map.state.npz), which LOAD restores; off by
+    # default: the file is as large as the map (78 KiB per Bayesian block)
+    "kVolumetricIntegrationB200SaveMapState": False,
 }
 
 
@@ -85,6 +88,7 @@ def make_semantic_integrator_class(Base, api):
         """GPU semantic voxel-grid integrator; `use_semantic_probabilistic` selects Bayesian fusion (:131-141)."""
 
         _defaults = DEFAULT_PARAMETERS
+        _api = api
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
@@ -111,6 +115,12 @@ def make_semantic_integrator_class(Base, api):
             self.last_integrated_id = -1
             self.last_instance_map = {}
             self._init_gpu_rectify()
+
+        def _after_load(self):
+            """The restored grid has no association yet, and until the next keyframe the output represents it as
+            objects when the configuration integrates instance ids."""
+            self.last_instance_map = {}
+            self.integrated_instance_ids = bool(self.b200_parameters["kVolumetricSemanticIntegrationUseInstanceIds"])
 
         def _make_grid(self, p, side, constructor_kwargs):
             probabilistic = bool(constructor_kwargs.get("use_semantic_probabilistic", False))
@@ -266,7 +276,10 @@ def make_semantic_integrator_class(Base, api):
                                 min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"]))
                             if len(v.points):
                                 write_ply_points(self.last_input_task.load_save_path, v.points, v.colors)
+                            self._save_map_state(self.last_input_task.load_save_path)
                             last_output = api.VolumetricIntegrationOutput(ttype)
+                        elif ttype == TaskType.LOAD:
+                            self._load_map_state(self.last_input_task, load_request_completed, load_request_condition)
                         elif ttype == TaskType.UPDATE_OUTPUT:
                             do_output = True
                         if do_output:
@@ -367,6 +380,7 @@ def load_pyslam_semantic_plugin():
     api = SimpleNamespace(
         USE_CPP=bool(USE_CPP),
         VolumetricIntegrationTaskType=B.VolumetricIntegrationTaskType,
+        VolumetricIntegrationTask=B.VolumetricIntegrationTask,
         VolumetricIntegrationOutput=B.VolumetricIntegrationOutput,
         VolumetricIntegrationMesh=B.VolumetricIntegrationMesh,
         VolumetricIntegrationPointCloud=B.VolumetricIntegrationPointCloud,

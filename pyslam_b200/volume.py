@@ -25,7 +25,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import _lib
+from . import _lib, map_state
 from ._lib import B2VConfig, BLOCK_SIZE, BLOCK_VOXELS, VOXEL_PLANES
 
 
@@ -67,7 +67,53 @@ class PointCloud:
         self.edge_ids = edge_ids                 # [N,4] int32 voxel (x,y,z) + axis of each zero crossing, if known
 
 
-class B200TsdfVolume:
+class _MapState:
+    """`save_state` / `load_state` of the TSDF volume and the voxel grids (`map_state` holds the file format).  A map
+    kind names itself in `_STATE_KIND` and provides `_state_config()` (what the voxels mean: must match to load),
+    `_state_arrays()` (per-block array specs, keys first), `_export_state()`, `_state_capacity()` (the most blocks it
+    can hold), `_clear_state()` and `_upload_state(blocks)`; the semantic grids add restored settings."""
+
+    _STATE_KIND = ""
+    _STATE_BOUNDS: dict = {}
+
+    def _state_semantic_kind(self) -> int:
+        return -1
+
+    def _state_settings(self) -> dict:
+        return {}
+
+    def _restore_settings(self, settings: dict) -> None:
+        pass
+
+    def save_state(self, path) -> None:
+        """Write the map's state to `path` (one uncompressed `.npz`; one file per shard for a sharded map), after the
+        work in flight is done.  The state is every block's raw voxels plus the configuration and settings a load
+        restores.  Not part of it: rectification maps and staged frames, bench counters and, on semantic grids, the
+        label-overflow counter (counts from 0 after a load) and the last association's instance map
+        (`remap_instance_ids` needs a new association, as on a fresh grid)."""
+        map_state.write(path, self._STATE_KIND, self._state_semantic_kind(), self._state_config(),
+                        self._state_settings(), self.shard_rank, self.shard_count, self._export_state())
+
+    def load_state(self, paths) -> None:
+        """Replace the map with the state in `paths`: one file, or a list such as the files of every shard of an
+        N-rank map.  Only the blocks this object owns under its own shard setting are kept (`sharding.owner_of`), so a
+        map saved by N ranks loads into any number of ranks, one included, with the same voxels bit for bit.  The
+        files are validated first: a wrong format version, kind or configuration, missing or malformed arrays,
+        duplicate keys, out-of-range values or more owned blocks than this object's ceiling raise ValueError and leave
+        the map as it was.  The blocks are uploaded in bounded chunks.  What is not part of the state: `save_state`."""
+        spec = self._state_arrays()
+        settings, blocks = map_state.read(
+            paths, self._STATE_KIND, self._state_semantic_kind(), self._state_config(),
+            {name: np.asarray(v).dtype for name, v in self._state_settings().items()}, spec, self.shard_rank,
+            self.shard_count, self._state_capacity(), self._STATE_BOUNDS)
+        self._clear_state()
+        block_bytes = sum(np.dtype(dt).itemsize * int(np.prod(shape)) for dt, shape in spec.values())
+        for a, b in map_state.chunks(len(blocks["keys"]), block_bytes):
+            self._upload_state({name: x[a:b] for name, x in blocks.items()})
+        self._restore_settings(settings)
+
+
+class B200TsdfVolume(_MapState):
     """H100-native TSDF + colour volume on 8^3 voxel blocks in a GPU hash table.
 
     Parameters mirror `o3d.pipelines.integration.ScalableTSDFVolume(voxel_length, sdf_trunc, ...)`
@@ -96,6 +142,7 @@ class B200TsdfVolume:
         self.device = int(device)
         self.shard_rank, self.shard_count = int(shard_rank), int(shard_count)
         self.volume_unit_resolution = int(volume_unit_resolution)
+        self.depth_sampling_stride = int(depth_sampling_stride)
         cfg = B2VConfig(voxel_length, block_size, sdf_trunc, depth_trunc, depth_sampling_stride,
                         capacity_blocks, device, shard_rank, shard_count, int(volume_unit_resolution),
                         float(voxel_length), float(sdf_trunc), self.max_capacity_blocks)
@@ -327,6 +374,39 @@ class B200TsdfVolume:
         x = np.ascontiguousarray(vox, np.float32).reshape(k.shape[0], VOXEL_PLANES, BLOCK_VOXELS)
         self._check(self._L.b2v_upload_blocks(self._h, k.shape[0], k.ctypes.data, x.ctypes.data),
                     "b2v_upload_blocks")
+
+    # ---- map state (_MapState) ----
+    _STATE_KIND = "tsdf"
+
+    def _state_config(self) -> dict:
+        return dict(voxel_size=np.float32(self.voxel_length), voxel_length=np.float64(self.voxel_length),
+                    sdf_trunc=np.float32(self.sdf_trunc), sdf_trunc_d=np.float64(self.sdf_trunc),
+                    depth_trunc=np.float32(self.depth_trunc), depth_stride=np.int32(self.depth_sampling_stride),
+                    unit_resolution=np.int32(self.volume_unit_resolution))
+
+    @staticmethod
+    def _state_arrays() -> dict:
+        return dict(keys=(np.int32, (3,)), vox=(np.float32, (VOXEL_PLANES, BLOCK_VOXELS)))
+
+    def _state_capacity(self) -> int:
+        return max(self.capacity_blocks, self.max_capacity_blocks)
+
+    def _export_state(self) -> dict:
+        """keys / vox of every block (b2v_dump_blocks, which waits for the frames in flight)."""
+        nb = self.num_blocks()
+        keys = np.zeros((nb, 3), np.int32)
+        vox = np.zeros((nb, VOXEL_PLANES, BLOCK_VOXELS), np.float32)
+        n = self._L.b2v_dump_blocks(self._h, keys.ctypes.data, None, vox.ctypes.data)
+        if n != nb:
+            raise RuntimeError(f"b2v_dump_blocks returned {n}, expected {nb}: {self._L.b2v_last_error(self._h).decode()}")
+        return dict(keys=keys, vox=vox)
+
+    def _clear_state(self) -> None:
+        self.reset()
+
+    def _upload_state(self, blocks: dict) -> None:
+        if len(blocks["keys"]):
+            self.upload_blocks(blocks["keys"], blocks["vox"])
 
     def export_blocks_torch(self):
         """(keys int32 [n,4] = {x,y,z,0}, vox float32 [n,5,512]) as torch CUDA tensors on this volume's device:
@@ -614,7 +694,7 @@ class VoxelGridData:
         self.confidences = None
 
 
-class _BlockGrid:
+class _BlockGrid(_MapState):
     """What the point-average and the semantic grids share: the library handle and its lifetime, the checks of
     `integrate`'s points and colours, the frame stage, carving and the read-outs both grids answer alike.  A subclass
     names its entry points by their prefix `_P` and stages frames with `_stage_frame`."""
@@ -627,6 +707,7 @@ class _BlockGrid:
         self._h = C.c_void_p()
         self.voxel_size = float(voxel_size)
         self._block_size = int(block_size)
+        self.capacity_blocks = int(capacity_blocks)
         self.max_capacity_blocks = int(max_capacity_blocks or 0)
         self.device = int(device)
         self._frame_gen, self._frame = 0, None
@@ -789,6 +870,18 @@ class _BlockGrid:
     def get_block_size(self) -> int:
         return self._block_size
 
+    # ---- map state (_MapState): the grid's kind adds its arrays, `_export_state` and `_upload_state` ----
+    _STATE_BOUNDS = {"count": (0, None)}
+
+    def _state_config(self) -> dict:
+        return dict(voxel_size=np.float64(self.voxel_size), block_size=np.int32(self._block_size))
+
+    def _state_capacity(self) -> int:
+        return max(self.capacity_blocks, self.max_capacity_blocks)
+
+    def _clear_state(self) -> None:
+        self.clear()
+
 
 class VoxelBlockGrid(_BlockGrid):
     """GPU drop-in for pySLAM's `volumetric.VoxelBlockGrid(voxel_size, block_size=8)`."""
@@ -860,6 +953,25 @@ class VoxelBlockGrid(_BlockGrid):
     def remove_low_confidence_voxels(self, min_confidence: float):
         # no-op for the non-semantic grid, as in the reference (voxel_block_grid.hpp:650-676)
         return None
+
+    _STATE_KIND = "grid"
+
+    @staticmethod
+    def _state_arrays() -> dict:
+        v = BLOCK_VOXELS
+        return dict(keys=(np.int32, (3,)), count=(np.int32, (v,)), pos_sum=(np.float32, (v, 3)),
+                    col_sum=(np.float32, (v, 3)))
+
+    def _export_state(self) -> dict:
+        d = self.dump_blocks()
+        del d["hashes"]
+        return d
+
+    def _upload_state(self, blocks: dict) -> None:
+        b = blocks
+        self._check(self._L.b2v_grid_upload_blocks(self._h, len(b["keys"]), b["keys"].ctypes.data,
+                                                   b["count"].ctypes.data, b["pos_sum"].ctypes.data,
+                                                   b["col_sum"].ctypes.data), "b2v_grid_upload_blocks")
 
     def dump_blocks(self):
         nb = self.num_blocks()
@@ -1058,6 +1170,9 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         of a sharded grid runs over all ranks (`sharding.assign_object_ids_to_instance_ids_sharded`)."""
         super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count,
                          self.KIND)
+        # mirrors of the library's settings (class defaults, voxel_data_semantic.h:107-108, 251-254), for save_state
+        self._depth_threshold = np.float32(10.0 if self.KIND == _lib.B2V_SEM_VOTING else 5.0)
+        self._depth_decay_rate = np.float32(0.07)
 
     def _stage_frame(self, images, labels, shape, filter_shadow_points, out):
         return self._L.b2v_sgrid_set_frame(self._h, *images, *labels, shape[0], shape[1], filter_shadow_points, out)
@@ -1065,9 +1180,71 @@ class VoxelBlockSemanticGrid(_BlockGrid):
     # ---- parameters (class-static in the reference, per grid here) ----
     def set_depth_threshold(self, depth_threshold: float):
         self._check(self._L.b2v_sgrid_set_depth_threshold(self._h, float(depth_threshold)), "set_depth_threshold")
+        self._depth_threshold = np.float32(depth_threshold)
 
     def set_depth_decay_rate(self, depth_decay_rate: float):
+        """Only the Bayesian grid has a decay rate (semantic_grid.hpp:31-36); the voting grid ignores it."""
         self._check(self._L.b2v_sgrid_set_depth_decay_rate(self._h, float(depth_decay_rate)), "set_depth_decay_rate")
+        if self.KIND == _lib.B2V_SEM_PROBABILISTIC:
+            self._depth_decay_rate = np.float32(depth_decay_rate)
+
+    # ---- map state (_MapState): the raw slots of b2v_sgrid_export_blocks, the settings and next_object_id ----
+    _STATE_KIND = "semantic"
+    _STATE_ARRAYS = ("count", "pos_sum", "col_sum", "object_id", "class_id", "counter", "ml_logp", "conf", "lab_obj",
+                     "lab_cls", "lab_logp")   # the order of b2v_sgrid_export_blocks / _upload_blocks
+
+    def _state_semantic_kind(self) -> int:
+        return self.KIND
+
+    @property
+    def _STATE_BOUNDS(self):
+        bounds = {"count": (0, None)}
+        if self.KIND == _lib.B2V_SEM_PROBABILISTIC:   # the number of label slots in use
+            bounds["counter"] = (0, _lib.B2V_SEM_MAX_LABELS)
+        return bounds
+
+    def _state_settings(self) -> dict:
+        return dict(depth_threshold=self._depth_threshold, depth_decay_rate=self._depth_decay_rate,
+                    next_object_id=np.int32(self.get_next_object_id()))
+
+    def _restore_settings(self, settings: dict) -> None:
+        self.set_depth_threshold(settings["depth_threshold"])
+        self.set_depth_decay_rate(settings["depth_decay_rate"])
+        self.set_next_object_id(int(settings["next_object_id"]))
+
+    def _state_arrays(self) -> dict:
+        v, k = BLOCK_VOXELS, _lib.B2V_SEM_MAX_LABELS
+        spec = dict(keys=(np.int32, (3,)), count=(np.int32, (v,)), pos_sum=(np.float64, (v, 3)),
+                    col_sum=(np.float32, (v, 3)), object_id=(np.int32, (v,)), class_id=(np.int32, (v,)),
+                    counter=(np.int32, (v,)))
+        if self.KIND == _lib.B2V_SEM_PROBABILISTIC:
+            spec.update(ml_logp=(np.float32, (v,)), conf=(np.float32, (v,)), lab_obj=(np.int32, (v, k)),
+                        lab_cls=(np.int32, (v, k)), lab_logp=(np.float32, (v, k)))
+        return spec
+
+    def export_blocks(self) -> dict:
+        """The raw state of every block (b2v_sgrid_export_blocks): keys [nb,3] and per-voxel arrays [nb,512,...] -
+        count, pos_sum (float64), col_sum, object_id, class_id, counter (the voting counter, or the number of label
+        slots in use) and, on the Bayesian grid, ml_logp, conf and the label slots lab_obj / lab_cls / lab_logp
+        [nb,512,8] in the kernel's own order.  Unlike `dump_blocks`, nothing is derived or reordered."""
+        spec = self._state_arrays()
+        nb = self.num_blocks()
+        d = {name: np.zeros((nb,) + shape, dt) for name, (dt, shape) in spec.items()}
+        if nb:
+            ptrs = [d[name].ctypes.data if name in d else None for name in self._STATE_ARRAYS]
+            n = self._L.b2v_sgrid_export_blocks(self._h, d["keys"].ctypes.data, *ptrs)
+            if n != nb:
+                raise RuntimeError(f"b2v_sgrid_export_blocks returned {n}, expected {nb}: "
+                                   f"{self._L.b2v_sgrid_last_error(self._h).decode()}")
+        return d
+
+    _export_state = export_blocks
+
+    def _upload_state(self, blocks: dict) -> None:
+        n = len(blocks["keys"])
+        ptrs = [blocks[name].ctypes.data if name in blocks and n else None for name in self._STATE_ARRAYS]
+        self._check(self._L.b2v_sgrid_upload_blocks(self._h, n, blocks["keys"].ctypes.data if n else None, *ptrs),
+                    "b2v_sgrid_upload_blocks")
 
     # ---- integrate (volumetric_grid_module.h: integrate(points, colors, class_ids, instance_ids, depths)) ----
     def integrate(self, points, colors=None, class_ids=None, instance_ids=None, depths=None):
