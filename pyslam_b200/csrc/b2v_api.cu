@@ -118,12 +118,12 @@ struct b2v_volume {
     b2v_config cfg{};
     VolumeGeometry geo{};
     cudaStream_t compute = nullptr, copy = nullptr, alloc = nullptr;
-    cudaStream_t last_stream = nullptr;  // caller stream of the most recent frame (synchronised on reads)
+    cudaStream_t update_stream = nullptr;  // stream of the most recent call's update kernels (see last_group_done)
     bool overlap = true;                 // allocate(g+1) on its own stream, concurrent with the update of group g
     bool use_tma = true;                 // stage image tiles with TMA when the layout allows it
     bool fuse = true;                    // b2v_integrate_batch fuses groups of up to kMaxGroup frames
     int group_frames = 16;               // frames per fused group (1..kMaxGroup), b2v_set_group_size
-    cudaEvent_t input_event = nullptr;   // b2v_set_input_event: readiness of the next batch's device inputs
+    cudaEvent_t input_event = nullptr;   // b2v_set_input_event: readiness of the next integrate call's device inputs
     uint32_t group_id = 0;               // groups enqueued since reset; group g uses group buffer g % kGroupBufs
     int last_group_count = 0;            // frames of the most recent group
     cudaEvent_t ev_in = nullptr;         // input fence recorded on the caller's stream
@@ -329,7 +329,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 105; }
+extern "C" int b2v_version(void) { return 106; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -487,12 +487,19 @@ extern "C" int b2v_destroy(b2v_volume *v) {
     return B2V_OK;
 }
 
-// waits for the volume's streams and the caller stream of the most recent frames, then mirrors the counters
+// Completion of the update of the most recent group, or nullptr when no group was enqueued since create or reset.
+// It marks the end of every call's updates so far, whatever their streams: the first group of a call on another
+// update stream than the previous call's waits for it (enqueue_frames), and the groups of one call share a stream.
+static cudaEvent_t last_group_done(const b2v_volume *v) {
+    return v->group_id ? v->ev_group_done[(v->group_id - 1) % kGroupBufs] : nullptr;
+}
+
+// waits for the volume's streams and the updates of every call so far, then mirrors the counters
 static int drain_and_copy_counters(b2v_volume *v) {
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
     B2V_CUDA(v, cudaStreamSynchronize(v->copy));
     B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
-    if (v->last_stream) B2V_CUDA(v, cudaStreamSynchronize(v->last_stream));
+    if (cudaEvent_t e = last_group_done(v)) B2V_CUDA(v, cudaEventSynchronize(e));
     B2V_CUDA(v, cudaMemcpyAsync(v->h_counters, v->meta.counters, kNumCounters * sizeof(uint32_t),
                                 cudaMemcpyDeviceToHost, v->compute));
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
@@ -632,7 +639,7 @@ static int ensure_staging16(b2v_volume *v, size_t pixels) {
     B2V_CUDA(v, cudaStreamSynchronize(v->compute));
     B2V_CUDA(v, cudaStreamSynchronize(v->copy));
     B2V_CUDA(v, cudaStreamSynchronize(v->alloc));
-    if (v->last_stream) B2V_CUDA(v, cudaStreamSynchronize(v->last_stream));
+    if (cudaEvent_t e = last_group_done(v)) B2V_CUDA(v, cudaEventSynchronize(e));
     B2V_CUDA(v, v->d_depth16.reserve(pixels * kStage));
     return B2V_OK;
 }
@@ -742,7 +749,13 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
         if (rc != B2V_OK) return rc;
     }
-    v->last_stream = stream ? cs : nullptr;
+    // This call's updates touch the blocks the previous call's did, and a block's running average depends on frame
+    // order: on another stream they wait for the previous call's last update (on the same stream, stream order does
+    // it).  Overlapped allocate kernels run on their own stream and are not held by this wait.
+    if (cs != v->update_stream) {
+        if (cudaEvent_t e = last_group_done(v)) B2V_CUDA(v, cudaStreamWaitEvent(cs, e, 0));
+        v->update_stream = cs;
+    }
     if (v->lam_H != height || v->lam_W != width || std::memcmp(v->lam_K, K, sizeof(v->lam_K)) != 0) {
         // the lambda image is read by update kernels of earlier frames that may still run, on the library's streams
         // or on a caller's; new intrinsics are rare, so the whole device is drained before the image is rewritten
@@ -883,7 +896,9 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
 extern "C" int b2v_integrate(b2v_volume *v, const float *depth, const uint8_t *color, int32_t height,
                              int32_t width, const double K[4], const double Tcw[16], void *stream) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    return enqueue_frames(v, "b2v_integrate", 1, depth, color, height, width, K, Tcw, stream, nullptr);
+    cudaEvent_t inputs_ready = v->input_event;  // one-shot
+    v->input_event = nullptr;
+    return enqueue_frames(v, "b2v_integrate", 1, depth, color, height, width, K, Tcw, stream, inputs_ready);
 }
 
 extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float *depth,

@@ -47,6 +47,23 @@ def _is_torch_cuda(x) -> bool:
     return hasattr(x, "data_ptr") and hasattr(x, "is_cuda") and bool(x.is_cuda)
 
 
+def _pinned_owner(x):
+    """The torch tensor behind a pinned host array (a numpy view of one included), or None.  The copy engine reads
+    pinned memory after the integrate call returns; pageable memory is staged before it returns."""
+    while x is not None:
+        if hasattr(x, "is_pinned"):
+            return x if x.is_pinned() else None
+        x = getattr(x, "base", None)
+    return None
+
+
+#: B200TsdfVolume holds the device and pinned inputs of the work in flight until a synchronising call.  Before a call
+#: that would take them past this many bytes it waits for the earlier calls and releases their inputs; a storage is
+#: counted once however often it is passed (a resident frame buffer, views into one pool), and an input larger than
+#: the bound is still held: the wait comes only when a later call brings another storage.
+HELD_INPUT_BYTES_MAX = 1 << 30
+
+
 class TriangleMesh:
     """Arrays shaped like `VolumetricIntegrationMesh` (volumetric_integrator_base.py:213-226)."""
 
@@ -153,7 +170,11 @@ class B200TsdfVolume(_MapState):
                 self._L.b2v_destroy(self._h)
                 self._h = C.c_void_p()
             raise RuntimeError(f"b2v_create failed (status {rc}): {msg}")
-        self._keepalive = []  # host arrays of frames still in flight
+        # Inputs the library may still read (device tensors, pinned host memory), by storage address, until a
+        # synchronising call; see HELD_INPUT_BYTES_MAX.
+        self._held, self._held_bytes = {}, 0
+        self._input_event_set = False     # set_input_event named the next call's input event
+        self._producer_event = None       # torch.cuda.Event: device inputs' producers on torch's current stream
 
     # ---- lifetime ----
     def close(self):
@@ -170,6 +191,36 @@ class B200TsdfVolume(_MapState):
     def _check(self, rc: int, what: str):
         if rc != _lib.B2V_OK:
             raise RuntimeError(f"{what} failed (status {rc}): {self._L.b2v_last_error(self._h).decode()}")
+
+    def _order_after_producer(self, tensor, stream):
+        """Device inputs without a caller stream are read on the library's streams, which do not wait for torch's:
+        the call's input event is then recorded on torch's current stream, after the inputs' producers (unless
+        set_input_event named one)."""
+        if stream or self._input_event_set:
+            return
+        import torch
+        if self._producer_event is None:
+            self._producer_event = torch.cuda.Event()
+        self._producer_event.record(torch.cuda.current_stream(tensor.device))
+        self._check(self._L.b2v_set_input_event(self._h, C.c_void_p(self._producer_event.cuda_event)),
+                    "b2v_set_input_event")
+
+    def _to_hold(self, inputs) -> dict:
+        """The storages of `inputs` the enqueued work may read after the call returns and that are not held yet:
+        device tensors and pinned host memory (a freed block would be handed to the next allocation while queued
+        kernels or copies still read it).  Pageable host arrays are staged before the call returns."""
+        new = {}
+        for x in inputs:
+            t = x if _is_torch_cuda(x) else _pinned_owner(x)
+            if t is not None and t.untyped_storage().data_ptr() not in self._held:
+                new[t.untyped_storage().data_ptr()] = t
+        return new
+
+    def _release_held(self) -> int:
+        """Wait for the work in flight and drop the inputs held for it, whatever the status (returned)."""
+        rc = self._L.b2v_synchronize(self._h)
+        self._held, self._held_bytes = {}, 0
+        return rc
 
     # ---- integrate ----
     def integrate(self, depth, color=None, K=None, pose=None, stream=None, depth_scale=None):
@@ -198,7 +249,6 @@ class B200TsdfVolume(_MapState):
             if depth.dim() != 2 or tuple(color.shape) != (H, W, 3):
                 raise RuntimeError("depth must be [H,W] and color [H,W,3]")
             dp, cp = depth.data_ptr(), color.data_ptr()
-            self._keepalive.append((depth, color))
         else:
             d = np.asarray(depth)
             c = np.asarray(color)
@@ -216,22 +266,16 @@ class B200TsdfVolume(_MapState):
             c = np.ascontiguousarray(c)
             H, W = d.shape
             dp, cp = d.ctypes.data, c.ctypes.data
-            self._keepalive.append((d, c))
+            depth, color = d, c
             if raw16:
-                rc = self._L.b2v_integrate_u16(self._h, dp, float(depth_scale), cp, H, W, K4.ctypes.data,
-                                               T.ctypes.data, None)
-                self._check(rc, "b2v_integrate_u16")
-                if len(self._keepalive) > 8:
-                    del self._keepalive[:-8]
+                self._enqueue("b2v_integrate_u16", self._L.b2v_integrate_u16,
+                              (dp, float(depth_scale), cp, H, W, K4.ctypes.data, T.ctypes.data, None), (d, c), None)
                 return
         if depth_scale is not None:
             raise RuntimeError("depth_scale is supported for host (numpy) uint16 depth images")
-        rc = self._L.b2v_integrate(self._h, dp, cp, H, W, K4.ctypes.data, T.ctypes.data,
-                                   C.c_void_p(stream) if stream else None)
-        self._check(rc, "b2v_integrate")
-        if len(self._keepalive) > 8:
-            # staging ring is 4 deep: anything older has been consumed by the copy engine
-            del self._keepalive[:-8]
+        self._enqueue("b2v_integrate", self._L.b2v_integrate,
+                      (dp, cp, H, W, K4.ctypes.data, T.ctypes.data, C.c_void_p(stream) if stream else None),
+                      (depth, color), stream)
 
     def integrate_batch(self, depths, colors, K, poses, stream=None, depth_scale=None):
         """n frames back to back (the rebuild(map) bulk path, base.py:1242-1318): depths [n,H,W] f32,
@@ -248,7 +292,7 @@ class B200TsdfVolume(_MapState):
                 raise RuntimeError("depth_scale goes with 16-bit depth images")
             H, W = int(depths.shape[1]), int(depths.shape[2])
             dp, cp = depths.data_ptr(), colors.data_ptr()
-            hold = (depths, colors)
+            inputs = (depths, colors)
         else:
             if raw16 and np.asarray(depths).dtype != np.uint16:
                 raise RuntimeError("depth_scale goes with uint16 depth images")
@@ -258,19 +302,40 @@ class B200TsdfVolume(_MapState):
                 raise RuntimeError("depths must be [n,H,W], colors [n,H,W,3], poses [n,4,4]")
             H, W = d.shape[1:]
             dp, cp = d.ctypes.data, c.ctypes.data
-            hold = (d, c)
+            inputs = (d, c)
+        s = C.c_void_p(stream) if stream else None
         if raw16:
-            rc = self._L.b2v_integrate_batch_u16(self._h, n, dp, float(depth_scale), cp, H, W, K4.ctypes.data,
-                                                 T.ctypes.data, C.c_void_p(stream) if stream else None)
+            self._enqueue("b2v_integrate_batch_u16", self._L.b2v_integrate_batch_u16,
+                          (n, dp, float(depth_scale), cp, H, W, K4.ctypes.data, T.ctypes.data, s), inputs, stream)
         else:
-            rc = self._L.b2v_integrate_batch(self._h, n, dp, cp, H, W, K4.ctypes.data, T.ctypes.data,
-                                             C.c_void_p(stream) if stream else None)
-        self._check(rc, "b2v_integrate_batch")
-        self._keepalive = [hold]
+            self._enqueue("b2v_integrate_batch", self._L.b2v_integrate_batch,
+                          (n, dp, cp, H, W, K4.ctypes.data, T.ctypes.data, s), inputs, stream)
+
+    def _enqueue(self, what, fn, args, inputs, stream):
+        """One integrate entry point: device inputs are ordered after their producers, and the inputs the enqueued
+        work reads are held."""
+        new = self._to_hold(inputs)
+        new_bytes = sum(t.untyped_storage().nbytes() for t in new.values())
+        if new_bytes and self._held and self._held_bytes + new_bytes > HELD_INPUT_BYTES_MAX:
+            # bounded: wait for the earlier calls and release their inputs first (only when this call brings new
+            # storage: inputs that stay resident, such as a reused frame buffer, are held once and cost no wait).
+            # A full pool is reported by the next synchronising call, as without this wait.
+            rc = self._release_held()
+            if rc not in (_lib.B2V_OK, _lib.B2V_ERR_CAPACITY):
+                self._check(rc, "b2v_synchronize")
+        if _is_torch_cuda(inputs[0]):
+            self._order_after_producer(inputs[0], stream)
+        try:
+            rc = fn(self._h, *args)
+        finally:
+            self._input_event_set = False     # one-shot: the call consumed it
+        self._check(rc, what)
+        self._held.update(new)
+        self._held_bytes += new_bytes
 
     def synchronize(self):
-        self._check(self._L.b2v_synchronize(self._h), "b2v_synchronize")
-        self._keepalive.clear()
+        """Wait for the work in flight; the inputs held for it are released."""
+        self._check(self._release_held(), "b2v_synchronize")
 
     def capacity(self):
         """(blocks the pool has storage for now, growths since creation); synchronises."""
@@ -280,8 +345,9 @@ class B200TsdfVolume(_MapState):
 
     def reset(self):
         """`self.volume.reset()` (tsdf.py:156; base.py:642)."""
-        self._check(self._L.b2v_reset(self._h), "b2v_reset")
-        self._keepalive.clear()
+        rc = self._L.b2v_reset(self._h)
+        self._held, self._held_bytes = {}, 0
+        self._check(rc, "b2v_reset")
 
     # ---- inspection ----
     def num_blocks(self) -> int:
@@ -319,9 +385,11 @@ class B200TsdfVolume(_MapState):
         self._check(self._L.b2v_set_fusion(self._h, 1 if enable else 0), "b2v_set_fusion")
 
     def set_input_event(self, cuda_event):
-        """The next integrate_batch call's device frames are ready when `cuda_event` (a raw cudaEvent_t handle, e.g.
-        `torch.cuda.Event.cuda_event`) fires; see b2v_set_input_event."""
+        """The next integrate / integrate_batch call's device frames are ready when `cuda_event` (a raw cudaEvent_t
+        handle, e.g. `torch.cuda.Event.cuda_event`) fires; see b2v_set_input_event.  Without it, the device frames of
+        a call without a stream wait for torch's current stream."""
         self._check(self._L.b2v_set_input_event(self._h, C.c_void_p(int(cuda_event))), "b2v_set_input_event")
+        self._input_event_set = True
 
     def set_group_size(self, frames: int):
         """Frames per fused group of integrate_batch (1..32, default 16); results do not depend on it."""
