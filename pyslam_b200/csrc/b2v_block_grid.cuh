@@ -44,18 +44,19 @@ struct ImagePoint {
     float u, v, depth;
 };
 
-// false when no voxel of the block can lie in the query's key range
-__device__ __forceinline__ bool block_in_range(const GridQuery &Q, const int4 key) {
+// false when no voxel of the block (side 1 << L) can lie in the query's key range
+template <int L> __device__ __forceinline__ bool block_in_range(const GridQuery &Q, const int4 key) {
     const int k[3] = {key.x, key.y, key.z};
 #pragma unroll
     for (int a = 0; a < 3; ++a)
-        if (k[a] < block_coord(Q.min_key[a]) || k[a] > block_coord(Q.max_key[a])) return false;
+        if (k[a] < grid_block_coord<L>(Q.min_key[a]) || k[a] > grid_block_coord<L>(Q.max_key[a])) return false;
     return true;
 }
 
-// voxel t (lx + 8 ly + 64 lz) of the block lies in the query's key range
-__device__ __forceinline__ bool voxel_in_range(const GridQuery &Q, const int4 key, int t) {
-    const int vk[3] = {key.x * kB + (t & 7), key.y * kB + ((t >> 3) & 7), key.z * kB + (t >> 6)};
+// voxel t (lx + B ly + B^2 lz) of the block lies in the query's key range
+template <int L> __device__ __forceinline__ bool voxel_in_range(const GridQuery &Q, const int4 key, int t) {
+    constexpr int kS = GridBlock<L>::kSide;
+    const int vk[3] = {key.x * kS + (t & (kS - 1)), key.y * kS + ((t >> L) & (kS - 1)), key.z * kS + (t >> (2 * L))};
 #pragma unroll
     for (int a = 0; a < 3; ++a)
         if (vk[a] < Q.min_key[a] || vk[a] > Q.max_key[a]) return false;
@@ -104,6 +105,30 @@ __device__ __forceinline__ uint32_t uploaded_block_index(const HashTable &T, con
     }
     __syncthreads();
     return s_idx;
+}
+
+// The same for uploaded block b (of n) and voxel t of the voxel-range CTA mapping (cta_voxel): B >= 8, the CTA lies in
+// one block and thread 0 finds it; B < 8, the CTA spans 512 / B^3 blocks and the thread of each block's voxel 0 finds
+// that block (kNoBlock past the n uploaded blocks).
+template <int L>
+__device__ __forceinline__ uint32_t uploaded_voxel_block(const HashTable &T, const int4 *keys, const uint32_t b,
+                                                         const int t, const uint32_t n, const uint32_t pool_capacity) {
+    if constexpr (3 * L >= 9) {
+        return uploaded_block_index(T, keys[b], pool_capacity);
+    } else {
+        __shared__ uint32_t s_idx[512 >> (3 * L)];
+        if (t == 0) {
+            uint32_t idx = kNoBlock;
+            if (b < n) {
+                const int4 key = keys[b];
+                const uint32_t slot = table_find(T, key.x, key.y, key.z);
+                idx = slot == kEmpty ? kNoBlock : T.entries[slot].w;
+            }
+            s_idx[threadIdx.x >> (3 * L)] = idx < pool_capacity ? idx : kNoBlock;
+        }
+        __syncthreads();
+        return s_idx[threadIdx.x >> (3 * L)];
+    }
 }
 
 }  // namespace b2v

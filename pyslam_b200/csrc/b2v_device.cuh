@@ -65,6 +65,37 @@ __host__ __device__ __forceinline__ uint32_t slot_hash(int x, int y, int z) {
 __host__ __device__ __forceinline__ int block_coord(int v) { return v >> kLog2B; }
 __host__ __device__ __forceinline__ int local_coord(int v) { return v & (kB - 1); }
 
+// ---- the sparse block grids (b2v_grid.cu, b2v_semantic.cu): block side B = 1 << L, L in [0, kMaxGridLog2B] ----
+// The same key rules with B a compile-time power of two: block key floor_div(v, B) = v >> L, local key v - B b =
+// v & (B - 1), voxel index lx + B ly + B^2 lz (voxel_hashing.h:139-161, voxel_block.h:67-70).  The TSDF volume keeps
+// kB above.  At L = 3 each of these is the expression of the helpers above.
+constexpr int kMaxGridLog2B = 4;   // B = 16
+template <int L> struct GridBlock {
+    static constexpr int kSide = 1 << L;
+    static constexpr int kVox = 1 << (3 * L);   // voxels per block
+};
+template <int L> __host__ __device__ __forceinline__ int grid_block_coord(int v) { return v >> L; }
+template <int L> __host__ __device__ __forceinline__ int grid_local_coord(int v) { return v & ((1 << L) - 1); }
+template <int L> __host__ __device__ __forceinline__ int grid_local_index(int vx, int vy, int vz) {
+    return grid_local_coord<L>(vx) + (grid_local_coord<L>(vy) << L) + (grid_local_coord<L>(vz) << (2 * L));
+}
+
+#ifdef __CUDACC__
+// Voxel-range CTA mapping of the grids' per-voxel passes: CTA c covers the 512 consecutive voxels [512 c, 512 c + 512)
+// of the pool, where voxel id = pool index * B^3 + local index.  *b: the pool index, *t: the local index of this
+// thread's voxel.  B = 8: one CTA per block (b = blockIdx.x, t = threadIdx.x); B = 16: eight CTAs per block; B < 8: a
+// CTA spans 512 / B^3 blocks, and the last CTA may reach past the blocks in use (callers bound b).
+template <int L> __device__ __forceinline__ void cta_voxel(uint32_t *b, int *t) {
+    if constexpr (3 * L >= 9) {
+        *b = blockIdx.x >> (3 * L - 9);
+        *t = static_cast<int>(((blockIdx.x & ((1u << (3 * L - 9)) - 1u)) << 9) + threadIdx.x);
+    } else {
+        *b = (blockIdx.x << (9 - 3 * L)) + (threadIdx.x >> (3 * L));
+        *t = static_cast<int>(threadIdx.x & ((1u << (3 * L)) - 1u));
+    }
+}
+#endif
+
 #ifdef __CUDACC__
 
 // (int32)floorf(x * inv_vs) with the multiply rounded on its own (never contracted)

@@ -6,6 +6,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -380,10 +381,28 @@ struct BlockIndex {
     // hash sharding (SURVEY.md 8e): the grid holds only the blocks with block_owner(key, shard_count) == shard_rank
     uint32_t shard_rank = 0, shard_count = 1;
 };
-// Block insert of every point (optional per-point mask `valid`): each block a point falls in gets a table entry and a
-// pool index (kNoBlock once the index passes index.capacity).  Points are float or double [n][3].
+// Block insert of every point (optional per-point mask `valid`): each block (side 1 << log2_block) a point falls in
+// gets a table entry and a pool index (kNoBlock once the index passes index.capacity).  Points are float or double
+// [n][3].
 cudaError_t launch_point_insert(const void *pts, bool pts_f64, const uint8_t *valid, int64_t n, float inv_vs,
-                                const HashTable &table, const BlockIndex &index, cudaStream_t stream);
+                                int log2_block, const HashTable &table, const BlockIndex &index, cudaStream_t stream);
+
+// The block sides the grids accept: B = 1, 2, 8, 16 (L = 0, 1, 3, 4).  B = 4 keeps the rejection the grids gave every
+// size but 8 before block sizes were supported, which their argument checks pin (tests/test_gpu_grid.py,
+// tests/test_gpu_semantic.py); the kernels and the key rules are written for any L in [0, kMaxGridLog2B].
+__host__ __device__ constexpr bool grid_log2_block_supported(int l) { return l == 0 || l == 1 || l == 3 || l == 4; }
+static_assert(kMaxGridLog2B == 4, "grid_log2_block_supported lists L = 0 .. 4");
+
+// The grids' block side B = 1 << L is a template parameter of their kernels: f(std::integral_constant<int, L>{}) for
+// a supported log2_block (grid_log2_block_supported), the one place a grid's runtime block size picks its kernels.
+template <typename F> decltype(auto) with_grid_block(int log2_block, F &&f) {
+    switch (log2_block) {
+    case 0: return f(std::integral_constant<int, 0>{});
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    default: return f(std::integral_constant<int, 4>{});
+    }
+}
 
 // Fused RGBD front-end: depth2pointcloud (pyslam/utilities/depth.py:45-85) + world transform
 // (pyslam/dense/volumetric_integrator_voxel_grid.py:262-281, volumetric_integrator_voxel_semantic_grid.py:411-436),
@@ -417,6 +436,7 @@ struct BlockGridCore {
     cudaStream_t stream = nullptr;
     // the reference stores the voxel size as float and inverts it in float (voxel_block_grid.h:225-226, .hpp:6)
     float inv_voxel_size = 0.0f;
+    int log2_block = 3;   // block side B = 1 << log2_block (block_size of create)
     HashTable table{};   // views of table_mem, block_keys, counters
     BlockIndex index{};
     // the table and block_keys are sized for index.capacity; a growable grid maps its storage on demand
@@ -429,12 +449,27 @@ struct BlockGridCore {
     DeviceBuffer<uint32_t> d_sums, d_offs, d_total;   // count -> scan of the read-outs
     std::string err;
 
+    // log2 of a supported block size (1, 2, 8, 16), else -1
+    static int log2_block_size(int32_t block_size);
+    // the most blocks of side 1 << log2_block a grid may hold: 2^31 voxels (the semantic sort key
+    // pool index * B^3 + local stays below its kBadVid), 2^22 blocks at B = 8, and at most 2^30 blocks (the table holds
+    // twice the blocks in a power of two of 32-bit slots)
+    static uint32_t max_blocks(int log2_block) {
+        return static_cast<uint32_t>(std::min<uint64_t>(1ull << 30, (1ull << 31) >> (3 * log2_block)));
+    }
     // the arguments both grids accept (max_capacity_blocks 0: a fixed grid)
     static bool valid_args(double voxel_size, int32_t block_size, uint32_t capacity_blocks,
                            uint32_t max_capacity_blocks);
     // stream, table, block index and counters for max(capacity_blocks, max_capacity_blocks) blocks; the grid then
     // maps its storage, sets index.pool_capacity and clears the index (clear_index) with its storage
-    int create(double voxel_size, uint32_t capacity_blocks, uint32_t max_capacity_blocks, int32_t device);
+    int create(double voxel_size, int32_t block_size, uint32_t capacity_blocks, uint32_t max_capacity_blocks,
+               int32_t device);
+    uint32_t block_voxels() const { return 1u << (3 * log2_block); }   // B^3
+    // CTAs of a per-voxel pass over n_blocks blocks (cta_voxel): one per 512 voxels
+    uint32_t voxel_ctas(uint32_t n_blocks) const {
+        return static_cast<uint32_t>((static_cast<uint64_t>(n_blocks) * block_voxels() + 511) / 512);
+    }
+    template <typename F> decltype(auto) dispatch(F &&f) const { return with_grid_block(log2_block, f); }
     void destroy();         // waits for the stream, destroys it and frees the pinned mirror
     int fetch_counters();   // h_counters := index.counters (synchronises)
     int read_counters();    // fetch_counters + B2V_ERR_CAPACITY ("hash table full" / "block pool full") on an error bit
@@ -458,10 +493,10 @@ struct BlockGridCore {
     // index is kNoBlock and the error flag says "block pool full").  Asynchronous.  A growable grid then maps storage
     // for the new pool count (resolve) before the grid's scatter kernel copies the voxels in.
     int insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys);
-    // room for n_blocks per-block counts in d_sums / offsets in d_offs
-    int ensure_scan(uint32_t n_blocks);
-    // exclusive scan of the per-block counts d_sums -> d_offs, and their total (synchronises)
-    cudaError_t scan_total(uint32_t n_blocks, uint32_t *total);
+    // room for n per-CTA counts in d_sums / offsets in d_offs (the CTAs of a per-voxel pass, voxel_ctas)
+    int ensure_scan(uint32_t n);
+    // exclusive scan of the per-CTA counts d_sums -> d_offs, and their total (synchronises)
+    cudaError_t scan_total(uint32_t n, uint32_t *total);
     GridQuery all_query(int min_count) const;
     // voxel_block_grid.hpp:828-831: keys in double with the float inverse voxel size
     GridQuery box_query(const double bbox[6], int min_count) const;

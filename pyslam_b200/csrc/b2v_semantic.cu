@@ -11,7 +11,7 @@
 // deterministic build processes the points of one call in input order, so this implementation does the same
 // per voxel:
 //   1. insert   one thread per point: block key (bit-exact, in the point's own precision) -> 128-bit-CAS table
-//   2. keys     one thread per point: sort key = pool_index * 512 + local voxel index
+//   2. keys     one thread per point: sort key = pool_index * B^3 + local voxel index
 //   3. sort     stable LSD radix sort of (key, point index) pairs (cub::DeviceRadixSort - library code)
 //   4. runs     the first element of every run of equal keys walks its run in input order and applies the
 //               reference's per-observation update: count, position_sum (float64), color_sum (float32), labels
@@ -56,7 +56,7 @@ struct SemBlockIndex {
 
 struct SemGrid {
     SemBlockIndex index;
-    int32_t *count;     // [V]            V = capacity * 512, voxel id = pool index * 512 + lx + 8 ly + 64 lz
+    int32_t *count;     // [V]            V = capacity * B^3, voxel id = pool index * B^3 + lx + B ly + B^2 lz
     double *pos;        // [V][3]
     float *col;         // [V][3]
     int32_t *obj, *cls; // [V]            current label (voting) / cached argmax (Bayesian)
@@ -73,7 +73,7 @@ struct SemGrid {
 // Only points whose block has a pool index in [lo, hi) get a key; the others get kBadVid, sort last and are left out
 // by the runs.  The first pass of a call covers the blocks with storage, [0, pool_capacity); after a growth the
 // keys -> sort -> runs passes are replayed over the blocks that just got storage.
-template <typename T>
+template <typename T, int L>
 __global__ void __launch_bounds__(256)
 sem_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, const int64_t n, const float inv_vs,
                 const HashTable H, const SemGrid G, const uint32_t lo, const uint32_t hi, uint32_t *__restrict__ vid,
@@ -84,12 +84,12 @@ sem_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, co
               vz = point_voxel_coord(pts[3 * i + 2], inv_vs);
     uint32_t key = kBadVid;
     const uint32_t slot = (valid == nullptr || valid[i])
-                              ? table_find(H, block_coord(vx), block_coord(vy), block_coord(vz))
+                              ? table_find(H, grid_block_coord<L>(vx), grid_block_coord<L>(vy), grid_block_coord<L>(vz))
                               : kEmpty;
     if (slot != kEmpty) {
         const uint32_t idx = H.entries[slot].w;
         if (idx >= lo && idx < hi)   // kNoBlock is past every window
-            key = idx * kVox + static_cast<uint32_t>(local_coord(vx) + (local_coord(vy) << 3) + (local_coord(vz) << 6));
+            key = idx * GridBlock<L>::kVox + static_cast<uint32_t>(grid_local_index<L>(vx, vy, vz));
     }
     vid[i] = key;
     order[i] = static_cast<uint32_t>(i);
@@ -334,8 +334,13 @@ __device__ __forceinline__ void sem_reset_voxel(const SemGrid &G, uint32_t v) { 
 
 // op 0: remove_low_count_voxels(a)  1: remove_low_confidence_segments(a)  2: remove_segment(a)
 // op 3: merge_segments(a, b)  (voxel_block_grid.hpp:625-647; voxel_block_semantic_grid.hpp:101-183)
-__global__ void __launch_bounds__(kVox) sem_edit_kernel(const SemGrid G, const int op, const int a, const int b) {
+// Per-voxel passes: one 512-thread CTA per 512 pool voxels (cta_voxel), so voxel id = blockIdx.x * 512 + threadIdx.x
+// whatever B; nv (the voxels of the blocks in use) bounds the last CTA when B < 8 and is not read at B >= 8.
+template <int L>
+__global__ void __launch_bounds__(kVox)
+sem_edit_kernel(const SemGrid G, const int op, const int a, const int b, const uint32_t nv) {
     const uint32_t v = blockIdx.x * kVox + threadIdx.x;
+    if (3 * L < 9 && v >= nv) return;
     const int c = G.count[v];
     if (op == 0) {
         if (c < a) sem_reset_voxel(G, v);
@@ -367,12 +372,13 @@ __global__ void __launch_bounds__(kVox) sem_edit_kernel(const SemGrid G, const i
 // ---- spatial filter: read-outs, carve and instance -> object association ----------------------------------------
 // the key range, then the fine test (box or frustum) on the voxel's float64 mean position.  Empty voxels never qualify
 // (get_voxels_in_bb, voxel_block_grid.hpp:822-1016; iterate_voxels_in_camera_frustrum, :1336-1460).
+template <int L>
 __device__ __forceinline__ bool sem_in_region(const SemGrid &G, const GridQuery &Q, uint32_t b, int t, ImagePoint *ip) {
     const int4 key = G.index.block_keys[b];
-    if (!block_in_range(Q, key)) return false;
-    const uint32_t v = b * kVox + t;
+    if (!block_in_range<L>(Q, key)) return false;
+    const uint32_t v = b * GridBlock<L>::kVox + t;
     const int c = G.count[v];
-    if (c < 1 || !voxel_in_range(Q, key, t)) return false;
+    if (c < 1 || !voxel_in_range<L>(Q, key, t)) return false;
     const double dc = static_cast<double>(c);
     double p[3];
 #pragma unroll
@@ -381,34 +387,50 @@ __device__ __forceinline__ bool sem_in_region(const SemGrid &G, const GridQuery 
 }
 
 // the read-out filter: count >= min_count and confidence >= min_conf (voxel_block_grid.hpp:797-803), then in box and
-// frustum mode (get_voxels_in_bb, get_voxels_in_camera_frustrum :1019-1195) the spatial filter
-__device__ __forceinline__ bool sem_keep(const SemGrid &G, const GridQuery &Q, uint32_t b, int t, float min_conf,
-                                         float *conf_out) {
-    const uint32_t v = b * kVox + t;
+// frustum mode (get_voxels_in_bb, get_voxels_in_camera_frustrum :1019-1195) the spatial filter.  A voxel of a block
+// past nb (the last CTA of a pass at B < 8) is never kept.
+template <int L>
+__device__ __forceinline__ bool sem_keep(const SemGrid &G, const GridQuery &Q, uint32_t b, int t, uint32_t nb,
+                                         float min_conf, float *conf_out) {
+    if (3 * L < 9 && b >= nb) {
+        *conf_out = 0.0f;
+        return false;
+    }
+    const uint32_t v = b * GridBlock<L>::kVox + t;
     const int c = G.count[v];
     const float conf = sem_confidence(G, v, c);
     *conf_out = conf;
     if (!(c >= Q.min_count && conf >= min_conf)) return false;
     if (Q.mode == kQueryAll) return true;
     ImagePoint ip;
-    return sem_in_region(G, Q, b, t, &ip);
+    return sem_in_region<L>(G, Q, b, t, &ip);
 }
 
+template <int L>
 __global__ void __launch_bounds__(kVox)
-sem_count_kernel(const SemGrid G, const GridQuery Q, const float min_conf, uint32_t *__restrict__ sums) {
+sem_count_kernel(const SemGrid G, const GridQuery Q, const float min_conf, uint32_t *__restrict__ sums,
+                 const uint32_t nb) {
     __shared__ uint32_t s_warp[16];
     float conf;
-    block_count_512(sem_keep(G, Q, blockIdx.x, threadIdx.x, min_conf, &conf), s_warp, sums + blockIdx.x);
+    uint32_t b;
+    int t;
+    cta_voxel<L>(&b, &t);
+    block_count_512(sem_keep<L>(G, Q, b, t, nb, min_conf, &conf), s_warp, sums + blockIdx.x);
 }
 
+template <int L>
 __global__ void __launch_bounds__(kVox)
 sem_emit_kernel(const SemGrid G, const GridQuery Q, const float min_conf,
                 const uint32_t *__restrict__ offs, double *__restrict__ out_pts, float *__restrict__ out_cols,
-                int32_t *__restrict__ out_cls, int32_t *__restrict__ out_obj, float *__restrict__ out_conf) {
+                int32_t *__restrict__ out_cls, int32_t *__restrict__ out_obj, float *__restrict__ out_conf,
+                const uint32_t nb) {
     __shared__ uint32_t s_warp[16];
     const uint32_t v = blockIdx.x * kVox + threadIdx.x;
     float conf;
-    const bool keep = sem_keep(G, Q, blockIdx.x, threadIdx.x, min_conf, &conf);
+    uint32_t b;
+    int t;
+    cta_voxel<L>(&b, &t);
+    const bool keep = sem_keep<L>(G, Q, b, t, nb, min_conf, &conf);
     const size_t pos = offs[blockIdx.x] + block_excl_scan_512(keep ? 1u : 0u, s_warp);
     if (!keep) return;
     const int c = G.count[v];
@@ -445,14 +467,19 @@ __device__ __forceinline__ void sem_set_object_id(const SemGrid &G, uint32_t v, 
 
 // carve (voxel_grid_carving.h:47-80): reset voxels in front of the observed surface by more than the threshold;
 // the depth image is indexed with truncated pixel coordinates, like at<float>(v, u)
+template <int L>
 __global__ void __launch_bounds__(kVox)
-sem_carve_kernel(const SemGrid G, const GridQuery Q, const float *__restrict__ depth, const float thr) {
-    const uint32_t b = blockIdx.x;
+sem_carve_kernel(const SemGrid G, const GridQuery Q, const float *__restrict__ depth, const float thr,
+                 const uint32_t nb) {
+    uint32_t b;
+    int t;
+    cta_voxel<L>(&b, &t);
+    if (3 * L < 9 && b >= nb) return;
     ImagePoint ip;
-    if (!sem_in_region(G, Q, b, threadIdx.x, &ip)) return;
+    if (!sem_in_region<L>(G, Q, b, t, &ip)) return;
     const float image_depth = depth[static_cast<size_t>(static_cast<int>(ip.v)) * Q.W + static_cast<int>(ip.u)];
     if (image_depth <= 0.0f || !isfinite(image_depth)) return;
-    if (ip.depth < image_depth - thr) sem_reset_voxel(G, b * kVox + threadIdx.x);
+    if (ip.depth < image_depth - thr) sem_reset_voxel(G, blockIdx.x * kVox + threadIdx.x);
 }
 
 // process_point of assign_object_ids_to_instance_ids (voxel_semantic_data_association.h:171-229): every voxel in
@@ -469,15 +496,19 @@ __device__ __forceinline__ unsigned long long assoc_key(int32_t inst, int32_t ob
            (static_cast<uint32_t>(obj) ^ 0x80000000u);
 }
 
+template <int L>
 __global__ void __launch_bounds__(kVox)
 sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__ class_img,
                  const int32_t *__restrict__ inst_img, const float *__restrict__ depth_img, const float thr,
                  const int do_carving, int32_t *__restrict__ pend, unsigned long long *__restrict__ records,
-                 uint32_t *__restrict__ n_records, const uint32_t cap_records) {
-    const uint32_t b = blockIdx.x;
+                 uint32_t *__restrict__ n_records, const uint32_t cap_records, const uint32_t nb) {
+    uint32_t b;
+    int t;
+    cta_voxel<L>(&b, &t);
+    if (3 * L < 9 && b >= nb) return;
     ImagePoint ip;
-    if (!sem_in_region(G, Q, b, threadIdx.x, &ip)) return;
-    const uint32_t v = b * kVox + threadIdx.x;
+    if (!sem_in_region<L>(G, Q, b, t, &ip)) return;
+    const uint32_t v = blockIdx.x * kVox + threadIdx.x;
     const size_t px = static_cast<size_t>(static_cast<int>(ip.v)) * Q.W + static_cast<int>(ip.u);
     const int32_t image_class = class_img[px];
     if (image_class < 0) return;
@@ -521,10 +552,12 @@ sem_assoc_triples_kernel(const unsigned long long *__restrict__ keys, const uint
 }
 
 // deferred assignment (voxel_semantic_data_association.h:354-370): pending voxels take their instance's final id
+template <int L>
 __global__ void __launch_bounds__(kVox)
 sem_assoc_apply_kernel(const SemGrid G, const int32_t *__restrict__ pend, const int32_t *__restrict__ map_inst,
-                       const int32_t *__restrict__ map_obj, const int n_map) {
+                       const int32_t *__restrict__ map_obj, const int n_map, const uint32_t nv) {
     const uint32_t v = blockIdx.x * kVox + threadIdx.x;
+    if (3 * L < 9 && v >= nv) return;
     const int32_t inst = pend[v];
     if (inst < 0) return;
     int lo = 0, hi = n_map - 1;
@@ -555,21 +588,23 @@ __global__ void sem_fill_kernel(const SemGrid G, const size_t v0, const size_t v
 struct SemUpload {
     void *dst[kSemArrays];
     const void *src[kSemArrays];
-    uint32_t block_bytes[kSemArrays];   // multiples of 16
+    uint32_t block_bytes[kSemArrays];   // multiples of sizeof(W)
     int32_t n_arrays;
 };
 
-// one CTA per uploaded block: every array's run of the block, 16 bytes per thread and step, replacing what the pool
-// block held
+// one CTA per uploaded block: every array's run of the block, one word W per thread and step, replacing what the pool
+// block held.  W = uint4 where every run is a multiple of 16 bytes (B >= 2), else uint32_t (B = 1).  A byte copy of
+// whole runs, not a per-voxel pass: it keeps one block per CTA at every B.
+template <typename W>
 __global__ void __launch_bounds__(256)
 sem_scatter_kernel(const int4 *__restrict__ keys, const SemUpload U, const HashTable T, const uint32_t pool_capacity) {
     const uint32_t b = blockIdx.x;
     const uint32_t idx = uploaded_block_index(T, keys[b], pool_capacity);
     if (idx == kNoBlock) return;
     for (int k = 0; k < U.n_arrays; ++k) {
-        const uint32_t words = U.block_bytes[k] / 16u;
-        const uint4 *src = static_cast<const uint4 *>(U.src[k]) + static_cast<size_t>(b) * words;
-        uint4 *dst = static_cast<uint4 *>(U.dst[k]) + static_cast<size_t>(idx) * words;
+        const uint32_t words = U.block_bytes[k] / static_cast<uint32_t>(sizeof(W));
+        const W *src = static_cast<const W *>(U.src[k]) + static_cast<size_t>(b) * words;
+        W *dst = static_cast<W *>(U.dst[k]) + static_cast<size_t>(idx) * words;
         for (uint32_t w = threadIdx.x; w < words; w += blockDim.x) dst[w] = src[w];
     }
 }
@@ -628,7 +663,7 @@ struct b2v_sgrid : BlockGridCore {
 extern "C" const char *b2v_sgrid_last_error(const b2v_sgrid *g) { return g ? g->err.c_str() : "null grid"; }
 
 static int sgrid_clear_device(b2v_sgrid *g, uint32_t used_blocks) {
-    const size_t nv = static_cast<size_t>(used_blocks) * kVox;
+    const size_t nv = static_cast<size_t>(used_blocks) * g->block_voxels();
     const int rc = g->clear_index();
     if (rc != B2V_OK || nv == 0) return rc;
     B2V_CUDA(g, cudaMemsetAsync(g->G.count, 0, nv * sizeof(int32_t), g->stream));
@@ -675,7 +710,7 @@ static bool sgrid_map_storage(b2v_sgrid *g, uint64_t blocks, std::string *err) {
     bool ok = true;
     uint64_t storage = g->index.capacity;
     for (int k = 0; k < na; ++k) {
-        const size_t block_bytes = arr[k].voxel_bytes * kVox;
+        const size_t block_bytes = arr[k].voxel_bytes * g->block_voxels();
         ok = ok && vmm_map(&g->store[k], static_cast<size_t>(blocks) * block_bytes, g->stream, err);
         storage = std::min<uint64_t>(storage, g->store[k].mapped / block_bytes);
     }
@@ -692,9 +727,10 @@ extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32
                                    uint32_t max_capacity_blocks, int32_t kind, int32_t device, b2v_sgrid **out) {
     if (!out) return B2V_ERR_INVALID_ARGUMENT;
     *out = nullptr;
-    // the sort key pool_index * 512 + voxel must stay below kBadVid: at most 2^22 blocks
+    // the sort key pool_index * B^3 + voxel must stay below kBadVid: at most 2^31 / B^3 blocks (2^22 at B = 8)
     if (!BlockGridCore::valid_args(voxel_size, block_size, capacity_blocks, max_capacity_blocks) ||
-        capacity_blocks > (1u << 22) || (kind != B2V_SEM_VOTING && kind != B2V_SEM_PROBABILISTIC))
+        capacity_blocks > BlockGridCore::max_blocks(BlockGridCore::log2_block_size(block_size)) ||
+        (kind != B2V_SEM_VOTING && kind != B2V_SEM_PROBABILISTIC))
         return B2V_ERR_INVALID_ARGUMENT;
     b2v_sgrid *g = new (std::nothrow) b2v_sgrid();
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
@@ -703,12 +739,12 @@ extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32
     g->G.depth_threshold = kind == B2V_SEM_VOTING ? 10.0f : 5.0f;
     g->G.depth_decay_rate = 0.07f;
     *out = g;
-    int rc = g->create(voxel_size, capacity_blocks, max_capacity_blocks, device);
+    int rc = g->create(voxel_size, block_size, capacity_blocks, max_capacity_blocks, device);
     if (rc != B2V_OK) return rc;
     SemArray arr[kSemArrays];
     const int na = sgrid_arrays(g, arr);
     for (int k = 0; k < na; ++k) {
-        if (!vmm_reserve(&g->store[k], static_cast<size_t>(g->index.capacity) * kVox * arr[k].voxel_bytes, device,
+        if (!vmm_reserve(&g->store[k], static_cast<size_t>(g->index.capacity) * g->block_voxels() * arr[k].voxel_bytes, device,
                          &g->err))
             return B2V_ERR_CUDA;
         *arr[k].ptr = reinterpret_cast<void *>(g->store[k].va);
@@ -782,12 +818,17 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
 static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid, uint32_t lo, uint32_t hi) {
     cudaStream_t s = g->stream;
     const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    if (in.pts_f64)
-        sem_keys_kernel<double><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n, g->inv_voxel_size,
-                                                     g->table, g->dev(), lo, hi, g->d_vid[0].get(), g->d_ord[0].get());
-    else
-        sem_keys_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n, g->inv_voxel_size,
-                                                    g->table, g->dev(), lo, hi, g->d_vid[0].get(), g->d_ord[0].get());
+    g->dispatch([&](auto l) {
+        constexpr int L = decltype(l)::value;
+        if (in.pts_f64)
+            sem_keys_kernel<double, L><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n,
+                                                            g->inv_voxel_size, g->table, g->dev(), lo, hi,
+                                                            g->d_vid[0].get(), g->d_ord[0].get());
+        else
+            sem_keys_kernel<float, L><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n,
+                                                           g->inv_voxel_size, g->table, g->dev(), lo, hi,
+                                                           g->d_vid[0].get(), g->d_ord[0].get());
+    });
     B2V_CUDA(g, cudaGetLastError());
     size_t tmp = g->d_sort_tmp.size();  // all 32 key bits: kBadVid (points without storage) must sort last
     B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp.get(), tmp, g->d_vid[0].get(), g->d_vid[1].get(),
@@ -805,8 +846,8 @@ static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8
 // maximum.  The staged inputs must stay alive until the call ends.
 static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
     ++g->generation;
-    B2V_CUDA(g, launch_point_insert(in.pts, in.pts_f64 != 0, valid, n, g->inv_voxel_size, g->table, g->index,
-                                    g->stream));
+    B2V_CUDA(g, launch_point_insert(in.pts, in.pts_f64 != 0, valid, n, g->inv_voxel_size, g->log2_block, g->table,
+                                    g->index, g->stream));
     const int rc = sgrid_apply(g, n, in, valid, 0, g->index.pool_capacity);
     if (rc != B2V_OK || !g->growable) return rc;
     return g->resolve(
@@ -815,8 +856,8 @@ static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const
             sgrid_map_storage(g, blocks, &map_err);
         },
         [&](uint32_t lo, uint32_t hi) {
-            sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * kVox,
-                                                        static_cast<size_t>(hi) * kVox);
+            sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
+                                                        static_cast<size_t>(hi) * g->block_voxels());
             B2V_CUDA(g, cudaGetLastError());
             return sgrid_apply(g, n, in, valid, lo, hi);
         });
@@ -926,11 +967,15 @@ static int64_t sgrid_run_readout(b2v_sgrid *g, const GridQuery &q, float min_con
         g->err = std::string("semantic read-out: ") + cudaGetErrorString(e);
         return static_cast<int64_t>(-1);
     };
-    if (g->ensure_scan(nb) != B2V_OK) return -1;
-    sem_count_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_sums.get());
+    const uint32_t nc = g->voxel_ctas(nb);
+    if (g->ensure_scan(nc) != B2V_OK) return -1;
+    g->dispatch([&](auto l) {
+        sem_count_kernel<decltype(l)::value><<<nc, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_sums.get(),
+                                                                        nb);
+    });
     uint32_t total = 0;
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = g->scan_total(nb, &total);
+    if (e == cudaSuccess) e = g->scan_total(nc, &total);
     if (e != cudaSuccess) return fail(e);
     if (total > g->d_out_obj.size()) {
         g->d_out_obj = {};   // reserved last: it holds the capacity only once every read-out buffer does
@@ -942,9 +987,11 @@ static int64_t sgrid_run_readout(b2v_sgrid *g, const GridQuery &q, float min_con
         if ((e = g->d_out_obj.reserve(cap)) != cudaSuccess) return fail(e);
     }
     if (total) {
-        sem_emit_kernel<<<nb, kVox, 0, g->stream>>>(g->dev(), q, min_confidence, g->d_offs.get(), g->d_out_pts.get(),
-                                                    g->d_out_cols.get(), g->d_out_cls.get(), g->d_out_obj.get(),
-                                                    g->d_out_conf.get());
+        g->dispatch([&](auto l) {
+            sem_emit_kernel<decltype(l)::value><<<nc, kVox, 0, g->stream>>>(
+                g->dev(), q, min_confidence, g->d_offs.get(), g->d_out_pts.get(), g->d_out_cols.get(),
+                g->d_out_cls.get(), g->d_out_obj.get(), g->d_out_conf.get(), nb);
+        });
         if ((e = cudaGetLastError()) != cudaSuccess) return fail(e);
     }
     g->last_n = total;
@@ -992,7 +1039,11 @@ static int sgrid_edit(b2v_sgrid *g, int op, int a, int b) {
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return B2V_ERR_CUDA;
     if (nb == 0) return B2V_OK;
-    sem_edit_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(g->dev(), op, a, b);
+    const uint32_t nbu = static_cast<uint32_t>(nb);
+    g->dispatch([&](auto l) {
+        sem_edit_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(g->dev(), op, a, b,
+                                                                                      nbu * g->block_voxels());
+    });
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
@@ -1007,8 +1058,8 @@ extern "C" int b2v_sgrid_merge_segments(b2v_sgrid *g, int32_t object_id1, int32_
     return sgrid_edit(g, 3, object_id1, object_id2);
 }
 
-// Parity hook.  Arrays are [nb][512]...; any output may be NULL.  `aux` = voting confidence counter, or the
-// number of label pairs of a Bayesian voxel; lab_* [nb][512][K] in ascending (object, class) order, padded with
+// Parity hook.  Arrays are [nb][B^3]...; any output may be NULL.  `aux` = voting confidence counter, or the
+// number of label pairs of a Bayesian voxel; lab_* [nb][B^3][K] in ascending (object, class) order, padded with
 // (-1, -1, -inf) (K <= B2V_SEM_MAX_LABELS).
 extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *hashes, int32_t *count, double *pos_sum,
                                          float *col_sum, int32_t *object_id, int32_t *class_id, float *confidence,
@@ -1017,7 +1068,7 @@ extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *
     if (!g) return -1;
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb <= 0) return nb;
-    const size_t nv = static_cast<size_t>(nb) * kVox;
+    const size_t nv = static_cast<size_t>(nb) * g->block_voxels();
     bool ok = true;
     auto d2h = [&](void *dst, const void *src, size_t bytes) {
         if (dst && src) ok = ok && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, g->stream) == cudaSuccess;
@@ -1116,8 +1167,12 @@ extern "C" int b2v_sgrid_carve(b2v_sgrid *g, const float K[4], int32_t width, in
     const float *d_depth = depth;
     const int rc = g->stage_input("b2v_sgrid_carve", height, width, false, &d_depth);
     if (rc != B2V_OK) return rc;
-    sem_carve_kernel<<<static_cast<unsigned>(nb), kVox, 0, g->stream>>>(
-        g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_depth, depth_threshold);
+    const GridQuery q = g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1);
+    const uint32_t nbu = static_cast<uint32_t>(nb);
+    g->dispatch([&](auto l) {
+        sem_carve_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(g->dev(), q, d_depth,
+                                                                                       depth_threshold, nbu);
+    });
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return B2V_OK;
@@ -1149,7 +1204,7 @@ static int64_t sgrid_assoc_votes(b2v_sgrid *g, const char *fn, const float K[4],
     }
     const int64_t nb = b2v_sgrid_num_blocks(g);
     if (nb < 0) return -1;
-    const size_t nv = static_cast<size_t>(nb) * kVox;
+    const size_t nv = static_cast<size_t>(nb) * g->block_voxels();
     ++g->generation;   // carving, and object id 0 for instance 0, change voxels
     uint32_t counts[2] = {0, 0};   // records, runs
     if (nb > 0) {
@@ -1164,10 +1219,13 @@ static int64_t sgrid_assoc_votes(b2v_sgrid *g, const char *fn, const float K[4],
         if (e == cudaSuccess) e = cudaMemsetAsync(g->d_pend.get(), 0xFF, nv * sizeof(int32_t), s);
         if (e == cudaSuccess) e = cudaMemsetAsync(n_records, 0, 2 * sizeof(uint32_t), s);
         if (e == cudaSuccess) {
-            sem_assoc_kernel<<<static_cast<unsigned>(nb), kVox, 0, s>>>(
-                g->dev(), g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1), d_cls, d_inst, d_depth,
-                depth_threshold, (do_carving && depth_image) ? 1 : 0, g->d_pend.get(), g->d_records.get(),
-                n_records, static_cast<uint32_t>(nv));
+            const GridQuery q = g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1);
+            const uint32_t nbu = static_cast<uint32_t>(nb);
+            g->dispatch([&](auto l) {
+                sem_assoc_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, s>>>(
+                    g->dev(), q, d_cls, d_inst, d_depth, depth_threshold, (do_carving && depth_image) ? 1 : 0,
+                    g->d_pend.get(), g->d_records.get(), n_records, static_cast<uint32_t>(nv), nbu);
+            });
             e = cudaGetLastError();
         }
         if (e == cudaSuccess) e = cudaMemcpyAsync(counts, n_records, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
@@ -1328,8 +1386,10 @@ static int64_t sgrid_assoc_resolve(b2v_sgrid *g, const char *fn, const int32_t *
         e = cudaMemcpyAsync(d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
     if (e == cudaSuccess && !new_id.empty() && g->votes_blocks > 0) {  // deferred assignment of this grid's pending voxels
         ++g->generation;
-        sem_assoc_apply_kernel<<<g->votes_blocks, kVox, 0, g->stream>>>(g->dev(), g->d_pend.get(), d_map, d_map + m,
-                                                                         static_cast<int>(m));
+        g->dispatch([&](auto l) {
+            sem_assoc_apply_kernel<decltype(l)::value><<<g->voxel_ctas(g->votes_blocks), kVox, 0, g->stream>>>(
+                g->dev(), g->d_pend.get(), d_map, d_map + m, static_cast<int>(m), g->votes_blocks * g->block_voxels());
+        });
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
@@ -1416,7 +1476,7 @@ extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys, int32_t 
                                     g->stream);
     for (int k = 0; k < na && e == cudaSuccess; ++k)
         if (out[k])
-            e = cudaMemcpyAsync(out[k], *arr[k].ptr, static_cast<size_t>(nb) * kVox * arr[k].voxel_bytes,
+            e = cudaMemcpyAsync(out[k], *arr[k].ptr, static_cast<size_t>(nb) * g->block_voxels() * arr[k].voxel_bytes,
                                 cudaMemcpyDeviceToHost, g->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
     if (e != cudaSuccess) {
@@ -1463,8 +1523,8 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
                 sgrid_map_storage(g, blocks, &map_err);
             },
             [&](uint32_t lo, uint32_t hi) {   // the cleared state for the voxels that just got storage
-                sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * kVox,
-                                                            static_cast<size_t>(hi) * kVox);
+                sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
+                                                            static_cast<size_t>(hi) * g->block_voxels());
                 B2V_CUDA(g, cudaGetLastError());
                 return B2V_OK;
             });
@@ -1472,21 +1532,30 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
     }
     SemUpload U{};
     U.n_arrays = na;
+    const size_t nvb = g->block_voxels();
     size_t block_bytes = 0;
-    for (int k = 0; k < na; ++k) block_bytes += arr[k].voxel_bytes * kVox;
+    bool runs16 = true;   // every run of a block a multiple of 16 bytes (B >= 2)
+    for (int k = 0; k < na; ++k) {
+        block_bytes += arr[k].voxel_bytes * nvb;
+        runs16 = runs16 && (arr[k].voxel_bytes * nvb) % 16 == 0;
+    }
     DeviceBuffer<uint8_t> d_src;
     B2V_CUDA(g, d_src.reserve(static_cast<size_t>(n_blocks) * block_bytes));
     size_t off = 0;
     for (int k = 0; k < na; ++k) {
-        const size_t bytes = static_cast<size_t>(n_blocks) * kVox * arr[k].voxel_bytes;
+        const size_t bytes = static_cast<size_t>(n_blocks) * nvb * arr[k].voxel_bytes;
         B2V_CUDA(g, cudaMemcpyAsync(d_src.get() + off, in[k], bytes, cudaMemcpyHostToDevice, g->stream));
         U.dst[k] = *arr[k].ptr;
         U.src[k] = d_src.get() + off;
-        U.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * kVox);
+        U.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * nvb);
         off += bytes;
     }
-    sem_scatter_kernel<<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(d_keys.get(), U, g->table,
-                                                                              g->index.pool_capacity);
+    if (runs16)
+        sem_scatter_kernel<uint4><<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(d_keys.get(), U, g->table,
+                                                                                         g->index.pool_capacity);
+    else
+        sem_scatter_kernel<uint32_t><<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(
+            d_keys.get(), U, g->table, g->index.pool_capacity);
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     return g->read_counters();

@@ -106,6 +106,8 @@ class B200PluginSetup:
         if constructor_kwargs:
             p.update({k: v for k, v in constructor_kwargs.items() if k in defaults})
         self.b200_parameters = p
+        # the keys the caller set (the rest hold the plugin's defaults)
+        self.b200_set_parameters = {k for k in defaults if k in (parameters_dict or {}) or k in (constructor_kwargs or {})}
         return p
 
     def _init_gpu_rectify(self):

@@ -72,12 +72,21 @@ DEFAULT_PARAMETERS = {
 }
 
 
-def _grid_args(p):
-    """Constructor arguments of either grid from the plugin parameters."""
-    return dict(voxel_size=p["kVolumetricIntegrationVoxelLength"], block_size=p["kVolumetricIntegrationBlockSize"],
-                capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
+def _grid_args(p, set_keys=()):
+    """Constructor arguments of either grid from the plugin parameters.  The capacities count blocks of the configured
+    kVolumetricIntegrationBlockSize B.  A capacity the caller did not set (not in `set_keys`) is the default's voxel
+    budget at that size: default * 512 / B^3 blocks, rounded up, so the default memory does not change with B; a value
+    the caller set is taken as given."""
+    B = int(p["kVolumetricIntegrationBlockSize"])
+
+    def blocks(key):
+        n = int(p[key])
+        return n if key in set_keys or B <= 0 else -(-n * 512 // B ** 3)
+
+    return dict(voxel_size=p["kVolumetricIntegrationVoxelLength"], block_size=B,
+                capacity_blocks=blocks("kVolumetricIntegrationB200CapacityBlocks"),
                 device=int(p["kVolumetricIntegrationB200Device"]),
-                max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None)
+                max_capacity_blocks=blocks("kVolumetricIntegrationB200MaxCapacityBlocks") or None)
 
 
 def make_semantic_integrator_class(Base, api):
@@ -125,7 +134,7 @@ def make_semantic_integrator_class(Base, api):
         def _make_grid(self, p, side, constructor_kwargs):
             probabilistic = bool(constructor_kwargs.get("use_semantic_probabilistic", False))
             grid_t = VoxelBlockSemanticProbabilisticGrid if probabilistic else VoxelBlockSemanticGrid
-            grid = grid_t(**_grid_args(p))
+            grid = grid_t(**_grid_args(p, self.b200_set_parameters))
             grid.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
             grid.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
             return grid
@@ -319,7 +328,7 @@ def make_voxel_grid_integrator_class(Base, api):
         _defaults = dict(DEFAULT_PARAMETERS, kVolumetricIntegrationB200CapacityBlocks=1 << 17)
 
         def _make_grid(self, p, side, constructor_kwargs):
-            return VoxelBlockGrid(**_grid_args(p))
+            return VoxelBlockGrid(**_grid_args(p, self.b200_set_parameters))
 
         def _integrate_raw_keyframe(self, kd, depth, scale):
             """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""

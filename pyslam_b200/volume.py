@@ -768,6 +768,9 @@ class _BlockGrid(_MapState):
     names its entry points by their prefix `_P` and stages frames with `_stage_frame`."""
 
     _P = ""
+    # block sides the grids take (pySLAM's kVolumetricIntegrationBlockSize): powers of two, so the block key stays a
+    # shift and the local key a mask; 4 keeps the rejection every size but 8 had before block sizes were supported
+    SUPPORTED_BLOCK_SIZES = (1, 2, 8, 16)
 
     def __init__(self, voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count,
                  *kind):
@@ -775,6 +778,7 @@ class _BlockGrid(_MapState):
         self._h = C.c_void_p()
         self.voxel_size = float(voxel_size)
         self._block_size = int(block_size)
+        self._block_voxels = self._block_size ** 3   # voxels per block: the per-voxel axis of dumps and uploads
         self.capacity_blocks = int(capacity_blocks)
         self.max_capacity_blocks = int(max_capacity_blocks or 0)
         self.device = int(device)
@@ -782,7 +786,10 @@ class _BlockGrid(_MapState):
         rc = self._c("create_ex")(float(voxel_size), int(block_size), int(capacity_blocks), self.max_capacity_blocks,
                                   *kind, int(device), C.byref(self._h))
         if rc != _lib.B2V_OK:
-            msg = self._c("last_error")(self._h).decode() if self._h else "invalid configuration"
+            msg = self._c("last_error")(self._h).decode() if self._h else (
+                "invalid configuration (block_size must be one of "
+                f"{', '.join(map(str, self.SUPPORTED_BLOCK_SIZES))}; got {block_size})"
+                if self._block_size not in self.SUPPORTED_BLOCK_SIZES else "invalid configuration")
             if self._h:
                 self._c("destroy")(self._h)
                 self._h = C.c_void_p()
@@ -1024,9 +1031,8 @@ class VoxelBlockGrid(_BlockGrid):
 
     _STATE_KIND = "grid"
 
-    @staticmethod
-    def _state_arrays() -> dict:
-        v = BLOCK_VOXELS
+    def _state_arrays(self) -> dict:
+        v = self._block_voxels
         return dict(keys=(np.int32, (3,)), count=(np.int32, (v,)), pos_sum=(np.float32, (v, 3)),
                     col_sum=(np.float32, (v, 3)))
 
@@ -1045,9 +1051,10 @@ class VoxelBlockGrid(_BlockGrid):
         nb = self.num_blocks()
         keys = np.zeros((nb, 3), np.int32)
         hashes = np.zeros(nb, np.uint64)
-        count = np.zeros((nb, BLOCK_VOXELS), np.int32)
-        pos = np.zeros((nb, BLOCK_VOXELS, 3), np.float32)
-        col = np.zeros((nb, BLOCK_VOXELS, 3), np.float32)
+        v = self._block_voxels
+        count = np.zeros((nb, v), np.int32)
+        pos = np.zeros((nb, v, 3), np.float32)
+        col = np.zeros((nb, v, 3), np.float32)
         n = self._L.b2v_grid_dump_blocks(self._h, keys.ctypes.data, hashes.ctypes.data,
                                          count.ctypes.data, pos.ctypes.data, col.ctypes.data)
         if n != nb:
@@ -1281,7 +1288,7 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         self.set_next_object_id(int(settings["next_object_id"]))
 
     def _state_arrays(self) -> dict:
-        v, k = BLOCK_VOXELS, _lib.B2V_SEM_MAX_LABELS
+        v, k = self._block_voxels, _lib.B2V_SEM_MAX_LABELS
         spec = dict(keys=(np.int32, (3,)), count=(np.int32, (v,)), pos_sum=(np.float64, (v, 3)),
                     col_sum=(np.float32, (v, 3)), object_id=(np.int32, (v,)), class_id=(np.int32, (v,)),
                     counter=(np.int32, (v,)))
@@ -1291,10 +1298,10 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         return spec
 
     def export_blocks(self) -> dict:
-        """The raw state of every block (b2v_sgrid_export_blocks): keys [nb,3] and per-voxel arrays [nb,512,...] -
+        """The raw state of every block (b2v_sgrid_export_blocks): keys [nb,3] and per-voxel arrays [nb,B^3,...] -
         count, pos_sum (float64), col_sum, object_id, class_id, counter (the voting counter, or the number of label
         slots in use) and, on the Bayesian grid, ml_logp, conf and the label slots lab_obj / lab_cls / lab_logp
-        [nb,512,8] in the kernel's own order.  Unlike `dump_blocks`, nothing is derived or reordered."""
+        [nb,B^3,8] in the kernel's own order.  Unlike `dump_blocks`, nothing is derived or reordered."""
         spec = self._state_arrays()
         nb = self.num_blocks()
         d = {name: np.zeros((nb,) + shape, dt) for name, (dt, shape) in spec.items()}
@@ -1517,8 +1524,8 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         return int(out.value)
 
     def dump_blocks(self, K: int = 8):
-        """Parity hook: per-block arrays [nb,512,...] incl. labels (see include/b2v.h)."""
-        nb, nv = self.num_blocks(), BLOCK_VOXELS
+        """Parity hook: per-block arrays [nb,B^3,...] incl. labels (see include/b2v.h)."""
+        nb, nv = self.num_blocks(), self._block_voxels
         d = dict(keys=np.zeros((nb, 3), np.int32), hashes=np.zeros(nb, np.uint64),
                  count=np.zeros((nb, nv), np.int32), pos_sum=np.zeros((nb, nv, 3), np.float64),
                  col_sum=np.zeros((nb, nv, 3), np.float32), object_id=np.zeros((nb, nv), np.int32),
