@@ -49,6 +49,7 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids", "b2v_grid_set_shard", "b2v_sgrid_set_shard",
     "b2v_sgrid_assoc_votes", "b2v_sgrid_copy_assoc_votes", "b2v_sgrid_assoc_resolve",
     "b2v_grid_upload_blocks", "b2v_sgrid_export_blocks", "b2v_sgrid_upload_blocks",
+    "b2v_sgrid_set_label_overflow", "b2v_sgrid_label_storage", "b2v_sgrid_export_labels", "b2v_sgrid_upload_labels",
 ]
 
 
@@ -180,6 +181,14 @@ def load() -> C.CDLL:
     L.b2v_sgrid_merge_segments.argtypes = [vp, i32, i32]
     L.b2v_sgrid_remove_segment.argtypes = [vp, i32]
     L.b2v_sgrid_label_overflows.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.b2v_sgrid_set_label_overflow.restype = C.c_int
+    L.b2v_sgrid_set_label_overflow.argtypes = [vp, C.c_uint64, C.c_uint64]
+    L.b2v_sgrid_label_storage.restype = C.c_int
+    L.b2v_sgrid_label_storage.argtypes = [vp, p_i64, p_i64, p_i64, p_i64]
+    L.b2v_sgrid_export_labels.restype = i64
+    L.b2v_sgrid_export_labels.argtypes = [vp] * 5
+    L.b2v_sgrid_upload_labels.restype = C.c_int
+    L.b2v_sgrid_upload_labels.argtypes = [vp, i64] + [vp] * 5
     L.b2v_sgrid_dump_blocks.restype = C.c_int64
     L.b2v_sgrid_dump_blocks.argtypes = [vp] * 10 + [i32] + [vp] * 3
     L.b2v_integrate_u16.restype = C.c_int

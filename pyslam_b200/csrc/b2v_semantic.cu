@@ -19,9 +19,12 @@
 // confidence read-out are evaluated in float64 and rounded (glibc's expf / logf are within 1 ulp of that).
 //
 // Bayesian labels: the reference keeps a std::map<(object, class), float> per voxel (typically 1-5 entries);
-// here a voxel has kSemLabels = 8 fixed slots.  A ninth distinct pair evicts the slot with the least evidence
-// that is not the current argmax (the first on ties) and bumps the overflow counter (b2v_sgrid_label_overflows) - a
-// documented deviation no reference KAT reaches; tests/test_gpu_semantic_edges.py checks the evicted slot.
+// here a voxel has kSemLabels = 8 fixed slots.  Without an overflow label store (the default) a ninth distinct pair
+// evicts the slot with the least evidence that is not the current argmax (the first on ties) and bumps the overflow
+// counter (b2v_sgrid_label_overflows); tests/test_gpu_semantic_edges.py checks the evicted slot.  With a store
+// (b2v_sgrid_set_label_overflow) a voxel links chunks of 8 more pairs from a grid-wide pool and never evicts below
+// the store's ceiling, so it holds the reference's unbounded map.  The store is a compile-time flag (kChain) of the
+// kernels that touch label pairs: their kChain = false instantiations are the grid without a store.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_run_length_encode.cuh>
 
@@ -33,6 +36,7 @@
 #include <map>
 #include <new>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/b2v.h"
@@ -68,6 +72,71 @@ struct SemGrid {
     int32_t kind;
     float depth_threshold, depth_decay_rate;
 };
+
+// ---- overflow label store ----------------------------------------------------------------------------------------
+// Pair s of a voxel (insertion order) is in-voxel slot s for s < kSemLabels, else entry (s - kSemLabels) % 8 of the
+// ((s - kSemLabels) / 8)-th chunk of the voxel's chain.  Chunks are taken from the pool's free list first, then fresh
+// from its mapped storage; edits that reset a voxel or collapse its labels push its chain onto the free list.
+constexpr int kChunkPairs = 8;
+constexpr uint64_t kMaxLabelChunks = 1ull << 25;   // 2^28 overflow pairs, 4 GiB of chunks
+struct alignas(16) LabelChunk {
+    int32_t obj[kChunkPairs], cls[kChunkPairs];
+    float logp[kChunkPairs];
+    uint32_t next;   // 1 + index of the next chunk of the chain, 0: the last
+    uint32_t pad[7];
+};
+static_assert(sizeof(LabelChunk) == 128, "chunk layout");
+
+enum LabelCounter : int {
+    kLcFree = 0,        // chunks on the free list
+    kLcFresh = 1,       // chunks ever taken from the storage (in use = fresh - free)
+    kLcTaken = 2,       // chunks requested by the runs of the current pass
+    kLcFirstFail = 3,   // the least request start of a run that got none (UINT_MAX: none)
+    kLcListed = 4,      // runs listed for the replay
+    kLcFull = 5,        // a run could not have chunks and no growth could give them: it evicted
+    kLcNum = 8
+};
+
+struct LabelStore {
+    uint32_t *head;           // [V] 1 + index of the voxel's first chunk, 0: none (zeroed memory is the cleared state)
+    LabelChunk *chunks;       // [mapped]
+    uint32_t *free_list;      // [mapped], kLcFree of them in use
+    uint32_t *ctr;            // LabelCounter
+    uint32_t *list;           // sorted position of the head of each run that found no chunks
+    const uint32_t *replay;   // non-NULL: thread r updates the run starting at replay[r], r < n_replay
+    uint32_t n_replay;
+    uint32_t mapped;          // chunks with storage
+    int32_t no_growth;        // the storage cannot grow: a run without chunks evicts instead of waiting for a replay
+};
+
+// visit the pairs of a voxel in slot order: f(slot, obj *, cls *, logp *) returns true to stop
+template <typename F>
+__device__ __forceinline__ void for_each_pair(const LabelStore &S, int32_t *lo, int32_t *lc, float *lp, int nl,
+                                              uint32_t head, F f) {
+    const int nr = nl < kSemLabels ? nl : kSemLabels;
+    for (int s = 0; s < nr; ++s)
+        if (f(s, lo + s, lc + s, lp + s)) return;
+    LabelChunk *c = nullptr;
+    for (int s = kSemLabels; s < nl; ++s) {
+        const int e = (s - kSemLabels) & (kChunkPairs - 1);
+        if (e == 0) c = S.chunks + ((c ? c->next : head) - 1);
+        if (f(s, c->obj + e, c->cls + e, c->logp + e)) return;
+    }
+}
+
+// push the voxel's chain onto the free list
+template <bool kChain> __device__ __forceinline__ void sem_release_labels(const LabelStore &S, uint32_t v) {
+    if constexpr (kChain) {
+        uint32_t link = S.head[v];
+        if (link == 0) return;
+        S.head[v] = 0;
+        while (link != 0) {
+            const uint32_t c = link - 1;
+            link = S.chunks[c].next;
+            S.free_list[atomicAdd(S.ctr + kLcFree, 1u)] = c;
+        }
+    }
+}
 
 // ---- 2. sort keys --------------------------------------------------------------------------------------------
 // Only points whose block has a pool index in [lo, hi) get a key; the others get kBadVid, sort last and are left out
@@ -168,10 +237,158 @@ __device__ float bayes_confidence(const int32_t *lo, const int32_t *lc, const fl
     return exp_rn(__fsub_rn(mlp, sum));
 }
 
+// the same over every pair of a voxel with an overflow chain
+__device__ float bayes_confidence_chain(const LabelStore &S, int32_t *lo, int32_t *lc, float *lp, int nl,
+                                        uint32_t head, int mo, int mc, float mlp) {
+    if (mo == -1 || mc == -1 || nl == 0) return 0.0f;
+    float sum = __uint_as_float(0xFF800000u);
+    long long prev = LLONG_MIN;
+    for (int k = 0; k < nl; ++k) {
+        long long best = LLONG_MAX;
+        float bl = 0.0f;
+        for_each_pair(S, lo, lc, lp, nl, head, [&](int, const int32_t *o, const int32_t *c, const float *l) {
+            const long long key = (static_cast<long long>(*o) << 32) + (static_cast<long long>(*c) + 0x80000000LL);
+            if (key > prev && key < best) {
+                best = key;
+                bl = *l;
+            }
+            return false;
+        });
+        if (best == LLONG_MAX) break;
+        prev = best;
+        sum = log_add_exp(sum, bl);
+    }
+    return exp_rn(__fsub_rn(mlp, sum));
+}
+
+// one Bayesian observation (object oo, class oc, evidence w) of a voxel with an overflow chain that can hold `cap`
+// pairs: the update of sem_runs_kernel over all of its pairs.  A new pair past `cap` evicts the weakest pair that is
+// not the argmax, the first in slot order on ties.
+__device__ __forceinline__ void bayes_observe_chain(const LabelStore &S, int32_t *lo, int32_t *lc, float *lp, int &nl,
+                                                    uint32_t head, int cap, int32_t oo, int32_t oc, float w,
+                                                    int32_t count, int32_t &obj, int32_t &cls, float &mlp,
+                                                    uint32_t *overflows) {
+    int32_t *po = nullptr, *pc = nullptr;
+    float *pl = nullptr;
+    for_each_pair(S, lo, lc, lp, nl, head, [&](int, int32_t *o, int32_t *c, float *l) {
+        if (*o != oo || *c != oc) return false;
+        po = o, pc = c, pl = l;
+        return true;
+    });
+    // slot s for a new pair (pl == nullptr before)
+    auto at = [&](int s) {
+        if (s < kSemLabels) {
+            po = lo + s, pc = lc + s, pl = lp + s;
+            return;
+        }
+        LabelChunk *c = S.chunks + (head - 1);
+        for (int q = (s - kSemLabels) / kChunkPairs; q > 0; --q) c = S.chunks + (c->next - 1);
+        const int e = (s - kSemLabels) & (kChunkPairs - 1);
+        po = c->obj + e, pc = c->cls + e, pl = c->logp + e;
+    };
+    if (count == 0) {  // initialize_semantics_log_prob: map[key] = w, argmax = key
+        if (pl == nullptr) {
+            at(nl < cap ? nl++ : 0);
+            *po = oo, *pc = oc;
+        }
+        *pl = w;
+        obj = oo, cls = oc, mlp = w;
+    } else if (pl != nullptr) {  // known pair: accumulate; a strictly larger value takes the argmax
+        *pl = __fadd_rn(*pl, w);
+        if (*po == obj && *pc == cls) {
+            mlp = *pl;
+        } else if (*pl > mlp) {
+            mlp = *pl;
+            obj = oo, cls = oc;
+        }
+    } else {  // new pair
+        if (nl < cap) {
+            at(nl++);
+        } else {  // out of slots: evict the weakest pair that is not the argmax
+            float least = 0.0f;
+            for_each_pair(S, lo, lc, lp, nl, head, [&](int, int32_t *o, int32_t *c, float *l) {
+                if (!(*o == obj && *c == cls) && (pl == nullptr || *l < least)) {
+                    po = o, pc = c, pl = l;
+                    least = *l;
+                }
+                return false;
+            });
+            atomicAdd(overflows, 1u);
+        }
+        *po = oo, *pc = oc, *pl = w;
+        if (w > mlp) {
+            mlp = w;
+            obj = oo, cls = oc;
+        }
+    }
+}
+
+// Chunks for the run of voxel v at sorted positions [j0, ...) before it applies anything: the run counts the distinct
+// pairs it adds to the voxel's nl pairs and, if they pass what its chain holds, takes the missing chunks with one
+// atomic and links them to the chain.  Returns the pairs the chain then holds (kSemLabels + 8 per chunk), or -1 when
+// the run got no chunks and must wait for the replay (it is listed).  Without growth (S.no_growth) such a run keeps
+// its chain and evicts.
+__device__ int sem_take_chunks(const LabelStore &S, const uint32_t *vid, const uint32_t *order, int64_t n, int64_t j0,
+                               const SemInputs &in, int32_t *lo, int32_t *lc, float *lp, int nl, uint32_t &head) {
+    const uint32_t v = vid[j0];
+    int chunks = 0;
+    uint32_t tail = 0;   // 1 + index of the chain's last chunk
+    for (uint32_t link = head; link != 0; link = S.chunks[link - 1].next) {
+        tail = link;
+        ++chunks;
+    }
+    int added = 0;
+    for (int64_t j = j0; j < n && vid[j] == v; ++j) {
+        const uint32_t i = order[j];
+        const int32_t oc = in.cls[i], oo = in.inst ? in.inst[i] : 0;
+        bool seen = false;
+        for (int64_t q = j - 1; q >= j0 && !seen; --q) {   // earlier in the run (the previous one first)
+            const uint32_t iq = order[q];
+            seen = in.cls[iq] == oc && (in.inst ? in.inst[iq] : 0) == oo;
+        }
+        if (!seen)
+            for_each_pair(S, lo, lc, lp, nl, head, [&](int, const int32_t *o, const int32_t *c, const float *) {
+                seen = *o == oo && *c == oc;
+                return seen;
+            });
+        added += seen ? 0 : 1;
+    }
+    const int have = kSemLabels + kChunkPairs * chunks;
+    const int over = nl + added - have;
+    if (over <= 0) return have;
+    const uint32_t need = static_cast<uint32_t>((over + kChunkPairs - 1) / kChunkPairs);
+    const uint32_t n_free = S.ctr[kLcFree], fresh = S.ctr[kLcFresh];
+    const uint32_t t = atomicAdd(S.ctr + kLcTaken, need);
+    if (static_cast<uint64_t>(t) + need > static_cast<uint64_t>(n_free) + (S.mapped - fresh)) {
+        atomicMin(S.ctr + kLcFirstFail, t);
+        if (S.no_growth) {
+            atomicOr(S.ctr + kLcFull, 1u);
+            return have;
+        }
+        S.list[atomicAdd(S.ctr + kLcListed, 1u)] = static_cast<uint32_t>(j0);
+        return -1;
+    }
+    for (uint32_t x = t; x < t + need; ++x) {   // free list from the top, then fresh chunks
+        const uint32_t c = x < n_free ? S.free_list[n_free - 1 - x] : fresh + (x - n_free);
+        S.chunks[c].next = 0;
+        if (tail == 0) head = c + 1;
+        else S.chunks[tail - 1].next = c + 1;
+        tail = c + 1;
+    }
+    return have + kChunkPairs * static_cast<int>(need);
+}
+
+template <bool kChain>
 __global__ void __launch_bounds__(128)
 sem_runs_kernel(const uint32_t *__restrict__ vid, const uint32_t *__restrict__ order, const int64_t n,
-                const SemInputs in, const SemGrid G) {
-    const int64_t j0 = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+                const SemInputs in, const SemGrid G, const LabelStore S) {
+    int64_t j0 = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if constexpr (kChain) {
+        if (S.replay != nullptr) {
+            if (j0 >= S.n_replay) return;
+            j0 = S.replay[j0];
+        }
+    }
     if (j0 >= n) return;
     const uint32_t v = vid[j0];
     if (v == kBadVid || (j0 > 0 && vid[j0 - 1] == v)) return;  // not the head of a run
@@ -195,6 +412,15 @@ sem_runs_kernel(const uint32_t *__restrict__ vid, const uint32_t *__restrict__ o
             lo[k] = G.lab_obj[static_cast<size_t>(v) * kSemLabels + k];
             lc[k] = G.lab_cls[static_cast<size_t>(v) * kSemLabels + k];
             lp[k] = G.lab_logp[static_cast<size_t>(v) * kSemLabels + k];
+        }
+    }
+    uint32_t head = 0;
+    int cap = kSemLabels;   // pairs the voxel can hold in this run
+    if constexpr (kChain) {
+        if (bayes && semantics) {
+            head = S.head[v];
+            cap = sem_take_chunks(S, vid, order, n, j0, in, lo, lc, lp, nl, head);
+            if (cap < 0) return;   // nothing written: the replay applies the whole run
         }
     }
 
@@ -247,6 +473,12 @@ sem_runs_kernel(const uint32_t *__restrict__ vid, const uint32_t *__restrict__ o
                 if (has_depth && !(depth <= G.depth_threshold))
                     w = __fmul_rn(exp_rn(__fmul_rn(-__fsub_rn(depth, G.depth_threshold), G.depth_decay_rate)),
                                   kBaseLogProb);
+                if constexpr (kChain) {
+                    bayes_observe_chain(S, lo, lc, lp, nl, head, cap, oo, oc, w, count, obj, cls, mlp,
+                                        G.index.counters + kBgLabelOverflow);
+                    ++count;
+                    continue;
+                }
                 int k = 0;
                 while (k < nl && !(lo[k] == oo && lc[k] == oc)) ++k;
                 if (count == 0) {  // initialize_semantics_log_prob: map[key] = w, argmax = key
@@ -304,7 +536,12 @@ sem_runs_kernel(const uint32_t *__restrict__ vid, const uint32_t *__restrict__ o
                 G.lab_cls[static_cast<size_t>(v) * kSemLabels + k] = lc[k];
                 G.lab_logp[static_cast<size_t>(v) * kSemLabels + k] = lp[k];
             }
-            G.conf[v] = bayes_confidence(lo, lc, lp, nl, obj, cls, mlp);
+            if constexpr (kChain) {
+                S.head[v] = head;
+                G.conf[v] = bayes_confidence_chain(S, lo, lc, lp, nl, head, obj, cls, mlp);
+            } else {
+                G.conf[v] = bayes_confidence(lo, lc, lp, nl, obj, cls, mlp);
+            }
         }
     }
 }
@@ -317,7 +554,9 @@ __device__ __forceinline__ float sem_confidence(const SemGrid &G, uint32_t v, in
     return fminf(1.0f, __fdiv_rn(static_cast<float>(G.counter[v]), static_cast<float>(count)));
 }
 
-__device__ __forceinline__ void sem_reset_voxel(const SemGrid &G, uint32_t v) {  // VoxelSemanticData*::reset()
+template <bool kChain>
+__device__ __forceinline__ void sem_reset_voxel(const SemGrid &G, const LabelStore &S, uint32_t v) {  // ::reset()
+    sem_release_labels<kChain>(S, v);
     G.count[v] = 0;
     for (int a = 0; a < 3; ++a) {
         G.pos[3 * static_cast<size_t>(v) + a] = 0.0;
@@ -336,21 +575,22 @@ __device__ __forceinline__ void sem_reset_voxel(const SemGrid &G, uint32_t v) { 
 // op 3: merge_segments(a, b)  (voxel_block_grid.hpp:625-647; voxel_block_semantic_grid.hpp:101-183)
 // Per-voxel passes: one 512-thread CTA per 512 pool voxels (cta_voxel), so voxel id = blockIdx.x * 512 + threadIdx.x
 // whatever B; nv (the voxels of the blocks in use) bounds the last CTA when B < 8 and is not read at B >= 8.
-template <int L>
+template <int L, bool kChain>
 __global__ void __launch_bounds__(kVox)
-sem_edit_kernel(const SemGrid G, const int op, const int a, const int b, const uint32_t nv) {
+sem_edit_kernel(const SemGrid G, const int op, const int a, const int b, const uint32_t nv, const LabelStore S) {
     const uint32_t v = blockIdx.x * kVox + threadIdx.x;
     if (3 * L < 9 && v >= nv) return;
     const int c = G.count[v];
     if (op == 0) {
-        if (c < a) sem_reset_voxel(G, v);
+        if (c < a) sem_reset_voxel<kChain>(G, S, v);
     } else if (op == 1) {
-        if (sem_confidence(G, v, c) < static_cast<float>(a)) sem_reset_voxel(G, v);
+        if (sem_confidence(G, v, c) < static_cast<float>(a)) sem_reset_voxel<kChain>(G, S, v);
     } else if (op == 2) {
-        if (G.obj[v] == a) sem_reset_voxel(G, v);
+        if (G.obj[v] == a) sem_reset_voxel<kChain>(G, S, v);
     } else if (G.obj[v] == b) {
         G.obj[v] = a;  // set_object_id
         if (G.kind == B2V_SEM_PROBABILISTIC) {
+            sem_release_labels<kChain>(S, v);
             // force_label_distribution (voxel_data_semantic.h:589-605): a single pair with log-probability 0
             const int32_t cl = G.cls[v];
             if (a >= 0 && cl >= 0) {
@@ -446,9 +686,11 @@ sem_emit_kernel(const SemGrid G, const GridQuery Q, const float min_conf,
 }
 
 // set_object_id (voxel_data_semantic.h:135, 455-460): the Bayesian voxel collapses onto the forced pair
-__device__ __forceinline__ void sem_set_object_id(const SemGrid &G, uint32_t v, int32_t id) {
+template <bool kChain>
+__device__ __forceinline__ void sem_set_object_id(const SemGrid &G, const LabelStore &S, uint32_t v, int32_t id) {
     G.obj[v] = id;
     if (G.kind == B2V_SEM_PROBABILISTIC) {
+        sem_release_labels<kChain>(S, v);
         const int32_t cl = G.cls[v];
         if (id >= 0 && cl >= 0) {
             G.counter[v] = 1;
@@ -467,10 +709,10 @@ __device__ __forceinline__ void sem_set_object_id(const SemGrid &G, uint32_t v, 
 
 // carve (voxel_grid_carving.h:47-80): reset voxels in front of the observed surface by more than the threshold;
 // the depth image is indexed with truncated pixel coordinates, like at<float>(v, u)
-template <int L>
+template <int L, bool kChain>
 __global__ void __launch_bounds__(kVox)
 sem_carve_kernel(const SemGrid G, const GridQuery Q, const float *__restrict__ depth, const float thr,
-                 const uint32_t nb) {
+                 const uint32_t nb, const LabelStore S) {
     uint32_t b;
     int t;
     cta_voxel<L>(&b, &t);
@@ -479,7 +721,7 @@ sem_carve_kernel(const SemGrid G, const GridQuery Q, const float *__restrict__ d
     if (!sem_in_region<L>(G, Q, b, t, &ip)) return;
     const float image_depth = depth[static_cast<size_t>(static_cast<int>(ip.v)) * Q.W + static_cast<int>(ip.u)];
     if (image_depth <= 0.0f || !isfinite(image_depth)) return;
-    if (ip.depth < image_depth - thr) sem_reset_voxel(G, blockIdx.x * kVox + threadIdx.x);
+    if (ip.depth < image_depth - thr) sem_reset_voxel<kChain>(G, S, blockIdx.x * kVox + threadIdx.x);
 }
 
 // process_point of assign_object_ids_to_instance_ids (voxel_semantic_data_association.h:171-229): every voxel in
@@ -496,12 +738,13 @@ __device__ __forceinline__ unsigned long long assoc_key(int32_t inst, int32_t ob
            (static_cast<uint32_t>(obj) ^ 0x80000000u);
 }
 
-template <int L>
+template <int L, bool kChain>
 __global__ void __launch_bounds__(kVox)
 sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__ class_img,
                  const int32_t *__restrict__ inst_img, const float *__restrict__ depth_img, const float thr,
                  const int do_carving, int32_t *__restrict__ pend, unsigned long long *__restrict__ records,
-                 uint32_t *__restrict__ n_records, const uint32_t cap_records, const uint32_t nb) {
+                 uint32_t *__restrict__ n_records, const uint32_t cap_records, const uint32_t nb,
+                 const LabelStore S) {
     uint32_t b;
     int t;
     cta_voxel<L>(&b, &t);
@@ -521,7 +764,7 @@ sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__
         const float image_depth = depth_img[px];
         if (image_depth <= 0.0f || !isfinite(image_depth)) return;
         if (do_carving && ip.depth < image_depth - thr) {
-            sem_reset_voxel(G, v);
+            sem_reset_voxel<kChain>(G, S, v);
             return;
         }
         if (ip.depth > image_depth + thr) return;
@@ -529,7 +772,7 @@ sem_assoc_kernel(const SemGrid G, const GridQuery Q, const int32_t *__restrict__
     if (point_object < 0) {
         if (image_instance == 0) {
             point_object = 0;
-            sem_set_object_id(G, v, 0);
+            sem_set_object_id<kChain>(G, S, v, 0);
         } else {
             point_object = kAssocPending;  // one new object id per instance id, handed out by the host
             pend[v] = image_instance;
@@ -552,10 +795,10 @@ sem_assoc_triples_kernel(const unsigned long long *__restrict__ keys, const uint
 }
 
 // deferred assignment (voxel_semantic_data_association.h:354-370): pending voxels take their instance's final id
-template <int L>
+template <int L, bool kChain>
 __global__ void __launch_bounds__(kVox)
 sem_assoc_apply_kernel(const SemGrid G, const int32_t *__restrict__ pend, const int32_t *__restrict__ map_inst,
-                       const int32_t *__restrict__ map_obj, const int n_map, const uint32_t nv) {
+                       const int32_t *__restrict__ map_obj, const int n_map, const uint32_t nv, const LabelStore S) {
     const uint32_t v = blockIdx.x * kVox + threadIdx.x;
     if (3 * L < 9 && v >= nv) return;
     const int32_t inst = pend[v];
@@ -565,7 +808,7 @@ sem_assoc_apply_kernel(const SemGrid G, const int32_t *__restrict__ pend, const 
         const int mid = (lo + hi) >> 1;
         const int32_t m = map_inst[mid];
         if (m == inst) {
-            if (map_obj[mid] >= 0) sem_set_object_id(G, v, map_obj[mid]);
+            if (map_obj[mid] >= 0) sem_set_object_id<kChain>(G, S, v, map_obj[mid]);
             return;
         }
         if (m < inst) lo = mid + 1; else hi = mid - 1;
@@ -652,13 +895,55 @@ struct b2v_sgrid : BlockGridCore {
     DeviceBuffer<int32_t> d_out_cls;
     DeviceBuffer<int32_t> d_out_obj;   // its size is the read-out capacity
     int64_t last_n = 0;
+    // overflow label store (b2v_sgrid_set_label_overflow): lab_max_chunks 0 = none, the kernels' kChain = false
+    uint32_t lab_max_chunks = 0;
+    uint32_t lab_mapped = 0;          // chunks with storage (the mapped granules may hold more)
+    int64_t lab_growths = 0;
+    bool lab_full = false;            // a run of the current call evicted for want of chunks past the ceiling
+    std::string lab_map_err;          // the chunk storage of the current call failed to grow (device memory)
+    VmmRange lab_head;                // [voxels] chain heads, mapped with the per-voxel arrays
+    VmmRange lab_chunks, lab_free;    // [lab_max_chunks] chunks and free list, mapped on demand
+    DeviceBuffer<uint32_t> d_lab_ctr;   // LabelCounter
+    DeviceBuffer<uint32_t> d_lab_list;  // runs listed for the replay; its size is their capacity
 
     SemGrid dev() const {   // the kernels' view
         SemGrid d = G;
         d.index = SemBlockIndex{index.block_keys, index.counters, index.capacity, index.pool_capacity};
         return d;
     }
+    LabelStore labels() const {   // the store as the kernels see it (all NULL without one)
+        LabelStore s{};
+        if (lab_max_chunks == 0) return s;
+        s.head = reinterpret_cast<uint32_t *>(lab_head.va);
+        s.chunks = reinterpret_cast<LabelChunk *>(lab_chunks.va);
+        s.free_list = reinterpret_cast<uint32_t *>(lab_free.va);
+        s.ctr = d_lab_ctr.get();
+        s.list = d_lab_list.get();
+        s.mapped = lab_mapped;
+        s.no_growth = lab_mapped >= lab_max_chunks ? 1 : 0;
+        return s;
+    }
 };
+
+// f(block size, chain flag) as integral constants: the kernels of the grid's block size and label store
+template <typename F> static void sgrid_dispatch(const b2v_sgrid *g, F &&f) {
+    g->dispatch([&](auto l) {
+        if (g->lab_max_chunks) f(l, std::true_type{});
+        else f(l, std::false_type{});
+    });
+}
+
+static bool sgrid_map_labels(b2v_sgrid *g, uint64_t chunks, std::string *err);
+static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+                            const int32_t *obj, const int32_t *cls, const float *logp);
+
+// an empty store: no chain, no chunk taken
+static int sgrid_label_reset(b2v_sgrid *g, size_t nv) {
+    static const uint32_t init[kLcNum] = {0, 0, 0, UINT32_MAX, 0, 0, 0, 0};
+    if (nv) B2V_CUDA(g, cudaMemsetAsync(reinterpret_cast<void *>(g->lab_head.va), 0, nv * sizeof(uint32_t), g->stream));
+    B2V_CUDA(g, cudaMemcpyAsync(g->d_lab_ctr.get(), init, sizeof(init), cudaMemcpyHostToDevice, g->stream));
+    return B2V_OK;
+}
 
 extern "C" const char *b2v_sgrid_last_error(const b2v_sgrid *g) { return g ? g->err.c_str() : "null grid"; }
 
@@ -673,7 +958,7 @@ static int sgrid_clear_device(b2v_sgrid *g, uint32_t used_blocks) {
     if (g->G.kind == B2V_SEM_PROBABILISTIC) B2V_CUDA(g, cudaMemsetAsync(g->G.conf, 0, nv * sizeof(float), g->stream));
     sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), 0, nv);
     B2V_CUDA(g, cudaGetLastError());
-    return B2V_OK;
+    return g->lab_max_chunks ? sgrid_label_reset(g, nv) : B2V_OK;
 }
 
 // the per-voxel arrays of the grid's kind and the bytes each holds per voxel
@@ -713,6 +998,11 @@ static bool sgrid_map_storage(b2v_sgrid *g, uint64_t blocks, std::string *err) {
         const size_t block_bytes = arr[k].voxel_bytes * g->block_voxels();
         ok = ok && vmm_map(&g->store[k], static_cast<size_t>(blocks) * block_bytes, g->stream, err);
         storage = std::min<uint64_t>(storage, g->store[k].mapped / block_bytes);
+    }
+    if (g->lab_max_chunks) {
+        const size_t block_bytes = sizeof(uint32_t) * g->block_voxels();
+        ok = ok && vmm_map(&g->lab_head, static_cast<size_t>(blocks) * block_bytes, g->stream, err);
+        storage = std::min<uint64_t>(storage, g->lab_head.mapped / block_bytes);
     }
     g->index.pool_capacity = static_cast<uint32_t>(storage);
     return ok;
@@ -769,6 +1059,54 @@ extern "C" int b2v_sgrid_set_shard(b2v_sgrid *g, int32_t shard_rank, int32_t sha
     return g->set_shard(shard_rank, shard_count);
 }
 
+extern "C" int b2v_sgrid_set_label_overflow(b2v_sgrid *g, uint64_t max_pairs, uint64_t initial_pairs) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (max_pairs == 0) return B2V_OK;
+    const uint64_t chunks = (max_pairs + kChunkPairs - 1) / kChunkPairs;
+    if (g->G.kind != B2V_SEM_PROBABILISTIC || g->lab_max_chunks != 0 || chunks > kMaxLabelChunks) {
+        g->err = g->G.kind != B2V_SEM_PROBABILISTIC ? "b2v_sgrid_set_label_overflow: the voting grid has no label set"
+                 : g->lab_max_chunks ? "b2v_sgrid_set_label_overflow: the store is already set"
+                                     : "b2v_sgrid_set_label_overflow: more than 2^28 overflow pairs";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    int rc = g->fetch_counters();
+    if (rc != B2V_OK) return rc;
+    if (g->h_counters[kBgPool] != 0) {
+        g->err = "b2v_sgrid_set_label_overflow: only on a grid without blocks";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    const size_t head_block = sizeof(uint32_t) * g->block_voxels();
+    B2V_CUDA(g, g->d_lab_ctr.reserve(kLcNum));
+    if (!vmm_reserve(&g->lab_head, static_cast<size_t>(g->index.capacity) * head_block, g->device, &g->err) ||
+        !vmm_reserve(&g->lab_chunks, static_cast<size_t>(chunks) * sizeof(LabelChunk), g->device, &g->err) ||
+        !vmm_reserve(&g->lab_free, static_cast<size_t>(chunks) * sizeof(uint32_t), g->device, &g->err) ||
+        !vmm_map(&g->lab_head, static_cast<size_t>(g->index.pool_capacity) * head_block, g->stream, &g->err))
+        return B2V_ERR_CUDA;
+    g->lab_max_chunks = static_cast<uint32_t>(chunks);
+    const uint64_t first = std::max<uint64_t>(1, (initial_pairs + kChunkPairs - 1) / kChunkPairs);
+    if (!sgrid_map_labels(g, first, &g->err)) return B2V_ERR_CUDA;
+    rc = sgrid_label_reset(g, 0);
+    if (rc != B2V_OK) return rc;
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return B2V_OK;
+}
+
+extern "C" int b2v_sgrid_label_storage(b2v_sgrid *g, int64_t *chunks_used, int64_t *chunks_mapped,
+                                       int64_t *chunks_max, int64_t *growths) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    uint32_t c[kLcNum] = {};
+    if (g->lab_max_chunks) {
+        B2V_CUDA(g, cudaMemcpyAsync(c, g->d_lab_ctr.get(), sizeof(c), cudaMemcpyDeviceToHost, g->stream));
+        B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    }
+    if (chunks_used) *chunks_used = static_cast<int64_t>(c[kLcFresh]) - c[kLcFree];
+    if (chunks_mapped) *chunks_mapped = g->lab_mapped;
+    if (chunks_max) *chunks_max = g->lab_max_chunks;
+    if (growths) *growths = g->lab_growths;
+    return B2V_OK;
+}
+
 extern "C" int b2v_sgrid_clear(b2v_sgrid *g) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     ++g->generation;
@@ -814,6 +1152,76 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
     return B2V_OK;
 }
 
+// map chunk storage for at least `chunks` chunks (at most the ceiling); false if a mapping failed
+static bool sgrid_map_labels(b2v_sgrid *g, uint64_t chunks, std::string *err) {
+    chunks = std::min<uint64_t>(chunks, g->lab_max_chunks);
+    const bool ok = vmm_map(&g->lab_chunks, static_cast<size_t>(chunks) * sizeof(LabelChunk), g->stream, err) &&
+                    vmm_map(&g->lab_free, static_cast<size_t>(chunks) * sizeof(uint32_t), g->stream, err);
+    const uint64_t held = std::min<uint64_t>(g->lab_chunks.mapped / sizeof(LabelChunk),
+                                             g->lab_free.mapped / sizeof(uint32_t));
+    g->lab_mapped = static_cast<uint32_t>(std::max<uint64_t>(g->lab_mapped, std::min(chunks, held)));
+    return ok;
+}
+
+// After a runs pass with a label store: the chunks its runs took leave the free list or the fresh storage, the pass
+// counters are re-armed, and *listed is the number of runs that got none.  *wanted: the chunks the storage must hold
+// for their replay.  Synchronises.
+static int sgrid_label_settle(b2v_sgrid *g, uint32_t *listed, uint64_t *wanted) {
+    uint32_t c[kLcNum];
+    B2V_CUDA(g, cudaMemcpyAsync(c, g->d_lab_ctr.get(), sizeof(c), cudaMemcpyDeviceToHost, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    // the runs that got chunks requested exactly [0, first fail) of the pass's requests
+    const uint32_t used = std::min(c[kLcTaken], c[kLcFirstFail]);
+    const uint32_t from_free = std::min(used, c[kLcFree]);
+    c[kLcFree] -= from_free;
+    c[kLcFresh] += used - from_free;
+    *wanted = c[kLcFresh] + std::max<int64_t>(0, static_cast<int64_t>(c[kLcTaken] - used) - c[kLcFree]);
+    *listed = c[kLcListed];
+    g->lab_full = g->lab_full || c[kLcFull] != 0;
+    c[kLcTaken] = 0;
+    c[kLcFirstFail] = UINT32_MAX;
+    c[kLcListed] = 0;
+    c[kLcFull] = 0;
+    B2V_CUDA(g, cudaMemcpyAsync(g->d_lab_ctr.get(), c, sizeof(c), cudaMemcpyHostToDevice, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return B2V_OK;
+}
+
+// sem_runs_kernel with a label store: the runs that found no chunks write nothing and are listed; the storage then
+// grows to hold them (at least doubling, at most the ceiling) and they are replayed over the same sorted pairs.  A
+// voxel's run is its only update in the pass, so the replay applies it from the state before the pass.  Past the
+// ceiling the replayed runs that still find no chunks evict (g->lab_full).
+static int sgrid_runs_chain(b2v_sgrid *g, int64_t n, const SemInputs &in) {
+    cudaStream_t s = g->stream;
+    if (g->d_lab_list.size() < static_cast<size_t>(n)) {
+        B2V_CUDA(g, cudaStreamSynchronize(s));
+        B2V_CUDA(g, g->d_lab_list.reserve(static_cast<size_t>(n) + n / 4 + 1024));
+    }
+    sem_runs_kernel<true><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(),
+                                                                                n, in, g->dev(), g->labels());
+    B2V_CUDA(g, cudaGetLastError());
+    uint32_t listed = 0;
+    uint64_t wanted = 0;
+    int rc = sgrid_label_settle(g, &listed, &wanted);
+    if (rc != B2V_OK || listed == 0) return rc;
+    if (wanted > g->lab_mapped && g->lab_mapped < g->lab_max_chunks) {
+        // a failed mapping still replays (the runs without chunks evict), then the call reports the device error
+        const uint32_t old = g->lab_mapped;
+        std::string map_err;
+        if (!sgrid_map_labels(g, std::max<uint64_t>(wanted, 2ull * old), &map_err) && g->lab_map_err.empty())
+            g->lab_map_err = "label storage could not grow: " + map_err;
+        if (g->lab_mapped > old) ++g->lab_growths;
+    }
+    LabelStore S = g->labels();
+    S.replay = g->d_lab_list.get();
+    S.n_replay = listed;
+    S.no_growth = 1;
+    sem_runs_kernel<true><<<(listed + 127) / 128, 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(), n, in, g->dev(),
+                                                              S);
+    B2V_CUDA(g, cudaGetLastError());
+    return sgrid_label_settle(g, &listed, &wanted);
+}
+
 // keys -> sort -> runs over the staged point records, for the points whose block's pool index lies in [lo, hi)
 static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid, uint32_t lo, uint32_t hi) {
     cudaStream_t s = g->stream;
@@ -833,8 +1241,9 @@ static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8
     size_t tmp = g->d_sort_tmp.size();  // all 32 key bits: kBadVid (points without storage) must sort last
     B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp.get(), tmp, g->d_vid[0].get(), g->d_vid[1].get(),
                                                g->d_ord[0].get(), g->d_ord[1].get(), n, 0, 32, s));
-    sem_runs_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(), n,
-                                                                          in, g->dev());
+    if (g->lab_max_chunks) return sgrid_runs_chain(g, n, in);
+    sem_runs_kernel<false><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(),
+                                                                                 n, in, g->dev(), LabelStore{});
     B2V_CUDA(g, cudaGetLastError());
     return B2V_OK;
 }
@@ -846,6 +1255,8 @@ static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8
 // maximum.  The staged inputs must stay alive until the call ends.
 static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid) {
     ++g->generation;
+    g->lab_full = false;
+    g->lab_map_err.clear();
     B2V_CUDA(g, launch_point_insert(in.pts, in.pts_f64 != 0, valid, n, g->inv_voxel_size, g->log2_block, g->table,
                                     g->index, g->stream));
     const int rc = sgrid_apply(g, n, in, valid, 0, g->index.pool_capacity);
@@ -861,6 +1272,20 @@ static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const
             B2V_CUDA(g, cudaGetLastError());
             return sgrid_apply(g, n, in, valid, lo, hi);
         });
+}
+
+// end of an integrate call: the counters, then B2V_ERR_CUDA if the label storage failed to grow, or "label storage
+// full" if a voxel evicted past the store's ceiling
+static int sgrid_finish(b2v_sgrid *g) {
+    const int rc = g->read_counters();
+    if (rc != B2V_OK) return rc;
+    if (!g->lab_map_err.empty()) {
+        g->err = g->lab_map_err;
+        return B2V_ERR_CUDA;
+    }
+    if (!g->lab_full) return rc;
+    g->err = "label storage full";
+    return B2V_ERR_CAPACITY;
 }
 
 extern "C" int b2v_sgrid_integrate(b2v_sgrid *g, int64_t n, const void *points, int32_t points_f64,
@@ -898,7 +1323,7 @@ extern "C" int b2v_sgrid_integrate(b2v_sgrid *g, int64_t n, const void *points, 
     in.cols_u8 = colors_u8 ? 1 : 0;
     rc = sgrid_fuse_staged(g, n, in, nullptr);
     if (rc != B2V_OK) return rc;
-    return g->read_counters();  // also the completion fence: the inputs are free when this returns
+    return sgrid_finish(g);  // also the completion fence: the inputs are free when this returns
 }
 
 extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const uint8_t *color,
@@ -933,7 +1358,7 @@ extern "C" int b2v_sgrid_integrate_rgbd(b2v_sgrid *g, const float *depth, const 
     in.depths = use_depths ? g->d_depths.get() : nullptr;
     rc = sgrid_fuse_staged(g, n, in, g->d_valid.get());
     if (rc != B2V_OK) return rc;
-    return g->read_counters();
+    return sgrid_finish(g);
 }
 
 extern "C" int64_t b2v_sgrid_num_blocks(b2v_sgrid *g) {
@@ -1040,9 +1465,9 @@ static int sgrid_edit(b2v_sgrid *g, int op, int a, int b) {
     if (nb < 0) return B2V_ERR_CUDA;
     if (nb == 0) return B2V_OK;
     const uint32_t nbu = static_cast<uint32_t>(nb);
-    g->dispatch([&](auto l) {
-        sem_edit_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(g->dev(), op, a, b,
-                                                                                      nbu * g->block_voxels());
+    sgrid_dispatch(g, [&](auto l, auto c) {
+        sem_edit_kernel<decltype(l)::value, decltype(c)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(
+            g->dev(), op, a, b, nbu * g->block_voxels(), g->labels());
     });
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
@@ -1083,6 +1508,8 @@ extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *
     d2h(aux, g->G.counter, nv * sizeof(int32_t));
     std::vector<int32_t> h_count, h_ctr, lo, lc;
     std::vector<float> lp;
+    std::vector<uint32_t> heads;
+    std::vector<LabelChunk> chunks;
     const bool bayes = g->G.kind == B2V_SEM_PROBABILISTIC;
     const bool want_labels = bayes && K > 0 && (lab_obj || lab_cls || lab_logp);
     if (confidence) {
@@ -1106,6 +1533,16 @@ extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *
         d2h(lo.data(), g->G.lab_obj, lo.size() * sizeof(int32_t));
         d2h(lc.data(), g->G.lab_cls, lc.size() * sizeof(int32_t));
         d2h(lp.data(), g->G.lab_logp, lp.size() * sizeof(float));
+        if (g->lab_max_chunks) {   // the chains: every chunk ever taken, fresh ones included
+            uint32_t c[kLcNum];
+            ok = ok && cudaMemcpyAsync(c, g->d_lab_ctr.get(), sizeof(c), cudaMemcpyDeviceToHost, g->stream) ==
+                           cudaSuccess &&
+                 cudaStreamSynchronize(g->stream) == cudaSuccess;
+            heads.resize(nv);
+            chunks.resize(ok ? c[kLcFresh] : 0);
+            d2h(heads.data(), reinterpret_cast<const void *>(g->lab_head.va), nv * sizeof(uint32_t));
+            d2h(chunks.data(), reinterpret_cast<const void *>(g->lab_chunks.va), chunks.size() * sizeof(LabelChunk));
+        }
     }
     ok = ok && cudaStreamSynchronize(g->stream) == cudaSuccess;
     if (!ok) {
@@ -1127,24 +1564,27 @@ extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *
         }
     if (want_labels) {
         const float ninf = -std::numeric_limits<float>::infinity();
-        for (size_t v = 0; v < nv; ++v) {
-            int idx[kSemLabels];
-            const int nl = h_ctr[v] < kSemLabels ? h_ctr[v] : kSemLabels;
-            for (int k = 0; k < nl; ++k) idx[k] = k;
-            for (int a = 1; a < nl; ++a)  // insertion sort by (object, class)
-                for (int q = a; q > 0; --q) {
-                    const size_t i0 = v * kSemLabels + idx[q - 1], i1 = v * kSemLabels + idx[q];
-                    if (lo[i0] < lo[i1] || (lo[i0] == lo[i1] && lc[i0] <= lc[i1])) break;
-                    const int t = idx[q];
-                    idx[q] = idx[q - 1];
-                    idx[q - 1] = t;
-                }
+        struct Pair {
+            int32_t o, c;
+            float l;
+        };
+        std::vector<Pair> pairs;
+        for (size_t v = 0; v < nv; ++v) {   // the voxel's pairs in slot order, then sorted by (object, class)
+            pairs.clear();
+            const int nl = heads.empty() ? std::min(h_ctr[v], kSemLabels) : h_ctr[v];
+            for (int k = 0; k < nl && k < kSemLabels; ++k)
+                pairs.push_back({lo[v * kSemLabels + k], lc[v * kSemLabels + k], lp[v * kSemLabels + k]});
+            for (uint32_t link = heads.empty() ? 0 : heads[v]; link != 0 && link <= chunks.size();
+                 link = chunks[link - 1].next)
+                for (int e = 0; e < kChunkPairs && static_cast<int>(pairs.size()) < nl; ++e)
+                    pairs.push_back({chunks[link - 1].obj[e], chunks[link - 1].cls[e], chunks[link - 1].logp[e]});
+            std::stable_sort(pairs.begin(), pairs.end(),
+                             [](const Pair &a, const Pair &b) { return a.o < b.o || (a.o == b.o && a.c < b.c); });
             for (int k = 0; k < K; ++k) {
-                const bool have = k < nl;
-                const size_t src = v * kSemLabels + (have ? idx[k] : 0);
-                if (lab_obj) lab_obj[v * K + k] = have ? lo[src] : -1;
-                if (lab_cls) lab_cls[v * K + k] = have ? lc[src] : -1;
-                if (lab_logp) lab_logp[v * K + k] = have ? lp[src] : ninf;
+                const bool have = k < static_cast<int>(pairs.size());
+                if (lab_obj) lab_obj[v * K + k] = have ? pairs[k].o : -1;
+                if (lab_cls) lab_cls[v * K + k] = have ? pairs[k].c : -1;
+                if (lab_logp) lab_logp[v * K + k] = have ? pairs[k].l : ninf;
             }
         }
     }
@@ -1169,9 +1609,9 @@ extern "C" int b2v_sgrid_carve(b2v_sgrid *g, const float K[4], int32_t width, in
     if (rc != B2V_OK) return rc;
     const GridQuery q = g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1);
     const uint32_t nbu = static_cast<uint32_t>(nb);
-    g->dispatch([&](auto l) {
-        sem_carve_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(g->dev(), q, d_depth,
-                                                                                       depth_threshold, nbu);
+    sgrid_dispatch(g, [&](auto l, auto c) {
+        sem_carve_kernel<decltype(l)::value, decltype(c)::value><<<g->voxel_ctas(nbu), kVox, 0, g->stream>>>(
+            g->dev(), q, d_depth, depth_threshold, nbu, g->labels());
     });
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
@@ -1221,10 +1661,10 @@ static int64_t sgrid_assoc_votes(b2v_sgrid *g, const char *fn, const float K[4],
         if (e == cudaSuccess) {
             const GridQuery q = g->frustum_query(K, width, height, Tcw, depth_max, depth_min, 1);
             const uint32_t nbu = static_cast<uint32_t>(nb);
-            g->dispatch([&](auto l) {
-                sem_assoc_kernel<decltype(l)::value><<<g->voxel_ctas(nbu), kVox, 0, s>>>(
+            sgrid_dispatch(g, [&](auto l, auto c) {
+                sem_assoc_kernel<decltype(l)::value, decltype(c)::value><<<g->voxel_ctas(nbu), kVox, 0, s>>>(
                     g->dev(), q, d_cls, d_inst, d_depth, depth_threshold, (do_carving && depth_image) ? 1 : 0,
-                    g->d_pend.get(), g->d_records.get(), n_records, static_cast<uint32_t>(nv), nbu);
+                    g->d_pend.get(), g->d_records.get(), n_records, static_cast<uint32_t>(nv), nbu, g->labels());
             });
             e = cudaGetLastError();
         }
@@ -1386,9 +1826,12 @@ static int64_t sgrid_assoc_resolve(b2v_sgrid *g, const char *fn, const int32_t *
         e = cudaMemcpyAsync(d_map + m, g->map_obj.data(), m * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream);
     if (e == cudaSuccess && !new_id.empty() && g->votes_blocks > 0) {  // deferred assignment of this grid's pending voxels
         ++g->generation;
-        g->dispatch([&](auto l) {
-            sem_assoc_apply_kernel<decltype(l)::value><<<g->voxel_ctas(g->votes_blocks), kVox, 0, g->stream>>>(
-                g->dev(), g->d_pend.get(), d_map, d_map + m, static_cast<int>(m), g->votes_blocks * g->block_voxels());
+        sgrid_dispatch(g, [&](auto l, auto c) {
+            sem_assoc_apply_kernel<decltype(l)::value, decltype(c)::value>
+                <<<g->voxel_ctas(g->votes_blocks), kVox, 0, g->stream>>>(g->dev(), g->d_pend.get(), d_map, d_map + m,
+                                                                        static_cast<int>(m),
+                                                                        g->votes_blocks * g->block_voxels(),
+                                                                        g->labels());
         });
         e = cudaGetLastError();
     }
@@ -1558,5 +2001,191 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
             d_keys.get(), U, g->table, g->index.pool_capacity);
     B2V_CUDA(g, cudaGetLastError());
     B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    if (g->lab_max_chunks) {   // the uploaded voxels hold their in-voxel pairs only until b2v_sgrid_upload_labels
+        rc = sgrid_set_labels(g, "b2v_sgrid_upload_blocks", n_blocks, keys, nullptr, nullptr, nullptr, nullptr);
+        if (rc != B2V_OK) return rc;
+    }
     return g->read_counters();
+}
+
+// ---- overflow label pairs of the map state ------------------------------------------------------------------------
+// Host copies of what the label store's host passes read: per-voxel counters and chain heads of the nb blocks in use,
+// the store's counters, every chunk ever taken and the free list.
+struct LabelHost {
+    int64_t nb = 0;
+    std::vector<int32_t> counter;
+    std::vector<uint32_t> head, free_list;
+    std::vector<LabelChunk> chunks;
+    uint32_t ctr[kLcNum] = {};
+};
+
+static int sgrid_fetch_labels(b2v_sgrid *g, LabelHost *h) {
+    h->nb = b2v_sgrid_num_blocks(g);
+    if (h->nb < 0) return B2V_ERR_CUDA;
+    const size_t nv = static_cast<size_t>(h->nb) * g->block_voxels();
+    h->counter.resize(nv);
+    h->head.resize(nv);
+    B2V_CUDA(g, cudaMemcpyAsync(h->ctr, g->d_lab_ctr.get(), sizeof(h->ctr), cudaMemcpyDeviceToHost, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    h->chunks.resize(h->ctr[kLcFresh]);
+    h->free_list.resize(h->ctr[kLcFree]);
+    if (nv) {
+        B2V_CUDA(g, cudaMemcpyAsync(h->counter.data(), g->G.counter, nv * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                                    g->stream));
+        B2V_CUDA(g, cudaMemcpyAsync(h->head.data(), reinterpret_cast<const void *>(g->lab_head.va),
+                                    nv * sizeof(uint32_t), cudaMemcpyDeviceToHost, g->stream));
+    }
+    if (!h->chunks.empty())
+        B2V_CUDA(g, cudaMemcpyAsync(h->chunks.data(), reinterpret_cast<const void *>(g->lab_chunks.va),
+                                    h->chunks.size() * sizeof(LabelChunk), cudaMemcpyDeviceToHost, g->stream));
+    if (!h->free_list.empty())
+        B2V_CUDA(g, cudaMemcpyAsync(h->free_list.data(), reinterpret_cast<const void *>(g->lab_free.va),
+                                    h->free_list.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, g->stream));
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    return B2V_OK;
+}
+
+// The uploaded blocks `keys` [n][3] that the grid holds get their overflow pairs: each voxel's chain goes back to the
+// pool, its counter keeps its in-voxel pairs (at most B2V_SEM_MAX_LABELS) and, if n_over is not NULL, it takes a new
+// chain of n_over[voxel] pairs from obj / cls / logp (slot order; the pairs of blocks the grid does not hold are
+// skipped).  Checks first and changes nothing on a bad argument or when the pool's ceiling cannot hold the pairs.
+static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+                            const int32_t *obj, const int32_t *cls, const float *logp) {
+    const size_t nvb = g->block_voxels();
+    LabelHost h;
+    int rc = sgrid_fetch_labels(g, &h);
+    if (rc != B2V_OK) return rc;
+    // pool index of every block in use, by key
+    std::vector<int4> hk(static_cast<size_t>(h.nb));
+    if (h.nb) {
+        B2V_CUDA(g, cudaMemcpy(hk.data(), g->index.block_keys, hk.size() * sizeof(int4), cudaMemcpyDeviceToHost));
+    }
+    std::map<std::tuple<int32_t, int32_t, int32_t>, uint32_t> pool;
+    for (int64_t b = 0; b < h.nb; ++b) pool[{hk[b].x, hk[b].y, hk[b].z}] = static_cast<uint32_t>(b);
+    std::vector<int64_t> idx(static_cast<size_t>(n_blocks), -1);
+    for (int64_t b = 0; b < n_blocks; ++b) {
+        const auto it = pool.find({keys[3 * b], keys[3 * b + 1], keys[3 * b + 2]});
+        if (it != pool.end()) idx[b] = it->second;
+    }
+    // checks: counts, and the chunks the new chains need against what the pool can give once the old ones are back
+    uint64_t need = 0, released = 0;
+    for (int64_t b = 0; b < n_blocks; ++b)
+        for (size_t t = 0; t < nvb; ++t) {
+            const int32_t m = n_over ? n_over[b * nvb + t] : 0;
+            if (m < 0 || (m > 0 && idx[b] >= 0 && h.counter[idx[b] * nvb + t] < kSemLabels)) {
+                g->err = std::string(fn) + ": overflow pairs of a voxel without " + std::to_string(kSemLabels) +
+                         " in-voxel pairs, or a negative count";
+                return B2V_ERR_INVALID_ARGUMENT;
+            }
+            if (idx[b] < 0) continue;
+            need += (static_cast<uint64_t>(m) + kChunkPairs - 1) / kChunkPairs;
+            for (uint32_t l = h.head[idx[b] * nvb + t]; l != 0; l = h.chunks[l - 1].next) ++released;
+        }
+    if (need > static_cast<uint64_t>(h.ctr[kLcFree]) + released + (g->lab_max_chunks - h.ctr[kLcFresh])) {
+        g->err = std::string(fn) + ": label storage full";
+        return B2V_ERR_CAPACITY;
+    }
+    // release, then new chains: chunks from the free list first, then fresh ones
+    size_t pos = 0;
+    for (int64_t b = 0; b < n_blocks; ++b)
+        for (size_t t = 0; t < nvb; ++t) {
+            const int32_t m = n_over ? n_over[b * nvb + t] : 0;
+            if (idx[b] < 0) {
+                pos += static_cast<size_t>(m);
+                continue;
+            }
+            const size_t v = idx[b] * nvb + t;
+            for (uint32_t l = h.head[v]; l != 0; l = h.chunks[l - 1].next) h.free_list.push_back(l - 1);
+            h.head[v] = 0;
+            h.counter[v] = std::min(h.counter[v], static_cast<int32_t>(kSemLabels)) + m;
+            uint32_t tail = 0;
+            for (int32_t e = 0; e < m; ++e, ++pos) {
+                if (e % kChunkPairs == 0) {
+                    uint32_t c;
+                    if (!h.free_list.empty()) {
+                        c = h.free_list.back();
+                        h.free_list.pop_back();
+                    } else {
+                        c = static_cast<uint32_t>(h.chunks.size());
+                        h.chunks.emplace_back();
+                    }
+                    h.chunks[c] = LabelChunk{};
+                    if (tail) h.chunks[tail - 1].next = c + 1;
+                    else h.head[v] = c + 1;
+                    tail = c + 1;
+                }
+                LabelChunk &c = h.chunks[tail - 1];
+                c.obj[e % kChunkPairs] = obj[pos];
+                c.cls[e % kChunkPairs] = cls[pos];
+                c.logp[e % kChunkPairs] = logp[pos];
+            }
+        }
+    std::string map_err;
+    if (h.chunks.size() > g->lab_mapped && !sgrid_map_labels(g, h.chunks.size(), &map_err)) {
+        g->err = std::string(fn) + ": label storage could not grow: " + map_err;
+        return B2V_ERR_CUDA;
+    }
+    h.ctr[kLcFree] = static_cast<uint32_t>(h.free_list.size());
+    h.ctr[kLcFresh] = static_cast<uint32_t>(h.chunks.size());
+    const size_t nv = h.counter.size();
+    if (nv) {
+        B2V_CUDA(g, cudaMemcpy(g->G.counter, h.counter.data(), nv * sizeof(int32_t), cudaMemcpyHostToDevice));
+        B2V_CUDA(g, cudaMemcpy(reinterpret_cast<void *>(g->lab_head.va), h.head.data(), nv * sizeof(uint32_t),
+                               cudaMemcpyHostToDevice));
+    }
+    if (!h.chunks.empty())
+        B2V_CUDA(g, cudaMemcpy(reinterpret_cast<void *>(g->lab_chunks.va), h.chunks.data(),
+                               h.chunks.size() * sizeof(LabelChunk), cudaMemcpyHostToDevice));
+    if (!h.free_list.empty())
+        B2V_CUDA(g, cudaMemcpy(reinterpret_cast<void *>(g->lab_free.va), h.free_list.data(),
+                               h.free_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    B2V_CUDA(g, cudaMemcpy(g->d_lab_ctr.get(), h.ctr, sizeof(h.ctr), cudaMemcpyHostToDevice));
+    return B2V_OK;
+}
+
+extern "C" int64_t b2v_sgrid_export_labels(b2v_sgrid *g, int32_t *n_over, int32_t *obj, int32_t *cls, float *logp) {
+    if (!g) return -1;
+    const size_t nvb = g->block_voxels();
+    if (g->lab_max_chunks == 0) {   // no store: no overflow pairs
+        const int64_t nb = b2v_sgrid_num_blocks(g);
+        if (nb > 0 && n_over) std::fill(n_over, n_over + static_cast<size_t>(nb) * nvb, 0);
+        return nb < 0 ? -1 : 0;
+    }
+    LabelHost h;
+    if (sgrid_fetch_labels(g, &h) != B2V_OK) return -1;
+    int64_t total = 0;
+    for (size_t v = 0; v < h.counter.size(); ++v) {
+        const int32_t m = h.counter[v] > kSemLabels ? h.counter[v] - kSemLabels : 0;
+        if (n_over) n_over[v] = m;
+        int32_t e = 0;
+        for (uint32_t l = h.head[v]; l != 0 && e < m; l = h.chunks[l - 1].next)
+            for (int k = 0; k < kChunkPairs && e < m; ++k, ++e) {
+                if (obj) obj[total + e] = h.chunks[l - 1].obj[k];
+                if (cls) cls[total + e] = h.chunks[l - 1].cls[k];
+                if (logp) logp[total + e] = h.chunks[l - 1].logp[k];
+            }
+        total += m;
+    }
+    return total;
+}
+
+extern "C" int b2v_sgrid_upload_labels(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+                                       const int32_t *obj, const int32_t *cls, const float *logp) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (n_blocks < 0 || (n_blocks > 0 && (!keys || !n_over))) {
+        g->err = "b2v_sgrid_upload_labels: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    const size_t nv = static_cast<size_t>(n_blocks) * g->block_voxels();
+    int64_t total = 0;
+    for (size_t v = 0; v < nv; ++v) total += n_over[v] > 0 ? n_over[v] : 0;
+    if (total == 0) return B2V_OK;
+    if (g->lab_max_chunks == 0 || !obj || !cls || !logp) {
+        g->err = g->lab_max_chunks == 0 ? "b2v_sgrid_upload_labels: overflow pairs for a grid without a label store"
+                                        : "b2v_sgrid_upload_labels: bad arguments";
+        return g->lab_max_chunks == 0 ? B2V_ERR_CAPACITY : B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(g, cudaSetDevice(g->device));
+    ++g->generation;
+    return sgrid_set_labels(g, "b2v_sgrid_upload_labels", n_blocks, keys, n_over, obj, cls, logp);
 }

@@ -61,6 +61,10 @@ DEFAULT_PARAMETERS = {
     # growth ceiling of the grid's storage: > CapacityBlocks starts with CapacityBlocks blocks and maps more on
     # demand, holding what a grid of this size from the start holds; 0 = fixed storage of CapacityBlocks
     "kVolumetricIntegrationB200MaxCapacityBlocks": 0,
+    # Bayesian grid (use_semantic_probabilistic): ceiling of the overflow label store, in (object, class) pairs past
+    # the 8 a voxel holds itself; below it no voxel evicts a pair and the labels equal the reference's unbounded map.
+    # 0 = no store (a ninth pair evicts the weakest); the voting grid has no label set and ignores it
+    "kVolumetricIntegrationB200LabelOverflowPairs": 0,
     "kVolumetricIntegrationB200Device": 0,
     "kVolumetricIntegrationB200GenerateObjects": True,   # kGenerateObjectsDefault (reference :84)
     # raw keyframe images to the grid (set_frame): upload once, undistort + BGR->RGB + depth widening + shadow filter
@@ -134,7 +138,13 @@ def make_semantic_integrator_class(Base, api):
         def _make_grid(self, p, side, constructor_kwargs):
             probabilistic = bool(constructor_kwargs.get("use_semantic_probabilistic", False))
             grid_t = VoxelBlockSemanticProbabilisticGrid if probabilistic else VoxelBlockSemanticGrid
-            grid = grid_t(**_grid_args(p, self.b200_set_parameters))
+            pairs = int(p["kVolumetricIntegrationB200LabelOverflowPairs"])
+            if pairs and not probabilistic:
+                getattr(Base, "print", print)("VolumetricIntegratorB200SemanticGrid: "
+                                              "kVolumetricIntegrationB200LabelOverflowPairs ignored: it applies to "
+                                              "use_semantic_probabilistic only")
+                pairs = 0
+            grid = grid_t(**_grid_args(p, self.b200_set_parameters), max_label_overflow_pairs=pairs)
             grid.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
             grid.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
             return grid

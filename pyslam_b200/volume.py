@@ -88,10 +88,13 @@ class _MapState:
     """`save_state` / `load_state` of the TSDF volume and the voxel grids (`map_state` holds the file format).  A map
     kind names itself in `_STATE_KIND` and provides `_state_config()` (what the voxels mean: must match to load),
     `_state_arrays()` (per-block array specs, keys first), `_export_state()`, `_state_capacity()` (the most blocks it
-    can hold), `_clear_state()` and `_upload_state(blocks)`; the semantic grids add restored settings."""
+    can hold), `_clear_state()` and `_upload_state(blocks)`; the semantic grids add restored settings, and a map with
+    `_STATE_LABELS` its overflow label pairs (`_export_labels()`, `_check_labels(labels)`, `_upload_labels(keys,
+    labels)`)."""
 
     _STATE_KIND = ""
     _STATE_BOUNDS: dict = {}
+    _STATE_LABELS = False   # the map has overflow label pairs (a Bayesian semantic grid)
 
     def _state_semantic_kind(self) -> int:
         return -1
@@ -109,7 +112,8 @@ class _MapState:
         label-overflow counter (counts from 0 after a load) and the last association's instance map
         (`remap_instance_ids` needs a new association, as on a fresh grid)."""
         map_state.write(path, self._STATE_KIND, self._state_semantic_kind(), self._state_config(),
-                        self._state_settings(), self.shard_rank, self.shard_count, self._export_state())
+                        self._state_settings(), self.shard_rank, self.shard_count, self._export_state(),
+                        self._export_labels() if self._STATE_LABELS else None)
 
     def load_state(self, paths) -> None:
         """Replace the map with the state in `paths`: one file, or a list such as the files of every shard of an
@@ -119,14 +123,20 @@ class _MapState:
         duplicate keys, out-of-range values or more owned blocks than this object's ceiling raise ValueError and leave
         the map as it was.  The blocks are uploaded in bounded chunks.  What is not part of the state: `save_state`."""
         spec = self._state_arrays()
-        settings, blocks = map_state.read(
+        settings, blocks, *labels = map_state.read(
             paths, self._STATE_KIND, self._state_semantic_kind(), self._state_config(),
             {name: np.asarray(v).dtype for name, v in self._state_settings().items()}, spec, self.shard_rank,
-            self.shard_count, self._state_capacity(), self._STATE_BOUNDS)
+            self.shard_count, self._state_capacity(), self._STATE_BOUNDS, labels=self._STATE_LABELS)
+        labels = labels[0] if labels else None
+        if labels is not None:
+            self._check_labels(labels)
         self._clear_state()
         block_bytes = sum(np.dtype(dt).itemsize * int(np.prod(shape)) for dt, shape in spec.values())
         for a, b in map_state.chunks(len(blocks["keys"]), block_bytes):
-            self._upload_state({name: x[a:b] for name, x in blocks.items()})
+            part = {name: x[a:b] for name, x in blocks.items()}
+            self._upload_state(part)
+            if labels is not None:
+                self._upload_labels(part["keys"], map_state.label_slice(labels, a, b))
         self._restore_settings(settings)
 
 
@@ -1237,14 +1247,32 @@ class VoxelBlockSemanticGrid(_BlockGrid):
     _P = "b2v_sgrid_"
 
     def __init__(self, voxel_size: float = 0.05, block_size: int = 8, capacity_blocks: int = 1 << 14,
-                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1):
+                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1,
+                 max_label_overflow_pairs: int = 0, initial_label_overflow_pairs: int | None = None):
         """`max_capacity_blocks`: growth ceiling (at most 2^22 blocks).  Above `capacity_blocks`, the per-voxel storage
         starts with `capacity_blocks` blocks and grows inside the integrate call that needs more; the grid then holds,
         bit for bit, what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or
         `capacity_blocks`) keeps the storage fixed.  `shard_rank` / `shard_count`: see `set_shard`; the association
-        of a sharded grid runs over all ranks (`sharding.assign_object_ids_to_instance_ids_sharded`)."""
+        of a sharded grid runs over all ranks (`sharding.assign_object_ids_to_instance_ids_sharded`).
+
+        `max_label_overflow_pairs` (Bayesian grid only; a non-zero value raises RuntimeError on the voting grid):
+        ceiling of the overflow label store, in (object, class) pairs past the 8 a voxel holds itself, shared by all
+        voxels and rounded up to chunks of 8.  Below it no voxel evicts a pair and the grid equals the reference's
+        unbounded label map; past it the integrate call evicts as without a store and raises ("label storage full").
+        0 (the default) is the grid without a store.  The store's storage starts with `initial_label_overflow_pairs`
+        (None: the ceiling, at most 2^17 pairs) and grows inside the integrate call that needs more."""
         super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count,
                          self.KIND)
+        max_pairs = int(max_label_overflow_pairs)
+        if max_pairs < 0:
+            raise RuntimeError("max_label_overflow_pairs must be >= 0")
+        if max_pairs:
+            first = min(max_pairs, 1 << 17) if initial_label_overflow_pairs is None else int(initial_label_overflow_pairs)
+            rc = self._L.b2v_sgrid_set_label_overflow(self._h, max_pairs, max(0, first))
+            if rc != _lib.B2V_OK:
+                msg = self._L.b2v_sgrid_last_error(self._h).decode()
+                self.close()
+                raise RuntimeError(f"max_label_overflow_pairs: {msg} (status {rc})")
         # mirrors of the library's settings (class defaults, voxel_data_semantic.h:107-108, 251-254), for save_state
         self._depth_threshold = np.float32(10.0 if self.KIND == _lib.B2V_SEM_VOTING else 5.0)
         self._depth_decay_rate = np.float32(0.07)
@@ -1314,6 +1342,47 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         return d
 
     _export_state = export_blocks
+
+    @property
+    def _STATE_LABELS(self):
+        return self.KIND == _lib.B2V_SEM_PROBABILISTIC
+
+    def export_labels(self) -> dict:
+        """The overflow label pairs (b2v_sgrid_export_labels): count int32 [nb,B^3] (each voxel's pairs past its 8
+        in-voxel slots, in the block order of `export_blocks`) and obj / cls int32, logp float32 [total], voxel after
+        voxel, each voxel's in slot order."""
+        nb = self.num_blocks()
+        count = np.zeros((nb, self._block_voxels), np.int32)
+        total = self._L.b2v_sgrid_export_labels(self._h, count.ctypes.data, None, None, None)
+        if total < 0:
+            raise RuntimeError(f"b2v_sgrid_export_labels failed: {self._L.b2v_sgrid_last_error(self._h).decode()}")
+        out = dict(count=count, obj=np.zeros(total, np.int32), cls=np.zeros(total, np.int32),
+                   logp=np.zeros(total, np.float32))
+        if total:
+            n = self._L.b2v_sgrid_export_labels(self._h, count.ctypes.data, out["obj"].ctypes.data,
+                                                out["cls"].ctypes.data, out["logp"].ctypes.data)
+            if n != total:
+                raise RuntimeError(f"b2v_sgrid_export_labels returned {n}, expected {total}")
+        return out
+
+    def _export_labels(self):
+        """The overflow pairs for the state file; None (the file of a grid without them) when no voxel has any."""
+        return self.export_labels() if self.label_storage()["used"] else None
+
+    def _check_labels(self, labels: dict) -> None:
+        """ValueError, before the map changes, when the label store's ceiling cannot hold the file's pairs."""
+        need = int(((labels["count"].astype(np.int64) + 7) // 8).sum())
+        have = self.label_storage()["max"]
+        if need > have:
+            raise ValueError(f"the state holds overflow label pairs in {need} chunks of 8 for this grid, more than its "
+                             f"max_label_overflow_pairs ceiling of {have} chunks")
+
+    def _upload_labels(self, keys, labels: dict) -> None:
+        n = len(keys)
+        arrs = [np.ascontiguousarray(labels[k]) for k in ("count", "obj", "cls", "logp")]
+        self._check(self._L.b2v_sgrid_upload_labels(self._h, n, np.ascontiguousarray(keys).ctypes.data if n else None,
+                                                    *[a.ctypes.data if a.size else None for a in arrs]),
+                    "b2v_sgrid_upload_labels")
 
     def _upload_state(self, blocks: dict) -> None:
         n = len(blocks["keys"])
@@ -1523,8 +1592,20 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         self._check(self._L.b2v_sgrid_label_overflows(self._h, C.byref(out)), "b2v_sgrid_label_overflows")
         return int(out.value)
 
-    def dump_blocks(self, K: int = 8):
-        """Parity hook: per-block arrays [nb,B^3,...] incl. labels (see include/b2v.h)."""
+    def label_storage(self) -> dict:
+        """The overflow label store in chunks of 8 pairs: `used` (in some voxel's chain), `mapped` (with storage),
+        `max` (the ceiling; 0 without a store) and `growths` of its storage."""
+        v = [C.c_int64(0) for _ in range(4)]
+        self._check(self._L.b2v_sgrid_label_storage(self._h, *map(C.byref, v)), "b2v_sgrid_label_storage")
+        return dict(zip(("used", "mapped", "max", "growths"), (int(x.value) for x in v)))
+
+    def dump_blocks(self, K: int | None = None):
+        """Parity hook: per-block arrays [nb,B^3,...] incl. labels (see include/b2v.h).  K: label pairs per voxel in
+        the dump; None: the largest pair count of a voxel (at least 8)."""
+        if K is None:
+            K = _lib.B2V_SEM_MAX_LABELS
+            if self.KIND == _lib.B2V_SEM_PROBABILISTIC and self.num_blocks():
+                K = max(K, int(self.export_blocks()["counter"].max()))
         nb, nv = self.num_blocks(), self._block_voxels
         d = dict(keys=np.zeros((nb, 3), np.int32), hashes=np.zeros(nb, np.uint64),
                  count=np.zeros((nb, nv), np.int32), pos_sum=np.zeros((nb, nv, 3), np.float64),
