@@ -50,6 +50,7 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_assoc_votes", "b2v_sgrid_copy_assoc_votes", "b2v_sgrid_assoc_resolve",
     "b2v_grid_upload_blocks", "b2v_sgrid_export_blocks", "b2v_sgrid_upload_blocks",
     "b2v_sgrid_set_label_overflow", "b2v_sgrid_label_storage", "b2v_sgrid_export_labels", "b2v_sgrid_upload_labels",
+    "b2v_grid_set_input_order_sums",
 ]
 
 
@@ -252,6 +253,8 @@ def load() -> C.CDLL:
     L.b2v_grid_integrate_f64.argtypes = [vp, vp, vp, i64]
     L.b2v_grid_integrate_ex.restype = C.c_int
     L.b2v_grid_integrate_ex.argtypes = [vp, vp, i32, vp, i32, i64]
+    L.b2v_grid_set_input_order_sums.restype = C.c_int
+    L.b2v_grid_set_input_order_sums.argtypes = [vp, i32]
     L.b2v_grid_integrate_rgbd.restype = C.c_int
     L.b2v_grid_integrate_rgbd.argtypes = [vp, vp, vp, i32, i32, vp, vp, C.c_float, C.c_float, i32]
     L.b2v_filter_shadow_points.restype = C.c_int

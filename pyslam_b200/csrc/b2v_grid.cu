@@ -10,7 +10,11 @@
 //         local index lx + B ly + B^2 lz (voxel_block.h:67-70) -- bit exact, for B = 1 << L (1, 2, 8, 16) a template
 //         parameter of every kernel that keys or walks voxels (with_grid_block picks the instantiation).
 //   sums: float atomics => same values as the reference up to summation order; sub-normal addends are kept
-//         (sum_add), as the reference's float adds keep them.
+//         (sum_add), as the reference's float adds keep them.  With input-order sums (b2v_grid_set_input_order_sums)
+//         each voxel instead adds its points in input order with IEEE float32 adds (voxel sort -> grid_runs_kernel),
+//         the sequential reference's sums bit for bit.
+#include <cub/device/device_radix_sort.cuh>
+
 #include <cmath>
 #include <cstring>
 #include <new>
@@ -202,6 +206,96 @@ grid_rgbd_accumulate_kernel(const RgbdParams P, const float *__restrict__ depth,
     for (int c = 0; c < 3; ++c)  // voxel_grid.py:271-273
         sum_add(fb + (4 + c) * kV + l, rgbd_color(rgb[3 * i + c]));
     atomicAdd(reinterpret_cast<int *>(blk) + l, 1);
+}
+
+// ---- voxel-order sort (both grids' input-order updates: BlockGridCore::sort_voxels) -------------------------
+// sort key of point i: pool index * B^3 + local index when its block has a pool index in [lo, hi), else kBadVid (also
+// for points masked out by `valid`); value: i.  A pass over [lo, hi) updates each voxel of those blocks once.
+template <typename T, int L>
+__global__ void __launch_bounds__(256)
+voxel_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, const int64_t n, const float inv_vs,
+                  const HashTable H, const uint32_t lo, const uint32_t hi, uint32_t *__restrict__ vid,
+                  uint32_t *__restrict__ order) {
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int vx = point_voxel_coord(pts[3 * i + 0], inv_vs), vy = point_voxel_coord(pts[3 * i + 1], inv_vs),
+              vz = point_voxel_coord(pts[3 * i + 2], inv_vs);
+    uint32_t key = kBadVid;
+    const uint32_t slot = (valid == nullptr || valid[i])
+                              ? table_find(H, grid_block_coord<L>(vx), grid_block_coord<L>(vy), grid_block_coord<L>(vz))
+                              : kEmpty;
+    if (slot != kEmpty) {
+        const uint32_t idx = H.entries[slot].w;
+        if (idx >= lo && idx < hi)   // kNoBlock is past every window
+            key = idx * GridBlock<L>::kVox + static_cast<uint32_t>(grid_local_index<L>(vx, vy, vz));
+    }
+    vid[i] = key;
+    order[i] = static_cast<uint32_t>(i);
+}
+
+// ---- input-order sums (b2v_grid_set_input_order_sums) ------------------------------------------------------
+// After the voxel-order sort each voxel's points of the pass are one run of equal keys, in input order (the sort is
+// stable).  The head of a run walks it from the voxel's stored values with the reference's per-point update
+// (voxel_data.h:53-57, 79-90): count + 1, position_sum += float32(x), color_sum += colour, each an IEEE float32 add
+// (--ftz=false keeps sub-normal addends), and writes each plane once.  The three sums of a group are independent
+// chains.  kBadVid ends the keys of the pass.  No colours (cols == nullptr): the colour sums are left as they are.
+template <typename Tp, typename Tc, int L>
+__global__ void __launch_bounds__(256)
+grid_runs_kernel(const uint32_t *__restrict__ vid, const uint32_t *__restrict__ order, const int64_t n,
+                 const Tp *__restrict__ pts, const Tc *__restrict__ cols, const GridMeta G) {
+    const int64_t j0 = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (j0 >= n) return;
+    const uint32_t v = vid[j0];
+    if (v == kBadVid || (j0 > 0 && vid[j0 - 1] == v)) return;  // not the head of a run
+    constexpr int kV = GridBlock<L>::kVox;
+    const int l = static_cast<int>(v & (kV - 1));
+    uint32_t *blk = G.pool + static_cast<size_t>(v >> (3 * L)) * kGridBlockWords<L>;
+    float *fb = reinterpret_cast<float *>(blk);
+    int count = reinterpret_cast<const int *>(blk)[l];
+    float px = fb[1 * kV + l], py = fb[2 * kV + l], pz = fb[3 * kV + l];
+    float cr = 0.0f, cg = 0.0f, cb = 0.0f;
+    if (cols != nullptr) cr = fb[4 * kV + l], cg = fb[5 * kV + l], cb = fb[6 * kV + l];
+    for (int64_t j = j0; j < n && vid[j] == v; ++j) {
+        const size_t i = order[j];
+        ++count;
+        px = __fadd_rn(px, static_cast<float>(pts[3 * i + 0]));
+        py = __fadd_rn(py, static_cast<float>(pts[3 * i + 1]));
+        pz = __fadd_rn(pz, static_cast<float>(pts[3 * i + 2]));
+        if (cols != nullptr) {
+            cr = __fadd_rn(cr, color_value(cols[3 * i + 0]));
+            cg = __fadd_rn(cg, color_value(cols[3 * i + 1]));
+            cb = __fadd_rn(cb, color_value(cols[3 * i + 2]));
+        }
+    }
+    reinterpret_cast<int *>(blk)[l] = count;
+    fb[1 * kV + l] = px;
+    fb[2 * kV + l] = py;
+    fb[3 * kV + l] = pz;
+    if (cols != nullptr) {
+        fb[4 * kV + l] = cr;
+        fb[5 * kV + l] = cg;
+        fb[6 * kV + l] = cb;
+    }
+}
+
+// integrate_rgbd with input-order sums: one thread per pixel writes the point record the front-end makes of it, from
+// the rgbd_point / rgbd_color of the atomic path, and a valid mask.  Invalid pixels are masked, not compacted, so each
+// voxel's run follows the row-major pixel order, the reference's point order.
+__global__ void __launch_bounds__(256)
+grid_rgbd_points_kernel(const RgbdParams P, const float *__restrict__ depth, const uint8_t *__restrict__ rgb,
+                        float *__restrict__ pts, float *__restrict__ cols, uint8_t *__restrict__ valid) {
+    const int64_t n = static_cast<int64_t>(P.H) * P.W;
+    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float pt[3];
+    const bool ok = rgbd_point(P, depth, i, pt);
+    valid[i] = ok ? 1 : 0;
+    if (!ok) return;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        pts[3 * i + a] = pt[a];
+        cols[3 * i + a] = rgbd_color(rgb[3 * i + a]);
+    }
 }
 
 // Per-voxel passes: one 512-thread CTA per 512 pool voxels (cta_voxel); nb, the blocks in use, bounds the last CTA
@@ -457,6 +551,40 @@ int BlockGridCore::insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4
     return B2V_OK;
 }
 
+int BlockGridCore::reserve_sort(size_t cap) {
+    size_t tmp = 0;
+    B2V_CUDA(this, cub::DeviceRadixSort::SortPairs(nullptr, tmp, sort.vid[0].get(), sort.vid[1].get(), sort.ord[0].get(),
+                                                  sort.ord[1].get(), static_cast<int64_t>(cap), 0, 32, stream));
+    B2V_CUDA(this, sort.tmp.reserve(tmp));
+    for (int k = 0; k < 2; ++k) {   // ord[1] last: it holds cap only once every buffer does
+        B2V_CUDA(this, sort.vid[k].reserve(cap));
+        B2V_CUDA(this, sort.ord[k].reserve(cap));
+    }
+    return B2V_OK;
+}
+
+cudaError_t BlockGridCore::sort_voxels(const void *pts, bool pts_f64, const uint8_t *valid, int64_t n, uint32_t lo,
+                                       uint32_t hi) {
+    if (n <= 0) return cudaSuccess;
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+    dispatch([&](auto l) {
+        constexpr int L = decltype(l)::value;
+        if (pts_f64)
+            voxel_keys_kernel<double, L><<<grid, 256, 0, stream>>>(static_cast<const double *>(pts), valid, n,
+                                                                   inv_voxel_size, table, lo, hi, sort.vid[0].get(),
+                                                                   sort.ord[0].get());
+        else
+            voxel_keys_kernel<float, L><<<grid, 256, 0, stream>>>(static_cast<const float *>(pts), valid, n,
+                                                                  inv_voxel_size, table, lo, hi, sort.vid[0].get(),
+                                                                  sort.ord[0].get());
+    });
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    size_t tmp = sort.tmp.size();  // all 32 key bits: kBadVid (points without storage) must sort last
+    return cub::DeviceRadixSort::SortPairs(sort.tmp.get(), tmp, sort.vid[0].get(), sort.vid[1].get(), sort.ord[0].get(),
+                                           sort.ord[1].get(), n, 0, 32, stream);
+}
+
 int BlockGridCore::ensure_scan(uint32_t n) {
     // room for twice the CTAs, so a growing map rarely reallocates
     if (n > d_sums.size()) B2V_CUDA(this, d_sums.reserve(static_cast<size_t>(n) * 2));
@@ -707,6 +835,10 @@ struct b2v_grid : BlockGridCore {
     VmmRange pool;
     DeviceBuffer<float> d_pts, d_cols, d_out_pts, d_out_cols;   // staging of host points, read-out
     int64_t last_n = 0;
+    bool input_order = false;   // b2v_grid_set_input_order_sums
+    // point records and mask of an input-order integrate_rgbd; d_valid's size is their capacity
+    DeviceBuffer<float> d_rec_pts, d_rec_cols;
+    DeviceBuffer<uint8_t> d_valid;
 
     GridMeta meta() const { return GridMeta{reinterpret_cast<uint32_t *>(pool.va), index}; }
     size_t block_bytes() const { return static_cast<size_t>(kGridPlanes) * block_voxels() * sizeof(uint32_t); }
@@ -807,14 +939,78 @@ static cudaError_t grid_accumulate(const b2v_grid *g, const void *pts, bool pts_
     return grid_accumulate_t(g, static_cast<const float *>(pts), cols, cols_u8, n, lo, hi);
 }
 
+// an input-order call takes at most this many points: the sort's values are uint32 point indices (as the semantic
+// grids' b2v_sgrid_integrate)
+constexpr int64_t kMaxOrderedPoints = 0x7FFFFFF0LL;
+
+extern "C" int b2v_grid_set_input_order_sums(b2v_grid *g, int32_t enable) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (enable && g->index.capacity > BlockGridCore::max_blocks(g->log2_block)) {
+        g->err = "b2v_grid_set_input_order_sums: the grid holds more than 2^31 voxels";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    g->input_order = enable != 0;
+    return B2V_OK;
+}
+
+// Room for n points of an input-order pass: the voxel sort and, with `records`, the point records of integrate_rgbd.
+// Queued passes may still read these buffers, so a reallocation waits for the stream.
+static int grid_reserve_ordered(b2v_grid *g, size_t n, bool records) {
+    const bool sort_short = n > g->sort.ord[1].size(), rec_short = records && n > g->d_valid.size();
+    if (!sort_short && !rec_short) return B2V_OK;
+    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
+    const size_t cap = n + n / 4 + 1024;
+    if (rec_short) {
+        B2V_CUDA(g, g->d_rec_pts.reserve(cap * 3));
+        B2V_CUDA(g, g->d_rec_cols.reserve(cap * 3));
+        B2V_CUDA(g, g->d_valid.reserve(cap));
+    }
+    return sort_short ? g->reserve_sort(cap) : B2V_OK;
+}
+
+// the input-order pass over the points whose block's pool index lies in [lo, hi): keys -> sort -> runs
+template <typename Tp>
+static cudaError_t grid_sum_in_order_t(b2v_grid *g, const Tp *p, const void *cols, bool cols_u8,
+                                       const uint8_t *valid, int64_t n, uint32_t lo, uint32_t hi) {
+    cudaError_t e = g->sort_voxels(p, sizeof(Tp) == sizeof(double), valid, n, lo, hi);
+    if (e != cudaSuccess) return e;
+    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
+    const uint32_t *vid = g->sort.vid[1].get(), *ord = g->sort.ord[1].get();
+    g->dispatch([&](auto l) {
+        constexpr int L = decltype(l)::value;
+        if (cols_u8)
+            grid_runs_kernel<Tp, uint8_t, L><<<grid, 256, 0, g->stream>>>(vid, ord, n, p,
+                                                                          static_cast<const uint8_t *>(cols), g->meta());
+        else
+            grid_runs_kernel<Tp, float, L><<<grid, 256, 0, g->stream>>>(vid, ord, n, p,
+                                                                        static_cast<const float *>(cols), g->meta());
+    });
+    return cudaGetLastError();
+}
+
+static cudaError_t grid_sum_in_order(b2v_grid *g, const void *pts, bool pts_f64, const void *cols, bool cols_u8,
+                                     const uint8_t *valid, int64_t n, uint32_t lo, uint32_t hi) {
+    if (pts_f64)
+        return grid_sum_in_order_t(g, static_cast<const double *>(pts), cols, cols_u8, valid, n, lo, hi);
+    return grid_sum_in_order_t(g, static_cast<const float *>(pts), cols, cols_u8, valid, n, lo, hi);
+}
+
 static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const void *colors, bool u8, int64_t n_points) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     if (n_points < 0 || (n_points > 0 && !points)) {
         g->err = "b2v_grid_integrate: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
+    if (g->input_order && n_points > kMaxOrderedPoints) {
+        g->err = "b2v_grid_integrate: more than 0x7FFFFFF0 points in one call with input-order sums";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
     if (n_points == 0) return B2V_OK;  // voxel_block_grid.hpp:22-24,121-123
     B2V_CUDA(g, cudaSetDevice(g->device));
+    if (g->input_order) {
+        const int rc = grid_reserve_ordered(g, static_cast<size_t>(n_points), false);
+        if (rc != B2V_OK) return rc;
+    }
     const void *d_p = points;
     const void *d_c = colors;
     const bool dev_p = is_device_pointer(points);
@@ -837,7 +1033,13 @@ static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const v
     }
     B2V_CUDA(g, launch_point_insert(d_p, f64, nullptr, n_points, g->inv_voxel_size, g->log2_block, g->table, g->index,
                                     g->stream));
-    B2V_CUDA(g, grid_accumulate(g, d_p, f64, d_c, u8, n_points, 0u, g->index.pool_capacity));
+    // a voxel's run is its only update in a pass, so the growth replay over the new blocks is exact in either mode
+    const bool ordered = g->input_order;
+    auto pass = [&](uint32_t lo, uint32_t hi) {
+        return ordered ? grid_sum_in_order(g, d_p, f64, d_c, u8, nullptr, n_points, lo, hi)
+                       : grid_accumulate(g, d_p, f64, d_c, u8, n_points, lo, hi);
+    };
+    B2V_CUDA(g, pass(0u, g->index.pool_capacity));
     if (!g->growable) return B2V_OK;
     return g->resolve(
         [&](uint64_t blocks) {
@@ -845,7 +1047,7 @@ static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const v
             grid_map_storage(g, blocks, &map_err);
         },
         [&](uint32_t lo, uint32_t hi) {
-            B2V_CUDA(g, grid_accumulate(g, d_p, f64, d_c, u8, n_points, lo, hi));
+            B2V_CUDA(g, pass(lo, hi));
             return B2V_OK;
         });
 }
@@ -871,13 +1073,39 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
         g->err = "b2v_grid_integrate_rgbd: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
+    const int64_t n = static_cast<int64_t>(height) * width;
+    if (g->input_order && n > kMaxOrderedPoints) {
+        g->err = "b2v_grid_integrate_rgbd: more than 0x7FFFFFF0 pixels with input-order sums";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
     const float *d_depth = depth;
     const uint8_t *d_color = color;
     // voxel_grid.py:238-245: depth2pointcloud sees the filtered depth
-    const int rc = g->stage_input("b2v_grid_integrate_rgbd", height, width, filter_shadow_points != 0, &d_depth,
-                                  &d_color);
+    int rc = g->stage_input("b2v_grid_integrate_rgbd", height, width, filter_shadow_points != 0, &d_depth, &d_color);
     if (rc != B2V_OK) return rc;
     const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
+    if (g->input_order) {   // point records -> the input-order path of b2v_grid_integrate
+        rc = grid_reserve_ordered(g, static_cast<size_t>(n), true);
+        if (rc != B2V_OK) return rc;
+        const float *pts = g->d_rec_pts.get(), *cols = g->d_rec_cols.get();
+        const uint8_t *valid = g->d_valid.get();
+        grid_rgbd_points_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, g->stream>>>(
+            P, d_depth, d_color, g->d_rec_pts.get(), g->d_rec_cols.get(), g->d_valid.get());
+        B2V_CUDA(g, cudaGetLastError());
+        B2V_CUDA(g, launch_point_insert(pts, false, valid, n, g->inv_voxel_size, g->log2_block, g->table, g->index,
+                                        g->stream));
+        B2V_CUDA(g, grid_sum_in_order(g, pts, false, cols, false, valid, n, 0u, g->index.pool_capacity));
+        if (!g->growable) return B2V_OK;
+        return g->resolve(
+            [&](uint64_t blocks) {
+                std::string map_err;   // a failed mapping surfaces as "block pool full"
+                grid_map_storage(g, blocks, &map_err);
+            },
+            [&](uint32_t lo, uint32_t hi) {
+                B2V_CUDA(g, grid_sum_in_order(g, pts, false, cols, false, valid, n, lo, hi));
+                return B2V_OK;
+            });
+    }
     const unsigned grid = static_cast<unsigned>((static_cast<size_t>(height) * width + 255) / 256);
     auto accumulate = [&](uint32_t lo, uint32_t hi) {
         g->dispatch([&](auto l) {

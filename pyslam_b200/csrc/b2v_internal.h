@@ -386,6 +386,8 @@ struct BlockIndex {
 // [n][3].
 cudaError_t launch_point_insert(const void *pts, bool pts_f64, const uint8_t *valid, int64_t n, float inv_vs,
                                 int log2_block, const HashTable &table, const BlockIndex &index, cudaStream_t stream);
+// sort key of a point without storage in the pass's window: above every voxel id, so it sorts last
+constexpr uint32_t kBadVid = 0xFFFFFFFFu;
 
 // The block sides the grids accept: B = 1, 2, 8, 16 (L = 0, 1, 3, 4).  B = 4 keeps the rejection the grids gave every
 // size but 8 before block sizes were supported, which their argument checks pin (tests/test_gpu_grid.py,
@@ -493,6 +495,18 @@ struct BlockGridCore {
     // index is kNoBlock and the error flag says "block pool full").  Asynchronous.  A growable grid then maps storage
     // for the new pool count (resolve) before the grid's scatter kernel copies the voxels in.
     int insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys);
+    // Voxel-order sort of the input-order updates (the semantic grids, the point grid's input-order sums): per point
+    // the key pool index * B^3 + local index (kBadVid where the point is masked out by `valid` or its block has no
+    // pool index in [lo, hi)) and the point index, sorted stably over all 32 key bits into vid[1] / ord[1], so each
+    // voxel's points form one run in input order.  vid[0] / ord[0] and tmp are the sort's scratch.
+    struct VoxelSort {
+        DeviceBuffer<uint32_t> vid[2], ord[2];
+        DeviceBuffer<uint8_t> tmp;
+    } sort;
+    // room for `cap` points in `sort`; a short buffer is reallocated, so the caller synchronises first
+    int reserve_sort(size_t cap);
+    // keys -> sort of n float or double [n][3] points (asynchronous; needs reserve_sort(>= n))
+    cudaError_t sort_voxels(const void *pts, bool pts_f64, const uint8_t *valid, int64_t n, uint32_t lo, uint32_t hi);
     // room for n per-CTA counts in d_sums / offsets in d_offs (the CTAs of a per-voxel pass, voxel_ctas)
     int ensure_scan(uint32_t n);
     // exclusive scan of the per-CTA counts d_sums -> d_offs, and their total (synchronises)

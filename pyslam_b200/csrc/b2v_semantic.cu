@@ -46,7 +46,6 @@
 namespace b2v {
 
 constexpr int kSemLabels = B2V_SEM_MAX_LABELS;
-constexpr uint32_t kBadVid = 0xFFFFFFFFu;
 constexpr float kBaseLogProb = 0.10536051565782628f;  // voxel_data_semantic.h:287, -log(0.9)
 constexpr int kSemArrays = 11;   // per-voxel arrays of a Bayesian grid (a voting grid has the first 6)
 
@@ -138,31 +137,10 @@ template <bool kChain> __device__ __forceinline__ void sem_release_labels(const 
     }
 }
 
-// ---- 2. sort keys --------------------------------------------------------------------------------------------
+// ---- 2. sort keys: BlockGridCore::sort_voxels (b2v_grid.cu) ------------------------------------------------
 // Only points whose block has a pool index in [lo, hi) get a key; the others get kBadVid, sort last and are left out
 // by the runs.  The first pass of a call covers the blocks with storage, [0, pool_capacity); after a growth the
 // keys -> sort -> runs passes are replayed over the blocks that just got storage.
-template <typename T, int L>
-__global__ void __launch_bounds__(256)
-sem_keys_kernel(const T *__restrict__ pts, const uint8_t *__restrict__ valid, const int64_t n, const float inv_vs,
-                const HashTable H, const SemGrid G, const uint32_t lo, const uint32_t hi, uint32_t *__restrict__ vid,
-                uint32_t *__restrict__ order) {
-    const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int vx = point_voxel_coord(pts[3 * i + 0], inv_vs), vy = point_voxel_coord(pts[3 * i + 1], inv_vs),
-              vz = point_voxel_coord(pts[3 * i + 2], inv_vs);
-    uint32_t key = kBadVid;
-    const uint32_t slot = (valid == nullptr || valid[i])
-                              ? table_find(H, grid_block_coord<L>(vx), grid_block_coord<L>(vy), grid_block_coord<L>(vz))
-                              : kEmpty;
-    if (slot != kEmpty) {
-        const uint32_t idx = H.entries[slot].w;
-        if (idx >= lo && idx < hi)   // kNoBlock is past every window
-            key = idx * GridBlock<L>::kVox + static_cast<uint32_t>(grid_local_index<L>(vx, vy, vz));
-    }
-    vid[i] = key;
-    order[i] = static_cast<uint32_t>(i);
-}
 
 // ---- fused front-end: depth2pointcloud + world transform of one labelled RGBD frame ------------------------
 // (pyslam/utilities/depth.py:45-85; pyslam/dense/volumetric_integrator_voxel_semantic_grid.py:392-453).  One
@@ -868,8 +846,6 @@ struct b2v_sgrid : BlockGridCore {
     DeviceBuffer<double> d_pts;
     DeviceBuffer<float> d_cols, d_depths;
     DeviceBuffer<int32_t> d_cls, d_inst;
-    DeviceBuffer<uint32_t> d_vid[2], d_ord[2];
-    DeviceBuffer<uint8_t> d_sort_tmp;
     DeviceBuffer<uint8_t> d_valid;   // per-point mask of the fused RGBD front-end; its size is the staging capacity
     // instance -> object association: votes (records -> sort -> runs -> triples), then resolve
     DeviceBuffer<int32_t> d_pend;                  // [voxels] instance id of a pending voxel, else -1
@@ -1140,14 +1116,8 @@ static int sgrid_ensure_stage(b2v_sgrid *g, size_t n) {
     B2V_CUDA(g, g->d_cls.reserve(cap));
     B2V_CUDA(g, g->d_inst.reserve(cap));
     B2V_CUDA(g, g->d_depths.reserve(cap));
-    for (int k = 0; k < 2; ++k) {
-        B2V_CUDA(g, g->d_vid[k].reserve(cap));
-        B2V_CUDA(g, g->d_ord[k].reserve(cap));
-    }
-    size_t tmp = 0;
-    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(nullptr, tmp, g->d_vid[0].get(), g->d_vid[1].get(), g->d_ord[0].get(),
-                                               g->d_ord[1].get(), static_cast<int64_t>(cap), 0, 32, g->stream));
-    B2V_CUDA(g, g->d_sort_tmp.reserve(tmp));
+    const int rc = g->reserve_sort(cap);
+    if (rc != B2V_OK) return rc;
     B2V_CUDA(g, g->d_valid.reserve(cap));
     return B2V_OK;
 }
@@ -1197,8 +1167,8 @@ static int sgrid_runs_chain(b2v_sgrid *g, int64_t n, const SemInputs &in) {
         B2V_CUDA(g, cudaStreamSynchronize(s));
         B2V_CUDA(g, g->d_lab_list.reserve(static_cast<size_t>(n) + n / 4 + 1024));
     }
-    sem_runs_kernel<true><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(),
-                                                                                n, in, g->dev(), g->labels());
+    sem_runs_kernel<true><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(
+        g->sort.vid[1].get(), g->sort.ord[1].get(), n, in, g->dev(), g->labels());
     B2V_CUDA(g, cudaGetLastError());
     uint32_t listed = 0;
     uint64_t wanted = 0;
@@ -1216,8 +1186,8 @@ static int sgrid_runs_chain(b2v_sgrid *g, int64_t n, const SemInputs &in) {
     S.replay = g->d_lab_list.get();
     S.n_replay = listed;
     S.no_growth = 1;
-    sem_runs_kernel<true><<<(listed + 127) / 128, 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(), n, in, g->dev(),
-                                                              S);
+    sem_runs_kernel<true><<<(listed + 127) / 128, 128, 0, s>>>(g->sort.vid[1].get(), g->sort.ord[1].get(), n, in,
+                                                              g->dev(), S);
     B2V_CUDA(g, cudaGetLastError());
     return sgrid_label_settle(g, &listed, &wanted);
 }
@@ -1225,25 +1195,10 @@ static int sgrid_runs_chain(b2v_sgrid *g, int64_t n, const SemInputs &in) {
 // keys -> sort -> runs over the staged point records, for the points whose block's pool index lies in [lo, hi)
 static int sgrid_apply(b2v_sgrid *g, int64_t n, const SemInputs &in, const uint8_t *valid, uint32_t lo, uint32_t hi) {
     cudaStream_t s = g->stream;
-    const unsigned grid = static_cast<unsigned>((n + 255) / 256);
-    g->dispatch([&](auto l) {
-        constexpr int L = decltype(l)::value;
-        if (in.pts_f64)
-            sem_keys_kernel<double, L><<<grid, 256, 0, s>>>(static_cast<const double *>(in.pts), valid, n,
-                                                            g->inv_voxel_size, g->table, g->dev(), lo, hi,
-                                                            g->d_vid[0].get(), g->d_ord[0].get());
-        else
-            sem_keys_kernel<float, L><<<grid, 256, 0, s>>>(static_cast<const float *>(in.pts), valid, n,
-                                                           g->inv_voxel_size, g->table, g->dev(), lo, hi,
-                                                           g->d_vid[0].get(), g->d_ord[0].get());
-    });
-    B2V_CUDA(g, cudaGetLastError());
-    size_t tmp = g->d_sort_tmp.size();  // all 32 key bits: kBadVid (points without storage) must sort last
-    B2V_CUDA(g, cub::DeviceRadixSort::SortPairs(g->d_sort_tmp.get(), tmp, g->d_vid[0].get(), g->d_vid[1].get(),
-                                               g->d_ord[0].get(), g->d_ord[1].get(), n, 0, 32, s));
+    B2V_CUDA(g, g->sort_voxels(in.pts, in.pts_f64 != 0, valid, n, lo, hi));
     if (g->lab_max_chunks) return sgrid_runs_chain(g, n, in);
-    sem_runs_kernel<false><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(g->d_vid[1].get(), g->d_ord[1].get(),
-                                                                                 n, in, g->dev(), LabelStore{});
+    sem_runs_kernel<false><<<static_cast<unsigned>((n + 127) / 128), 128, 0, s>>>(
+        g->sort.vid[1].get(), g->sort.ord[1].get(), n, in, g->dev(), LabelStore{});
     B2V_CUDA(g, cudaGetLastError());
     return B2V_OK;
 }

@@ -65,6 +65,10 @@ DEFAULT_PARAMETERS = {
     # the 8 a voxel holds itself; below it no voxel evicts a pair and the labels equal the reference's unbounded map.
     # 0 = no store (a ninth pair evicts the weakest); the voting grid has no label set and ignores it
     "kVolumetricIntegrationB200LabelOverflowPairs": 0,
+    # voxel-grid plugin: each voxel sums its points in input order (VoxelBlockGrid(input_order_sums=True)), so the
+    # map equals the reference's sequential build bit for bit and is the same on every run; the semantic grids always
+    # sum in input order and do not read it
+    "kVolumetricIntegrationB200InputOrderSums": False,
     "kVolumetricIntegrationB200Device": 0,
     "kVolumetricIntegrationB200GenerateObjects": True,   # kGenerateObjectsDefault (reference :84)
     # raw keyframe images to the grid (set_frame): upload once, undistort + BGR->RGB + depth widening + shadow filter
@@ -338,7 +342,8 @@ def make_voxel_grid_integrator_class(Base, api):
         _defaults = dict(DEFAULT_PARAMETERS, kVolumetricIntegrationB200CapacityBlocks=1 << 17)
 
         def _make_grid(self, p, side, constructor_kwargs):
-            return VoxelBlockGrid(**_grid_args(p, self.b200_set_parameters))
+            return VoxelBlockGrid(**_grid_args(p, self.b200_set_parameters),
+                                  input_order_sums=bool(p["kVolumetricIntegrationB200InputOrderSums"]))
 
         def _integrate_raw_keyframe(self, kd, depth, scale):
             """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""

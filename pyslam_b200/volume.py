@@ -974,12 +974,31 @@ class VoxelBlockGrid(_BlockGrid):
     _P = "b2v_grid_"
 
     def __init__(self, voxel_size: float, block_size: int = 8, capacity_blocks: int = 1 << 17,
-                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1):
+                 device: int = 0, max_capacity_blocks: int | None = None, shard_rank: int = 0, shard_count: int = 1,
+                 input_order_sums: bool = False):
         """`max_capacity_blocks`: growth ceiling of the block pool.  Above `capacity_blocks`, the pool starts with
         `capacity_blocks` blocks of storage and grows inside the integrate call that needs more; the grid then holds
         what a grid created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the
-        pool fixed.  `shard_rank` / `shard_count`: see `set_shard`."""
+        pool fixed.  `shard_rank` / `shard_count`: see `set_shard`.
+
+        `input_order_sums`: each voxel adds its points in input order with IEEE float32 adds instead of float atomics,
+        so the position and colour sums equal the sequential reference's bit for bit and are the same on every run, in
+        every shard layout and after every growth.  Off (the default), the sums equal the reference's up to the order
+        of the atomic adds, which no two runs share; keys, hashes and counts are the same either way.  A call in this
+        mode takes at most 0x7FFFFFF0 points.  Saved map states load into a grid of either mode."""
         super().__init__(voxel_size, block_size, capacity_blocks, device, max_capacity_blocks, shard_rank, shard_count)
+        self._input_order_sums = bool(input_order_sums)
+        if self._input_order_sums:
+            rc = self._L.b2v_grid_set_input_order_sums(self._h, 1)
+            if rc != _lib.B2V_OK:
+                msg = self._L.b2v_grid_last_error(self._h).decode()
+                self.close()
+                raise RuntimeError(f"input_order_sums: {msg} (status {rc})")
+
+    @property
+    def input_order_sums(self) -> bool:
+        """True when each voxel sums its points in input order (see the constructor)."""
+        return self._input_order_sums
 
     def _stage_frame(self, images, labels, shape, filter_shadow_points, out):
         if labels[0] is not None or labels[1] is not None:
