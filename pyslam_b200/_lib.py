@@ -29,13 +29,13 @@ EXPORTED_SYMBOLS = [
     "b2v_create", "b2v_destroy", "b2v_reset", "b2v_last_error", "b2v_integrate",
     "b2v_integrate_batch", "b2v_integrate_u16", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_capacity",
     "b2v_num_blocks", "b2v_last_frame_stats", "b2v_last_mesh_stats",
-    "b2v_counters", "b2v_set_overlap", "b2v_set_fusion", "b2v_set_group_size", "b2v_set_input_event", "b2v_set_rectification", "b2v_remap", "b2v_profile_enable", "b2v_profile_read", "b2v_dump_blocks", "b2v_upload_blocks", "b2v_export_blocks_device", "b2v_import_blocks_device", "b2v_last_touched_keys", "b2v_extract_mesh", "b2v_copy_mesh",
+    "b2v_counters", "b2v_set_overlap", "b2v_set_fusion", "b2v_set_group_size", "b2v_set_input_event", "b2v_set_rectification", "b2v_remap", "b2v_profile_enable", "b2v_profile_read", "b2v_export_blocks", "b2v_upload_blocks", "b2v_last_touched_keys", "b2v_block_key_hashes", "b2v_extract_mesh", "b2v_copy_mesh",
     "b2v_extract_points", "b2v_copy_points", "b2v_export_halo_device", "b2v_extract_mesh_with_halo",
     "b2v_extract_points_with_halo", "b2v_weld_mesh_device", "b2v_weld_last_error", "b2v_grid_create", "b2v_grid_create_ex", "b2v_grid_capacity",
     "b2v_grid_destroy", "b2v_grid_clear",
     "b2v_grid_last_error", "b2v_grid_integrate", "b2v_grid_integrate_f64", "b2v_grid_integrate_ex", "b2v_grid_integrate_rgbd", "b2v_filter_shadow_points", "b2v_grid_synchronize", "b2v_grid_num_blocks",
     "b2v_grid_size", "b2v_grid_get_voxels", "b2v_grid_copy_voxels",
-    "b2v_grid_remove_low_count_voxels", "b2v_grid_dump_blocks", "b2v_grid_carve",
+    "b2v_grid_remove_low_count_voxels", "b2v_grid_export_blocks", "b2v_grid_carve",
     "b2v_grid_get_voxels_in_frustum", "b2v_grid_get_voxels_in_bb", "b2v_version", "b2v_device_sm_count", "b2v_selftest_division",
     "b2v_sgrid_create", "b2v_sgrid_create_ex", "b2v_sgrid_capacity", "b2v_sgrid_destroy", "b2v_sgrid_last_error", "b2v_sgrid_clear",
     "b2v_sgrid_set_depth_threshold", "b2v_sgrid_set_depth_decay_rate", "b2v_sgrid_integrate",
@@ -43,7 +43,7 @@ EXPORTED_SYMBOLS = [
     "b2v_sgrid_num_blocks", "b2v_sgrid_get_voxels", "b2v_sgrid_copy_voxels", "b2v_sgrid_get_voxels_in_bb",
     "b2v_sgrid_get_voxels_in_frustum",
     "b2v_sgrid_remove_low_count_voxels", "b2v_sgrid_remove_low_confidence_segments", "b2v_sgrid_merge_segments",
-    "b2v_sgrid_remove_segment", "b2v_sgrid_label_overflows", "b2v_sgrid_dump_blocks", "b2v_sgrid_carve",
+    "b2v_sgrid_remove_segment", "b2v_sgrid_label_overflows", "b2v_sgrid_carve",
     "b2v_sgrid_assign_object_ids_to_instance_ids", "b2v_sgrid_copy_instance_map", "b2v_sgrid_set_next_object_id",
     "b2v_sgrid_get_next_object_id", "b2v_grid_set_rectification", "b2v_grid_set_frame", "b2v_sgrid_set_rectification",
     "b2v_sgrid_set_frame", "b2v_sgrid_remap_instance_ids", "b2v_grid_set_shard", "b2v_sgrid_set_shard",
@@ -190,16 +190,10 @@ def load() -> C.CDLL:
     L.b2v_sgrid_export_labels.argtypes = [vp] * 5
     L.b2v_sgrid_upload_labels.restype = C.c_int
     L.b2v_sgrid_upload_labels.argtypes = [vp, i64] + [vp] * 5
-    L.b2v_sgrid_dump_blocks.restype = C.c_int64
-    L.b2v_sgrid_dump_blocks.argtypes = [vp] * 10 + [i32] + [vp] * 3
     L.b2v_integrate_u16.restype = C.c_int
     L.b2v_integrate_u16.argtypes = [vp, vp, C.c_float, vp, i32, i32, vp, vp, vp]
     L.b2v_integrate_batch_u16.restype = C.c_int
     L.b2v_integrate_batch_u16.argtypes = [vp, i32, vp, C.c_float, vp, i32, i32, vp, vp, vp]
-    L.b2v_export_blocks_device.restype = C.c_int64
-    L.b2v_export_blocks_device.argtypes = [vp, vp, vp, C.c_int64]
-    L.b2v_import_blocks_device.restype = C.c_int
-    L.b2v_import_blocks_device.argtypes = [vp, C.c_int64, vp, vp]
     L.b2v_set_rectification.restype = C.c_int
     L.b2v_set_rectification.argtypes = [vp, vp, vp, i32, i32, i32]
     L.b2v_remap.restype = C.c_int
@@ -210,12 +204,14 @@ def load() -> C.CDLL:
     L.b2v_set_input_event.argtypes = [vp, vp]
     L.b2v_set_group_size.restype = C.c_int
     L.b2v_set_group_size.argtypes = [vp, i32]
-    L.b2v_dump_blocks.restype = i64
-    L.b2v_dump_blocks.argtypes = [vp, vp, vp, vp]
+    L.b2v_export_blocks.restype = i64
+    L.b2v_export_blocks.argtypes = [vp, vp, vp, i64]
     L.b2v_upload_blocks.restype = C.c_int
     L.b2v_upload_blocks.argtypes = [vp, i64, vp, vp]
     L.b2v_last_touched_keys.restype = i64
     L.b2v_last_touched_keys.argtypes = [vp, vp, i64]
+    L.b2v_block_key_hashes.restype = C.c_int
+    L.b2v_block_key_hashes.argtypes = [vp, i64, vp]
     L.b2v_extract_mesh.restype = C.c_int
     L.b2v_extract_mesh.argtypes = [vp, p_i64, p_i64]
     L.b2v_copy_mesh.restype = C.c_int
@@ -277,10 +273,10 @@ def load() -> C.CDLL:
     L.b2v_grid_get_voxels_in_frustum.argtypes = [vp, vp, i32, i32, vp, C.c_float, C.c_float, i32]
     L.b2v_grid_get_voxels_in_bb.restype = i64
     L.b2v_grid_get_voxels_in_bb.argtypes = [vp, vp, i32]
-    L.b2v_grid_dump_blocks.restype = i64
-    L.b2v_grid_dump_blocks.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.b2v_grid_export_blocks.restype = i64
+    L.b2v_grid_export_blocks.argtypes = [vp, vp, vp]
     L.b2v_grid_upload_blocks.restype = C.c_int
-    L.b2v_grid_upload_blocks.argtypes = [vp, i64, vp, vp, vp, vp]
+    L.b2v_grid_upload_blocks.argtypes = [vp, i64, vp, vp]
     L.b2v_sgrid_export_blocks.restype = i64
     L.b2v_sgrid_export_blocks.argtypes = [vp] * 13
     L.b2v_sgrid_upload_blocks.restype = C.c_int

@@ -329,7 +329,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 109; }
+extern "C" int b2v_version(void) { return 110; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -1069,34 +1069,26 @@ extern "C" int b2v_counters(b2v_volume *v, int64_t *block_updates, int64_t *kern
     return rc;
 }
 
-extern "C" int64_t b2v_dump_blocks(b2v_volume *v, int32_t *keys, uint64_t *hashes, float *voxels) {
+// The blocks cross the ABI in the pool's own layout: keys int4 {x, y, z, 0}, voxels [nb][5][512].
+extern "C" int64_t b2v_export_blocks(b2v_volume *v, int32_t *keys4, float *voxels, int64_t max_blocks) {
     if (!v) return -1;
     if (read_counters(v) == B2V_ERR_CUDA) return -1;
     const uint32_t nb = block_count(v);
+    if (!keys4 && !voxels) return nb;
+    if (static_cast<int64_t>(nb) > max_blocks) {
+        v->err = "b2v_export_blocks: destination too small";
+        return -1;
+    }
     if (nb == 0) return 0;
-    if (keys) {
-        std::vector<int4> tmp(nb);
-        if (cudaMemcpy(tmp.data(), v->meta.block_keys, nb * sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
-            return -1;
-        for (uint32_t i = 0; i < nb; ++i) {
-            keys[3 * i + 0] = tmp[i].x;
-            keys[3 * i + 1] = tmp[i].y;
-            keys[3 * i + 2] = tmp[i].z;
-        }
-    }
-    if (hashes) {
-        DeviceBuffer<uint64_t> d_h;
-        if (d_h.reserve(nb) != cudaSuccess) return -1;
-        cudaError_t e = launch_block_hashes(v->meta.block_keys, d_h.get(), nb, v->compute);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-        if (e == cudaSuccess) e = cudaMemcpy(hashes, d_h.get(), nb * sizeof(uint64_t), cudaMemcpyDeviceToHost);
-        v->launches += 1;
-        if (e != cudaSuccess) return -1;
-    }
-    if (voxels) {
-        if (cudaMemcpy(voxels, v->meta.pool, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
-                       cudaMemcpyDeviceToHost) != cudaSuccess)
-            return -1;
+    cudaError_t e = cudaSuccess;
+    if (keys4) e = cudaMemcpyAsync(keys4, v->meta.block_keys, nb * sizeof(int4), cudaMemcpyDefault, v->compute);
+    if (e == cudaSuccess && voxels)
+        e = cudaMemcpyAsync(voxels, v->meta.pool, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
+                            cudaMemcpyDefault, v->compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
+    if (e != cudaSuccess) {
+        v->err = std::string("b2v_export_blocks: ") + cudaGetErrorString(e);
+        return -1;
     }
     return nb;
 }
@@ -1109,9 +1101,9 @@ static int grow_for_blocks(b2v_volume *v, int64_t n_blocks) {
     return pool_grow(v, static_cast<uint64_t>(v->h_counters[kCtrPool]) + static_cast<uint64_t>(n_blocks));
 }
 
-extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t *keys, const float *voxels) {
+extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t *keys4, const float *voxels) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    if (n_blocks < 0 || (n_blocks > 0 && (!keys || !voxels))) {
+    if (n_blocks < 0 || (n_blocks > 0 && (!keys4 || !voxels))) {
         v->err = "b2v_upload_blocks: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
@@ -1122,21 +1114,27 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
         if (rc == B2V_ERR_CUDA) return rc;
     }
     const size_t n = static_cast<size_t>(n_blocks);
-    std::vector<int4> k4(n);
-    for (size_t i = 0; i < n; ++i) k4[i] = make_int4(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2], 0);
-    DeviceBuffer<int4> d_k;
-    DeviceBuffer<float> d_v;
+    // device arrays are read in place; host ones are staged on the compute stream
+    const int4 *d_keys = reinterpret_cast<const int4 *>(keys4);
+    const float *d_vox = voxels;
+    DeviceBuffer<int4> k_stage;
+    DeviceBuffer<float> v_stage;
     DeviceBuffer<uint32_t> d_i;
-    cudaError_t e = d_k.reserve(n);
-    if (e == cudaSuccess) e = d_v.reserve(n * kBlockFloats);
-    if (e == cudaSuccess) e = d_i.reserve(n);
+    cudaError_t e = d_i.reserve(n);
+    if (e == cudaSuccess && !is_device_pointer(keys4)) {
+        e = k_stage.reserve(n);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(k_stage.get(), keys4, n * sizeof(int4), cudaMemcpyHostToDevice, v->compute);
+        d_keys = k_stage.get();
+    }
+    if (e == cudaSuccess && !is_device_pointer(voxels)) {
+        e = v_stage.reserve(n * kBlockFloats);
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(v_stage.get(), voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice,
+                                v->compute);
+        d_vox = v_stage.get();
+    }
     if (e == cudaSuccess)
-        e = cudaMemcpyAsync(d_k.get(), k4.data(), n * sizeof(int4), cudaMemcpyHostToDevice, v->compute);
-    if (e == cudaSuccess)
-        e = cudaMemcpyAsync(d_v.get(), voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice, v->compute);
-    if (e == cudaSuccess)
-        e = launch_upload_blocks(d_k.get(), d_v.get(), static_cast<uint32_t>(n), d_i.get(), v->table, v->meta,
-                                 v->compute);
+        e = launch_upload_blocks(d_keys, d_vox, static_cast<uint32_t>(n), d_i.get(), v->table, v->meta, v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
     v->launches += 2;
     if (e != cudaSuccess) {
@@ -1146,81 +1144,31 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
     return read_counters(v);
 }
 
-// Device-to-device block exchange (multi-GPU mesh gather, SURVEY.md 8e): keys as int32 x 4 {x, y, z, 0}
-extern "C" int64_t b2v_export_blocks_device(b2v_volume *v, int32_t *d_keys4, float *d_voxels, int64_t max_blocks) {
-    if (!v) return -1;
-    if (read_counters(v) == B2V_ERR_CUDA) return -1;
-    const uint32_t nb = block_count(v);
-    if (!d_keys4 && !d_voxels) return nb;
-    if (static_cast<int64_t>(nb) > max_blocks) {
-        v->err = "b2v_export_blocks_device: destination too small";
-        return -1;
-    }
-    if (nb == 0) return 0;
-    cudaError_t e = cudaSuccess;
-    if (d_keys4) e = cudaMemcpyAsync(d_keys4, v->meta.block_keys, nb * sizeof(int4), cudaMemcpyDeviceToDevice, v->compute);
-    if (e == cudaSuccess && d_voxels)
-        e = cudaMemcpyAsync(d_voxels, v->meta.pool, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
-                            cudaMemcpyDeviceToDevice, v->compute);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    if (e != cudaSuccess) {
-        v->err = std::string("b2v_export_blocks_device: ") + cudaGetErrorString(e);
-        return -1;
-    }
-    return nb;
-}
-
-extern "C" int b2v_import_blocks_device(b2v_volume *v, int64_t n_blocks, const int32_t *d_keys4, const float *d_voxels) {
-    if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    if (n_blocks < 0 || (n_blocks > 0 && (!d_keys4 || !d_voxels))) {
-        v->err = "b2v_import_blocks_device: bad arguments";
-        return B2V_ERR_INVALID_ARGUMENT;
-    }
-    if (n_blocks == 0) return B2V_OK;
-    B2V_CUDA(v, cudaSetDevice(v->cfg.device));
-    {
-        const int rc = grow_for_blocks(v, n_blocks);
-        if (rc == B2V_ERR_CUDA) return rc;
-    }
-    DeviceBuffer<uint32_t> d_i;
-    cudaError_t e = d_i.reserve(static_cast<size_t>(n_blocks));
-    if (e == cudaSuccess)
-        e = launch_upload_blocks(reinterpret_cast<const int4 *>(d_keys4), d_voxels, static_cast<uint32_t>(n_blocks),
-                                 d_i.get(), v->table, v->meta, v->compute);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    v->launches += 2;
-    if (e != cudaSuccess) {
-        v->err = std::string("b2v_import_blocks_device: ") + cudaGetErrorString(e);
-        return B2V_ERR_CUDA;
-    }
-    return read_counters(v);
-}
-
-extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys, int64_t max_keys) {
+extern "C" int64_t b2v_last_touched_keys(b2v_volume *v, int32_t *keys4, int64_t max_keys) {
     if (!v) return -1;
     if (read_counters(v) == B2V_ERR_CUDA) return -1;
     if (v->group_id == 0) return 0;
     const int buf = static_cast<int>((v->group_id - 1) % kGroupBufs);  // the most recent group's touched blocks
     uint32_t n = v->h_counters[group_ctr(buf, kGcUnion)];
     if (n > v->meta.capacity) n = v->meta.capacity;
-    if (!keys) return n;
+    if (!keys4) return n;
     if (static_cast<int64_t>(n) > max_keys) n = static_cast<uint32_t>(max_keys);
     if (n == 0) return 0;
     DeviceBuffer<int4> d_k;
     if (d_k.reserve(n) != cudaSuccess) return -1;
-    std::vector<int4> tmp(n);
     const uint32_t *list = v->meta.union_slots + static_cast<size_t>(buf) * v->meta.capacity;
     cudaError_t e = launch_gather_active_keys(v->table, list, n, d_k.get(), v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
-    if (e == cudaSuccess) e = cudaMemcpy(tmp.data(), d_k.get(), n * sizeof(int4), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(keys4, d_k.get(), n * sizeof(int4), cudaMemcpyDeviceToHost);
     v->launches += 1;
     if (e != cudaSuccess) return -1;
-    for (uint32_t i = 0; i < n; ++i) {
-        keys[3 * i + 0] = tmp[i].x;
-        keys[3 * i + 1] = tmp[i].y;
-        keys[3 * i + 2] = tmp[i].z;
-    }
     return n;
+}
+
+extern "C" int b2v_block_key_hashes(const int32_t *keys4, int64_t n, uint64_t *hashes) {
+    if (n < 0 || (n > 0 && (!keys4 || !hashes))) return B2V_ERR_INVALID_ARGUMENT;
+    for (int64_t i = 0; i < n; ++i) hashes[i] = block_key_hash(keys4[4 * i], keys4[4 * i + 1], keys4[4 * i + 2]);
+    return B2V_OK;
 }
 
 // ---- mesh / point cloud ---------------------------------------------------------------------

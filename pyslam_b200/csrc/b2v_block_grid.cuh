@@ -92,43 +92,4 @@ __device__ __forceinline__ bool region_contains(const GridQuery &Q, const double
     return frustum_contains(Q, p, ip);
 }
 
-// ---- block upload (b2v_grid_upload_blocks, b2v_sgrid_upload_blocks) -------------------------------------------
-// Pool index of the uploaded block `key` that this CTA scatters, for every thread of the CTA: kNoBlock when the block
-// has no table entry (another shard owns it) or no storage (the pool is full).  The keys went through
-// block_import_kernel in an earlier launch, so the table holds their final entries.
-__device__ __forceinline__ uint32_t uploaded_block_index(const HashTable &T, const int4 key, const uint32_t pool_capacity) {
-    __shared__ uint32_t s_idx;
-    if (threadIdx.x == 0) {
-        const uint32_t slot = table_find(T, key.x, key.y, key.z);
-        const uint32_t idx = slot == kEmpty ? kNoBlock : T.entries[slot].w;
-        s_idx = idx < pool_capacity ? idx : kNoBlock;
-    }
-    __syncthreads();
-    return s_idx;
-}
-
-// The same for uploaded block b (of n) and voxel t of the voxel-range CTA mapping (cta_voxel): B >= 8, the CTA lies in
-// one block and thread 0 finds it; B < 8, the CTA spans 512 / B^3 blocks and the thread of each block's voxel 0 finds
-// that block (kNoBlock past the n uploaded blocks).
-template <int L>
-__device__ __forceinline__ uint32_t uploaded_voxel_block(const HashTable &T, const int4 *keys, const uint32_t b,
-                                                         const int t, const uint32_t n, const uint32_t pool_capacity) {
-    if constexpr (3 * L >= 9) {
-        return uploaded_block_index(T, keys[b], pool_capacity);
-    } else {
-        __shared__ uint32_t s_idx[512 >> (3 * L)];
-        if (t == 0) {
-            uint32_t idx = kNoBlock;
-            if (b < n) {
-                const int4 key = keys[b];
-                const uint32_t slot = table_find(T, key.x, key.y, key.z);
-                idx = slot == kEmpty ? kNoBlock : T.entries[slot].w;
-            }
-            s_idx[threadIdx.x >> (3 * L)] = idx < pool_capacity ? idx : kNoBlock;
-        }
-        __syncthreads();
-        return s_idx[threadIdx.x >> (3 * L)];
-    }
-}
-
 }  // namespace b2v

@@ -402,27 +402,28 @@ grid_carve_kernel(const GridMeta G, const GridQuery Q, const float *__restrict__
     }
 }
 
-// block upload: one CTA per 512 uploaded voxels (cta_voxel over the n uploaded blocks) copies them, in the layout of
-// b2v_grid_dump_blocks (count [B^3], pos_sum / col_sum [B^3][3]), into the planes of their pool blocks, replacing
-// what the blocks held
-template <int L>
-__global__ void __launch_bounds__(kVox)
-grid_scatter_kernel(const int4 *__restrict__ keys, const int32_t *__restrict__ count, const float *__restrict__ pos,
-                    const float *__restrict__ col, const HashTable T, const GridMeta G, const uint32_t n) {
-    constexpr int kV = GridBlock<L>::kVox;
-    uint32_t b;
-    int t;
-    cta_voxel<L>(&b, &t);
-    const uint32_t idx = uploaded_voxel_block<L>(T, keys, b, t, n, G.index.pool_capacity);
+// block upload (BlockGridCore::scatter_blocks): one CTA per uploaded block copies every array's run of the block, one
+// word W per thread and step, over its pool block's run.  W = uint4 where every run is a multiple of 16 bytes, else
+// uint32_t.  A block without a table entry (another shard owns it) or storage (the pool is full) is skipped.  The keys
+// went through block_import_kernel in an earlier launch, so the table holds their final entries.
+template <typename W>
+__global__ void __launch_bounds__(256)
+block_scatter_kernel(const int4 *__restrict__ keys, const BlockArrays A, const HashTable T, const uint32_t pool_capacity) {
+    __shared__ uint32_t s_idx;
+    if (threadIdx.x == 0) {
+        const int4 key = keys[blockIdx.x];
+        const uint32_t slot = table_find(T, key.x, key.y, key.z);
+        const uint32_t idx = slot == kEmpty ? kNoBlock : T.entries[slot].w;
+        s_idx = idx < pool_capacity ? idx : kNoBlock;
+    }
+    __syncthreads();
+    const uint32_t idx = s_idx;
     if (idx == kNoBlock) return;
-    const size_t v = static_cast<size_t>(b) * kV + t;
-    uint32_t *blk = G.pool + static_cast<size_t>(idx) * kGridBlockWords<L>;
-    float *fb = reinterpret_cast<float *>(blk);
-    reinterpret_cast<int32_t *>(blk)[t] = count[v];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        fb[(1 + c) * kV + t] = pos[3 * v + c];
-        fb[(4 + c) * kV + t] = col[3 * v + c];
+    for (int k = 0; k < A.n_arrays; ++k) {
+        const uint32_t words = A.block_bytes[k] / static_cast<uint32_t>(sizeof(W));
+        const W *src = static_cast<const W *>(A.src[k]) + static_cast<size_t>(blockIdx.x) * words;
+        W *dst = static_cast<W *>(A.dst[k]) + static_cast<size_t>(idx) * words;
+        for (uint32_t w = threadIdx.x; w < words; w += blockDim.x) dst[w] = src[w];
     }
 }
 
@@ -539,15 +540,41 @@ int BlockGridCore::clear_index() {
     return B2V_OK;
 }
 
-int BlockGridCore::insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys) {
-    std::vector<int4> k4(static_cast<size_t>(n));
-    for (size_t i = 0; i < k4.size(); ++i) k4[i] = make_int4(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2], 0);
-    B2V_CUDA(this, d_keys->reserve(k4.size()));
-    // a pageable source is staged before the call returns, so k4 may go
-    B2V_CUDA(this, cudaMemcpyAsync(d_keys->get(), k4.data(), k4.size() * sizeof(int4), cudaMemcpyHostToDevice, stream));
+int BlockGridCore::insert_keys(int64_t n, const int32_t *keys4, DeviceBuffer<int4> *d_keys) {
+    B2V_CUDA(this, d_keys->reserve(static_cast<size_t>(n)));
+    B2V_CUDA(this, cudaMemcpyAsync(d_keys->get(), keys4, static_cast<size_t>(n) * sizeof(int4), cudaMemcpyHostToDevice,
+                                   stream));
     block_import_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
         d_keys->get(), static_cast<uint32_t>(n), table, index);
     B2V_CUDA(this, cudaGetLastError());
+    return B2V_OK;
+}
+
+int BlockGridCore::scatter_blocks(int64_t n, const int4 *d_keys, const BlockArrays &arrays) {
+    BlockArrays A = arrays;   // with src[k] staged on the device, one array after the other
+    size_t bytes = 0;
+    bool runs16 = true;
+    for (int k = 0; k < A.n_arrays; ++k) {
+        bytes += static_cast<size_t>(n) * A.block_bytes[k];
+        runs16 = runs16 && A.block_bytes[k] % 16 == 0;
+    }
+    DeviceBuffer<uint8_t> d_src;
+    B2V_CUDA(this, d_src.reserve(bytes));
+    size_t off = 0;
+    for (int k = 0; k < A.n_arrays; ++k) {
+        const size_t run = static_cast<size_t>(n) * A.block_bytes[k];
+        B2V_CUDA(this, cudaMemcpyAsync(d_src.get() + off, arrays.src[k], run, cudaMemcpyHostToDevice, stream));
+        A.src[k] = d_src.get() + off;
+        off += run;
+    }
+    if (runs16)
+        block_scatter_kernel<uint4><<<static_cast<unsigned>(n), 256, 0, stream>>>(d_keys, A, table,
+                                                                                 index.pool_capacity);
+    else
+        block_scatter_kernel<uint32_t><<<static_cast<unsigned>(n), 256, 0, stream>>>(d_keys, A, table,
+                                                                                    index.pool_capacity);
+    B2V_CUDA(this, cudaGetLastError());
+    B2V_CUDA(this, cudaStreamSynchronize(stream));
     return B2V_OK;
 }
 
@@ -1250,79 +1277,43 @@ extern "C" int b2v_grid_carve(b2v_grid *g, const float K[4], int32_t width, int3
     return B2V_OK;
 }
 
-extern "C" int64_t b2v_grid_dump_blocks(b2v_grid *g, int32_t *keys, uint64_t *hashes, int32_t *count,
-                                        float *pos_sum, float *col_sum) {
+extern "C" int64_t b2v_grid_export_blocks(b2v_grid *g, int32_t *keys4, uint32_t *blocks) {
     if (!g) return -1;
     if (g->read_counters() == B2V_ERR_CUDA) return -1;
     const uint32_t nb = g->block_count();
-    if (nb == 0) return 0;
-    std::vector<int4> k(nb);
-    if (cudaMemcpy(k.data(), g->index.block_keys, nb * sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+    cudaError_t e = cudaSuccess;
+    if (nb && keys4)
+        e = cudaMemcpyAsync(keys4, g->index.block_keys, nb * sizeof(int4), cudaMemcpyDeviceToHost, g->stream);
+    if (nb && blocks && e == cudaSuccess)
+        e = cudaMemcpyAsync(blocks, reinterpret_cast<const void *>(g->pool.va), nb * g->block_bytes(),
+                            cudaMemcpyDeviceToHost, g->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(g->stream);
+    if (e != cudaSuccess) {
+        g->err = std::string("b2v_grid_export_blocks: ") + cudaGetErrorString(e);
         return -1;
-    for (uint32_t i = 0; i < nb; ++i) {
-        if (keys) {
-            keys[3 * i + 0] = k[i].x;
-            keys[3 * i + 1] = k[i].y;
-            keys[3 * i + 2] = k[i].z;
-        }
-        if (hashes) hashes[i] = block_key_hash(k[i].x, k[i].y, k[i].z);
-    }
-    if (count || pos_sum || col_sum) {
-        const size_t nv = g->block_voxels(), words = kGridPlanes * nv;
-        std::vector<uint32_t> raw(static_cast<size_t>(nb) * words);
-        if (cudaMemcpy(raw.data(), g->meta().pool, raw.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost) != cudaSuccess)
-            return -1;
-        for (size_t b = 0; b < nb; ++b) {
-            const uint32_t *blk = raw.data() + b * words;
-            const float *fb = reinterpret_cast<const float *>(blk);
-            for (size_t l = 0; l < nv; ++l) {
-                if (count) count[b * nv + l] = static_cast<int32_t>(blk[l]);
-                for (size_t c = 0; c < 3; ++c) {
-                    if (pos_sum) pos_sum[(b * nv + l) * 3 + c] = fb[(1 + c) * nv + l];
-                    if (col_sum) col_sum[(b * nv + l) * 3 + c] = fb[(4 + c) * nv + l];
-                }
-            }
-        }
     }
     return nb;
 }
 
-extern "C" int b2v_grid_upload_blocks(b2v_grid *g, int64_t n_blocks, const int32_t *keys, const int32_t *count,
-                                      const float *pos_sum, const float *col_sum) {
+extern "C" int b2v_grid_upload_blocks(b2v_grid *g, int64_t n_blocks, const int32_t *keys4, const uint32_t *blocks) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
-    if (n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && (!keys || !count || !pos_sum || !col_sum))) {
+    if (n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && (!keys4 || !blocks))) {
         g->err = "b2v_grid_upload_blocks: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     if (n_blocks == 0) return B2V_OK;
     B2V_CUDA(g, cudaSetDevice(g->device));
-    DeviceBuffer<int4> d_keys;
-    int rc = g->insert_keys(n_blocks, keys, &d_keys);
-    if (rc != B2V_OK) return rc;
-    if (g->growable) {   // new storage is mapped zeroed: the cleared state of a voxel
-        rc = g->resolve(
-            [&](uint64_t blocks) {
-                std::string map_err;   // a failed mapping surfaces as "block pool full"
-                grid_map_storage(g, blocks, &map_err);
-            },
-            [](uint32_t, uint32_t) { return B2V_OK; });
-        if (rc != B2V_OK) return rc;
-    }
-    const size_t nv = static_cast<size_t>(n_blocks) * g->block_voxels();
-    DeviceBuffer<int32_t> d_count;
-    DeviceBuffer<float> d_pos, d_col;
-    B2V_CUDA(g, d_count.reserve(nv));
-    B2V_CUDA(g, d_pos.reserve(nv * 3));
-    B2V_CUDA(g, d_col.reserve(nv * 3));
-    B2V_CUDA(g, cudaMemcpyAsync(d_count.get(), count, nv * sizeof(int32_t), cudaMemcpyHostToDevice, g->stream));
-    B2V_CUDA(g, cudaMemcpyAsync(d_pos.get(), pos_sum, nv * 3 * sizeof(float), cudaMemcpyHostToDevice, g->stream));
-    B2V_CUDA(g, cudaMemcpyAsync(d_col.get(), col_sum, nv * 3 * sizeof(float), cudaMemcpyHostToDevice, g->stream));
-    const uint32_t nu = static_cast<uint32_t>(n_blocks);
-    g->dispatch([&](auto l) {
-        grid_scatter_kernel<decltype(l)::value><<<g->voxel_ctas(nu), kVox, 0, g->stream>>>(
-            d_keys.get(), d_count.get(), d_pos.get(), d_col.get(), g->table, g->meta(), nu);
-    });
-    B2V_CUDA(g, cudaGetLastError());
-    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
-    return g->read_counters();
+    BlockArrays a{};
+    a.n_arrays = 1;
+    a.dst[0] = reinterpret_cast<void *>(g->pool.va);
+    a.src[0] = blocks;
+    a.block_bytes[0] = static_cast<uint32_t>(g->block_bytes());
+    const int rc = g->upload_blocks(
+        n_blocks, keys4, a,
+        [&](uint64_t storage_blocks) {
+            std::string map_err;   // a failed mapping surfaces as "block pool full"
+            grid_map_storage(g, storage_blocks, &map_err);
+        },
+        [](uint32_t, uint32_t) { return B2V_OK; });   // new storage is mapped zeroed: the cleared state of a voxel
+    return rc == B2V_OK ? g->read_counters() : rc;
 }

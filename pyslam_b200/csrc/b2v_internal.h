@@ -275,9 +275,6 @@ cudaError_t launch_selftest_division(unsigned long long *d_bad, uint64_t pairs, 
 // fused update of a group of frames (each block is read and written once per group)
 cudaError_t launch_integrate_group(const GroupArgs &args, const HashTable &table, const PoolMeta &meta,
                                    int group_buf, int grid_ctas, int sm_count, cudaStream_t stream);
-// hashes[i] = BlockKeyHash(block_keys[i])
-cudaError_t launch_block_hashes(const int4 *block_keys, uint64_t *hashes, uint32_t n,
-                                cudaStream_t stream);
 // keys of the slots in a touched list
 cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *slots,
                                       uint32_t n, int4 *out, cudaStream_t stream);
@@ -432,6 +429,16 @@ struct GridQuery {
     int32_t W, H;
 };
 
+// The per-voxel arrays of a grid's blocks as a block upload copies them: array k holds a run of block_bytes[k] bytes
+// per block at dst[k] + pool index * block_bytes[k], and the uploaded blocks' runs follow one another in src[k].
+constexpr int kMaxBlockArrays = 11;
+struct BlockArrays {
+    void *dst[kMaxBlockArrays];
+    const void *src[kMaxBlockArrays];
+    uint32_t block_bytes[kMaxBlockArrays];
+    int32_t n_arrays;
+};
+
 // The host half both grids share: device and stream, table, block index, counters, growth, scan buffers.
 struct BlockGridCore {
     int device = 0;
@@ -490,11 +497,16 @@ struct BlockGridCore {
     // in one call belong to one block and a block's index never changes, so every voxel is updated by exactly one of
     // the passes.  If the storage cannot grow, the blocks past it are dropped ("block pool full").  Synchronises.
     template <typename MapStorage, typename Replay> int resolve(MapStorage map_storage, Replay replay);
-    // First half of a block upload: the HOST keys int32 [n][3] as int4 in *d_keys, and each inserted into the table
-    // with a pool index (block_insert: a sharded grid skips the blocks it does not own; past index.capacity the
-    // index is kNoBlock and the error flag says "block pool full").  Asynchronous.  A growable grid then maps storage
-    // for the new pool count (resolve) before the grid's scatter kernel copies the voxels in.
-    int insert_keys(int64_t n, const int32_t *keys, DeviceBuffer<int4> *d_keys);
+    // Block upload of both grids (b2v_grid_upload_blocks, b2v_sgrid_upload_blocks): the n HOST keys int32 [n][4]
+    // {x, y, z, 0} go through the block insert (a sharded grid skips the blocks it does not own; past index.capacity
+    // the index is kNoBlock and the error flag says "block pool full"), a growable grid maps storage for the new pool
+    // count (resolve with the grid's map_storage, and fill(lo, hi) setting the blocks that got storage to the cleared
+    // state), then every block's run of each array replaces its pool block's run.  Synchronises.
+    template <typename MapStorage, typename Fill>
+    int upload_blocks(int64_t n, const int32_t *keys4, const BlockArrays &arrays, MapStorage map_storage, Fill fill);
+    // its steps: the keys into *d_keys and the table (asynchronous); the copy of the runs (synchronises)
+    int insert_keys(int64_t n, const int32_t *keys4, DeviceBuffer<int4> *d_keys);
+    int scatter_blocks(int64_t n, const int4 *d_keys, const BlockArrays &arrays);
     // Voxel-order sort of the input-order updates (the semantic grids, the point grid's input-order sums): per point
     // the key pool index * B^3 + local index (kBadVid where the point is masked out by `valid` or its block has no
     // pool index in [lo, hi)) and the point index, sorted stably over all 32 key bits into vid[1] / ord[1], so each
@@ -566,6 +578,15 @@ template <typename MapStorage, typename Replay> int BlockGridCore::resolve(MapSt
                                                   index.counters + kBgError, stream));
     B2V_CUDA(this, cudaStreamSynchronize(stream));
     return B2V_OK;
+}
+
+template <typename MapStorage, typename Fill>
+int BlockGridCore::upload_blocks(int64_t n, const int32_t *keys4, const BlockArrays &arrays, MapStorage map_storage,
+                                 Fill fill) {
+    DeviceBuffer<int4> d_keys;
+    int rc = insert_keys(n, keys4, &d_keys);
+    if (rc == B2V_OK && growable) rc = resolve(map_storage, fill);
+    return rc == B2V_OK ? scatter_blocks(n, d_keys.get(), arrays) : rc;
 }
 
 // raw uint16 depth -> float32 metres (b2v_prep.cu)

@@ -32,7 +32,6 @@
 #include <climits>
 #include <cmath>
 #include <cstring>
-#include <limits>
 #include <map>
 #include <new>
 #include <string>
@@ -48,6 +47,7 @@ namespace b2v {
 constexpr int kSemLabels = B2V_SEM_MAX_LABELS;
 constexpr float kBaseLogProb = 0.10536051565782628f;  // voxel_data_semantic.h:287, -log(0.9)
 constexpr int kSemArrays = 11;   // per-voxel arrays of a Bayesian grid (a voting grid has the first 6)
+static_assert(kSemArrays <= kMaxBlockArrays, "a block upload carries every array");
 
 // the block index as the semantic kernels read it: BlockIndex without the shard fields, which only the block insert
 // reads (the 24-byte layout keeps sem_runs_kernel's label slots in a local-memory frame, as before the shard fields)
@@ -803,33 +803,6 @@ __global__ void sem_fill_kernel(const SemGrid G, const size_t v0, const size_t v
     }
 }
 
-// ---- block upload (b2v_sgrid_upload_blocks) ------------------------------------------------------------------
-// The grid's per-voxel arrays (sgrid_arrays order): each uploaded block is a contiguous run of block_bytes[k] bytes in
-// src[k] (the layout of b2v_sgrid_export_blocks) and goes to its pool block's run in dst[k].
-struct SemUpload {
-    void *dst[kSemArrays];
-    const void *src[kSemArrays];
-    uint32_t block_bytes[kSemArrays];   // multiples of sizeof(W)
-    int32_t n_arrays;
-};
-
-// one CTA per uploaded block: every array's run of the block, one word W per thread and step, replacing what the pool
-// block held.  W = uint4 where every run is a multiple of 16 bytes (B >= 2), else uint32_t (B = 1).  A byte copy of
-// whole runs, not a per-voxel pass: it keeps one block per CTA at every B.
-template <typename W>
-__global__ void __launch_bounds__(256)
-sem_scatter_kernel(const int4 *__restrict__ keys, const SemUpload U, const HashTable T, const uint32_t pool_capacity) {
-    const uint32_t b = blockIdx.x;
-    const uint32_t idx = uploaded_block_index(T, keys[b], pool_capacity);
-    if (idx == kNoBlock) return;
-    for (int k = 0; k < U.n_arrays; ++k) {
-        const uint32_t words = U.block_bytes[k] / static_cast<uint32_t>(sizeof(W));
-        const W *src = static_cast<const W *>(U.src[k]) + static_cast<size_t>(b) * words;
-        W *dst = static_cast<W *>(U.dst[k]) + static_cast<size_t>(idx) * words;
-        for (uint32_t w = threadIdx.x; w < words; w += blockDim.x) dst[w] = src[w];
-    }
-}
-
 }  // namespace b2v
 
 // ====================================================================================================================
@@ -910,7 +883,7 @@ template <typename F> static void sgrid_dispatch(const b2v_sgrid *g, F &&f) {
 }
 
 static bool sgrid_map_labels(b2v_sgrid *g, uint64_t chunks, std::string *err);
-static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys4, const int32_t *n_over,
                             const int32_t *obj, const int32_t *cls, const float *logp);
 
 // an empty store: no chain, no chunk taken
@@ -1438,115 +1411,6 @@ extern "C" int b2v_sgrid_merge_segments(b2v_sgrid *g, int32_t object_id1, int32_
     return sgrid_edit(g, 3, object_id1, object_id2);
 }
 
-// Parity hook.  Arrays are [nb][B^3]...; any output may be NULL.  `aux` = voting confidence counter, or the
-// number of label pairs of a Bayesian voxel; lab_* [nb][B^3][K] in ascending (object, class) order, padded with
-// (-1, -1, -inf) (K <= B2V_SEM_MAX_LABELS).
-extern "C" int64_t b2v_sgrid_dump_blocks(b2v_sgrid *g, int32_t *keys, uint64_t *hashes, int32_t *count, double *pos_sum,
-                                         float *col_sum, int32_t *object_id, int32_t *class_id, float *confidence,
-                                         int32_t *aux, int32_t K, int32_t *lab_obj, int32_t *lab_cls,
-                                         float *lab_logp) {
-    if (!g) return -1;
-    const int64_t nb = b2v_sgrid_num_blocks(g);
-    if (nb <= 0) return nb;
-    const size_t nv = static_cast<size_t>(nb) * g->block_voxels();
-    bool ok = true;
-    auto d2h = [&](void *dst, const void *src, size_t bytes) {
-        if (dst && src) ok = ok && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, g->stream) == cudaSuccess;
-    };
-    std::vector<int4> hk(static_cast<size_t>(nb));
-    d2h(hk.data(), g->index.block_keys, hk.size() * sizeof(int4));
-    d2h(count, g->G.count, nv * sizeof(int32_t));
-    d2h(pos_sum, g->G.pos, nv * 3 * sizeof(double));
-    d2h(col_sum, g->G.col, nv * 3 * sizeof(float));
-    d2h(object_id, g->G.obj, nv * sizeof(int32_t));
-    d2h(class_id, g->G.cls, nv * sizeof(int32_t));
-    d2h(aux, g->G.counter, nv * sizeof(int32_t));
-    std::vector<int32_t> h_count, h_ctr, lo, lc;
-    std::vector<float> lp;
-    std::vector<uint32_t> heads;
-    std::vector<LabelChunk> chunks;
-    const bool bayes = g->G.kind == B2V_SEM_PROBABILISTIC;
-    const bool want_labels = bayes && K > 0 && (lab_obj || lab_cls || lab_logp);
-    if (confidence) {
-        if (bayes) {
-            d2h(confidence, g->G.conf, nv * sizeof(float));
-        } else {
-            h_count.resize(nv);
-            h_ctr.resize(nv);
-            d2h(h_count.data(), g->G.count, nv * sizeof(int32_t));
-            d2h(h_ctr.data(), g->G.counter, nv * sizeof(int32_t));
-        }
-    }
-    if (want_labels) {
-        if (h_ctr.empty()) {
-            h_ctr.resize(nv);
-            d2h(h_ctr.data(), g->G.counter, nv * sizeof(int32_t));
-        }
-        lo.resize(nv * kSemLabels);
-        lc.resize(nv * kSemLabels);
-        lp.resize(nv * kSemLabels);
-        d2h(lo.data(), g->G.lab_obj, lo.size() * sizeof(int32_t));
-        d2h(lc.data(), g->G.lab_cls, lc.size() * sizeof(int32_t));
-        d2h(lp.data(), g->G.lab_logp, lp.size() * sizeof(float));
-        if (g->lab_max_chunks) {   // the chains: every chunk ever taken, fresh ones included
-            uint32_t c[kLcNum];
-            ok = ok && cudaMemcpyAsync(c, g->d_lab_ctr.get(), sizeof(c), cudaMemcpyDeviceToHost, g->stream) ==
-                           cudaSuccess &&
-                 cudaStreamSynchronize(g->stream) == cudaSuccess;
-            heads.resize(nv);
-            chunks.resize(ok ? c[kLcFresh] : 0);
-            d2h(heads.data(), reinterpret_cast<const void *>(g->lab_head.va), nv * sizeof(uint32_t));
-            d2h(chunks.data(), reinterpret_cast<const void *>(g->lab_chunks.va), chunks.size() * sizeof(LabelChunk));
-        }
-    }
-    ok = ok && cudaStreamSynchronize(g->stream) == cudaSuccess;
-    if (!ok) {
-        g->err = "b2v_sgrid_dump_blocks: device copy failed";
-        return -1;
-    }
-    for (int64_t b = 0; b < nb; ++b) {
-        if (keys) {
-            keys[3 * b + 0] = hk[b].x;
-            keys[3 * b + 1] = hk[b].y;
-            keys[3 * b + 2] = hk[b].z;
-        }
-        if (hashes) hashes[b] = block_key_hash(hk[b].x, hk[b].y, hk[b].z);
-    }
-    if (confidence && !bayes)
-        for (size_t v = 0; v < nv; ++v) {
-            const float c = h_count[v] ? static_cast<float>(h_ctr[v]) / static_cast<float>(h_count[v]) : 0.0f;
-            confidence[v] = h_count[v] ? (c < 1.0f ? c : 1.0f) : 0.0f;
-        }
-    if (want_labels) {
-        const float ninf = -std::numeric_limits<float>::infinity();
-        struct Pair {
-            int32_t o, c;
-            float l;
-        };
-        std::vector<Pair> pairs;
-        for (size_t v = 0; v < nv; ++v) {   // the voxel's pairs in slot order, then sorted by (object, class)
-            pairs.clear();
-            const int nl = heads.empty() ? std::min(h_ctr[v], kSemLabels) : h_ctr[v];
-            for (int k = 0; k < nl && k < kSemLabels; ++k)
-                pairs.push_back({lo[v * kSemLabels + k], lc[v * kSemLabels + k], lp[v * kSemLabels + k]});
-            for (uint32_t link = heads.empty() ? 0 : heads[v]; link != 0 && link <= chunks.size();
-                 link = chunks[link - 1].next)
-                for (int e = 0; e < kChunkPairs && static_cast<int>(pairs.size()) < nl; ++e)
-                    pairs.push_back({chunks[link - 1].obj[e], chunks[link - 1].cls[e], chunks[link - 1].logp[e]});
-            std::stable_sort(pairs.begin(), pairs.end(),
-                             [](const Pair &a, const Pair &b) { return a.o < b.o || (a.o == b.o && a.c < b.c); });
-            for (int k = 0; k < K; ++k) {
-                const bool have = k < static_cast<int>(pairs.size());
-                if (lab_obj) lab_obj[v * K + k] = have ? pairs[k].o : -1;
-                if (lab_cls) lab_cls[v * K + k] = have ? pairs[k].c : -1;
-                if (lab_logp) lab_logp[v * K + k] = have ? pairs[k].l : ninf;
-            }
-        }
-    }
-    return nb;
-}
-
-
 // ---- carve / instance -> object association -------------------------------------------------------------------------
 extern "C" int b2v_sgrid_carve(b2v_sgrid *g, const float K[4], int32_t width, int32_t height, const double Tcw[16],
                                float depth_max, float depth_min, const float *depth, float depth_threshold) {
@@ -1859,7 +1723,7 @@ extern "C" int b2v_sgrid_copy_instance_map(b2v_sgrid *g, int32_t *instance_ids, 
 }
 
 // ---- raw block export / upload (map state) --------------------------------------------------------------------------
-extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys, int32_t *count, double *pos_sum, float *col_sum,
+extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys4, int32_t *count, double *pos_sum, float *col_sum,
                                            int32_t *object_id, int32_t *class_id, int32_t *counter, float *ml_logp,
                                            float *conf, int32_t *lab_obj, int32_t *lab_cls, float *lab_logp) {
     if (!g) return -1;
@@ -1869,9 +1733,10 @@ extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys, int32_t 
                                    lab_obj, lab_cls, lab_logp};
     SemArray arr[kSemArrays];
     const int na = sgrid_arrays(g, arr);
-    std::vector<int4> hk(static_cast<size_t>(nb));
-    cudaError_t e = cudaMemcpyAsync(hk.data(), g->index.block_keys, hk.size() * sizeof(int4), cudaMemcpyDeviceToHost,
-                                    g->stream);
+    cudaError_t e = cudaSuccess;
+    if (keys4)
+        e = cudaMemcpyAsync(keys4, g->index.block_keys, static_cast<size_t>(nb) * sizeof(int4), cudaMemcpyDeviceToHost,
+                            g->stream);
     for (int k = 0; k < na && e == cudaSuccess; ++k)
         if (out[k])
             e = cudaMemcpyAsync(out[k], *arr[k].ptr, static_cast<size_t>(nb) * g->block_voxels() * arr[k].voxel_bytes,
@@ -1881,16 +1746,10 @@ extern "C" int64_t b2v_sgrid_export_blocks(b2v_sgrid *g, int32_t *keys, int32_t 
         g->err = std::string("b2v_sgrid_export_blocks: ") + cudaGetErrorString(e);
         return -1;
     }
-    if (keys)
-        for (int64_t b = 0; b < nb; ++b) {
-            keys[3 * b + 0] = hk[b].x;
-            keys[3 * b + 1] = hk[b].y;
-            keys[3 * b + 2] = hk[b].z;
-        }
     return nb;
 }
 
-extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys, const int32_t *count,
+extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys4, const int32_t *count,
                                        const double *pos_sum, const float *col_sum, const int32_t *object_id,
                                        const int32_t *class_id, const int32_t *counter, const float *ml_logp,
                                        const float *conf, const int32_t *lab_obj, const int32_t *lab_cls,
@@ -1900,7 +1759,7 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
                                         lab_obj, lab_cls, lab_logp};
     SemArray arr[kSemArrays];
     const int na = sgrid_arrays(g, arr);
-    bool bad = n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && !keys);
+    bool bad = n_blocks < 0 || n_blocks > INT32_MAX || (n_blocks > 0 && !keys4);
     for (int k = 0; k < na; ++k) bad = bad || (n_blocks > 0 && !in[k]);
     if (bad) {
         g->err = "b2v_sgrid_upload_blocks: bad arguments";
@@ -1911,53 +1770,28 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
     g->has_instance_map = false;
     if (n_blocks == 0) return B2V_OK;
     B2V_CUDA(g, cudaSetDevice(g->device));
-    DeviceBuffer<int4> d_keys;
-    int rc = g->insert_keys(n_blocks, keys, &d_keys);
+    BlockArrays a{};
+    a.n_arrays = na;
+    for (int k = 0; k < na; ++k) {
+        a.dst[k] = *arr[k].ptr;
+        a.src[k] = in[k];
+        a.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * g->block_voxels());
+    }
+    int rc = g->upload_blocks(
+        n_blocks, keys4, a,
+        [&](uint64_t blocks) {
+            std::string map_err;   // a failed mapping surfaces as "block pool full"
+            sgrid_map_storage(g, blocks, &map_err);
+        },
+        [&](uint32_t lo, uint32_t hi) {   // the cleared state for the voxels that just got storage
+            sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
+                                                        static_cast<size_t>(hi) * g->block_voxels());
+            B2V_CUDA(g, cudaGetLastError());
+            return B2V_OK;
+        });
     if (rc != B2V_OK) return rc;
-    if (g->growable) {
-        rc = g->resolve(
-            [&](uint64_t blocks) {
-                std::string map_err;   // a failed mapping surfaces as "block pool full"
-                sgrid_map_storage(g, blocks, &map_err);
-            },
-            [&](uint32_t lo, uint32_t hi) {   // the cleared state for the voxels that just got storage
-                sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
-                                                            static_cast<size_t>(hi) * g->block_voxels());
-                B2V_CUDA(g, cudaGetLastError());
-                return B2V_OK;
-            });
-        if (rc != B2V_OK) return rc;
-    }
-    SemUpload U{};
-    U.n_arrays = na;
-    const size_t nvb = g->block_voxels();
-    size_t block_bytes = 0;
-    bool runs16 = true;   // every run of a block a multiple of 16 bytes (B >= 2)
-    for (int k = 0; k < na; ++k) {
-        block_bytes += arr[k].voxel_bytes * nvb;
-        runs16 = runs16 && (arr[k].voxel_bytes * nvb) % 16 == 0;
-    }
-    DeviceBuffer<uint8_t> d_src;
-    B2V_CUDA(g, d_src.reserve(static_cast<size_t>(n_blocks) * block_bytes));
-    size_t off = 0;
-    for (int k = 0; k < na; ++k) {
-        const size_t bytes = static_cast<size_t>(n_blocks) * nvb * arr[k].voxel_bytes;
-        B2V_CUDA(g, cudaMemcpyAsync(d_src.get() + off, in[k], bytes, cudaMemcpyHostToDevice, g->stream));
-        U.dst[k] = *arr[k].ptr;
-        U.src[k] = d_src.get() + off;
-        U.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * nvb);
-        off += bytes;
-    }
-    if (runs16)
-        sem_scatter_kernel<uint4><<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(d_keys.get(), U, g->table,
-                                                                                         g->index.pool_capacity);
-    else
-        sem_scatter_kernel<uint32_t><<<static_cast<unsigned>(n_blocks), 256, 0, g->stream>>>(
-            d_keys.get(), U, g->table, g->index.pool_capacity);
-    B2V_CUDA(g, cudaGetLastError());
-    B2V_CUDA(g, cudaStreamSynchronize(g->stream));
     if (g->lab_max_chunks) {   // the uploaded voxels hold their in-voxel pairs only until b2v_sgrid_upload_labels
-        rc = sgrid_set_labels(g, "b2v_sgrid_upload_blocks", n_blocks, keys, nullptr, nullptr, nullptr, nullptr);
+        rc = sgrid_set_labels(g, "b2v_sgrid_upload_blocks", n_blocks, keys4, nullptr, nullptr, nullptr, nullptr);
         if (rc != B2V_OK) return rc;
     }
     return g->read_counters();
@@ -2000,11 +1834,11 @@ static int sgrid_fetch_labels(b2v_sgrid *g, LabelHost *h) {
     return B2V_OK;
 }
 
-// The uploaded blocks `keys` [n][3] that the grid holds get their overflow pairs: each voxel's chain goes back to the
+// The uploaded blocks `keys4` [n][4] that the grid holds get their overflow pairs: each voxel's chain goes back to the
 // pool, its counter keeps its in-voxel pairs (at most B2V_SEM_MAX_LABELS) and, if n_over is not NULL, it takes a new
 // chain of n_over[voxel] pairs from obj / cls / logp (slot order; the pairs of blocks the grid does not hold are
 // skipped).  Checks first and changes nothing on a bad argument or when the pool's ceiling cannot hold the pairs.
-static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, const int32_t *keys4, const int32_t *n_over,
                             const int32_t *obj, const int32_t *cls, const float *logp) {
     const size_t nvb = g->block_voxels();
     LabelHost h;
@@ -2019,7 +1853,7 @@ static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, cons
     for (int64_t b = 0; b < h.nb; ++b) pool[{hk[b].x, hk[b].y, hk[b].z}] = static_cast<uint32_t>(b);
     std::vector<int64_t> idx(static_cast<size_t>(n_blocks), -1);
     for (int64_t b = 0; b < n_blocks; ++b) {
-        const auto it = pool.find({keys[3 * b], keys[3 * b + 1], keys[3 * b + 2]});
+        const auto it = pool.find({keys4[4 * b], keys4[4 * b + 1], keys4[4 * b + 2]});
         if (it != pool.end()) idx[b] = it->second;
     }
     // checks: counts, and the chunks the new chains need against what the pool can give once the old ones are back
@@ -2124,10 +1958,10 @@ extern "C" int64_t b2v_sgrid_export_labels(b2v_sgrid *g, int32_t *n_over, int32_
     return total;
 }
 
-extern "C" int b2v_sgrid_upload_labels(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys, const int32_t *n_over,
+extern "C" int b2v_sgrid_upload_labels(b2v_sgrid *g, int64_t n_blocks, const int32_t *keys4, const int32_t *n_over,
                                        const int32_t *obj, const int32_t *cls, const float *logp) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
-    if (n_blocks < 0 || (n_blocks > 0 && (!keys || !n_over))) {
+    if (n_blocks < 0 || (n_blocks > 0 && (!keys4 || !n_over))) {
         g->err = "b2v_sgrid_upload_labels: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
@@ -2142,5 +1976,5 @@ extern "C" int b2v_sgrid_upload_labels(b2v_sgrid *g, int64_t n_blocks, const int
     }
     B2V_CUDA(g, cudaSetDevice(g->device));
     ++g->generation;
-    return sgrid_set_labels(g, "b2v_sgrid_upload_labels", n_blocks, keys, n_over, obj, cls, logp);
+    return sgrid_set_labels(g, "b2v_sgrid_upload_labels", n_blocks, keys4, n_over, obj, cls, logp);
 }

@@ -211,7 +211,7 @@ def gather_blocks(keys, vox, dst: int = 0, group=None, device=None):
 
 def gather_blocks_device(volume, dst: int = 0, group=None):
     """Device-resident gather over NCCL: every rank exports its blocks device-to-device
-    (`b2v_export_blocks_device`), the payloads travel GPU to GPU (NVLink), nothing touches host memory.
+    (`b2v_export_blocks`), the payloads travel GPU to GPU (NVLink), nothing touches host memory.
     Returns (keys int32 [n,4], vox float32 [n,5,512]) CUDA tensors on dst, (None, None) elsewhere."""
     import torch
     import torch.distributed as dist

@@ -47,6 +47,23 @@ def _is_torch_cuda(x) -> bool:
     return hasattr(x, "data_ptr") and hasattr(x, "is_cuda") and bool(x.is_cuda)
 
 
+def _keys4(keys) -> np.ndarray:
+    """Block keys [n,3] as the library takes them: int32 [n,4] = {x, y, z, 0}, the table's own key layout."""
+    k = np.asarray(keys, np.int32).reshape(-1, 3)
+    k4 = np.zeros((k.shape[0], 4), np.int32)
+    k4[:, :3] = k
+    return k4
+
+
+def _block_hashes(keys) -> np.ndarray:
+    """The reference's BlockKeyHash of block keys [n,3] (b2v_block_key_hashes: the hash the kernels use)."""
+    k4 = _keys4(keys)
+    h = np.zeros(len(k4), np.uint64)
+    if len(k4) and _lib.load().b2v_block_key_hashes(k4.ctypes.data, len(k4), h.ctypes.data) != _lib.B2V_OK:
+        raise RuntimeError("b2v_block_key_hashes failed")
+    return h
+
+
 def _pinned_owner(x):
     """The torch tensor behind a pinned host array (a numpy view of one included), or None.  The copy engine reads
     pinned memory after the integrate call returns; pageable memory is staged before it returns."""
@@ -429,26 +446,32 @@ class B200TsdfVolume(_MapState):
 
     def last_touched_keys(self) -> np.ndarray:
         n = self._L.b2v_last_touched_keys(self._h, None, 0)
-        keys = np.zeros((max(int(n), 0), 3), np.int32)
+        keys = np.zeros((max(int(n), 0), 4), np.int32)
         if n > 0:
             self._L.b2v_last_touched_keys(self._h, keys.ctypes.data, int(n))
-        return keys
+        return np.ascontiguousarray(keys[:, :3])
+
+    def _export_blocks(self, empty):
+        """(keys int32 [nb,4] = {x,y,z,0}, vox float32 [nb,5,512]) of every block in arrays `empty(shape, dtype name)`
+        makes, host or device (b2v_export_blocks, which waits for the frames in flight)."""
+        n = self._L.b2v_export_blocks(self._h, None, None, 0)
+        if n < 0:
+            raise RuntimeError(self._L.b2v_last_error(self._h).decode())
+        keys, vox = empty((n, 4), "int32"), empty((n, VOXEL_PLANES, BLOCK_VOXELS), "float32")
+        ptr = (lambda a: a.data_ptr()) if hasattr(keys, "data_ptr") else (lambda a: a.ctypes.data)
+        if n and self._L.b2v_export_blocks(self._h, ptr(keys), ptr(vox), n) != n:
+            raise RuntimeError(self._L.b2v_last_error(self._h).decode())
+        return keys, vox
 
     def dump_blocks(self):
         """Parity hook: keys int32 [nb,3], hashes uint64 [nb] (reference BlockKeyHash),
         vox float32 [nb,5,512] planes (tsdf, weight, r, g, b)."""
-        nb = self.num_blocks()
-        keys = np.zeros((nb, 3), np.int32)
-        hashes = np.zeros(nb, np.uint64)
-        vox = np.zeros((nb, VOXEL_PLANES, BLOCK_VOXELS), np.float32)
-        n = self._L.b2v_dump_blocks(self._h, keys.ctypes.data, hashes.ctypes.data, vox.ctypes.data)
-        if n != nb:
-            raise RuntimeError(f"b2v_dump_blocks returned {n}, expected {nb}")
-        return dict(keys=keys, hashes=hashes, vox=vox)
+        d = self._export_state()
+        return dict(keys=d["keys"], hashes=_block_hashes(d["keys"]), vox=d["vox"])
 
     def upload_blocks(self, keys, vox):
         """Restore / seed blocks: keys int32 [n,3] (unique), vox float32 [n,5,512]."""
-        k = np.ascontiguousarray(keys, np.int32).reshape(-1, 3)
+        k = _keys4(keys)
         x = np.ascontiguousarray(vox, np.float32).reshape(k.shape[0], VOXEL_PLANES, BLOCK_VOXELS)
         self._check(self._L.b2v_upload_blocks(self._h, k.shape[0], k.ctypes.data, x.ctypes.data),
                     "b2v_upload_blocks")
@@ -470,14 +493,8 @@ class B200TsdfVolume(_MapState):
         return max(self.capacity_blocks, self.max_capacity_blocks)
 
     def _export_state(self) -> dict:
-        """keys / vox of every block (b2v_dump_blocks, which waits for the frames in flight)."""
-        nb = self.num_blocks()
-        keys = np.zeros((nb, 3), np.int32)
-        vox = np.zeros((nb, VOXEL_PLANES, BLOCK_VOXELS), np.float32)
-        n = self._L.b2v_dump_blocks(self._h, keys.ctypes.data, None, vox.ctypes.data)
-        if n != nb:
-            raise RuntimeError(f"b2v_dump_blocks returned {n}, expected {nb}: {self._L.b2v_last_error(self._h).decode()}")
-        return dict(keys=keys, vox=vox)
+        keys4, vox = self._export_blocks(np.empty)
+        return dict(keys=np.ascontiguousarray(keys4[:, :3]), vox=vox)
 
     def _clear_state(self) -> None:
         self.reset()
@@ -490,26 +507,17 @@ class B200TsdfVolume(_MapState):
         """(keys int32 [n,4] = {x,y,z,0}, vox float32 [n,5,512]) as torch CUDA tensors on this volume's device:
         device-to-device copies of the block keys and the block pool (multi-GPU mesh gather)."""
         import torch
-        n = self._L.b2v_export_blocks_device(self._h, None, None, 0)
-        if n < 0:
-            raise RuntimeError(self._L.b2v_last_error(self._h).decode())
         dev = torch.device("cuda", self.device)
-        keys = torch.empty((n, 4), dtype=torch.int32, device=dev)
-        vox = torch.empty((n, VOXEL_PLANES, BLOCK_VOXELS), dtype=torch.float32, device=dev)
-        if n:
-            got = self._L.b2v_export_blocks_device(self._h, keys.data_ptr(), vox.data_ptr(), n)
-            if got != n:
-                raise RuntimeError(self._L.b2v_last_error(self._h).decode())
-        return keys, vox
+        return self._export_blocks(lambda shape, dt: torch.empty(shape, dtype=getattr(torch, dt), device=dev))
 
     def import_blocks_torch(self, keys, vox):
-        """Inverse of export_blocks_torch: contiguous torch CUDA tensors on this volume's device."""
+        """Inverse of export_blocks_torch: contiguous torch CUDA tensors on this volume's device, read in place."""
         if keys.shape[0] == 0:
             return
         if not (keys.is_cuda and vox.is_cuda and keys.is_contiguous() and vox.is_contiguous()):
             raise RuntimeError("keys and vox must be contiguous CUDA tensors")
-        self._check(self._L.b2v_import_blocks_device(self._h, int(keys.shape[0]), keys.data_ptr(), vox.data_ptr()),
-                    "b2v_import_blocks_device")
+        self._check(self._L.b2v_upload_blocks(self._h, int(keys.shape[0]), keys.data_ptr(), vox.data_ptr()),
+                    "b2v_upload_blocks")
 
     # ---- outputs ----
     def extract_mesh(self) -> TriangleMesh:
@@ -1059,6 +1067,7 @@ class VoxelBlockGrid(_BlockGrid):
         return None
 
     _STATE_KIND = "grid"
+    _PLANES = 7   # a pool block's 32-bit planes of B^3 voxels: count (int32), pos_sum x, y, z, col_sum r, g, b
 
     def _state_arrays(self) -> dict:
         v = self._block_voxels
@@ -1066,29 +1075,37 @@ class VoxelBlockGrid(_BlockGrid):
                     col_sum=(np.float32, (v, 3)))
 
     def _export_state(self) -> dict:
-        d = self.dump_blocks()
-        del d["hashes"]
-        return d
+        """keys int32 [nb,3], count int32 [nb,B^3], pos_sum / col_sum float32 [nb,B^3,3] of every block, from the
+        pool blocks of b2v_grid_export_blocks."""
+        nb = self.num_blocks()
+        keys4 = np.empty((nb, 4), np.int32)
+        raw = np.empty((nb, self._PLANES, self._block_voxels), np.uint32)
+        n = self._L.b2v_grid_export_blocks(self._h, keys4.ctypes.data, raw.ctypes.data)
+        if n != nb:
+            raise RuntimeError(f"b2v_grid_export_blocks returned {n}, expected {nb}")
+
+        def xyz(p):
+            return np.ascontiguousarray(raw[:, p:p + 3].transpose(0, 2, 1)).view(np.float32)
+        return dict(keys=np.ascontiguousarray(keys4[:, :3]), count=np.ascontiguousarray(raw[:, 0]).view(np.int32),
+                    pos_sum=xyz(1), col_sum=xyz(4))
 
     def _upload_state(self, blocks: dict) -> None:
         b = blocks
-        self._check(self._L.b2v_grid_upload_blocks(self._h, len(b["keys"]), b["keys"].ctypes.data,
-                                                   b["count"].ctypes.data, b["pos_sum"].ctypes.data,
-                                                   b["col_sum"].ctypes.data), "b2v_grid_upload_blocks")
+        n, v = len(b["keys"]), self._block_voxels
+        raw = np.empty((n, self._PLANES, v), np.uint32)
+        raw[:, 0] = np.asarray(b["count"], np.int32).reshape(n, v).view(np.uint32)
+        for p, name in ((1, "pos_sum"), (4, "col_sum")):
+            raw[:, p:p + 3] = np.asarray(b[name], np.float32).reshape(n, v, 3).view(np.uint32).transpose(0, 2, 1)
+        keys4 = _keys4(b["keys"])
+        self._check(self._L.b2v_grid_upload_blocks(self._h, n, keys4.ctypes.data, raw.ctypes.data),
+                    "b2v_grid_upload_blocks")
 
     def dump_blocks(self):
-        nb = self.num_blocks()
-        keys = np.zeros((nb, 3), np.int32)
-        hashes = np.zeros(nb, np.uint64)
-        v = self._block_voxels
-        count = np.zeros((nb, v), np.int32)
-        pos = np.zeros((nb, v, 3), np.float32)
-        col = np.zeros((nb, v, 3), np.float32)
-        n = self._L.b2v_grid_dump_blocks(self._h, keys.ctypes.data, hashes.ctypes.data,
-                                         count.ctypes.data, pos.ctypes.data, col.ctypes.data)
-        if n != nb:
-            raise RuntimeError(f"b2v_grid_dump_blocks returned {n}, expected {nb}")
-        return dict(keys=keys, hashes=hashes, count=count, pos_sum=pos, col_sum=col)
+        """Parity hook: keys int32 [nb,3], hashes uint64 [nb] (reference BlockKeyHash), count int32 [nb,B^3],
+        pos_sum / col_sum float32 [nb,B^3,3]."""
+        d = self._export_state()
+        return dict(keys=d["keys"], hashes=_block_hashes(d["keys"]), count=d["count"], pos_sum=d["pos_sum"],
+                    col_sum=d["col_sum"])
 
     # ---- spatial queries and carving (SURVEY.md §8(f) rank 3) ----
     def _collect(self, n):
@@ -1347,17 +1364,19 @@ class VoxelBlockSemanticGrid(_BlockGrid):
     def export_blocks(self) -> dict:
         """The raw state of every block (b2v_sgrid_export_blocks): keys [nb,3] and per-voxel arrays [nb,B^3,...] -
         count, pos_sum (float64), col_sum, object_id, class_id, counter (the voting counter, or the number of label
-        slots in use) and, on the Bayesian grid, ml_logp, conf and the label slots lab_obj / lab_cls / lab_logp
+        pairs) and, on the Bayesian grid, ml_logp, conf and the label slots lab_obj / lab_cls / lab_logp
         [nb,B^3,8] in the kernel's own order.  Unlike `dump_blocks`, nothing is derived or reordered."""
         spec = self._state_arrays()
         nb = self.num_blocks()
         d = {name: np.zeros((nb,) + shape, dt) for name, (dt, shape) in spec.items()}
         if nb:
+            keys4 = np.zeros((nb, 4), np.int32)
             ptrs = [d[name].ctypes.data if name in d else None for name in self._STATE_ARRAYS]
-            n = self._L.b2v_sgrid_export_blocks(self._h, d["keys"].ctypes.data, *ptrs)
+            n = self._L.b2v_sgrid_export_blocks(self._h, keys4.ctypes.data, *ptrs)
             if n != nb:
                 raise RuntimeError(f"b2v_sgrid_export_blocks returned {n}, expected {nb}: "
                                    f"{self._L.b2v_sgrid_last_error(self._h).decode()}")
+            d["keys"] = np.ascontiguousarray(keys4[:, :3])
         return d
 
     _export_state = export_blocks
@@ -1397,16 +1416,16 @@ class VoxelBlockSemanticGrid(_BlockGrid):
                              f"max_label_overflow_pairs ceiling of {have} chunks")
 
     def _upload_labels(self, keys, labels: dict) -> None:
-        n = len(keys)
+        n, keys4 = len(keys), _keys4(keys)
         arrs = [np.ascontiguousarray(labels[k]) for k in ("count", "obj", "cls", "logp")]
-        self._check(self._L.b2v_sgrid_upload_labels(self._h, n, np.ascontiguousarray(keys).ctypes.data if n else None,
+        self._check(self._L.b2v_sgrid_upload_labels(self._h, n, keys4.ctypes.data if n else None,
                                                     *[a.ctypes.data if a.size else None for a in arrs]),
                     "b2v_sgrid_upload_labels")
 
     def _upload_state(self, blocks: dict) -> None:
-        n = len(blocks["keys"])
+        n, keys4 = len(blocks["keys"]), _keys4(blocks["keys"])
         ptrs = [blocks[name].ctypes.data if name in blocks and n else None for name in self._STATE_ARRAYS]
-        self._check(self._L.b2v_sgrid_upload_blocks(self._h, n, blocks["keys"].ctypes.data if n else None, *ptrs),
+        self._check(self._L.b2v_sgrid_upload_blocks(self._h, n, keys4.ctypes.data if n else None, *ptrs),
                     "b2v_sgrid_upload_blocks")
 
     # ---- integrate (volumetric_grid_module.h: integrate(points, colors, class_ids, instance_ids, depths)) ----
@@ -1619,27 +1638,49 @@ class VoxelBlockSemanticGrid(_BlockGrid):
         return dict(zip(("used", "mapped", "max", "growths"), (int(x.value) for x in v)))
 
     def dump_blocks(self, K: int | None = None):
-        """Parity hook: per-block arrays [nb,B^3,...] incl. labels (see include/b2v.h).  K: label pairs per voxel in
-        the dump; None: the largest pair count of a voxel (at least 8)."""
+        """Parity hook: per-block arrays [nb,B^3,...] derived from `export_blocks` and `export_labels` - keys,
+        hashes (reference BlockKeyHash), count, pos_sum, col_sum, object_id, class_id, confidence (the Bayesian
+        `conf`; on the voting grid min(float32(counter) / float32(count), 1), 0 without points), aux (`counter`) and
+        lab_obj / lab_cls / lab_logp [nb,B^3,K]: a Bayesian voxel's label pairs, in-voxel slots then overflow chain,
+        stably sorted by (object, class), the first K, padded with (-1, -1, -inf).  K: None gives the largest pair
+        count of a voxel (at least 8)."""
+        raw = self.export_blocks()
+        nb, nv = raw["count"].shape
+        bayes = self.KIND == _lib.B2V_SEM_PROBABILISTIC
+        counter = raw["counter"]
         if K is None:
-            K = _lib.B2V_SEM_MAX_LABELS
-            if self.KIND == _lib.B2V_SEM_PROBABILISTIC and self.num_blocks():
-                K = max(K, int(self.export_blocks()["counter"].max()))
-        nb, nv = self.num_blocks(), self._block_voxels
-        d = dict(keys=np.zeros((nb, 3), np.int32), hashes=np.zeros(nb, np.uint64),
-                 count=np.zeros((nb, nv), np.int32), pos_sum=np.zeros((nb, nv, 3), np.float64),
-                 col_sum=np.zeros((nb, nv, 3), np.float32), object_id=np.zeros((nb, nv), np.int32),
-                 class_id=np.zeros((nb, nv), np.int32), confidence=np.zeros((nb, nv), np.float32),
-                 aux=np.zeros((nb, nv), np.int32), lab_obj=np.full((nb, nv, K), -1, np.int32),
-                 lab_cls=np.full((nb, nv, K), -1, np.int32), lab_logp=np.full((nb, nv, K), -np.inf, np.float32))
-        if nb:
-            n = self._L.b2v_sgrid_dump_blocks(
-                self._h, d["keys"].ctypes.data, d["hashes"].ctypes.data, d["count"].ctypes.data,
-                d["pos_sum"].ctypes.data, d["col_sum"].ctypes.data, d["object_id"].ctypes.data,
-                d["class_id"].ctypes.data, d["confidence"].ctypes.data, d["aux"].ctypes.data, int(K),
-                d["lab_obj"].ctypes.data, d["lab_cls"].ctypes.data, d["lab_logp"].ctypes.data)
-            if n != nb:
-                raise RuntimeError(f"b2v_sgrid_dump_blocks returned {n}, expected {nb}")
+            K = max(_lib.B2V_SEM_MAX_LABELS, int(counter.max()) if bayes and nb else 0)
+        if bayes:
+            confidence = raw["conf"]
+        else:
+            count = raw["count"]
+            with np.errstate(divide="ignore", invalid="ignore"):
+                ratio = counter.astype(np.float32) / count.astype(np.float32)
+            confidence = np.where(count != 0, np.minimum(ratio, np.float32(1)), np.float32(0)).astype(np.float32)
+        d = dict(keys=raw["keys"], hashes=_block_hashes(raw["keys"]), count=raw["count"],
+                 pos_sum=raw["pos_sum"], col_sum=raw["col_sum"], object_id=raw["object_id"],
+                 class_id=raw["class_id"], confidence=confidence, aux=counter,
+                 lab_obj=np.full((nb, nv, K), -1, np.int32), lab_cls=np.full((nb, nv, K), -1, np.int32),
+                 lab_logp=np.full((nb, nv, K), -np.inf, np.float32))
+        if bayes and K > 0 and nb:
+            # every pair with its voxel: the in-voxel slots in use, then the overflow pairs, each part in slot order
+            L = _lib.B2V_SEM_MAX_LABELS
+            slots = np.arange(L)[None, :] < np.minimum(counter.reshape(-1), L)[:, None]
+            vox = [np.nonzero(slots)[0]]
+            pairs = [[raw[name].reshape(-1, L)[slots]] for name in ("lab_obj", "lab_cls", "lab_logp")]
+            over = self._export_labels()
+            if over is not None:
+                vox.append(np.repeat(np.arange(nb * nv), over["count"].reshape(-1)))
+                for p, name in zip(pairs, ("obj", "cls", "logp")):
+                    p.append(over[name])
+            vox = np.concatenate(vox)
+            obj, cls, logp = (np.concatenate(p) for p in pairs)
+            order = np.lexsort((cls, obj, vox))   # stable: equal pairs keep slot order
+            vox, obj, cls, logp = vox[order], obj[order], cls[order], logp[order]
+            rank = np.arange(len(vox)) - np.searchsorted(vox, vox)   # position among the voxel's sorted pairs
+            keep = rank < K
+            for name, x in (("lab_obj", obj), ("lab_cls", cls), ("lab_logp", logp)):
+                d[name].reshape(nb * nv, K)[vox[keep], rank[keep]] = x[keep]
         return d
 
 
