@@ -26,18 +26,18 @@ VOXEL_PLANES = 5
 
 #: every symbol include/b2v.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
-    "b2v_create", "b2v_destroy", "b2v_reset", "b2v_last_error", "b2v_integrate",
-    "b2v_integrate_batch", "b2v_integrate_u16", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_capacity",
+    "b2v_create", "b2v_destroy", "b2v_reset", "b2v_last_error",
+    "b2v_integrate_batch", "b2v_integrate_batch_u16", "b2v_synchronize", "b2v_capacity",
     "b2v_num_blocks", "b2v_last_frame_stats", "b2v_last_mesh_stats",
     "b2v_counters", "b2v_set_overlap", "b2v_set_fusion", "b2v_set_group_size", "b2v_set_input_event", "b2v_set_rectification", "b2v_remap", "b2v_profile_enable", "b2v_profile_read", "b2v_export_blocks", "b2v_upload_blocks", "b2v_last_touched_keys", "b2v_block_key_hashes", "b2v_extract_mesh", "b2v_copy_mesh",
-    "b2v_extract_points", "b2v_copy_points", "b2v_export_halo_device", "b2v_extract_mesh_with_halo",
-    "b2v_extract_points_with_halo", "b2v_weld_mesh_device", "b2v_weld_last_error", "b2v_grid_create", "b2v_grid_create_ex", "b2v_grid_capacity",
+    "b2v_extract_points", "b2v_export_halo_device", "b2v_extract_mesh_with_halo",
+    "b2v_extract_points_with_halo", "b2v_weld_mesh_device", "b2v_weld_last_error", "b2v_grid_create_ex", "b2v_grid_capacity",
     "b2v_grid_destroy", "b2v_grid_clear",
-    "b2v_grid_last_error", "b2v_grid_integrate", "b2v_grid_integrate_f64", "b2v_grid_integrate_ex", "b2v_grid_integrate_rgbd", "b2v_filter_shadow_points", "b2v_grid_synchronize", "b2v_grid_num_blocks",
+    "b2v_grid_last_error", "b2v_grid_integrate_ex", "b2v_grid_integrate_rgbd", "b2v_filter_shadow_points", "b2v_grid_synchronize", "b2v_grid_num_blocks",
     "b2v_grid_size", "b2v_grid_get_voxels", "b2v_grid_copy_voxels",
     "b2v_grid_remove_low_count_voxels", "b2v_grid_export_blocks", "b2v_grid_carve",
     "b2v_grid_get_voxels_in_frustum", "b2v_grid_get_voxels_in_bb", "b2v_version", "b2v_device_sm_count", "b2v_selftest_division",
-    "b2v_sgrid_create", "b2v_sgrid_create_ex", "b2v_sgrid_capacity", "b2v_sgrid_destroy", "b2v_sgrid_last_error", "b2v_sgrid_clear",
+    "b2v_sgrid_create_ex", "b2v_sgrid_capacity", "b2v_sgrid_destroy", "b2v_sgrid_last_error", "b2v_sgrid_clear",
     "b2v_sgrid_set_depth_threshold", "b2v_sgrid_set_depth_decay_rate", "b2v_sgrid_integrate",
     "b2v_sgrid_integrate_rgbd",
     "b2v_sgrid_num_blocks", "b2v_sgrid_get_voxels", "b2v_sgrid_copy_voxels", "b2v_sgrid_get_voxels_in_bb",
@@ -115,8 +115,6 @@ def load() -> C.CDLL:
     L.b2v_reset.argtypes = [vp]
     L.b2v_last_error.restype = C.c_char_p
     L.b2v_last_error.argtypes = [vp]
-    L.b2v_integrate.restype = C.c_int
-    L.b2v_integrate.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp]
     L.b2v_integrate_batch.restype = C.c_int
     L.b2v_integrate_batch.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp]
     L.b2v_synchronize.restype = C.c_int
@@ -137,8 +135,6 @@ def load() -> C.CDLL:
     L.b2v_profile_enable.argtypes = [vp, i32]
     L.b2v_profile_read.restype = C.c_int
     L.b2v_profile_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), p_i64, p_i64]
-    L.b2v_sgrid_create.restype = C.c_int
-    L.b2v_sgrid_create.argtypes = [C.c_double, i32, C.c_uint32, i32, i32, C.POINTER(vp)]
     L.b2v_sgrid_create_ex.restype = C.c_int
     L.b2v_sgrid_create_ex.argtypes = [C.c_double, i32, C.c_uint32, C.c_uint32, i32, i32, C.POINTER(vp)]
     L.b2v_sgrid_capacity.restype = C.c_int
@@ -190,8 +186,6 @@ def load() -> C.CDLL:
     L.b2v_sgrid_export_labels.argtypes = [vp] * 5
     L.b2v_sgrid_upload_labels.restype = C.c_int
     L.b2v_sgrid_upload_labels.argtypes = [vp, i64] + [vp] * 5
-    L.b2v_integrate_u16.restype = C.c_int
-    L.b2v_integrate_u16.argtypes = [vp, vp, C.c_float, vp, i32, i32, vp, vp, vp]
     L.b2v_integrate_batch_u16.restype = C.c_int
     L.b2v_integrate_batch_u16.argtypes = [vp, i32, vp, C.c_float, vp, i32, i32, vp, vp, vp]
     L.b2v_set_rectification.restype = C.c_int
@@ -218,8 +212,6 @@ def load() -> C.CDLL:
     L.b2v_copy_mesh.argtypes = [vp, vp, vp, vp, vp]
     L.b2v_extract_points.restype = C.c_int
     L.b2v_extract_points.argtypes = [vp, p_i64]
-    L.b2v_copy_points.restype = C.c_int
-    L.b2v_copy_points.argtypes = [vp, vp, vp]
     L.b2v_export_halo_device.restype = C.c_int
     L.b2v_export_halo_device.argtypes = [vp, i32, vp, vp, vp, vp, i64, i64]
     L.b2v_extract_mesh_with_halo.restype = C.c_int
@@ -231,8 +223,6 @@ def load() -> C.CDLL:
     L.b2v_weld_last_error.restype = C.c_char_p
     L.b2v_weld_last_error.argtypes = []
 
-    L.b2v_grid_create.restype = C.c_int
-    L.b2v_grid_create.argtypes = [C.c_float, i32, u32, i32, C.POINTER(vp)]
     L.b2v_grid_create_ex.restype = C.c_int
     L.b2v_grid_create_ex.argtypes = [C.c_float, i32, u32, u32, i32, C.POINTER(vp)]
     L.b2v_grid_capacity.restype = C.c_int
@@ -243,10 +233,6 @@ def load() -> C.CDLL:
     L.b2v_grid_clear.argtypes = [vp]
     L.b2v_grid_last_error.restype = C.c_char_p
     L.b2v_grid_last_error.argtypes = [vp]
-    L.b2v_grid_integrate.restype = C.c_int
-    L.b2v_grid_integrate.argtypes = [vp, vp, vp, i64]
-    L.b2v_grid_integrate_f64.restype = C.c_int
-    L.b2v_grid_integrate_f64.argtypes = [vp, vp, vp, i64]
     L.b2v_grid_integrate_ex.restype = C.c_int
     L.b2v_grid_integrate_ex.argtypes = [vp, vp, i32, vp, i32, i64]
     L.b2v_grid_set_input_order_sums.restype = C.c_int

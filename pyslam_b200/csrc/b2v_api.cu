@@ -137,9 +137,8 @@ struct b2v_volume {
     // TMA descriptors are cached per image address (encoding costs ~1 us of host time each)
     std::unordered_map<uintptr_t, FrameMaps> map_cache;
     int map_H = 0, map_W = 0;
-    // raw 16-bit depth input (b2v_integrate_u16 / b2v_integrate_batch_u16): uploaded as is, widened on the device
+    // raw 16-bit depth input (b2v_integrate_batch_u16): uploaded as is, widened on the device
     DeviceBuffer<uint16_t> d_depth16;   // same slots as d_depth; allocated on first use
-    float in_u16_scale = 0.0f;          // > 0 while a *_u16 entry point runs: `depth` pointers are uint16_t
     DeviceBuffer<float> d_depth;        // staging of host frames (and of widened uint16 depth), see stage_slot
     DeviceBuffer<uint8_t> d_color;
     DeviceBuffer<Texel> d_tex;      // texel images, written by the allocate kernels and read by the update kernels
@@ -329,7 +328,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 110; }
+extern "C" int b2v_version(void) { return 111; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -720,10 +719,13 @@ static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d
 
 // Enqueues n_frames frames, contiguous in the caller's arrays, as groups in the group buffers: groups of up to
 // group_frames frames on the fused kernels when fusion is on and there are two frames or more, else groups of one
-// frame on the frame-by-frame kernels.  inputs_ready: an event after which device frames are ready, or nullptr.
-static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, const float *depth, const uint8_t *color,
-                          int32_t height, int32_t width, const double K[4], const double *Tcw, void *stream,
-                          cudaEvent_t inputs_ready) {
+// frame on the frame-by-frame kernels.  depth is float32 metres (u16_scale = 0) or raw uint16 widened on the device
+// to float32(depth) * u16_scale (u16_scale > 0).  Consumes the input event of b2v_set_input_event.
+static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, const void *depth, float u16_scale,
+                          const uint8_t *color, int32_t height, int32_t width, const double K[4], const double *Tcw,
+                          void *stream) {
+    const cudaEvent_t inputs_ready = v->input_event;  // one-shot: consumed by bad arguments too
+    v->input_event = nullptr;
     if (n_frames < 0 || (n_frames > 0 && (!depth || !color || !Tcw || !K)) || height <= 0 || width <= 0) {
         v->err = std::string(what) + ": bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
@@ -742,8 +744,9 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
     }
     cudaStream_t cs = stream ? static_cast<cudaStream_t>(stream) : v->compute;
     cudaStream_t as = v->overlap ? v->alloc : cs;  // stream of the allocate kernels
-    const bool u16 = v->in_u16_scale > 0.0f;       // `depth` is really const uint16_t *
-    const uint16_t *depth16 = reinterpret_cast<const uint16_t *>(depth);
+    const bool u16 = u16_scale > 0.0f;
+    const float *depth32 = static_cast<const float *>(depth);
+    const uint16_t *depth16 = static_cast<const uint16_t *>(depth);
     {
         int rc = ensure_staging(v, pixels);
         if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
@@ -812,7 +815,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
                 B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_depth16, pixels, s0), depth16 + pixels * g0,
                                             pixels * sizeof(uint16_t) * count, cudaMemcpyHostToDevice, v->copy));
             else if (!dev_depth)
-                B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_depth, pixels, s0), depth + pixels * g0,
+                B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_depth, pixels, s0), depth32 + pixels * g0,
                                             pixels * sizeof(float) * count, cudaMemcpyHostToDevice, v->copy));
             if (!dev_color)
                 B2V_CUDA(v, cudaMemcpyAsync(stage_slot(v->d_color, pixels * 3, s0), color + pixels * 3 * g0,
@@ -823,7 +826,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         if (u16) {  // widen the group's raw depth into its (contiguous) float staging slots in one launch
             const uint16_t *src = dev_depth ? depth16 + pixels * g0 : stage_slot(v->d_depth16, pixels, s0);
             B2V_CUDA(v, launch_depth_u16_to_f32(src, stage_slot(v->d_depth, pixels, s0), pixels * count,
-                                                v->in_u16_scale, as));
+                                                u16_scale, as));
             v->launches += 1;
         }
         static thread_local GroupAllocArgs aargs;  // ~15 KB: keep it off the stack
@@ -836,7 +839,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         for (int k = 0; k < count; ++k) {
             const size_t f = static_cast<size_t>(g0 + k);
             // (widened) staging
-            const float *d_depth = dev_depth && !u16 ? depth + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
+            const float *d_depth = dev_depth && !u16 ? depth32 + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
             const uint8_t *d_color = dev_color ? color + pixels * 3 * f : stage_slot(v->d_color, pixels * 3, s0 + k);
             Texel *tex = stage_slot(v->d_tex, texel_pitch(pixels), s0 + k);
             const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s0 + k, as);
@@ -893,22 +896,11 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
     return B2V_OK;
 }
 
-extern "C" int b2v_integrate(b2v_volume *v, const float *depth, const uint8_t *color, int32_t height,
-                             int32_t width, const double K[4], const double Tcw[16], void *stream) {
-    if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    cudaEvent_t inputs_ready = v->input_event;  // one-shot
-    v->input_event = nullptr;
-    return enqueue_frames(v, "b2v_integrate", 1, depth, color, height, width, K, Tcw, stream, inputs_ready);
-}
-
 extern "C" int b2v_integrate_batch(b2v_volume *v, int32_t n_frames, const float *depth,
                                    const uint8_t *color, int32_t height, int32_t width,
                                    const double K[4], const double *Tcw, void *stream) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    cudaEvent_t inputs_ready = v->input_event;  // one-shot
-    v->input_event = nullptr;
-    return enqueue_frames(v, "b2v_integrate_batch", n_frames, depth, color, height, width, K, Tcw, stream,
-                          inputs_ready);
+    return enqueue_frames(v, "b2v_integrate_batch", n_frames, depth, 0.0f, color, height, width, K, Tcw, stream);
 }
 
 // Raw 16-bit depth (e.g. TUM / ScanNet PNGs): uploaded as uint16 (2 instead of 4 bytes per pixel over PCIe) and
@@ -922,25 +914,8 @@ extern "C" int b2v_integrate_batch_u16(b2v_volume *v, int32_t n_frames, const ui
         v->err = "b2v_integrate_batch_u16: depth_scale must be positive";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    v->in_u16_scale = depth_scale;
-    const int rc = b2v_integrate_batch(v, n_frames, reinterpret_cast<const float *>(depth), color, height, width, K,
-                                       Tcw, stream);
-    v->in_u16_scale = 0.0f;
-    return rc;
-}
-
-extern "C" int b2v_integrate_u16(b2v_volume *v, const uint16_t *depth, float depth_scale, const uint8_t *color,
-                                 int32_t height, int32_t width, const double K[4], const double Tcw[16],
-                                 void *stream) {
-    if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    if (!(depth_scale > 0.0f)) {
-        v->err = "b2v_integrate_u16: depth_scale must be positive";
-        return B2V_ERR_INVALID_ARGUMENT;
-    }
-    v->in_u16_scale = depth_scale;
-    const int rc = b2v_integrate(v, reinterpret_cast<const float *>(depth), color, height, width, K, Tcw, stream);
-    v->in_u16_scale = 0.0f;
-    return rc;
+    return enqueue_frames(v, "b2v_integrate_batch_u16", n_frames, depth, depth_scale, color, height, width, K, Tcw,
+                          stream);
 }
 
 extern "C" int b2v_set_input_event(b2v_volume *v, void *event) {
@@ -1267,10 +1242,6 @@ extern "C" int b2v_copy_mesh(b2v_volume *v, double *vertices, double *colors, in
 extern "C" int b2v_extract_points(b2v_volume *v, int64_t *n_points) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
     return extract_common(v, false, n_points, nullptr);
-}
-
-extern "C" int b2v_copy_points(b2v_volume *v, double *points, double *colors) {
-    return b2v_copy_mesh(v, points, colors, nullptr, nullptr);
 }
 
 // ---- sharded extraction: face-halo exchange (b2v_shard.cu) --------------------------------------------------------

@@ -881,17 +881,20 @@ static bool grid_map_storage(b2v_grid *g, uint64_t blocks, std::string *err) {
     return ok;
 }
 
+// the storage growth of BlockGridCore::resolve / upload_blocks
+static auto grid_grow_storage(b2v_grid *g) {
+    return [g](uint64_t blocks) {
+        std::string map_err;   // a failed mapping surfaces as "block pool full"
+        grid_map_storage(g, blocks, &map_err);
+    };
+}
+
 static int grid_clear_device(b2v_grid *g, uint32_t used_blocks) {
     const int rc = g->clear_index();
     if (rc != B2V_OK) return rc;
     B2V_CUDA(g, cudaMemsetAsync(reinterpret_cast<void *>(g->pool.va), 0, static_cast<size_t>(used_blocks) * g->block_bytes(),
                                 g->stream));
     return B2V_OK;
-}
-
-extern "C" int b2v_grid_create(float voxel_size, int32_t block_size, uint32_t capacity_blocks,
-                               int32_t device, b2v_grid **out) {
-    return b2v_grid_create_ex(voxel_size, block_size, capacity_blocks, 0, device, out);
 }
 
 extern "C" int b2v_grid_create_ex(float voxel_size, int32_t block_size, uint32_t capacity_blocks,
@@ -1022,18 +1025,20 @@ static cudaError_t grid_sum_in_order(b2v_grid *g, const void *pts, bool pts_f64,
     return grid_sum_in_order_t(g, static_cast<const float *>(pts), cols, cols_u8, valid, n, lo, hi);
 }
 
-static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const void *colors, bool u8, int64_t n_points) {
+extern "C" int b2v_grid_integrate_ex(b2v_grid *g, const void *points, int32_t points_f64, const void *colors,
+                                     int32_t colors_u8, int64_t n_points) {
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     if (n_points < 0 || (n_points > 0 && !points)) {
-        g->err = "b2v_grid_integrate: bad arguments";
+        g->err = "b2v_grid_integrate_ex: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     if (g->input_order && n_points > kMaxOrderedPoints) {
-        g->err = "b2v_grid_integrate: more than 0x7FFFFFF0 points in one call with input-order sums";
+        g->err = "b2v_grid_integrate_ex: more than 0x7FFFFFF0 points in one call with input-order sums";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     if (n_points == 0) return B2V_OK;  // voxel_block_grid.hpp:22-24,121-123
     B2V_CUDA(g, cudaSetDevice(g->device));
+    const bool f64 = points_f64 != 0, u8 = colors_u8 != 0;
     if (g->input_order) {
         const int rc = grid_reserve_ordered(g, static_cast<size_t>(n_points), false);
         if (rc != B2V_OK) return rc;
@@ -1068,28 +1073,10 @@ static int grid_integrate_any(b2v_grid *g, const void *points, bool f64, const v
     };
     B2V_CUDA(g, pass(0u, g->index.pool_capacity));
     if (!g->growable) return B2V_OK;
-    return g->resolve(
-        [&](uint64_t blocks) {
-            std::string map_err;   // a failed mapping surfaces as "block pool full"
-            grid_map_storage(g, blocks, &map_err);
-        },
-        [&](uint32_t lo, uint32_t hi) {
-            B2V_CUDA(g, pass(lo, hi));
-            return B2V_OK;
-        });
-}
-
-extern "C" int b2v_grid_integrate(b2v_grid *g, const float *points, const float *colors, int64_t n_points) {
-    return grid_integrate_any(g, points, false, colors, false, n_points);
-}
-
-extern "C" int b2v_grid_integrate_f64(b2v_grid *g, const double *points, const float *colors, int64_t n_points) {
-    return grid_integrate_any(g, points, true, colors, false, n_points);
-}
-
-extern "C" int b2v_grid_integrate_ex(b2v_grid *g, const void *points, int32_t points_f64, const void *colors,
-                                     int32_t colors_u8, int64_t n_points) {
-    return grid_integrate_any(g, points, points_f64 != 0, colors, colors_u8 != 0, n_points);
+    return g->resolve(grid_grow_storage(g), [&](uint32_t lo, uint32_t hi) {
+        B2V_CUDA(g, pass(lo, hi));
+        return B2V_OK;
+    });
 }
 
 extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const uint8_t *color, int32_t height,
@@ -1111,7 +1098,7 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
     int rc = g->stage_input("b2v_grid_integrate_rgbd", height, width, filter_shadow_points != 0, &d_depth, &d_color);
     if (rc != B2V_OK) return rc;
     const RgbdParams P = rgbd_params(K, Twc, min_depth, max_depth, height, width);
-    if (g->input_order) {   // point records -> the input-order path of b2v_grid_integrate
+    if (g->input_order) {   // point records -> the input-order path of b2v_grid_integrate_ex
         rc = grid_reserve_ordered(g, static_cast<size_t>(n), true);
         if (rc != B2V_OK) return rc;
         const float *pts = g->d_rec_pts.get(), *cols = g->d_rec_cols.get();
@@ -1123,15 +1110,10 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
                                         g->stream));
         B2V_CUDA(g, grid_sum_in_order(g, pts, false, cols, false, valid, n, 0u, g->index.pool_capacity));
         if (!g->growable) return B2V_OK;
-        return g->resolve(
-            [&](uint64_t blocks) {
-                std::string map_err;   // a failed mapping surfaces as "block pool full"
-                grid_map_storage(g, blocks, &map_err);
-            },
-            [&](uint32_t lo, uint32_t hi) {
-                B2V_CUDA(g, grid_sum_in_order(g, pts, false, cols, false, valid, n, lo, hi));
-                return B2V_OK;
-            });
+        return g->resolve(grid_grow_storage(g), [&](uint32_t lo, uint32_t hi) {
+            B2V_CUDA(g, grid_sum_in_order(g, pts, false, cols, false, valid, n, lo, hi));
+            return B2V_OK;
+        });
     }
     const unsigned grid = static_cast<unsigned>((static_cast<size_t>(height) * width + 255) / 256);
     auto accumulate = [&](uint32_t lo, uint32_t hi) {
@@ -1147,16 +1129,11 @@ extern "C" int b2v_grid_integrate_rgbd(b2v_grid *g, const float *depth, const ui
     accumulate(0u, g->index.pool_capacity);
     B2V_CUDA(g, cudaGetLastError());
     if (!g->growable) return B2V_OK;
-    return g->resolve(
-        [&](uint64_t blocks) {
-            std::string map_err;   // a failed mapping surfaces as "block pool full"
-            grid_map_storage(g, blocks, &map_err);
-        },
-        [&](uint32_t lo, uint32_t hi) {
-            accumulate(lo, hi);
-            B2V_CUDA(g, cudaGetLastError());
-            return B2V_OK;
-        });
+    return g->resolve(grid_grow_storage(g), [&](uint32_t lo, uint32_t hi) {
+        accumulate(lo, hi);
+        B2V_CUDA(g, cudaGetLastError());
+        return B2V_OK;
+    });
 }
 
 extern "C" int b2v_grid_set_rectification(b2v_grid *g, const float *map_x, const float *map_y, int32_t height,
@@ -1308,12 +1285,8 @@ extern "C" int b2v_grid_upload_blocks(b2v_grid *g, int64_t n_blocks, const int32
     a.dst[0] = reinterpret_cast<void *>(g->pool.va);
     a.src[0] = blocks;
     a.block_bytes[0] = static_cast<uint32_t>(g->block_bytes());
-    const int rc = g->upload_blocks(
-        n_blocks, keys4, a,
-        [&](uint64_t storage_blocks) {
-            std::string map_err;   // a failed mapping surfaces as "block pool full"
-            grid_map_storage(g, storage_blocks, &map_err);
-        },
-        [](uint32_t, uint32_t) { return B2V_OK; });   // new storage is mapped zeroed: the cleared state of a voxel
+    // new storage is mapped zeroed, which is the cleared state of a voxel: nothing to fill
+    const int rc = g->upload_blocks(n_blocks, keys4, a, grid_grow_storage(g),
+                                    [](uint32_t, uint32_t) { return B2V_OK; });
     return rc == B2V_OK ? g->read_counters() : rc;
 }

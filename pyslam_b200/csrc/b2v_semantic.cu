@@ -957,9 +957,12 @@ static bool sgrid_map_storage(b2v_sgrid *g, uint64_t blocks, std::string *err) {
     return ok;
 }
 
-extern "C" int b2v_sgrid_create(double voxel_size, int32_t block_size, uint32_t capacity_blocks, int32_t kind,
-                                int32_t device, b2v_sgrid **out) {
-    return b2v_sgrid_create_ex(voxel_size, block_size, capacity_blocks, 0, kind, device, out);
+// the storage growth of BlockGridCore::resolve / upload_blocks
+static auto sgrid_grow_storage(b2v_sgrid *g) {
+    return [g](uint64_t blocks) {
+        std::string map_err;   // a failed mapping surfaces as "block pool full"
+        sgrid_map_storage(g, blocks, &map_err);
+    };
 }
 
 extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32_t capacity_blocks,
@@ -1189,17 +1192,12 @@ static int sgrid_fuse_staged(b2v_sgrid *g, int64_t n, const SemInputs &in, const
                                     g->index, g->stream));
     const int rc = sgrid_apply(g, n, in, valid, 0, g->index.pool_capacity);
     if (rc != B2V_OK || !g->growable) return rc;
-    return g->resolve(
-        [&](uint64_t blocks) {
-            std::string map_err;   // a failed mapping surfaces as "block pool full"
-            sgrid_map_storage(g, blocks, &map_err);
-        },
-        [&](uint32_t lo, uint32_t hi) {
-            sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
-                                                        static_cast<size_t>(hi) * g->block_voxels());
-            B2V_CUDA(g, cudaGetLastError());
-            return sgrid_apply(g, n, in, valid, lo, hi);
-        });
+    return g->resolve(sgrid_grow_storage(g), [&](uint32_t lo, uint32_t hi) {
+        sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
+                                                    static_cast<size_t>(hi) * g->block_voxels());
+        B2V_CUDA(g, cudaGetLastError());
+        return sgrid_apply(g, n, in, valid, lo, hi);
+    });
 }
 
 // end of an integrate call: the counters, then B2V_ERR_CUDA if the label storage failed to grow, or "label storage
@@ -1777,18 +1775,13 @@ extern "C" int b2v_sgrid_upload_blocks(b2v_sgrid *g, int64_t n_blocks, const int
         a.src[k] = in[k];
         a.block_bytes[k] = static_cast<uint32_t>(arr[k].voxel_bytes * g->block_voxels());
     }
-    int rc = g->upload_blocks(
-        n_blocks, keys4, a,
-        [&](uint64_t blocks) {
-            std::string map_err;   // a failed mapping surfaces as "block pool full"
-            sgrid_map_storage(g, blocks, &map_err);
-        },
-        [&](uint32_t lo, uint32_t hi) {   // the cleared state for the voxels that just got storage
-            sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
-                                                        static_cast<size_t>(hi) * g->block_voxels());
-            B2V_CUDA(g, cudaGetLastError());
-            return B2V_OK;
-        });
+    int rc = g->upload_blocks(n_blocks, keys4, a, sgrid_grow_storage(g), [&](uint32_t lo, uint32_t hi) {
+        // the cleared state for the voxels that just got storage
+        sem_fill_kernel<<<592, 256, 0, g->stream>>>(g->dev(), static_cast<size_t>(lo) * g->block_voxels(),
+                                                    static_cast<size_t>(hi) * g->block_voxels());
+        B2V_CUDA(g, cudaGetLastError());
+        return B2V_OK;
+    });
     if (rc != B2V_OK) return rc;
     if (g->lab_max_chunks) {   // the uploaded voxels hold their in-voxel pairs only until b2v_sgrid_upload_labels
         rc = sgrid_set_labels(g, "b2v_sgrid_upload_blocks", n_blocks, keys4, nullptr, nullptr, nullptr, nullptr);

@@ -295,13 +295,13 @@ class B200TsdfVolume(_MapState):
             dp, cp = d.ctypes.data, c.ctypes.data
             depth, color = d, c
             if raw16:
-                self._enqueue("b2v_integrate_u16", self._L.b2v_integrate_u16,
-                              (dp, float(depth_scale), cp, H, W, K4.ctypes.data, T.ctypes.data, None), (d, c), None)
+                self._enqueue("b2v_integrate_batch_u16", self._L.b2v_integrate_batch_u16,
+                              (1, dp, float(depth_scale), cp, H, W, K4.ctypes.data, T.ctypes.data, None), (d, c), None)
                 return
         if depth_scale is not None:
             raise RuntimeError("depth_scale is supported for host (numpy) uint16 depth images")
-        self._enqueue("b2v_integrate", self._L.b2v_integrate,
-                      (dp, cp, H, W, K4.ctypes.data, T.ctypes.data, C.c_void_p(stream) if stream else None),
+        self._enqueue("b2v_integrate_batch", self._L.b2v_integrate_batch,
+                      (1, dp, cp, H, W, K4.ctypes.data, T.ctypes.data, C.c_void_p(stream) if stream else None),
                       (depth, color), stream)
 
     def integrate_batch(self, depths, colors, K, poses, stream=None, depth_scale=None):
@@ -524,13 +524,7 @@ class B200TsdfVolume(_MapState):
         """north_star `extract_mesh()` == Open3D `extract_triangle_mesh()` (tsdf.py:239,260)."""
         nv, nt = C.c_int64(0), C.c_int64(0)
         self._check(self._L.b2v_extract_mesh(self._h, C.byref(nv), C.byref(nt)), "b2v_extract_mesh")
-        V = np.zeros((nv.value, 3), np.float64)   # float64 like Open3D's TriangleMesh, computed in float64
-        Cc = np.zeros((nv.value, 3), np.float64)
-        E = np.zeros((nv.value, 4), np.int32)
-        T = np.zeros((nt.value, 3), np.int32)
-        self._check(self._L.b2v_copy_mesh(self._h, V.ctypes.data, Cc.ctypes.data, E.ctypes.data,
-                                          T.ctypes.data), "b2v_copy_mesh")
-        return TriangleMesh(V, T, Cc, E)
+        return self._copy_mesh(nv.value, nt.value)
 
     extract_triangle_mesh = extract_mesh
 
@@ -580,6 +574,7 @@ class B200TsdfVolume(_MapState):
         return PointCloud(m.vertices, m.vertex_colors, m.edge_ids)
 
     def _copy_mesh(self, nv: int, nt: int) -> TriangleMesh:
+        """The result of the last extraction (b2v_copy_mesh), float64 like Open3D's TriangleMesh."""
         V = np.zeros((nv, 3), np.float64)
         Cc = np.zeros((nv, 3), np.float64)
         E = np.zeros((nv, 4), np.int32)
@@ -591,10 +586,8 @@ class B200TsdfVolume(_MapState):
     def extract_point_cloud(self) -> PointCloud:
         n = C.c_int64(0)
         self._check(self._L.b2v_extract_points(self._h, C.byref(n)), "b2v_extract_points")
-        P = np.zeros((n.value, 3), np.float64)
-        Cc = np.zeros((n.value, 3), np.float64)
-        self._check(self._L.b2v_copy_points(self._h, P.ctypes.data, Cc.ctypes.data), "b2v_copy_points")
-        return PointCloud(P, Cc)
+        m = self._copy_mesh(n.value, 0)
+        return PointCloud(m.vertices, m.vertex_colors, m.edge_ids)
 
 
 def filter_shadow_points(depth, delta_depth=None, delta_x=2, delta_y=2, fill_value=-1, device=0):
@@ -1023,7 +1016,7 @@ class VoxelBlockGrid(_BlockGrid):
         pts, cols, cu8 = self._points_colors(points, colors)
         self._check(self._L.b2v_grid_integrate_ex(self._h, pts.ctypes.data, 1 if pts.dtype == np.float64 else 0,
                                                   None if cols is None else cols.ctypes.data, cu8, pts.shape[0]),
-                    "b2v_grid_integrate")
+                    "b2v_grid_integrate_ex")
         self._check(self._L.b2v_grid_synchronize(self._h), "b2v_grid_synchronize")
 
     def integrate_rgbd(self, depth, color, K, Twc, max_depth=np.inf, min_depth=0.0, filter_shadow_points=False):
