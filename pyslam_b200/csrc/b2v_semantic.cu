@@ -1902,10 +1902,14 @@ static int sgrid_set_labels(b2v_sgrid *g, const char *fn, int64_t n_blocks, cons
                 c.logp[e % kChunkPairs] = logp[pos];
             }
         }
-    std::string map_err;
-    if (h.chunks.size() > g->lab_mapped && !sgrid_map_labels(g, h.chunks.size(), &map_err)) {
-        g->err = std::string(fn) + ": label storage could not grow: " + map_err;
-        return B2V_ERR_CUDA;
+    if (h.chunks.size() > g->lab_mapped) {   // a growth of the chunk storage, counted as the runs' growths are
+        const uint32_t old = g->lab_mapped;
+        std::string map_err;
+        if (!sgrid_map_labels(g, h.chunks.size(), &map_err)) {
+            g->err = std::string(fn) + ": label storage could not grow: " + map_err;
+            return B2V_ERR_CUDA;
+        }
+        if (g->lab_mapped > old) ++g->lab_growths;
     }
     h.ctr[kLcFree] = static_cast<uint32_t>(h.free_list.size());
     h.ctr[kLcFresh] = static_cast<uint32_t>(h.chunks.size());
