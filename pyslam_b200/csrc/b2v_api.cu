@@ -44,9 +44,11 @@ void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], 
                            p->pose.Rwc[3 * i + 2] * Tcw[11]);
     p->tau_d = g.unit_shift > 0 ? g.tau_d : static_cast<double>(g.tau);
     p->unit_len = g.voxel_length * static_cast<double>(kB << g.unit_shift);
-    IntFrame &I = p->I;
-    for (int i = 0; i < 12; ++i) I.E[i] = static_cast<float>(Tcw[i]);
-    for (int i = 0; i < 3; ++i) I.Es[i] = I.E[4 * i + 2] * g.vs;  // extrinsic_f * voxel_length_f, column 2
+    IntPose &E = p->E;
+    for (int i = 0; i < 12; ++i) E.E[i] = static_cast<float>(Tcw[i]);
+    for (int i = 0; i < 3; ++i) E.Es[i] = E.E[4 * i + 2] * g.vs;  // extrinsic_f * voxel_length_f, column 2
+    E.pad = 0.0f;
+    IntConsts &I = p->I;
     I.fxf = static_cast<float>(K[0]);
     I.fyf = static_cast<float>(K[1]);
     I.cxf = static_cast<float>(K[2]);
@@ -59,6 +61,7 @@ void fill_frame_params(FrameParams *p, const double K[4], const double Tcw[16], 
     I.pixels = W * H;
     I.tex = nullptr;
     I.lam = nullptr;
+    I.tex_pitch = 0;
     p->inv_fx = 1.0f / I.fxf;
     p->inv_fy = 1.0f / I.fyf;
     p->inv_vs = 1.0f / g.vs;  // voxel_block_grid.hpp:6
@@ -508,7 +511,7 @@ static int drain_and_copy_counters(b2v_volume *v) {
 static int launch_group_update(b2v_volume *v, int buf, cudaStream_t cs) {
     const GroupArgs &a = v->gargs[buf];
     B2V_CUDA(v, v->gfused[buf] ? launch_integrate_group(a, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs)
-                               : launch_integrate(a.f[0], a.V, v->table, v->meta, buf, v->grid_ctas, cs));
+                               : launch_integrate(a, v->table, v->meta, buf, v->grid_ctas, cs));
     v->launches += v->gfused[buf] ? 2 : 1;  // update (+ the mask clear of a fused group)
     return B2V_OK;
 }
@@ -847,16 +850,20 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             FrameParams P;
             fill_frame_params(&P, K, Tcw + 16 * f, height, width, v->geo);
             P.group_buf = buf;
-            P.I.tex = tex;
-            P.I.lam = v->d_lambda.get();
-            if (k == 0) aargs.P = P;
+            if (k == 0) {  // the update constants of frame 0 serve the group: one set of intrinsics per call
+                P.I.tex = tex;
+                P.I.lam = v->d_lambda.get();
+                P.I.tex_pitch = static_cast<int64_t>(texel_pitch(pixels));
+                args.C = P.I;
+                aargs.P = P;
+            }
             aargs.pose[k] = P.pose;
             aargs.depth[k] = d_depth;
             aargs.color[k] = d_color;
             aargs.tex[k] = tex;
             const FrameMaps *fm = frame_maps(v, d_depth, d_color, height, width);
             if (fm) aargs.maps[k] = *fm; else aargs.use_tma = 0;
-            args.f[k] = P.I;
+            args.f[k] = P.E;
         }
         cudaEvent_t *pe = nullptr;
         if (v->prof_enabled) {

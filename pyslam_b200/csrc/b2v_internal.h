@@ -104,19 +104,26 @@ __device__ __forceinline__ float texel_channel(const Texel &t, int c) {
     return __fsub_rn(__uint_as_float(__byte_perm(t.rgb, 0x4B000000u, 0x7440u + c)), 8388608.0f);
 }
 
-// Constants of the projective update of one frame (Open3D UniformTSDFVolume::IntegrateWithDepthToCameraDistance-
-// Multiplier): passed in kernel-parameter space, so the kernels read them as constant-bank operands.
-struct IntFrame {
-    float E[12];     // Tcw rows 0..2 as float32 (extrinsic.cast<float>())
-    float Es[3];     // E[2], E[6], E[10] times voxel_length_f (extrinsic_scaled_f(:, 2)): the per-z-step increment
+// Constants of the projective update (Open3D UniformTSDFVolume::IntegrateWithDepthToCameraDistanceMultiplier), split
+// into what the frames of a group share and what each frame has of its own.  The shared part sits in kernel-parameter
+// space at fixed offsets, so the kernels read it as constant-bank operands.
+struct IntConsts {
     float fxf, fyf, cxf, cyf;
     float safe_w, safe_h;   // W - 0.0001f, H - 0.0001f
     float tau, inv_tau;
     int32_t W;
     int32_t pixels;         // W * H: the index that voxels projecting outside the image gather (see below)
-    const Texel *tex;       // texels of the frame
-    const float *lam;       // lambda image of the frame's intrinsics, same pixel index as tex
+    const Texel *tex;       // texels of frame 0 of the group; frame k's start k * tex_pitch texels later
+    const float *lam;       // lambda image of the intrinsics, same pixel index as the texels
+    int64_t tex_pitch;
 };
+// The camera pose of one frame, 64 bytes: a frame step reads it with four 16-byte loads.
+struct alignas(16) IntPose {
+    float E[12];     // Tcw rows 0..2 as float32 (extrinsic.cast<float>())
+    float Es[3];     // E[2], E[6], E[10] times voxel_length_f (extrinsic_scaled_f(:, 2)): the per-z-step increment
+    float pad;
+};
+static_assert(sizeof(IntPose) == 64, "IntPose is four float4");
 // Texel and lambda images hold one element past the W * H pixels.  The update kernels gather it, instead of
 // predicating the loads, for a voxel outside the image.  Its lambda is NaN (written with the lambda image), so the
 // voxel's sdf is NaN and the update skips it whatever the texel there holds; the texel buffers are allocated for the
@@ -136,7 +143,8 @@ struct FrameParams {
     FramePose pose;
     double tau_d;    // sdf_trunc as float64 (unit mode: the value Open3D holds; D1: (double)sdf_trunc_f)
     double unit_len; // voxel_length * unit resolution, float64 (volume_unit_length_)
-    IntFrame I;
+    IntConsts I;     // update constants (tex, lam, tex_pitch: set by the caller)
+    IntPose E;       // update pose
     float inv_fx, inv_fy;   // 1.0f / fx, 1.0f / fy (lambda image)
     float inv_vs, depth_trunc;
     int32_t unit_shift;     // log2(blocks per unit side): 0 = 8^3 units (D1 allocation), 1 = Open3D's 16^3 units
@@ -159,7 +167,8 @@ constexpr int kMaxGroup = 32;   // frames per fused group (bits of the membershi
 // may run while group g is still being integrated
 constexpr int kGroupBufs = 4;
 struct GroupArgs {
-    IntFrame f[kMaxGroup];
+    IntPose f[kMaxGroup];
+    IntConsts C;
     VolumeConsts V;
     int32_t count;
 };
@@ -267,8 +276,9 @@ cudaError_t launch_allocate(const GroupAllocArgs &args, const HashTable &table, 
 cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &table,
                                   const PoolMeta &meta, int sm_count, cudaStream_t stream);
 // projective TSDF + colour update of every block touched by the one-frame group in group buffer group_buf
-cudaError_t launch_integrate(const IntFrame &f, const VolumeConsts &vc, const HashTable &table,
-                             const PoolMeta &meta, int group_buf, int grid_ctas, cudaStream_t stream);
+// (frame 0 of args)
+cudaError_t launch_integrate(const GroupArgs &args, const HashTable &table, const PoolMeta &meta, int group_buf,
+                             int grid_ctas, cudaStream_t stream);
 int integrate_max_resident_ctas_per_sm();
 // d_bad[0]: reciprocals (3 x 2^23 inputs), d_bad[1]: quotients (`pairs` inputs) whose fast path differs from IEEE
 cudaError_t launch_selftest_division(unsigned long long *d_bad, uint64_t pairs, cudaStream_t stream);
