@@ -20,7 +20,7 @@ from types import SimpleNamespace
 
 import numpy as np
 
-from . import map_state
+from . import map_state, shard_plugin, sharding
 from .volume import B200TsdfVolume
 
 # defaults copied by value from the reference's parameter table (pyslam/config_parameters.py:311,
@@ -38,6 +38,9 @@ DEFAULT_PARAMETERS = {
     # bit-identical to a pool of this size from the start; 0 = fixed pool of CapacityBlocks
     "kVolumetricIntegrationB200MaxCapacityBlocks": 0,
     "kVolumetricIntegrationB200Device": 0,
+    # CUDA device ids of a map hash-sharded over several GPUs: with N >= 2 ids this process is rank 0 on the first and
+    # starts N - 1 worker processes on the others (shard_plugin.py); empty or one id: one map on one device
+    "kVolumetricIntegrationB200Devices": [],
     # undistort + BGR->RGB on the GPU (b2v_set_rectification) instead of the base class's cv2.remap / cvtColor
     "kVolumetricIntegrationB200GpuRectify": True,
     # when the input queue holds a backlog (rebuild(map) re-enqueues every keyframe, base.py:1242-1318), up to this
@@ -120,6 +123,72 @@ class B200PluginSetup:
             self.volume.set_rectification(m1, m2, swap_rb=True)
             self._gpu_rectify = True
 
+    # what a worker's plugin takes over from rank 0's before it builds its shard (shard_plugin.worker_plugin)
+    _SHARD_ATTRS = ("b200_parameters", "b200_set_parameters", "volumetric_integration_depth_trunc", "_side",
+                    "_probabilistic")
+
+    def _start_map(self):
+        """Build the map (`_build_map`): on one device, or with two or more kVolumetricIntegrationB200Devices as rank 0
+        of a sharded map whose workers build theirs in the same SETUP op.  Bad device lists raise RuntimeError."""
+        p = self.b200_parameters
+        devices = shard_plugin.parse_devices(p["kVolumetricIntegrationB200Devices"])
+        self._shards = None
+        if devices and "kVolumetricIntegrationB200Device" in self.b200_set_parameters:
+            getattr(type(self), "print", print)(f"{type(self).__name__}: kVolumetricIntegrationB200Device ignored: "
+                                                "kVolumetricIntegrationB200Devices places the map")
+        if len(devices) == 1:
+            p["kVolumetricIntegrationB200Device"] = devices[0]
+        if len(devices) < 2:
+            self._build_map()
+            return
+        c = self.camera
+        fx, fy, cx, cy = self._intrinsics()
+        attrs = {k: getattr(self, k) for k in self._SHARD_ATTRS if hasattr(self, k)}
+        attrs.update(camera=SimpleNamespace(fx=fx, fy=fy, cx=cx, cy=cy, width=getattr(c, "width", None),
+                                            height=getattr(c, "height", None)),
+                     calib_map1=getattr(self, "calib_map1", None), calib_map2=getattr(self, "calib_map2", None),
+                     depth_estimator=None if getattr(self, "depth_estimator", None) is None else True)
+        group = shard_plugin.ShardGroup(devices)
+        try:
+            group.plugin, self._shards = self, group
+            group.run("setup", dict(kind=self._SHARD_KIND, factory=shard_plugin.WORKER_FACTORY, attrs=attrs))
+        except BaseException:
+            self._shards = None
+            group.close()
+            if getattr(self, "volume", None) is not None:
+                self.volume.close()
+            raise
+
+    def _op_setup(self, meta):
+        self._build_map()
+
+    def _map_placement(self) -> dict:
+        """Device and shard arguments of the map's constructor."""
+        s = self._shards
+        if s is None:
+            return dict(device=int(self.b200_parameters["kVolumetricIntegrationB200Device"]))
+        return dict(device=s.device, shard_rank=s.rank, shard_count=s.world)
+
+    def _map_call(self, op, meta=None, **arrays):
+        """`_op_<op>(meta, **arrays)` on this map, or on every rank's shard of a sharded map (rank 0's result)."""
+        if getattr(self, "_shards", None) is None:
+            return getattr(self, "_op_" + op)(meta or {}, **arrays)
+        return self._shards.run(op, meta, arrays)
+
+    def _op_reset(self, meta):
+        self.volume.reset()
+
+    def _op_save_state(self, meta):
+        self.volume.save_state(map_state.shard_state_path(meta["path"], self._shards.rank, self._shards.world))
+
+    def _op_load_state(self, meta):
+        self.volume.load_state(meta["paths"])
+        self._after_load()
+
+    def _stop_shards(self):
+        if getattr(self, "_shards", None) is not None:
+            self._shards.close()
+
     def load(self, path):
         """The LOAD task of the map saved in directory `path`, the mirror of the base class's `save(path)`: it reads
         `path/dense_map.state.npz` (written by SAVE with kVolumetricIntegrationB200SaveMapState).  The integrator then
@@ -131,17 +200,22 @@ class B200PluginSetup:
 
     def _save_map_state(self, ply_path):
         """The part of SAVE that writes the map's state beside the .ply, when kVolumetricIntegrationB200SaveMapState."""
-        if self.b200_parameters["kVolumetricIntegrationB200SaveMapState"]:
+        if not self.b200_parameters["kVolumetricIntegrationB200SaveMapState"]:
+            return
+        if self._shards is None:
             self.volume.save_state(map_state.state_path(ply_path))
+        else:   # every rank writes its own shard file (dense_map.state.<r>-of-<N>.npz)
+            map_state.remove_other_states(ply_path, self._shards.world)
+            self._shards.run("save_state", dict(path=ply_path))
 
     def _load_map_state(self, task, completed, condition):
-        """LOAD: replace the map with the state file beside `task.load_save_path`; the next output shows it.  The
-        waiter is notified either way; `completed` becomes 1 only on success (a failure raises, leaving the map as it
-        was, and the task loop logs it)."""
+        """LOAD: replace the map with the state beside `task.load_save_path` (`map_state.state_files`: the single file,
+        or the shard files of a map saved by several ranks); the next output shows it.  The waiter is notified either
+        way; `completed` becomes 1 only on success on every rank (a failure raises, leaving the map as it was, and the
+        task loop logs it)."""
         loaded = False
         try:
-            self.volume.load_state(map_state.state_path(task.load_save_path))
-            self._after_load()
+            self._map_call("load_state", dict(paths=map_state.state_files(task.load_save_path)))
             loaded = True
         finally:
             with condition:
@@ -171,6 +245,7 @@ def make_integrator_class(Base, api):
         """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
 
         _api = api
+        _SHARD_KIND = "tsdf"
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
@@ -188,14 +263,17 @@ def make_integrator_class(Base, api):
             self.volumetric_integration_depth_trunc = (
                 p["kVolumetricIntegrationTsdfDepthTruncOutdoor"] if outdoor
                 else p["kVolumetricIntegrationTsdfDepthTruncIndoor"])
+            self._start_map()
+
+        def _build_map(self):
+            p = self.b200_parameters
             self.volume = B200TsdfVolume(
                 voxel_length=p["kVolumetricIntegrationVoxelLength"],
                 sdf_trunc=p["kVolumetricIntegrationTSdfTrunc"],
                 depth_trunc=self.volumetric_integration_depth_trunc,
                 capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None,
-                device=int(p["kVolumetricIntegrationB200Device"]),
-                volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]))
+                volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]), **self._map_placement())
             self.last_output = None
             self.last_integrated_id = -1
             self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call
@@ -217,10 +295,35 @@ def make_integrator_class(Base, api):
             p = self.b200_parameters
             mesh_out, pc_out = None, None
             if p["kVolumetricIntegrationTsdfExtractMesh"]:
-                mesh_out = api.VolumetricIntegrationMesh(self.volume.extract_triangle_mesh())
+                mesh_out = api.VolumetricIntegrationMesh(self._map_call("mesh"))
             else:
-                pc_out = api.VolumetricIntegrationPointCloud(self.volume.extract_point_cloud())
+                pc_out = api.VolumetricIntegrationPointCloud(self._map_call("points"))
             return api.VolumetricIntegrationOutput(task_type, self.last_integrated_id, pc_out, mesh_out)
+
+        def _op_mesh(self, meta):
+            if self._shards is None:
+                return self.volume.extract_triangle_mesh()
+            return sharding.extract_mesh_sharded(self.volume)
+
+        def _op_points(self, meta):
+            if self._shards is None:
+                return self.volume.extract_point_cloud()
+            return sharding.extract_point_cloud_sharded(self.volume)
+
+        def _integrate_sharded(self, frames, K4, fused):
+            """The frames on every rank's shard: one fused batch when the unsharded plugin fuses them, else one call
+            per frame.  Rank 0 uploads each batch once (raw uint16 depth stays 16-bit) and broadcasts it."""
+            for part in ([frames] if fused else [[f] for f in frames]):
+                scale = part[0][3]
+                self._shards.run(
+                    "integrate", dict(K=K4, poses=np.stack([np.asarray(f[0].pose, np.float64) for f in part]),
+                                      scale=scale),
+                    dict(depths=np.ascontiguousarray(np.stack([f[2] for f in part]),
+                                                     np.float32 if scale is None else np.uint16),
+                         colors=np.ascontiguousarray(np.stack([f[1] for f in part]), np.uint8)))
+
+        def _op_integrate(self, meta, depths, colors):
+            self.volume.integrate_batch(depths, colors, meta["K"], meta["poses"], depth_scale=meta["scale"])
 
         def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
                                is_running, load_request_completed, load_request_condition,
@@ -238,7 +341,7 @@ def make_integrator_class(Base, api):
                     except Exception:
                         pass
                     if task is not None and task.task_type == TaskType.RESET:
-                        self.volume.reset()
+                        self._map_call("reset")
                     if self._has_deferred:
                         self.last_input_task, self._deferred_task, self._has_deferred = self._deferred_task, None, False
                     else:
@@ -273,7 +376,9 @@ def make_integrator_class(Base, api):
                                 same = all(f[1].shape == frames[0][1].shape and f[2].shape == frames[0][2].shape
                                            and f[2].dtype == frames[0][2].dtype and f[3] == frames[0][3]
                                            for f in frames)
-                                if len(frames) > 1 and same:
+                                if self._shards is not None:
+                                    self._integrate_sharded(frames, K4, len(frames) > 1 and same)
+                                elif len(frames) > 1 and same:
                                     # one C call: groups of frames fused per block visit (b2v_integrate_batch)
                                     self.volume.integrate_batch(np.stack([f[2] for f in frames]),
                                                                 np.stack([f[1] for f in frames]), K4,
@@ -293,10 +398,10 @@ def make_integrator_class(Base, api):
                         elif ttype == TaskType.SAVE:
                             path = self.last_input_task.load_save_path
                             if self.b200_parameters["kVolumetricIntegrationTsdfExtractMesh"]:
-                                m = self.volume.extract_triangle_mesh()
+                                m = self._map_call("mesh")
                                 write_ply_mesh(path, m.vertices, m.triangles, m.vertex_colors)
                             else:
-                                pc = self.volume.extract_point_cloud()
+                                pc = self._map_call("points")
                                 write_ply_points(path, pc.points, pc.colors)
                             self._save_map_state(path)
                             last_output = api.VolumetricIntegrationOutput(ttype)
@@ -324,6 +429,7 @@ def make_integrator_class(Base, api):
             time_volumetric_integration.value = time.perf_counter() - t_start
 
         def _stop_volume_integrator_implementation(self):
+            self._stop_shards()
             if getattr(self, "volume", None) is not None:
                 self.volume.close()
 

@@ -28,8 +28,11 @@ from __future__ import annotations
 import time
 import traceback
 
+from types import SimpleNamespace
+
 import numpy as np
 
+from . import sharding
 from .integrator import B200PluginSetup, raw_depth, write_ply_points
 from .volume import (CameraFrustrum, VoxelBlockGrid, VoxelBlockSemanticGrid, VoxelBlockSemanticProbabilisticGrid,
                      filter_shadow_points, remap_instance_ids)
@@ -70,6 +73,8 @@ DEFAULT_PARAMETERS = {
     # sum in input order and do not read it
     "kVolumetricIntegrationB200InputOrderSums": False,
     "kVolumetricIntegrationB200Device": 0,
+    # device ids of a map sharded over several GPUs (integrator.py has the same parameter)
+    "kVolumetricIntegrationB200Devices": [],
     "kVolumetricIntegrationB200GenerateObjects": True,   # kGenerateObjectsDefault (reference :84)
     # raw keyframe images to the grid (set_frame): upload once, undistort + BGR->RGB + depth widening + shadow filter
     # on the GPU instead of the base class's cv2.remap / cvtColor (integrator.py has the same switch)
@@ -106,6 +111,8 @@ def make_semantic_integrator_class(Base, api):
 
         _defaults = DEFAULT_PARAMETERS
         _api = api
+        _SHARD_KIND = "semantic"
+        _LABELS = True     # the grid takes class and instance images
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
@@ -120,9 +127,14 @@ def make_semantic_integrator_class(Base, api):
             env_t = getattr(api, "DatasetEnvironmentType", None)
             if env_t is not None and hasattr(env_t, "INDOOR"):
                 indoor = environment_type == env_t.INDOOR
-            side = "Indoor" if indoor else "Outdoor"
-            self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{side}"]
-            self.volume = self._make_grid(p, side, constructor_kwargs or {})
+            self._side = "Indoor" if indoor else "Outdoor"
+            self._probabilistic = bool((constructor_kwargs or {}).get("use_semantic_probabilistic", False))
+            self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{self._side}"]
+            self._start_map()
+
+        def _build_map(self):
+            p, side = self.b200_parameters, self._side
+            self.volume = self._make_grid(p, side, {"use_semantic_probabilistic": self._probabilistic})
             fx, fy, cx, cy = self._intrinsics()
             self.camera_frustrum = CameraFrustrum(
                 fx, fy, cx, cy, self.camera.width, self.camera.height, np.eye(4),
@@ -148,7 +160,8 @@ def make_semantic_integrator_class(Base, api):
                                               "kVolumetricIntegrationB200LabelOverflowPairs ignored: it applies to "
                                               "use_semantic_probabilistic only")
                 pairs = 0
-            grid = grid_t(**_grid_args(p, self.b200_set_parameters), max_label_overflow_pairs=pairs)
+            grid = grid_t(**dict(_grid_args(p, self.b200_set_parameters), **self._map_placement()),
+                          max_label_overflow_pairs=pairs)
             grid.set_depth_threshold(p[f"kVolumetricSemanticProbabilisticIntegrationDepthThreshold{side}"])
             grid.set_depth_decay_rate(p[f"kVolumetricSemanticProbabilisticIntegrationDepthDecayRate{side}"])
             return grid
@@ -162,14 +175,23 @@ def make_semantic_integrator_class(Base, api):
                 return None   # the frustum's label / carve calls reject such frames: the host path handles them
             return raw_depth(kd.depth, self.camera, getattr(api, "USE_CPP", False))
 
-        def _integrate_raw_keyframe(self, kd, depth, scale):
+        def _uses_instances(self, classes, instances):
+            """The frame's instance ids are associated and integrated (host arrays)."""
+            return (self._LABELS and bool(self.b200_parameters["kVolumetricSemanticIntegrationUseInstanceIds"])
+                    and instances is not None and np.asarray(instances).size > 0 and classes is not None)
+
+        def _assign_object_ids(self, *args, **kwargs):
+            """The grid's association; over all ranks for a sharded grid."""
+            if self._shards is None:
+                return self.volume.assign_object_ids_to_instance_ids(*args, **kwargs)
+            return sharding.assign_object_ids_to_instance_ids_sharded(self.volume, *args, **kwargs)
+
+        def _integrate_raw(self, kd, depth, scale, use_instances):
             """The loop body on the raw images: one set_frame uploads, rectifies and shadow-filters them on the
             device; association (or carving), the instance remap and the integration read the staged images."""
             p = self.b200_parameters
             flt = bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"])
             classes, instances = kd.semantic_img, kd.semantic_instances_img
-            use_instances = (bool(p["kVolumetricSemanticIntegrationUseInstanceIds"]) and instances is not None
-                             and np.asarray(instances).size > 0 and classes is not None)
             fr = self.volume.set_frame(depth, kd.img, class_image=classes,
                                        instance_image=instances if use_instances else None, depth_scale=scale,
                                        filter_shadow_points=flt)
@@ -178,7 +200,7 @@ def make_semantic_integrator_class(Base, api):
             carve_thr = float(p["kVolumetricIntegrationVoxelGridCarvingDepthThreshold"])
             object_image = None
             if use_instances:   # association and carving see the filtered depth (:349-362, :371-388)
-                self.last_instance_map = self.volume.assign_object_ids_to_instance_ids(
+                self.last_instance_map = self._assign_object_ids(
                     self.camera_frustrum, fr.class_image, fr.instance_image, fr.filtered_depth,
                     depth_threshold=carve_thr, do_carving=bool(p["kVolumetricIntegrationVoxelGridUseCarving"]),
                     min_vote_ratio=float(p["kVolumetricSemanticIntegrationMinVoteRatio"]),
@@ -197,22 +219,68 @@ def make_semantic_integrator_class(Base, api):
             return True
 
         def _integrate_keyframe(self, kd):
-            """The reference loop body for one keyframe (:300-461)."""
+            """The reference loop body for one keyframe (:300-461): on the raw images, or on the ones the base class
+            prepared on the host; on every rank's shard of a sharded grid."""
             raw = self._raw_frame(kd)
+            if self._shards is not None:
+                return self._integrate_keyframe_sharded(kd, raw)
             if raw is not None:
-                return self._integrate_raw_keyframe(kd, *raw)
-            p = self.b200_parameters
+                return self._integrate_raw(kd, *raw, self._uses_instances(kd.semantic_img, kd.semantic_instances_img))
             rect = self.estimate_depth_if_needed_and_rectify(kd)
             color, depth = rect[0], rect[1]
             classes = rect[3] if len(rect) > 3 else None
             instances = rect[4] if len(rect) > 4 else None
             if color is None or depth is None:
                 return False
+            return self._integrate_prepared(kd, color, depth, classes, instances)
+
+        def _labels(self, classes, instances, use_instances, raw):
+            """The label images of a broadcast keyframe: none for the point-average grid; int32 (what set_frame
+            converts them to) on the raw path, where an empty image is no image."""
+            if not self._LABELS:
+                return {}
+            out = {}
+            for name, img in (("classes", classes), ("instances", instances if use_instances or not raw else None)):
+                if img is not None and raw:
+                    img = np.ascontiguousarray(img, np.int32) if np.asarray(img).size else None
+                out[name] = img
+            return out
+
+        def _integrate_keyframe_sharded(self, kd, raw):
+            """Rank 0's part of INTEGRATE: broadcast the keyframe (raw images, or the host-prepared ones when the
+            frame takes the host path); every rank then runs the loop body on its shard (`_op_frame`)."""
+            meta = dict(id=kd.id, pose=np.asarray(kd.pose, np.float64), raw=raw is not None)
+            if raw is not None:
+                depth, scale = raw
+                use = self._uses_instances(kd.semantic_img, kd.semantic_instances_img)
+                meta.update(scale=scale, use_instances=use)
+                arrays = dict(depth=depth, img=kd.img,
+                              **self._labels(kd.semantic_img, kd.semantic_instances_img, use, True))
+            else:
+                rect = self.estimate_depth_if_needed_and_rectify(kd)
+                color, depth = rect[0], rect[1]
+                if color is None or depth is None:
+                    return False
+                arrays = dict(depth=depth, img=color, **self._labels(rect[3] if len(rect) > 3 else None,
+                                                                     rect[4] if len(rect) > 4 else None, False, False))
+            self._shards.run("frame", meta, arrays)
+            return True
+
+        def _op_frame(self, meta, depth, img, classes=None, instances=None):
+            kd = SimpleNamespace(id=meta["id"], pose=meta["pose"], img=img, semantic_img=classes,
+                                 semantic_instances_img=instances)
+            if meta["raw"]:
+                return self._integrate_raw(kd, depth, meta["scale"], meta["use_instances"])
+            host = [x.cpu().numpy() if hasattr(x, "cpu") else x for x in (img, depth, classes, instances)]
+            return self._integrate_prepared(kd, *host)
+
+        def _integrate_prepared(self, kd, color, depth, classes, instances):
+            """The loop body on images the base class prepared on the host."""
+            p = self.b200_parameters
             depth = np.ascontiguousarray(depth, np.float32)
             flt = bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"])
             self.integrated_instance_ids = False
-            use_instances = (bool(p["kVolumetricSemanticIntegrationUseInstanceIds"]) and instances is not None
-                             and np.asarray(instances).size > 0 and classes is not None)
+            use_instances = self._uses_instances(classes, instances)
             self.camera_frustrum.set_T_cw(kd.pose)
             carve_thr = float(p["kVolumetricIntegrationVoxelGridCarvingDepthThreshold"])
             object_image = None
@@ -220,7 +288,7 @@ def make_semantic_integrator_class(Base, api):
                 # association and carving look at the FILTERED depth image (:349-362, :371-388)
                 depth_used = filter_shadow_points(depth) if flt else depth
                 if use_instances:
-                    self.last_instance_map = self.volume.assign_object_ids_to_instance_ids(
+                    self.last_instance_map = self._assign_object_ids(
                         self.camera_frustrum, classes, instances, depth_used, depth_threshold=carve_thr,
                         do_carving=bool(p["kVolumetricIntegrationVoxelGridUseCarving"]),
                         min_vote_ratio=float(p["kVolumetricSemanticIntegrationMinVoteRatio"]),
@@ -244,9 +312,9 @@ def make_semantic_integrator_class(Base, api):
             if (p["kVolumetricIntegrationB200GenerateObjects"] and getattr(self, "integrated_instance_ids", False)
                     and ObjList is not None):
                 # reference :523-587: objects only when instance ids are available
-                grp = self.volume.get_object_segments(
+                grp = self._map_call("segments", dict(
                     min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
-                    min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"]))
+                    min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"])))
                 sem_rgb = getattr(api, "sem_img_to_rgb", None)      # SemanticMappingShared.sem_img_to_rgb
                 ids_rgb = getattr(api, "ids_to_rgb_float", None)    # IdsColorTable.ids_to_rgb_float
                 n = len(grp.object_vector)
@@ -256,13 +324,23 @@ def make_semantic_integrator_class(Base, api):
                             if ids_rgb is not None and n else np.zeros((n, 3), np.float32))
                 objects = ObjList(grp, sem_cols, obj_cols, n)
                 return api.VolumetricIntegrationOutput(task_type, self.last_integrated_id, None, None, objects)
-            v = self.volume.get_voxels(min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
-                                       min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"]))
+            v = self._map_call("voxels", dict(min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
+                                              min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"])))
             pc = api.VolumetricIntegrationPointCloud(points=np.ascontiguousarray(v.points, np.float32),
                                                      colors=np.ascontiguousarray(v.colors, np.float32))
             pc.semantics = v.class_ids if len(v.class_ids) else None
             pc.object_ids = v.object_ids if len(v.object_ids) else None
             return api.VolumetricIntegrationOutput(task_type, self.last_integrated_id, pc, None)
+
+        def _op_voxels(self, meta):
+            if self._shards is None:
+                return self.volume.get_voxels(**meta)
+            return sharding.get_voxels_sharded(self.volume, **meta)
+
+        def _op_segments(self, meta):
+            if self._shards is None:
+                return self.volume.get_object_segments(**meta)
+            return sharding.get_object_segments_sharded(self.volume, **meta)
 
         def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
                                is_running, load_request_completed, load_request_condition,
@@ -279,7 +357,7 @@ def make_semantic_integrator_class(Base, api):
                     except Exception:
                         pass
                     if task is not None and task.task_type == TaskType.RESET:
-                        self.volume.reset()
+                        self._map_call("reset")
                     self.last_input_task = q_in.get()  # blocking
                     if self.last_input_task is None:
                         is_running.value = 0
@@ -294,9 +372,9 @@ def make_semantic_integrator_class(Base, api):
                                         do_output = False
                         elif ttype == TaskType.SAVE:
                             p = self.b200_parameters
-                            v = self.volume.get_voxels(
+                            v = self._map_call("voxels", dict(
                                 min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
-                                min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"]))
+                                min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"])))
                             if len(v.points):
                                 write_ply_points(self.last_input_task.load_save_path, v.points, v.colors)
                             self._save_map_state(self.last_input_task.load_save_path)
@@ -325,6 +403,7 @@ def make_semantic_integrator_class(Base, api):
             time_volumetric_integration.value = time.perf_counter() - t_start
 
         def _stop_volume_integrator_implementation(self):
+            self._stop_shards()
             if getattr(self, "volume", None) is not None:
                 self.volume.close()
 
@@ -340,12 +419,14 @@ def make_voxel_grid_integrator_class(Base, api):
 
     class VolumetricIntegratorB200VoxelGrid(SemanticCls):
         _defaults = dict(DEFAULT_PARAMETERS, kVolumetricIntegrationB200CapacityBlocks=1 << 17)
+        _SHARD_KIND = "voxel_grid"
+        _LABELS = False
 
         def _make_grid(self, p, side, constructor_kwargs):
-            return VoxelBlockGrid(**_grid_args(p, self.b200_set_parameters),
+            return VoxelBlockGrid(**dict(_grid_args(p, self.b200_set_parameters), **self._map_placement()),
                                   input_order_sums=bool(p["kVolumetricIntegrationB200InputOrderSums"]))
 
-        def _integrate_raw_keyframe(self, kd, depth, scale):
+        def _integrate_raw(self, kd, depth, scale, use_instances):
             """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
             p = self.b200_parameters
             fr = self.volume.set_frame(depth, kd.img, depth_scale=scale,
@@ -361,15 +442,8 @@ def make_voxel_grid_integrator_class(Base, api):
             self.last_integrated_id = kd.id
             return True
 
-        def _integrate_keyframe(self, kd):
-            raw = self._raw_frame(kd)
-            if raw is not None:
-                return self._integrate_raw_keyframe(kd, *raw)
+        def _integrate_prepared(self, kd, color, depth, classes, instances):
             p = self.b200_parameters
-            rect = self.estimate_depth_if_needed_and_rectify(kd)
-            color, depth = rect[0], rect[1]
-            if color is None or depth is None:
-                return False
             depth = np.ascontiguousarray(depth, np.float32)
             if p["kVolumetricIntegrationVoxelGridUseCarving"]:
                 self.camera_frustrum.set_T_cw(kd.pose)
@@ -384,7 +458,7 @@ def make_voxel_grid_integrator_class(Base, api):
             return True
 
         def _make_output(self, task_type):
-            v = self.volume.get_voxels(min_count=int(self.b200_parameters["kVolumetricIntegrationVoxelGridMinCount"]))
+            v = self._map_call("voxels", dict(min_count=int(self.b200_parameters["kVolumetricIntegrationVoxelGridMinCount"])))
             pc = api.VolumetricIntegrationPointCloud(points=np.ascontiguousarray(v.points, np.float32),
                                                      colors=np.ascontiguousarray(v.colors, np.float32))
             return api.VolumetricIntegrationOutput(task_type, self.last_integrated_id, pc, None)

@@ -35,6 +35,55 @@ def state_path(ply_path: str) -> str:
     return os.path.splitext(ply_path)[0] + ".state.npz"
 
 
+def shard_state_path(ply_path: str, rank: int, count: int) -> str:
+    """The state file rank `rank` of a `count`-rank plugin writes beside `dense_map.ply`:
+    `dense_map.state.<rank>-of-<count>.npz`."""
+    return os.path.splitext(ply_path)[0] + f".state.{rank}-of-{count}.npz"
+
+
+def _shard_sets(ply_path: str) -> dict:
+    """count -> {rank: path} of the shard state files beside `ply_path`."""
+    head = os.path.basename(os.path.splitext(ply_path)[0]) + ".state."
+    folder = os.path.dirname(ply_path) or "."
+    sets = {}
+    for name in os.listdir(folder) if os.path.isdir(folder) else ():
+        if not (name.startswith(head) and name.endswith(".npz")):
+            continue
+        rank, sep, count = name[len(head):-4].partition("-of-")
+        if sep and rank.isdigit() and count.isdigit():
+            sets.setdefault(int(count), {})[int(rank)] = os.path.join(os.path.dirname(ply_path), name)
+    return sets
+
+
+def state_files(ply_path: str):
+    """What LOAD reads for the map saved as `ply_path`: the single state file when it exists, else the complete set of
+    shard files (a list in rank order), else the single file's path (whose load then reports it missing).  ValueError
+    when shard files exist but form no complete set, or more than one."""
+    single = state_path(ply_path)
+    if os.path.exists(single):
+        return single
+    sets = _shard_sets(ply_path)
+    full = [n for n, s in sets.items() if sorted(s) == list(range(n))]
+    if sets and len(full) != 1:
+        raise ValueError(f"{single} is missing and the shard state files beside it form "
+                         f"{'no complete set' if not full else 'more than one set'}: "
+                         f"{sorted(os.path.basename(p) for s in sets.values() for p in s.values())}")
+    if not sets:
+        return single
+    return [sets[full[0]][r] for r in range(full[0])]
+
+
+def remove_other_states(ply_path: str, count: int) -> None:
+    """Before a `count`-rank plugin writes its shard files: remove the single file and the shard files of other rank
+    counts beside `ply_path`, so that `state_files` finds the new set."""
+    if os.path.exists(state_path(ply_path)):
+        os.remove(state_path(ply_path))
+    for n, s in _shard_sets(ply_path).items():
+        if n != count:
+            for p in s.values():
+                os.remove(p)
+
+
 def write(path, kind: str, semantic_kind: int, config: dict, settings: dict, shard_rank: int, shard_count: int,
           arrays: dict, labels: dict | None = None) -> None:
     """Write one state file at `path` (exactly that name).  `config` / `settings`: numpy scalars; `arrays`: the
