@@ -1091,10 +1091,6 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
     }
     if (n_blocks == 0) return B2V_OK;
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
-    {
-        const int rc = grow_for_blocks(v, n_blocks);
-        if (rc == B2V_ERR_CUDA) return rc;
-    }
     const size_t n = static_cast<size_t>(n_blocks);
     // device arrays are read in place; host ones are staged on the compute stream
     const int4 *d_keys = reinterpret_cast<const int4 *>(keys4);
@@ -1114,6 +1110,25 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
             e = cudaMemcpyAsync(v_stage.get(), voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice,
                                 v->compute);
         d_vox = v_stage.get();
+    }
+    // the weights are checked before the pool grows or any block is written: a rejected upload leaves the volume as
+    // it was (d_i's first element counts the bad weights)
+    uint32_t bad = 0;
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_i.get(), 0, sizeof(uint32_t), v->compute);
+    if (e == cudaSuccess) e = launch_upload_check(d_vox, static_cast<uint32_t>(n), d_i.get(), v->compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_i.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, v->compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
+    if (e != cudaSuccess) {
+        v->err = std::string("b2v_upload_blocks: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    if (bad) {
+        v->err = "b2v_upload_blocks: " + std::to_string(bad) + " voxel weights outside [0, 2^24]; nothing was uploaded";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    {
+        const int rc = grow_for_blocks(v, n_blocks);
+        if (rc == B2V_ERR_CUDA) return rc;
     }
     if (e == cudaSuccess)
         e = launch_upload_blocks(d_keys, d_vox, static_cast<uint32_t>(n), d_i.get(), v->table, v->meta, v->compute);

@@ -290,6 +290,9 @@ cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *sl
                                       uint32_t n, int4 *out, cudaStream_t stream);
 
 // find-or-create the blocks of `keys` (unique) and copy `vox` [n][5][512] into them
+// the largest weight a voxel may hold: w + 1 is exact below it and rounds back to it there (integration saturates)
+constexpr float kWeightMax = 16777216.0f;  // 2^24
+cudaError_t launch_upload_check(const float *vox, uint32_t n, uint32_t *bad, cudaStream_t stream);
 cudaError_t launch_upload_blocks(const int4 *keys, const float *vox, uint32_t n, uint32_t *scratch_idx,
                                  const HashTable &table, const PoolMeta &meta, cudaStream_t stream);
 

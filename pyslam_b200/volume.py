@@ -79,6 +79,7 @@ def _pinned_owner(x):
 #: counted once however often it is passed (a resident frame buffer, views into one pool), and an input larger than
 #: the bound is still held: the wait comes only when a later call brings another storage.
 HELD_INPUT_BYTES_MAX = 1 << 30
+WEIGHT_MAX = 2.0 ** 24   # the largest voxel weight a TSDF block may hold (include/b2v.h)
 
 
 class TriangleMesh:
@@ -122,6 +123,9 @@ class _MapState:
     def _restore_settings(self, settings: dict) -> None:
         pass
 
+    def _check_blocks(self, blocks: dict) -> None:
+        """Raise ValueError for block values the map does not take (checked before the map is cleared)."""
+
     def save_state(self, path) -> None:
         """Write the map's state to `path` (one uncompressed `.npz`; one file per shard for a sharded map), after the
         work in flight is done.  The state is every block's raw voxels plus the configuration and settings a load
@@ -145,6 +149,7 @@ class _MapState:
             {name: np.asarray(v).dtype for name, v in self._state_settings().items()}, spec, self.shard_rank,
             self.shard_count, self._state_capacity(), self._STATE_BOUNDS, labels=self._STATE_LABELS)
         labels = labels[0] if labels else None
+        self._check_blocks(blocks)
         if labels is not None:
             self._check_labels(labels)
         self._clear_state()
@@ -470,7 +475,8 @@ class B200TsdfVolume(_MapState):
         return dict(keys=d["keys"], hashes=_block_hashes(d["keys"]), vox=d["vox"])
 
     def upload_blocks(self, keys, vox):
-        """Restore / seed blocks: keys int32 [n,3] (unique), vox float32 [n,5,512]."""
+        """Restore / seed blocks: keys int32 [n,3] (unique), vox float32 [n,5,512].  Every weight must lie in
+        [0, 2^24] (include/b2v.h); otherwise RuntimeError and the volume is unchanged."""
         k = _keys4(keys)
         x = np.ascontiguousarray(vox, np.float32).reshape(k.shape[0], VOXEL_PLANES, BLOCK_VOXELS)
         self._check(self._L.b2v_upload_blocks(self._h, k.shape[0], k.ctypes.data, x.ctypes.data),
@@ -498,6 +504,11 @@ class B200TsdfVolume(_MapState):
 
     def _clear_state(self) -> None:
         self.reset()
+
+    def _check_blocks(self, blocks: dict) -> None:
+        w = blocks["vox"][:, 1]
+        if w.size and not np.all((w >= 0) & (w <= WEIGHT_MAX)):
+            raise ValueError("voxel weights outside [0, 2^24] in the state")
 
     def _upload_state(self, blocks: dict) -> None:
         if len(blocks["keys"]):
