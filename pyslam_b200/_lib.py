@@ -85,6 +85,12 @@ class B2VConfig(C.Structure):
     ]
 
 
+class B2VConfigEx(C.Structure):
+    """b2v_config with its last field, color_f64 (b2v_version() >= 112).  The field sits in what is B2VConfig's tail
+    padding, so both have the header's size, and a B2VConfig (ctypes zero-fills it) creates a float32-colour volume."""
+    _fields_ = B2VConfig._fields_ + [("color_f64", C.c_int32)]
+
+
 _lib = None
 
 
@@ -108,7 +114,7 @@ def load() -> C.CDLL:
     L.b2v_selftest_division.argtypes = [i32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
 
     L.b2v_create.restype = C.c_int
-    L.b2v_create.argtypes = [C.POINTER(B2VConfig), C.POINTER(vp)]
+    L.b2v_create.argtypes = [C.POINTER(B2VConfigEx), C.POINTER(vp)]
     L.b2v_destroy.restype = C.c_int
     L.b2v_destroy.argtypes = [vp]
     L.b2v_reset.restype = C.c_int

@@ -231,8 +231,6 @@ CUmemAllocationProp pool_prop(int device) {
     return p;
 }
 
-constexpr size_t kBlockBytes = static_cast<size_t>(kBlockFloats) * sizeof(float);
-
 bool cu_failed(CUresult r, const char *what, std::string *err) {
     if (r == CUDA_SUCCESS) return false;
     *err = std::string(what) + ": CUresult " + std::to_string(r);
@@ -297,8 +295,10 @@ void b2v::vmm_release(VmmRange *r) {
 }
 
 // reserve the address range of meta.capacity blocks
+static size_t block_bytes(const b2v_volume *v) { return tsdf_block_bytes(v->cfg.color_f64 != 0); }
+
 static int pool_reserve(b2v_volume *v) {
-    if (!vmm_reserve(&v->pool, static_cast<size_t>(v->meta.capacity) * kBlockBytes, v->cfg.device, &v->err))
+    if (!vmm_reserve(&v->pool, static_cast<size_t>(v->meta.capacity) * block_bytes(v), v->cfg.device, &v->err))
         return B2V_ERR_CUDA;
     v->meta.pool = reinterpret_cast<float *>(v->pool.va);
     return B2V_OK;
@@ -307,8 +307,8 @@ static int pool_reserve(b2v_volume *v) {
 // map (and zero: allocation relies on a zeroed pool) storage for at least `blocks` blocks, in whole granules, up to
 // the reservation; pool_capacity follows
 static int pool_map(b2v_volume *v, uint64_t blocks) {
-    if (!vmm_map(&v->pool, static_cast<size_t>(blocks) * kBlockBytes, v->compute, &v->err)) return B2V_ERR_CUDA;
-    v->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(v->meta.capacity, v->pool.mapped / kBlockBytes));
+    if (!vmm_map(&v->pool, static_cast<size_t>(blocks) * block_bytes(v), v->compute, &v->err)) return B2V_ERR_CUDA;
+    v->meta.pool_capacity = static_cast<uint32_t>(std::min<size_t>(v->meta.capacity, v->pool.mapped / block_bytes(v)));
     return B2V_OK;
 }
 
@@ -331,7 +331,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 111; }
+extern "C" int b2v_version(void) { return 112; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -362,6 +362,7 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
         !(cfg->depth_trunc > 0.0f) || cfg->capacity_blocks == 0 || cfg->shard_count < 1 ||
         cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_count ||
         (cfg->unit_resolution != 0 && cfg->unit_resolution != 8 && cfg->unit_resolution != 16) ||
+        (cfg->color_f64 != 0 && cfg->color_f64 != 1) ||
         (cfg->max_capacity_blocks != 0 &&
          (cfg->max_capacity_blocks < cfg->capacity_blocks || cfg->max_capacity_blocks > (1u << 30))) ||
         static_cast<float>(cfg->voxel_length > 0.0 ? cfg->voxel_length : cfg->voxel_size) != cfg->voxel_size ||
@@ -455,7 +456,7 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     int sms = 0;
     B2V_CUDA(v, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
     // persistent grid: exactly one wave of resident CTAs (B2V_INT_CTAS_PER_SM overrides, for tuning)
-    int per_sm = integrate_max_resident_ctas_per_sm();
+    int per_sm = integrate_max_resident_ctas_per_sm(cfg->color_f64 != 0);
     if (const char *e = std::getenv("B2V_INT_CTAS_PER_SM")) {
         const int n = std::atoi(e);
         if (n >= 1 && n <= 32) per_sm = n;
@@ -510,8 +511,9 @@ static int drain_and_copy_counters(b2v_volume *v) {
 
 static int launch_group_update(b2v_volume *v, int buf, cudaStream_t cs) {
     const GroupArgs &a = v->gargs[buf];
-    B2V_CUDA(v, v->gfused[buf] ? launch_integrate_group(a, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs)
-                               : launch_integrate(a, v->table, v->meta, buf, v->grid_ctas, cs));
+    const bool f64 = v->cfg.color_f64 != 0;
+    B2V_CUDA(v, v->gfused[buf] ? launch_integrate_group(a, v->table, v->meta, buf, v->grid_ctas, v->sm_count, cs, f64)
+                               : launch_integrate(a, v->table, v->meta, buf, v->grid_ctas, cs, f64));
     v->launches += v->gfused[buf] ? 2 : 1;  // update (+ the mask clear of a fused group)
     return B2V_OK;
 }
@@ -570,7 +572,7 @@ extern "C" int b2v_reset(b2v_volume *v) {
     if (rc != B2V_OK) return rc;
     std::memset(v->h_skip, 0, kGroupBufs * sizeof(uint32_t));
     const uint32_t nb = block_count(v);
-    B2V_CUDA(v, cudaMemsetAsync(v->meta.pool, 0, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
+    B2V_CUDA(v, cudaMemsetAsync(v->meta.pool, 0, static_cast<size_t>(nb) * block_bytes(v),
                                 v->compute));
     B2V_CUDA(v, cudaMemsetAsync(v->meta.block_flags, 0, static_cast<size_t>(nb) * sizeof(uint32_t), v->compute));
     rc = volume_clear_device(v);
@@ -1051,7 +1053,7 @@ extern "C" int b2v_counters(b2v_volume *v, int64_t *block_updates, int64_t *kern
     return rc;
 }
 
-// The blocks cross the ABI in the pool's own layout: keys int4 {x, y, z, 0}, voxels [nb][5][512].
+// The blocks cross the ABI in the pool's own layout: keys int4 {x, y, z, 0}, voxels nb blocks of TsdfBlock<TC>.
 extern "C" int64_t b2v_export_blocks(b2v_volume *v, int32_t *keys4, float *voxels, int64_t max_blocks) {
     if (!v) return -1;
     if (read_counters(v) == B2V_ERR_CUDA) return -1;
@@ -1065,7 +1067,7 @@ extern "C" int64_t b2v_export_blocks(b2v_volume *v, int32_t *keys4, float *voxel
     cudaError_t e = cudaSuccess;
     if (keys4) e = cudaMemcpyAsync(keys4, v->meta.block_keys, nb * sizeof(int4), cudaMemcpyDefault, v->compute);
     if (e == cudaSuccess && voxels)
-        e = cudaMemcpyAsync(voxels, v->meta.pool, static_cast<size_t>(nb) * kBlockFloats * sizeof(float),
+        e = cudaMemcpyAsync(voxels, v->meta.pool, static_cast<size_t>(nb) * block_bytes(v),
                             cudaMemcpyDefault, v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
     if (e != cudaSuccess) {
@@ -1105,9 +1107,9 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
         d_keys = k_stage.get();
     }
     if (e == cudaSuccess && !is_device_pointer(voxels)) {
-        e = v_stage.reserve(n * kBlockFloats);
+        e = v_stage.reserve(n * (block_bytes(v) / sizeof(float)));
         if (e == cudaSuccess)
-            e = cudaMemcpyAsync(v_stage.get(), voxels, n * kBlockFloats * sizeof(float), cudaMemcpyHostToDevice,
+            e = cudaMemcpyAsync(v_stage.get(), voxels, n * block_bytes(v), cudaMemcpyHostToDevice,
                                 v->compute);
         d_vox = v_stage.get();
     }
@@ -1115,7 +1117,7 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
     // it was (d_i's first element counts the bad weights)
     uint32_t bad = 0;
     if (e == cudaSuccess) e = cudaMemsetAsync(d_i.get(), 0, sizeof(uint32_t), v->compute);
-    if (e == cudaSuccess) e = launch_upload_check(d_vox, static_cast<uint32_t>(n), d_i.get(), v->compute);
+    if (e == cudaSuccess) e = launch_upload_check(d_vox, static_cast<uint32_t>(n), d_i.get(), v->compute, v->cfg.color_f64 != 0);
     if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, d_i.get(), sizeof(uint32_t), cudaMemcpyDeviceToHost, v->compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
     if (e != cudaSuccess) {
@@ -1131,7 +1133,8 @@ extern "C" int b2v_upload_blocks(b2v_volume *v, int64_t n_blocks, const int32_t 
         if (rc == B2V_ERR_CUDA) return rc;
     }
     if (e == cudaSuccess)
-        e = launch_upload_blocks(d_keys, d_vox, static_cast<uint32_t>(n), d_i.get(), v->table, v->meta, v->compute);
+        e = launch_upload_blocks(d_keys, d_vox, static_cast<uint32_t>(n), d_i.get(), v->table, v->meta, v->compute,
+                                 v->cfg.color_f64 != 0);
     if (e == cudaSuccess) e = cudaStreamSynchronize(v->compute);
     v->launches += 2;
     if (e != cudaSuccess) {
@@ -1205,9 +1208,9 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     cudaStream_t cs = v->compute;
     const int sms = v->sm_count;
     if (mesh) {
-        B2V_CUDA(v, launch_mesh_classify(v->table, v->meta, v->mb, sms, cs));
+        B2V_CUDA(v, launch_mesh_classify(v->table, v->meta, v->mb, sms, cs, v->cfg.color_f64 != 0));
     } else {
-        B2V_CUDA(v, launch_point_masks(v->table, v->meta, v->mb, sms, cs));
+        B2V_CUDA(v, launch_point_masks(v->table, v->meta, v->mb, sms, cs, v->cfg.color_f64 != 0));
     }
     B2V_CUDA(v, launch_mesh_scan(v->mb, sms, cs));
     B2V_CUDA(v, cudaMemcpyAsync(v->h_totals, v->mb.totals, kNumMeshTotals * sizeof(uint32_t), cudaMemcpyDeviceToHost, cs));
@@ -1218,7 +1221,8 @@ static int extract_common(b2v_volume *v, bool mesh, int64_t *n_vertices, int64_t
     B2V_CUDA(v, v->mesh.edge_ids.reserve(nv * 4));
     B2V_CUDA(v, v->mesh.triangles.reserve(nt * 3));
     v->mb = mesh_view(v, nb);
-    B2V_CUDA(v, launch_mesh_vertices(v->meta, v->mb, v->geo.voxel_length, v->geo.unit_shift, !mesh, v->h_totals[kMtVertexBlocks], cs));
+    B2V_CUDA(v, launch_mesh_vertices(v->meta, v->mb, v->geo.voxel_length, v->geo.unit_shift, !mesh, v->h_totals[kMtVertexBlocks], cs,
+                                     v->cfg.color_f64 != 0));
     if (mesh) B2V_CUDA(v, launch_mesh_triangles(v->mb, v->h_totals[kMtTriangleBlocks], cs));
     B2V_CUDA(v, cudaStreamSynchronize(cs));
     v->launches += mesh ? 6 : 5;
@@ -1314,7 +1318,7 @@ extern "C" int b2v_export_halo_device(b2v_volume *v, int32_t world, int64_t *rec
                 v->err = "b2v_export_halo_device: destination too small";
                 out = B2V_ERR_INVALID_ARGUMENT;
             } else {
-                e = launch_halo_emit(v->meta, nb, world, d_offs.get(), d_headers, d_payload, cs);
+                e = launch_halo_emit(v->meta, nb, world, d_offs.get(), d_headers, d_payload, cs, v->cfg.color_f64 != 0);
                 if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
             }
         }
@@ -1378,7 +1382,7 @@ static int extract_with_halo(b2v_volume *v, bool mesh, int64_t n_records, const 
     if (e == cudaSuccess) e = cudaMemsetAsync(h->meta.counters, 0, kNumCounters * sizeof(uint32_t), cs);
     if (e == cudaSuccess)
         e = launch_halo_import(v->meta, nb, d_headers, d_payload, nr, d_sizes.get(), d_offs.get(), d_part.get(),
-                               d_tot.get(), h->table, h->meta, cs);
+                               d_tot.get(), h->table, h->meta, cs, v->cfg.color_f64 != 0);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h->meta.counters + kCtrPool, &head[0], sizeof(uint32_t), cudaMemcpyHostToDevice, cs);
     if (e == cudaSuccess) e = cudaMemcpyAsync(&head[1], h->meta.counters + kCtrError, sizeof(uint32_t), cudaMemcpyDeviceToHost, cs);
     if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
@@ -1387,7 +1391,7 @@ static int extract_with_halo(b2v_volume *v, bool mesh, int64_t n_records, const 
         return B2V_ERR_CUDA;
     }
     if (head[1]) {
-        v->err = (head[1] & 4u) ? "halo import: a record has an invalid mask"
+        v->err = (head[1] & 4u) ? "halo import: a record has an invalid mask (or another colour precision)"
                  : (head[1] & 8u) ? "halo import: a block key arrived twice (records of another world size?)"
                                   : "halo import: scratch table full";
         return B2V_ERR_INVALID_ARGUMENT;

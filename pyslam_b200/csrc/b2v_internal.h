@@ -173,10 +173,34 @@ struct GroupArgs {
     int32_t count;
 };
 
+// Block layout of the TSDF pool, by colour type TC.  Every block holds the tsdf and weight float32 planes, then the
+// r, g, b planes of TC (voxel index lx + 8 ly + 64 lz in each plane).  TC = float is the default volume: five float32
+// planes, kBlockFloats floats (10 KiB) per block.  TC = double is the float64-colour volume (b2v_config.color_f64):
+// Open3D's Vector3d colour, 16 KiB per block.  Every kernel that reads or writes the pool has its body templated on
+// TC and two entry points: `name` (float, the default volume's kernel as it always was) and `name_c64` (double).
+template <typename TC> struct TsdfBlock {
+    static constexpr int kFloats = 2 * kVox + 3 * kVox * static_cast<int>(sizeof(TC) / sizeof(float));
+    static constexpr size_t kBytes = static_cast<size_t>(kFloats) * sizeof(float);
+    // colour plane c (0 = r) of the block at blk
+    __host__ __device__ static TC *color(float *blk, int c) { return reinterpret_cast<TC *>(blk + 2 * kVox) + c * kVox; }
+    __host__ __device__ static const TC *color(const float *blk, int c) {
+        return reinterpret_cast<const TC *>(blk + 2 * kVox) + c * kVox;
+    }
+    // colour c of voxel v of the block at blk
+    __host__ __device__ static TC color_at(const float *blk, int c, int v) {
+        if constexpr (sizeof(TC) == sizeof(float)) return blk[(2 + c) * kVox + v];
+        else return color(blk, c)[v];
+    }
+};
+static_assert(TsdfBlock<float>::kFloats == kBlockFloats && TsdfBlock<double>::kBytes == 16384, "block layouts");
+inline size_t tsdf_block_bytes(bool color_f64) {
+    return color_f64 ? TsdfBlock<double>::kBytes : TsdfBlock<float>::kBytes;
+}
+
 // Device-resident bookkeeping of one volume.  Everything indexed by table slot or pool index is sized for the
 // maximum capacity; only the pool's storage grows (a growable volume maps it on demand, see b2v_api.cu).
 struct PoolMeta {
-    float *pool;              // [pool_capacity][5][512] float32 planes: tsdf, weight, r, g, b
+    float *pool;              // [pool_capacity] blocks of TsdfBlock<TC>::kFloats floats (see TsdfBlock)
     int4 *block_keys;         // [capacity] key of pool block i (w unused)
     uint32_t *counters;       // device counters, see Counter
     uint32_t *group_mask;     // [kGroupBufs][table capacity] bit k: the slot is touched by frame k of the group
@@ -277,24 +301,25 @@ cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &t
                                   const PoolMeta &meta, int sm_count, cudaStream_t stream);
 // projective TSDF + colour update of every block touched by the one-frame group in group buffer group_buf
 // (frame 0 of args)
+// color_f64: the volume's colour type (TsdfBlock), here and in every launcher below that takes it
 cudaError_t launch_integrate(const GroupArgs &args, const HashTable &table, const PoolMeta &meta, int group_buf,
-                             int grid_ctas, cudaStream_t stream);
-int integrate_max_resident_ctas_per_sm();
+                             int grid_ctas, cudaStream_t stream, bool color_f64);
+int integrate_max_resident_ctas_per_sm(bool color_f64);
 // d_bad[0]: reciprocals (3 x 2^23 inputs), d_bad[1]: quotients (`pairs` inputs) whose fast path differs from IEEE
 cudaError_t launch_selftest_division(unsigned long long *d_bad, uint64_t pairs, cudaStream_t stream);
 // fused update of a group of frames (each block is read and written once per group)
 cudaError_t launch_integrate_group(const GroupArgs &args, const HashTable &table, const PoolMeta &meta,
-                                   int group_buf, int grid_ctas, int sm_count, cudaStream_t stream);
+                                   int group_buf, int grid_ctas, int sm_count, cudaStream_t stream, bool color_f64);
 // keys of the slots in a touched list
 cudaError_t launch_gather_active_keys(const HashTable &table, const uint32_t *slots,
                                       uint32_t n, int4 *out, cudaStream_t stream);
 
-// find-or-create the blocks of `keys` (unique) and copy `vox` [n][5][512] into them
+// find-or-create the blocks of `keys` (unique) and copy `vox` (n blocks in the pool's layout) into them
 // the largest weight a voxel may hold: w + 1 is exact below it and rounds back to it there (integration saturates)
 constexpr float kWeightMax = 16777216.0f;  // 2^24
-cudaError_t launch_upload_check(const float *vox, uint32_t n, uint32_t *bad, cudaStream_t stream);
+cudaError_t launch_upload_check(const float *vox, uint32_t n, uint32_t *bad, cudaStream_t stream, bool color_f64);
 cudaError_t launch_upload_blocks(const int4 *keys, const float *vox, uint32_t n, uint32_t *scratch_idx,
-                                 const HashTable &table, const PoolMeta &meta, cudaStream_t stream);
+                                 const HashTable &table, const PoolMeta &meta, cudaStream_t stream, bool color_f64);
 
 // ---- pool growth (growable volumes) ----
 // one thread, between a group's allocation and its update: if pool indices past the storage were handed out
@@ -332,14 +357,14 @@ enum MeshTotal : int { kMtVertices = 0, kMtTriangles = 1, kMtVertexBlocks = 2, k
 // neighbour lookup (7 hash probes per block) + candidate tiles from the blocks' sign summaries, then the
 // marching-cubes case per voxel + vertex ownership masks of the candidates (Open3D ExtractTriangleMesh semantics)
 cudaError_t launch_mesh_classify(const HashTable &table, const PoolMeta &meta, const MeshBuffers &mb, int grid_ctas,
-                                 cudaStream_t stream);
+                                 cudaStream_t stream, bool color_f64);
 // the same front end + zero-crossing masks of Open3D ExtractPointCloud (no cube validity requirement)
 cudaError_t launch_point_masks(const HashTable &table, const PoolMeta &meta, const MeshBuffers &mb, int grid_ctas,
-                               cudaStream_t stream);
+                               cudaStream_t stream, bool color_f64);
 // per-block sums + exclusive scans -> offs, totals
 cudaError_t launch_mesh_scan(const MeshBuffers &mb, int grid_ctas, cudaStream_t stream);
 cudaError_t launch_mesh_vertices(const PoolMeta &meta, const MeshBuffers &mb, double voxel_length, int unit_shift,
-                                 bool points, uint32_t work_blocks, cudaStream_t stream);
+                                 bool points, uint32_t work_blocks, cudaStream_t stream, bool color_f64);
 cudaError_t launch_mesh_triangles(const MeshBuffers &mb, uint32_t work_blocks, cudaStream_t stream);
 
 // ---- face-halo exchange of a sharded volume (b2v_shard.cu) ----
@@ -350,15 +375,23 @@ constexpr int kHaloMaxVoxels = 169;
 // dest_offs [2][world + 1]: the first record / payload voxel of each destination (index world: the totals)
 cudaError_t launch_halo_count(const PoolMeta &meta, uint32_t nb, uint32_t world, uint32_t *counts, uint32_t *offs,
                               uint32_t *partials, uint32_t *totals, uint32_t *dest_offs, cudaStream_t stream);
-// headers int32 [records][4] = {key x, y, z, mask}, payload float32 [voxels][5], at the positions of launch_halo_count
+// headers int32 [records][4] = {key x, y, z, mask}, payload [voxels][HaloVoxel<TC>::kWords], at the positions of
+// launch_halo_count.  A float64-colour volume sets kHaloColorF64 in every mask it sends and imports only such records.
+constexpr int kHaloColorF64 = B2V_HALO_COLOR_F64;
+template <typename TC> struct HaloVoxel {   // {tsdf, weight, r, g, b}: float32 tsdf, weight and colour of type TC
+    static constexpr int kWords = 2 + 3 * static_cast<int>(sizeof(TC) / sizeof(float));   // 5 or 8 float32 words
+    static constexpr int kMaskFlag = sizeof(TC) == sizeof(double) ? kHaloColorF64 : 0;
+};
+inline int halo_voxel_words(bool color_f64) { return color_f64 ? HaloVoxel<double>::kWords : HaloVoxel<float>::kWords; }
 cudaError_t launch_halo_emit(const PoolMeta &meta, uint32_t nb, uint32_t world, const uint32_t *offs, int32_t *headers,
-                             float *payload, cudaStream_t stream);
+                             float *payload, cudaStream_t stream, bool color_f64);
 // scratch dst := src blocks [0, n_owned) at the same pool indices + the records as zero-filled halo blocks at
 // [n_owned, n_owned + n_records); the table must be empty.  sizes / offs [n_records], partials, totals: scan scratch.
 // dst.counters[kCtrError]: bit 1 table full, bit 2 a record with a bad mask, bit 3 a key imported twice
 cudaError_t launch_halo_import(const PoolMeta &src, uint32_t n_owned, const int32_t *headers, const float *payload,
                                uint32_t n_records, uint32_t *sizes, uint32_t *offs, uint32_t *partials,
-                               uint32_t *totals, const HashTable &table, const PoolMeta &dst, cudaStream_t stream);
+                               uint32_t *totals, const HashTable &table, const PoolMeta &dst, cudaStream_t stream,
+                               bool color_f64);
 // weld of concatenated mesh pieces by edge id: vertices in order of first occurrence, triangles remapped
 struct WeldArgs {
     uint32_t nv, nt;

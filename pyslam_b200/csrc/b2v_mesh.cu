@@ -135,8 +135,8 @@ constexpr int kClsCtasPerSm = 10;  // 48 registers: the persistent grid is exact
 // merged into the global masks with one atomic per non-zero word; owners in a neighbouring block are set directly.
 // The own voxels of the CTA's next tile are loaded while the current one is classified.
 
-__global__ void __launch_bounds__(kClsThreads, kClsCtasPerSm)
-mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
+template <typename TC>
+__device__ __forceinline__ void mesh_classify_kernel_body(const PoolMeta M, const MeshBuffers mb) {
     __shared__ uint32_t s_neg[81], s_val[81];
     __shared__ uint32_t s_cube[kVox / 4];
     __shared__ uint32_t s_own[kVox / 4];
@@ -152,7 +152,7 @@ mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
     if (it < n) {
         b = cand[it];
         if (t < 8) nbr_t = mb.nbr[b * 8 + t];
-        const float *own = M.pool + static_cast<size_t>(b) * kBlockFloats;
+        const float *own = M.pool + static_cast<size_t>(b) * TsdfBlock<TC>::kFloats;
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             f0[k] = own[t + kClsThreads * k];
@@ -186,7 +186,7 @@ mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
         if (it_next < n) {
             b_next = cand[it_next];
             if (t < 8) nbr_t = mb.nbr[b_next * 8 + t];
-            const float *own = M.pool + static_cast<size_t>(b_next) * kBlockFloats;
+            const float *own = M.pool + static_cast<size_t>(b_next) * TsdfBlock<TC>::kFloats;
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 f0[k] = own[t + kClsThreads * k];
@@ -200,7 +200,7 @@ mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
             const int x = h & 15, y = (h >> 4) & 15, z = h >> 8;
             const int pb = s_nbr[(x >> 3) | ((y >> 3) << 1) | ((z >> 3) << 2)];
             if (pb >= 0) {
-                const float *blk = M.pool + static_cast<size_t>(pb) * kBlockFloats;
+                const float *blk = M.pool + static_cast<size_t>(pb) * TsdfBlock<TC>::kFloats;
                 const int v = (x & 7) + ((y & 7) << 3) + ((z & 7) << 6);
                 const float f = blk[v], w = blk[kVox + v];
                 if (f < 0.0f) atomicOr(&s_neg[y + 9 * z], 1u << x);
@@ -260,10 +260,20 @@ mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
     }
 }
 
+__global__ void __launch_bounds__(kClsThreads, kClsCtasPerSm)
+mesh_classify_kernel(const PoolMeta M, const MeshBuffers mb) {
+    mesh_classify_kernel_body<float>(M, mb);
+}
+// the float64-colour instantiation
+__global__ void __launch_bounds__(kClsThreads, kClsCtasPerSm)
+mesh_classify_kernel_c64(const PoolMeta M, const MeshBuffers mb) {
+    mesh_classify_kernel_body<double>(M, mb);
+}
+
 // ---- pass 1b: zero-crossing masks (point cloud) ---------------------------------------------
 
-__global__ void __launch_bounds__(kVox)
-point_masks_kernel(const PoolMeta M, const MeshBuffers mb) {
+template <typename TC>
+__device__ __forceinline__ void point_masks_kernel_body(const PoolMeta M, const MeshBuffers mb) {
     __shared__ int s_nbr[8];
     __shared__ uint8_t s_m[kVox];
     const int t = threadIdx.x;
@@ -273,7 +283,7 @@ point_masks_kernel(const PoolMeta M, const MeshBuffers mb) {
         const uint32_t b = cand[it];
         if (t < 8) s_nbr[t] = mb.nbr[b * 8 + t];
         __syncthreads();
-        const float *blk = M.pool + static_cast<size_t>(b) * kBlockFloats;
+        const float *blk = M.pool + static_cast<size_t>(b) * TsdfBlock<TC>::kFloats;
         const float f0 = blk[t], w0 = blk[kVox + t];
         const int l[3] = {t & 7, (t >> 3) & 7, t >> 6};
         unsigned m = 0;
@@ -284,7 +294,7 @@ point_masks_kernel(const PoolMeta M, const MeshBuffers mb) {
                 q[a] += 1;
                 const int pb = s_nbr[(q[0] >> 3) | ((q[1] >> 3) << 1) | ((q[2] >> 3) << 2)];
                 if (pb < 0) continue;
-                const float *nb = M.pool + static_cast<size_t>(pb) * kBlockFloats;
+                const float *nb = M.pool + static_cast<size_t>(pb) * TsdfBlock<TC>::kFloats;
                 const int v = (q[0] & 7) + ((q[1] & 7) << 3) + ((q[2] & 7) << 6);
                 const float f1 = nb[v], w1 = nb[kVox + v];
                 if (w1 != 0.0f && f1 < 0.98f && f1 >= -0.98f && f0 * f1 < 0.0f) m |= 1u << a;
@@ -301,6 +311,16 @@ point_masks_kernel(const PoolMeta M, const MeshBuffers mb) {
         }
         __syncthreads();
     }
+}
+
+__global__ void __launch_bounds__(kVox)
+point_masks_kernel(const PoolMeta M, const MeshBuffers mb) {
+    point_masks_kernel_body<float>(M, mb);
+}
+// the float64-colour instantiation
+__global__ void __launch_bounds__(kVox)
+point_masks_kernel_c64(const PoolMeta M, const MeshBuffers mb) {
+    point_masks_kernel_body<double>(M, mb);
 }
 
 // ---- pass 2: per-block sums and their exclusive scans ---------------------------------------
@@ -386,14 +406,15 @@ mesh_block_sums_kernel(const MeshBuffers mb) {
 //     pt = vl/2 + vl * e;  pt[a] += |f0| vl / (|f0| + |f1|);  colour (|f1| c0/255 + |f0| c1/255) / (|f0| + |f1|)
 // points = true: ExtractPointCloud: p0 = (vl/2 + vl * x_in_unit) + unit * L, p1 = p0 + vl on the axis,
 //     p = (p0 r1 + p1 r0) / (r0 + r1) with float32 r0 = |f0|, r1 = |f1| (their sum in float32), colour
-//     ((c0 r1 + c1 r0) / (r0 + r1)) / 255 in float32, widened
+//     ((c0 r1 + c1 r0) / (r0 + r1)) / 255 in float32, widened.  With float64 colour (TC = double) the colour terms
+//     are float64: c r widens r, the sum r0 + r1 is widened after its float32 add, and 255 is widened.
 // One CTA per block with output.  The block's vertices are first listed in shared memory at the positions pass 2 gave
 // them, then every lane emits one listed vertex: no lane idles on a voxel without output, stores are consecutive.
 constexpr int kEmitThreads = 128;
 
-template <bool kPoints>
-__global__ void __launch_bounds__(kEmitThreads)
-mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, const int unit_shift) {
+template <typename TC, bool kPoints>
+__device__ __forceinline__ void mesh_vertices_kernel_body(const PoolMeta M, const MeshBuffers mb, const double vl,
+                                                          const int unit_shift) {
     __shared__ unsigned short s_list[3 * kVox];   // voxel << 2 | axis
     const uint32_t b = mb.work[blockIdx.x];       // blocks with at least one vertex
     const int t = threadIdx.x;
@@ -414,14 +435,15 @@ mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, co
     const uint32_t nv = mb.sums[b];
     const uint32_t vbase = mb.offs[b];
     const int *nbr = mb.nbr + static_cast<size_t>(b) * 8;
-    const float *blk = M.pool + static_cast<size_t>(b) * kBlockFloats;
+    const float *blk = M.pool + static_cast<size_t>(b) * TsdfBlock<TC>::kFloats;
     const int4 key = M.block_keys[b];
     const double half = __dmul_rn(vl, 0.5);
     for (uint32_t i = t; i < nv; i += kEmitThreads) {
         const int en = s_list[i];
         const int v0 = en >> 2, a = en & 3;
         const float r0 = fabsf(blk[v0]);
-        const float c0[3] = {blk[2 * kVox + v0], blk[3 * kVox + v0], blk[4 * kVox + v0]};
+        const TC c0[3] = {TsdfBlock<TC>::color_at(blk, 0, v0), TsdfBlock<TC>::color_at(blk, 1, v0),
+                          TsdfBlock<TC>::color_at(blk, 2, v0)};
         const int l[3] = {v0 & 7, (v0 >> 3) & 7, v0 >> 6};
         const int g[3] = {key.x * kB + l[0], key.y * kB + l[1], key.z * kB + l[2]};
         double p[3];
@@ -440,7 +462,7 @@ mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, co
         }
         const int q[3] = {l[0] + (a == 0), l[1] + (a == 1), l[2] + (a == 2)};
         const int pb = nbr[(q[0] >> 3) | ((q[1] >> 3) << 1) | ((q[2] >> 3) << 2)];
-        const float *nb = M.pool + static_cast<size_t>(pb) * kBlockFloats;
+        const float *nb = M.pool + static_cast<size_t>(pb) * TsdfBlock<TC>::kFloats;
         const int v1 = (q[0] & 7) + ((q[1] & 7) << 3) + ((q[2] & 7) << 6);
         const float r1 = fabsf(nb[v1]);
         const double pa = a == 0 ? p[0] : (a == 1 ? p[1] : p[2]);
@@ -452,9 +474,15 @@ mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, co
                            static_cast<double>(rs));
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
-                const float c1 = nb[(2 + k) * kVox + v1];
-                const float num = __fadd_rn(__fmul_rn(c0[k], r1), __fmul_rn(c1, r0));
-                col[k] = static_cast<double>(__fdiv_rn(__fdiv_rn(num, rs), 255.0f));
+                const TC c1 = TsdfBlock<TC>::color_at(nb, k, v1);
+                if constexpr (std::is_same<TC, float>::value) {
+                    const float num = __fadd_rn(__fmul_rn(c0[k], r1), __fmul_rn(c1, r0));
+                    col[k] = static_cast<double>(__fdiv_rn(__fdiv_rn(num, rs), 255.0f));
+                } else {
+                    const double num = __dadd_rn(__dmul_rn(c0[k], static_cast<double>(r1)),
+                                                 __dmul_rn(c1, static_cast<double>(r0)));
+                    col[k] = __ddiv_rn(__ddiv_rn(num, static_cast<double>(rs)), 255.0);
+                }
             }
         } else {
             const double f0 = static_cast<double>(r0), f1 = static_cast<double>(r1);
@@ -463,7 +491,7 @@ mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, co
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 const double d0 = __ddiv_rn(static_cast<double>(c0[k]), 255.0);
-                const double d1 = __ddiv_rn(static_cast<double>(nb[(2 + k) * kVox + v1]), 255.0);
+                const double d1 = __ddiv_rn(static_cast<double>(TsdfBlock<TC>::color_at(nb, k, v1)), 255.0);
                 col[k] = __ddiv_rn(__dadd_rn(__dmul_rn(f1, d0), __dmul_rn(f0, d1)), fs);
             }
         }
@@ -478,6 +506,18 @@ mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, co
         }
         reinterpret_cast<int4 *>(mb.edge_ids)[vid] = make_int4(g[0], g[1], g[2], a);
     }
+}
+
+template <bool kPoints>
+__global__ void __launch_bounds__(kEmitThreads)
+mesh_vertices_kernel(const PoolMeta M, const MeshBuffers mb, const double vl, const int unit_shift) {
+    mesh_vertices_kernel_body<float, kPoints>(M, mb, vl, unit_shift);
+}
+// the float64-colour instantiation
+template <bool kPoints>
+__global__ void __launch_bounds__(kEmitThreads)
+mesh_vertices_kernel_c64(const PoolMeta M, const MeshBuffers mb, const double vl, const int unit_shift) {
+    mesh_vertices_kernel_body<double, kPoints>(M, mb, vl, unit_shift);
 }
 
 // ---- pass 3b: triangles ----------------------------------------------------------------------
@@ -547,20 +587,20 @@ static cudaError_t launch_mesh_front(const HashTable &table, const PoolMeta &met
 }
 
 cudaError_t launch_mesh_classify(const HashTable &table, const PoolMeta &meta, const MeshBuffers &mb, int sms,
-                                 cudaStream_t stream) {
+                                 cudaStream_t stream, bool color_f64) {
     cudaError_t e = launch_mesh_front(table, meta, mb, stream);
     if (e != cudaSuccess || mb.n_blocks == 0) return e;
     const unsigned grid = min(mb.n_blocks, static_cast<unsigned>(sms) * kClsCtasPerSm);
-    mesh_classify_kernel<<<grid, kClsThreads, 0, stream>>>(meta, mb);
+    (color_f64 ? mesh_classify_kernel_c64 : mesh_classify_kernel)<<<grid, kClsThreads, 0, stream>>>(meta, mb);
     return cudaGetLastError();
 }
 
 cudaError_t launch_point_masks(const HashTable &table, const PoolMeta &meta, const MeshBuffers &mb, int sms,
-                               cudaStream_t stream) {
+                               cudaStream_t stream, bool color_f64) {
     cudaError_t e = launch_mesh_front(table, meta, mb, stream);
     if (e != cudaSuccess || mb.n_blocks == 0) return e;
     const unsigned grid = min(mb.n_blocks, static_cast<unsigned>(sms) * (2048u / kVox));
-    point_masks_kernel<<<grid, kVox, 0, stream>>>(meta, mb);
+    (color_f64 ? point_masks_kernel_c64 : point_masks_kernel)<<<grid, kVox, 0, stream>>>(meta, mb);
     return cudaGetLastError();
 }
 
@@ -575,12 +615,11 @@ cudaError_t launch_mesh_scan(const MeshBuffers &mb, int sms, cudaStream_t stream
 }
 
 cudaError_t launch_mesh_vertices(const PoolMeta &meta, const MeshBuffers &mb, double voxel_length, int unit_shift,
-                                 bool points, uint32_t work_blocks, cudaStream_t stream) {
+                                 bool points, uint32_t work_blocks, cudaStream_t stream, bool color_f64) {
     if (work_blocks == 0) return cudaSuccess;
-    if (points)
-        mesh_vertices_kernel<true><<<work_blocks, kEmitThreads, 0, stream>>>(meta, mb, voxel_length, unit_shift);
-    else
-        mesh_vertices_kernel<false><<<work_blocks, kEmitThreads, 0, stream>>>(meta, mb, voxel_length, unit_shift);
+    const auto kernel = points ? (color_f64 ? mesh_vertices_kernel_c64<true> : mesh_vertices_kernel<true>)
+                               : (color_f64 ? mesh_vertices_kernel_c64<false> : mesh_vertices_kernel<false>);
+    kernel<<<work_blocks, kEmitThreads, 0, stream>>>(meta, mb, voxel_length, unit_shift);
     return cudaGetLastError();
 }
 

@@ -4,7 +4,8 @@
 // only the voxels whose local coordinate is 0 on every axis where o is 1: a 64-voxel face, an 8-voxel line or one
 // corner voxel.  A rank therefore sends, for each owned block H and each rank r != own owning some H-o, ONE record:
 // the header {key.x, key.y, key.z, mask} (bit o-1 of the 7-bit mask: r owns H-o) and the union of the needed voxels
-// in increasing voxel index (at most 169 voxels, 5 float32 channels each: tsdf, weight, r, g, b).  Records are grouped
+// in increasing voxel index (at most 169 voxels of HaloVoxel<TC>::kWords float32 words each: tsdf, weight, r, g, b,
+// the colour as float32 or, in a float64-colour volume, as float64 with kHaloColorF64 set in the mask).  Records are grouped
 // by destination, and inside a destination ordered by the sender's pool index (count -> scan -> emit).
 //
 // The receiver imports its own blocks (pool indices [0, n_owned)) and the records as zero-filled halo blocks after
@@ -97,7 +98,51 @@ __global__ void halo_dest_offsets_kernel(const uint32_t *__restrict__ offs, cons
     out[world + 1 + r] = r < world ? offs[plane + static_cast<size_t>(r) * nb] : totals[1];
 }
 
+// one voxel of a float64-colour block as a halo payload record {tsdf, weight, r, g, b as float64} and back (the
+// default volume's kernels copy its five float32 planes in place)
+__device__ __forceinline__ void halo_put_f64(float *out, const float *blk, const int v) {
+    out[0] = blk[v];
+    out[1] = blk[kVox + v];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) reinterpret_cast<double *>(out + 2)[c] = TsdfBlock<double>::color(blk, c)[v];
+}
+// voxel q of a record's payload `in` into voxel v of the block at blk
+__device__ __forceinline__ void halo_get_f64(float *blk, const float *in, const uint32_t q, const int v) {
+    constexpr int kWords = HaloVoxel<double>::kWords;
+    blk[v] = in[q * kWords];
+    blk[kVox + v] = in[q * kWords + 1];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        TsdfBlock<double>::color(blk, c)[v] = reinterpret_cast<const double *>(in + q * kWords + 2)[c];
+}
+
 // one CTA per owned block: its records' headers and voxels at the positions the scan gave them
+template <typename TC>   // TC = double: the float64-colour kernel
+__device__ __forceinline__ void halo_emit_kernel_body(const PoolMeta M, uint32_t nb, uint32_t world,
+                                                      const uint32_t *__restrict__ offs, int4 *__restrict__ headers,
+                                                      float *__restrict__ payload) {
+    constexpr int kWords = HaloVoxel<TC>::kWords;
+    const uint32_t b = blockIdx.x;
+    const int4 k = M.block_keys[b];
+    uint32_t dest[7], masks[7];
+    const int n = halo_dests(k, world, dest, masks);
+    const size_t plane = static_cast<size_t>(world) * nb;
+    const float *blk = M.pool + static_cast<size_t>(b) * TsdfBlock<TC>::kFloats;
+    for (int j = 0; j < n; ++j) {
+        const size_t i = static_cast<size_t>(dest[j]) * nb + b;
+        const uint32_t rec = offs[i];
+        const size_t voff = offs[plane + i];
+        if (threadIdx.x == 0)
+            headers[rec] = make_int4(k.x, k.y, k.z, static_cast<int>(masks[j]) | HaloVoxel<TC>::kMaskFlag);
+        const uint32_t cnt = g_halo_cnt[masks[j]];
+        for (uint32_t q = threadIdx.x; q < cnt; q += blockDim.x) {
+            const int v = g_halo_vox[masks[j]][q];
+            halo_put_f64(payload + (voff + q) * kWords, blk, v);
+        }
+    }
+}
+
+// the default volume's kernel, written out (as an inlined body it would compile to different SASS)
 __global__ void __launch_bounds__(128)
 halo_emit_kernel(const PoolMeta M, uint32_t nb, uint32_t world, const uint32_t *__restrict__ offs,
                  int4 *__restrict__ headers, float *__restrict__ payload) {
@@ -121,6 +166,12 @@ halo_emit_kernel(const PoolMeta M, uint32_t nb, uint32_t world, const uint32_t *
         }
     }
 }
+// the float64-colour instantiation
+__global__ void __launch_bounds__(128)
+halo_emit_kernel_c64(const PoolMeta M, uint32_t nb, uint32_t world, const uint32_t *__restrict__ offs,
+                 int4 *__restrict__ headers, float *__restrict__ payload) {
+    halo_emit_kernel_body<double>(M, nb, world, offs, headers, payload);
+}
 
 cudaError_t launch_halo_count(const PoolMeta &meta, uint32_t nb, uint32_t world, uint32_t *counts, uint32_t *offs,
                               uint32_t *partials, uint32_t *totals, uint32_t *dest_offs, cudaStream_t stream) {
@@ -142,9 +193,10 @@ cudaError_t launch_halo_count(const PoolMeta &meta, uint32_t nb, uint32_t world,
 }
 
 cudaError_t launch_halo_emit(const PoolMeta &meta, uint32_t nb, uint32_t world, const uint32_t *offs, int32_t *headers,
-                             float *payload, cudaStream_t stream) {
+                             float *payload, cudaStream_t stream, bool color_f64) {
     if (nb == 0) return cudaSuccess;
-    halo_emit_kernel<<<nb, 128, 0, stream>>>(meta, nb, world, offs, reinterpret_cast<int4 *>(headers), payload);
+    (color_f64 ? halo_emit_kernel_c64 : halo_emit_kernel)<<<nb, 128, 0, stream>>>(
+        meta, nb, world, offs, reinterpret_cast<int4 *>(headers), payload);
     return cudaGetLastError();
 }
 
@@ -163,29 +215,89 @@ __device__ __forceinline__ void insert_at(const HashTable &T, const PoolMeta &D,
 }
 
 // one CTA per owned block: the live block b becomes scratch block b (voxels, sign summary, table entry)
-__global__ void __launch_bounds__(128)
-halo_copy_owned_kernel(const PoolMeta S, const HashTable T, const PoolMeta D) {
+template <typename TC>
+__device__ __forceinline__ void halo_copy_owned_kernel_body(const PoolMeta S, const HashTable T, const PoolMeta D) {
+    constexpr int kFloats = TsdfBlock<TC>::kFloats;
     const uint32_t b = blockIdx.x;
-    const float4 *src = reinterpret_cast<const float4 *>(S.pool + static_cast<size_t>(b) * kBlockFloats);
-    float4 *dst = reinterpret_cast<float4 *>(D.pool + static_cast<size_t>(b) * kBlockFloats);
-    for (int i = threadIdx.x; i < kBlockFloats / 4; i += blockDim.x) dst[i] = src[i];
+    const float4 *src = reinterpret_cast<const float4 *>(S.pool + static_cast<size_t>(b) * kFloats);
+    float4 *dst = reinterpret_cast<float4 *>(D.pool + static_cast<size_t>(b) * kFloats);
+    for (int i = threadIdx.x; i < kFloats / 4; i += blockDim.x) dst[i] = src[i];
     if (threadIdx.x == 0) {
         D.block_flags[b] = S.block_flags[b];
         insert_at(T, D, S.block_keys[b], b);
     }
 }
 
+__global__ void __launch_bounds__(128)
+halo_copy_owned_kernel(const PoolMeta S, const HashTable T, const PoolMeta D) {
+    halo_copy_owned_kernel_body<float>(S, T, D);
+}
+// the float64-colour instantiation
+__global__ void __launch_bounds__(128)
+halo_copy_owned_kernel_c64(const PoolMeta S, const HashTable T, const PoolMeta D) {
+    halo_copy_owned_kernel_body<double>(S, T, D);
+}
+
 // counts[j] = voxels of record j (the receiver's payload offsets come from their scan); a bad mask counts 0 and is
-// reported by the import
-__global__ void halo_record_sizes_kernel(const int4 *__restrict__ headers, uint32_t n, uint32_t *__restrict__ counts) {
+// reported by the import.  A record of the other colour type (kHaloColorF64 set or missing) has a bad mask.
+template <typename TC>
+__device__ __forceinline__ void halo_record_sizes_kernel_body(const int4 *__restrict__ headers, uint32_t n,
+                                                              uint32_t *__restrict__ counts) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
-    const int m = headers[j].w;
+    const int m = headers[j].w - HaloVoxel<TC>::kMaskFlag;
     counts[j] = (m > 0 && m < 128) ? g_halo_cnt[m] : 0u;
+}
+
+__global__ void
+halo_record_sizes_kernel(const int4 *__restrict__ headers, uint32_t n, uint32_t *__restrict__ counts) {
+    halo_record_sizes_kernel_body<float>(headers, n, counts);
+}
+// the float64-colour instantiation
+__global__ void
+halo_record_sizes_kernel_c64(const int4 *__restrict__ headers, uint32_t n, uint32_t *__restrict__ counts) {
+    halo_record_sizes_kernel_body<double>(headers, n, counts);
 }
 
 // one CTA per record: a zero-filled block at pool index base + j with the record's voxels scattered into it; its sign
 // summary is computed from what was written
+template <typename TC>   // TC = double: the float64-colour kernel
+__device__ __forceinline__ void halo_import_kernel_body(const int4 *__restrict__ headers,
+                                                        const float *__restrict__ payload,
+                                                        const uint32_t *__restrict__ offs, uint32_t base,
+                                                        const HashTable T, const PoolMeta D) {
+    constexpr int kFloats = TsdfBlock<TC>::kFloats, kWords = HaloVoxel<TC>::kWords;
+    const uint32_t j = blockIdx.x;
+    const int4 h = headers[j];
+    const int hm = h.w - HaloVoxel<TC>::kMaskFlag;
+    const uint32_t idx = base + j;
+    float *blk = D.pool + static_cast<size_t>(idx) * kFloats;
+    float4 *b4 = reinterpret_cast<float4 *>(blk);
+    for (int i = threadIdx.x; i < kFloats / 4; i += blockDim.x) b4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    __syncthreads();
+    const bool ok = hm > 0 && hm < 128;
+    bool neg = false, pos = false;
+    if (ok) {
+        const uint32_t cnt = g_halo_cnt[hm];
+        const float *in = payload + static_cast<size_t>(offs[j]) * kWords;
+        for (uint32_t q = threadIdx.x; q < cnt; q += blockDim.x) {
+            const int v = g_halo_vox[hm][q];
+            halo_get_f64(blk, in, q, v);
+            const float f = in[q * kWords], w = in[q * kWords + 1];
+            neg |= w != 0.0f && f < 0.0f;
+            pos |= w != 0.0f && !(f < 0.0f);
+        }
+    }
+    const int any_neg = __syncthreads_or(neg);
+    const int any_pos = __syncthreads_or(pos);
+    if (threadIdx.x == 0) {
+        if (!ok) atomicOr(D.counters + kCtrError, 4u);
+        D.block_flags[idx] = (any_neg ? 1u : 0u) | (any_pos ? 2u : 0u);
+        insert_at(T, D, make_int4(h.x, h.y, h.z, 0), idx);
+    }
+}
+
+// the default volume's kernel, written out (as an inlined body it would compile to different SASS)
 __global__ void __launch_bounds__(128)
 halo_import_kernel(const int4 *__restrict__ headers, const float *__restrict__ payload, const uint32_t *__restrict__ offs,
                    uint32_t base, const HashTable T, const PoolMeta D) {
@@ -218,20 +330,30 @@ halo_import_kernel(const int4 *__restrict__ headers, const float *__restrict__ p
         insert_at(T, D, make_int4(h.x, h.y, h.z, 0), idx);
     }
 }
+// the float64-colour instantiation
+__global__ void __launch_bounds__(128)
+halo_import_kernel_c64(const int4 *__restrict__ headers, const float *__restrict__ payload, const uint32_t *__restrict__ offs,
+                   uint32_t base, const HashTable T, const PoolMeta D) {
+    halo_import_kernel_body<double>(headers, payload, offs, base, T, D);
+}
 
 cudaError_t launch_halo_import(const PoolMeta &src, uint32_t n_owned, const int32_t *headers, const float *payload,
                                uint32_t n_records, uint32_t *sizes, uint32_t *offs, uint32_t *partials,
-                               uint32_t *totals, const HashTable &table, const PoolMeta &dst, cudaStream_t stream) {
+                               uint32_t *totals, const HashTable &table, const PoolMeta &dst, cudaStream_t stream,
+                               bool color_f64) {
     cudaError_t e = upload_halo_tables_once();
     if (e != cudaSuccess) return e;
-    if (n_owned) halo_copy_owned_kernel<<<n_owned, 128, 0, stream>>>(src, table, dst);
+    if (n_owned)
+        (color_f64 ? halo_copy_owned_kernel_c64 : halo_copy_owned_kernel)<<<n_owned, 128, 0, stream>>>(src, table, dst);
     if (n_records) {
         const int4 *h4 = reinterpret_cast<const int4 *>(headers);
-        halo_record_sizes_kernel<<<(n_records + 255) / 256, 256, 0, stream>>>(h4, n_records, sizes);
+        (color_f64 ? halo_record_sizes_kernel_c64 : halo_record_sizes_kernel)<<<(n_records + 255) / 256, 256, 0,
+                                                                                stream>>>(h4, n_records, sizes);
         const dim3 chunks((n_records + 1023) / 1024, 1);
         scan_reduce_kernel<<<chunks, 1024, 0, stream>>>(sizes, partials, n_records);
         scan_apply_kernel<<<chunks, 1024, 0, stream>>>(sizes, offs, partials, totals, n_records);
-        halo_import_kernel<<<n_records, 128, 0, stream>>>(h4, payload, offs, n_owned, table, dst);
+        (color_f64 ? halo_import_kernel_c64 : halo_import_kernel)<<<n_records, 128, 0, stream>>>(h4, payload, offs,
+                                                                                                 n_owned, table, dst);
     }
     return cudaGetLastError();
 }

@@ -51,6 +51,9 @@ DEFAULT_PARAMETERS = {
     # SAVE also writes the map's state beside dense_map.ply (dense_map.state.npz), which LOAD restores; off by default:
     # the file is as large as the map (10 KiB per TSDF block)
     "kVolumetricIntegrationB200SaveMapState": False,
+    # keep each voxel's colour as Open3D does, a float64 running mean: voxel, mesh and point-cloud colours equal
+    # Open3D's bit for bit, at 16 KiB per block instead of 10 KiB (INTEGRATION.md section 2)
+    "kVolumetricIntegrationB200ColorFloat64": False,
 }
 
 
@@ -273,7 +276,8 @@ def make_integrator_class(Base, api):
                 depth_trunc=self.volumetric_integration_depth_trunc,
                 capacity_blocks=int(p["kVolumetricIntegrationB200CapacityBlocks"]),
                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None,
-                volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]), **self._map_placement())
+                volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]),
+                color_float64=bool(p["kVolumetricIntegrationB200ColorFloat64"]), **self._map_placement())
             self.last_output = None
             self.last_integrated_id = -1
             self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call

@@ -212,7 +212,8 @@ def gather_blocks(keys, vox, dst: int = 0, group=None, device=None):
 def gather_blocks_device(volume, dst: int = 0, group=None):
     """Device-resident gather over NCCL: every rank exports its blocks device-to-device
     (`b2v_export_blocks`), the payloads travel GPU to GPU (NVLink), nothing touches host memory.
-    Returns (keys int32 [n,4], vox float32 [n,5,512]) CUDA tensors on dst, (None, None) elsewhere."""
+    Returns (keys int32 [n,4], vox float32 [n,5,512], or a float64-colour volume's raw layout [n,4096]) CUDA tensors
+    on dst, (None, None) elsewhere."""
     import torch
     import torch.distributed as dist
 
@@ -249,9 +250,9 @@ def extract_mesh_distributed(volume, dst: int = 0, group=None, device=None, capa
     on_device = dist.get_backend(group) == "nccl"
     if on_device:
         keys, vox = gather_blocks_device(volume, dst=dst, group=group)
-    else:
-        d = volume.dump_blocks()
-        keys, vox = gather_blocks(d["keys"], d["vox"], dst=dst, group=group, device=device)
+    else:   # the blocks in the volume's raw layout, which gather_blocks moves word for word
+        keys4, raw = volume._export_blocks(np.empty)
+        keys, vox = gather_blocks(keys4[:, :3], raw, dst=dst, group=group, device=device)
     if dist.get_rank(group) != dst:
         return None
     cap = capacity_blocks or max(2 * len(keys), 1024)
@@ -261,14 +262,15 @@ def extract_mesh_distributed(volume, dst: int = 0, group=None, device=None, capa
             scratch.close()
         scratch = B200TsdfVolume(volume.voxel_length, volume.sdf_trunc, volume.depth_trunc,
                                  capacity_blocks=cap, device=volume.device,
-                                 volume_unit_resolution=volume.volume_unit_resolution)
+                                 volume_unit_resolution=volume.volume_unit_resolution,
+                                 color_float64=volume.color_float64)
         volume._mesh_scratch = scratch
     else:
         scratch.reset()
     if on_device:
         scratch.import_blocks_torch(keys, vox)
     else:
-        scratch.upload_blocks(keys, vox)
+        scratch._upload_raw(keys, vox)
     return scratch.extract_mesh()
 
 
@@ -276,7 +278,8 @@ def extract_mesh_distributed(volume, dst: int = 0, group=None, device=None, capa
 
 def halo_records(volume, world: int):
     """The halo records `volume` (one shard of a `world`-rank sharding) sends each rank: a list of `world` pairs
-    (headers int32 [n,4] = {x,y,z,mask}, payload float32 [m,5]) of CUDA tensors; the volume's own rank gets empty ones."""
+    (headers int32 [n,4] = {x,y,z,mask}, payload float32 [m,5], or [m,8] with float64 colour) of CUDA tensors; the
+    volume's own rank gets empty ones."""
     headers, payload, nrec, nvox = volume.export_halo_torch(world)
     return list(zip(headers.split(nrec), payload.split(nvox)))
 
@@ -290,7 +293,7 @@ def _concat_records(records):
     if not records:
         return torch.zeros((0, 4), dtype=torch.int32), torch.zeros((0, 5), dtype=torch.float32)
     return torch.cat([torch.as_tensor(h).reshape(-1, 4) for h, _ in records]), \
-        torch.cat([torch.as_tensor(x).reshape(-1, 5) for _, x in records])
+        torch.cat([torch.as_tensor(x).reshape(-1, torch.as_tensor(x).shape[-1]) for _, x in records])
 
 
 def mesh_piece(volume, records):
@@ -348,17 +351,20 @@ def _exchange_halo(volume, group):
     headers, payload, nrec, nvox = volume.export_halo_torch(world)
     dev = headers.device if on_device else torch.device("cpu")
     headers, payload = headers.to(dev), payload.to(dev)
-    mine = torch.tensor([nrec, nvox], dtype=torch.int64, device=dev)
+    # row 2: the payload's words per voxel, which tell the ranks' colour precisions apart
+    mine = torch.tensor([nrec, nvox, [payload.shape[1]] * world], dtype=torch.int64, device=dev)
     sizes = [torch.zeros_like(mine) for _ in range(world)]
     dist.all_gather(sizes, mine, group=group)
     sizes = [s.cpu() for s in sizes]
+    if any(int(sizes[s][2, 0]) != payload.shape[1] for s in range(world)):
+        raise ValueError("the ranks of a sharded volume must all keep float32 colour or all float64 colour")
     in_rec = [int(sizes[s][0, rank]) for s in range(world)]
     in_vox = [int(sizes[s][1, rank]) for s in range(world)]
     rh = torch.empty((sum(in_rec), 4), dtype=torch.int32, device=dev)
     rx = torch.empty((sum(in_vox), payload.shape[1]), dtype=torch.float32, device=dev)
     dist.all_to_all_single(rh, headers, output_split_sizes=in_rec, input_split_sizes=nrec, group=group)
     dist.all_to_all_single(rx, payload, output_split_sizes=in_vox, input_split_sizes=nvox, group=group)
-    sent = [int(sizes[s][0].sum()) * 16 + int(sizes[s][1].sum()) * 20 for s in range(world)]
+    sent = [int(sizes[s][0].sum()) * 16 + int(sizes[s][1].sum()) * 4 * payload.shape[1] for s in range(world)]
     return rh, rx, sent
 
 

@@ -26,7 +26,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib, map_state
-from ._lib import B2VConfig, BLOCK_SIZE, BLOCK_VOXELS, VOXEL_PLANES
+from ._lib import B2VConfigEx, BLOCK_SIZE, BLOCK_VOXELS, VOXEL_PLANES
 
 
 def _as_K4(K) -> np.ndarray:
@@ -173,13 +173,17 @@ class B200TsdfVolume(_MapState):
     def __init__(self, voxel_length: float, sdf_trunc: float, depth_trunc: float = 4.0,
                  capacity_blocks: int = 1 << 18, device: int = 0, depth_sampling_stride: int = 4,
                  block_size: int = BLOCK_SIZE, shard_rank: int = 0, shard_count: int = 1,
-                 volume_unit_resolution: int = 16, max_capacity_blocks: int | None = None):
+                 volume_unit_resolution: int = 16, max_capacity_blocks: int | None = None,
+                 color_float64: bool = False):
         """`volume_unit_resolution`: Open3D's parameter of that name.  16 (the reference's value) allocates every
         8^3 block of each 16^3 unit `ScalableTSDFVolume::LocateVolumeUnit` touches - the same voxels Open3D updates;
         8 is SURVEY decision D1 (the float32 pyslam key range of the +-sdf_trunc box, ~9 % fewer blocks).
         `max_capacity_blocks`: growth ceiling of the block pool.  Above `capacity_blocks`, the pool starts with
         `capacity_blocks` blocks of storage and grows on demand; the volume then holds, bit for bit, what a volume
-        created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the pool fixed."""
+        created with `capacity_blocks=max_capacity_blocks` holds.  None (or `capacity_blocks`) keeps the pool fixed.
+        `color_float64`: keep each voxel's colour as Open3D's TSDFVoxel does, a float64 running mean
+        (c * w + rgb) / (w + 1), so voxel, mesh and point-cloud colours equal Open3D's bit for bit.  A block then takes
+        16 KiB instead of 10 KiB; tsdf and weights are the same in both modes.  False keeps the float32 running mean."""
         self._L = _lib.load()
         self._h = C.c_void_p()
         self.voxel_length = float(voxel_length)
@@ -192,9 +196,10 @@ class B200TsdfVolume(_MapState):
         self.shard_rank, self.shard_count = int(shard_rank), int(shard_count)
         self.volume_unit_resolution = int(volume_unit_resolution)
         self.depth_sampling_stride = int(depth_sampling_stride)
-        cfg = B2VConfig(voxel_length, block_size, sdf_trunc, depth_trunc, depth_sampling_stride,
+        self.color_float64 = bool(color_float64)
+        cfg = B2VConfigEx(voxel_length, block_size, sdf_trunc, depth_trunc, depth_sampling_stride,
                         capacity_blocks, device, shard_rank, shard_count, int(volume_unit_resolution),
-                        float(voxel_length), float(sdf_trunc), self.max_capacity_blocks)
+                        float(voxel_length), float(sdf_trunc), self.max_capacity_blocks, int(self.color_float64))
         rc = self._L.b2v_create(C.byref(cfg), C.byref(self._h))
         if rc != _lib.B2V_OK:
             msg = self._L.b2v_last_error(self._h).decode() if self._h else "invalid configuration"
@@ -456,13 +461,18 @@ class B200TsdfVolume(_MapState):
             self._L.b2v_last_touched_keys(self._h, keys.ctypes.data, int(n))
         return np.ascontiguousarray(keys[:, :3])
 
+    def _raw_shape(self, n: int) -> tuple:
+        """Shape of n blocks in the pool's raw layout as float32 words: [n,5,512] planes (tsdf, weight, r, g, b), or
+        with float64 colour [n,4096], the tsdf and weight planes followed by the float64 r, g, b planes."""
+        return (n, RAW_F64_WORDS) if self.color_float64 else (n, VOXEL_PLANES, BLOCK_VOXELS)
+
     def _export_blocks(self, empty):
-        """(keys int32 [nb,4] = {x,y,z,0}, vox float32 [nb,5,512]) of every block in arrays `empty(shape, dtype name)`
-        makes, host or device (b2v_export_blocks, which waits for the frames in flight)."""
+        """(keys int32 [nb,4] = {x,y,z,0}, raw float32 blocks, `_raw_shape`) of every block in arrays
+        `empty(shape, dtype name)` makes, host or device (b2v_export_blocks, which waits for the frames in flight)."""
         n = self._L.b2v_export_blocks(self._h, None, None, 0)
         if n < 0:
             raise RuntimeError(self._L.b2v_last_error(self._h).decode())
-        keys, vox = empty((n, 4), "int32"), empty((n, VOXEL_PLANES, BLOCK_VOXELS), "float32")
+        keys, vox = empty((n, 4), "int32"), empty(self._raw_shape(n), "float32")
         ptr = (lambda a: a.data_ptr()) if hasattr(keys, "data_ptr") else (lambda a: a.ctypes.data)
         if n and self._L.b2v_export_blocks(self._h, ptr(keys), ptr(vox), n) != n:
             raise RuntimeError(self._L.b2v_last_error(self._h).decode())
@@ -470,15 +480,33 @@ class B200TsdfVolume(_MapState):
 
     def dump_blocks(self):
         """Parity hook: keys int32 [nb,3], hashes uint64 [nb] (reference BlockKeyHash),
-        vox float32 [nb,5,512] planes (tsdf, weight, r, g, b)."""
+        vox float32 [nb,5,512] planes (tsdf, weight, r, g, b).  With float64 colour also rgb64 float64 [nb,3,512], the
+        colours as the volume keeps them; vox then holds them rounded to float32."""
         d = self._export_state()
-        return dict(keys=d["keys"], hashes=_block_hashes(d["keys"]), vox=d["vox"])
+        out = dict(keys=d["keys"], hashes=_block_hashes(d["keys"]), vox=d["vox"])
+        if self.color_float64:
+            out["rgb64"] = d["rgb64"]
+            out["vox"] = np.concatenate([d["vox"], d["rgb64"].astype(np.float32)], axis=1)
+        return out
 
-    def upload_blocks(self, keys, vox):
-        """Restore / seed blocks: keys int32 [n,3] (unique), vox float32 [n,5,512].  Every weight must lie in
-        [0, 2^24] (include/b2v.h); otherwise RuntimeError and the volume is unchanged."""
+    def upload_blocks(self, keys, vox, rgb64=None):
+        """Restore / seed blocks: keys int32 [n,3] (unique), vox float32 [n,5,512].  A float64-colour volume takes
+        its colours from rgb64 float64 [n,3,512] (vox's colour planes are ignored) and requires it; a float32 volume
+        refuses it (ValueError).  Every weight must lie in [0, 2^24] (include/b2v.h); otherwise RuntimeError and the
+        volume is unchanged."""
+        if (rgb64 is None) == self.color_float64:
+            raise ValueError("upload_blocks: rgb64 is required by a float64-colour volume and refused by a float32 one")
         k = _keys4(keys)
-        x = np.ascontiguousarray(vox, np.float32).reshape(k.shape[0], VOXEL_PLANES, BLOCK_VOXELS)
+        n = k.shape[0]
+        x = np.ascontiguousarray(vox, np.float32).reshape(n, VOXEL_PLANES, BLOCK_VOXELS)
+        if self.color_float64:
+            x = _pack_f64_blocks(x[:, :2], np.asarray(rgb64, np.float64).reshape(n, 3, BLOCK_VOXELS))
+        self._upload_raw(keys, x)
+
+    def _upload_raw(self, keys, raw):
+        """upload_blocks from keys int32 [n,3] and host blocks in the raw layout (`_raw_shape`)"""
+        k = _keys4(keys)
+        x = np.ascontiguousarray(raw, np.float32).reshape(self._raw_shape(k.shape[0]))
         self._check(self._L.b2v_upload_blocks(self._h, k.shape[0], k.ctypes.data, x.ctypes.data),
                     "b2v_upload_blocks")
 
@@ -486,21 +514,35 @@ class B200TsdfVolume(_MapState):
     _STATE_KIND = "tsdf"
 
     def _state_config(self) -> dict:
-        return dict(voxel_size=np.float32(self.voxel_length), voxel_length=np.float64(self.voxel_length),
-                    sdf_trunc=np.float32(self.sdf_trunc), sdf_trunc_d=np.float64(self.sdf_trunc),
-                    depth_trunc=np.float32(self.depth_trunc), depth_stride=np.int32(self.depth_sampling_stride),
-                    unit_resolution=np.int32(self.volume_unit_resolution))
+        # The colour precision is recorded by float64-colour volumes only, so the files of float32 volumes keep the
+        # configuration they had before the mode existed.  Either way a file of the other mode does not load: a
+        # float32 file lacks color_f64, and a float64 file has an rgb64 array a float32 volume does not take.
+        c = dict(voxel_size=np.float32(self.voxel_length), voxel_length=np.float64(self.voxel_length),
+                 sdf_trunc=np.float32(self.sdf_trunc), sdf_trunc_d=np.float64(self.sdf_trunc),
+                 depth_trunc=np.float32(self.depth_trunc), depth_stride=np.int32(self.depth_sampling_stride),
+                 unit_resolution=np.int32(self.volume_unit_resolution))
+        if self.color_float64:
+            c["color_f64"] = np.int32(1)
+        return c
 
-    @staticmethod
-    def _state_arrays() -> dict:
+    def _state_arrays(self) -> dict:
+        """keys and vox [n,5,512] (float32 colour planes); a float64-colour volume keeps the tsdf and weight planes in
+        vox [n,2,512] and its colours in rgb64 float64 [n,3,512]."""
+        if self.color_float64:
+            return dict(keys=(np.int32, (3,)), vox=(np.float32, (2, BLOCK_VOXELS)),
+                        rgb64=(np.float64, (3, BLOCK_VOXELS)))
         return dict(keys=(np.int32, (3,)), vox=(np.float32, (VOXEL_PLANES, BLOCK_VOXELS)))
 
     def _state_capacity(self) -> int:
         return max(self.capacity_blocks, self.max_capacity_blocks)
 
     def _export_state(self) -> dict:
-        keys4, vox = self._export_blocks(np.empty)
-        return dict(keys=np.ascontiguousarray(keys4[:, :3]), vox=vox)
+        keys4, raw = self._export_blocks(np.empty)
+        keys = np.ascontiguousarray(keys4[:, :3])
+        if not self.color_float64:
+            return dict(keys=keys, vox=raw)
+        vox, rgb64 = _split_f64_blocks(raw)
+        return dict(keys=keys, vox=vox, rgb64=rgb64)
 
     def _clear_state(self) -> None:
         self.reset()
@@ -511,12 +553,17 @@ class B200TsdfVolume(_MapState):
             raise ValueError("voxel weights outside [0, 2^24] in the state")
 
     def _upload_state(self, blocks: dict) -> None:
-        if len(blocks["keys"]):
+        if not len(blocks["keys"]):
+            return
+        if self.color_float64:
+            self._upload_raw(blocks["keys"], _pack_f64_blocks(blocks["vox"], blocks["rgb64"]))
+        else:
             self.upload_blocks(blocks["keys"], blocks["vox"])
 
     def export_blocks_torch(self):
         """(keys int32 [n,4] = {x,y,z,0}, vox float32 [n,5,512]) as torch CUDA tensors on this volume's device:
-        device-to-device copies of the block keys and the block pool (multi-GPU mesh gather)."""
+        device-to-device copies of the block keys and the block pool (multi-GPU mesh gather).  A float64-colour
+        volume's vox is its raw layout, float32 [n,4096] (tsdf and weight planes, then the float64 r, g, b planes)."""
         import torch
         dev = torch.device("cuda", self.device)
         return self._export_blocks(lambda shape, dt: torch.empty(shape, dtype=getattr(torch, dt), device=dev))
@@ -527,6 +574,8 @@ class B200TsdfVolume(_MapState):
             return
         if not (keys.is_cuda and vox.is_cuda and keys.is_contiguous() and vox.is_contiguous()):
             raise RuntimeError("keys and vox must be contiguous CUDA tensors")
+        if tuple(vox.shape) != self._raw_shape(int(keys.shape[0])):
+            raise ValueError(f"vox must be the raw layout {self._raw_shape(int(keys.shape[0]))} of this volume")
         self._check(self._L.b2v_upload_blocks(self._h, int(keys.shape[0]), keys.data_ptr(), vox.data_ptr()),
                     "b2v_upload_blocks")
 
@@ -543,7 +592,8 @@ class B200TsdfVolume(_MapState):
     def export_halo_torch(self, world: int):
         """Halo records this shard sends the other ranks of a `world`-rank sharding (b2v_export_halo_device):
         (headers int32 [R,4] = {x,y,z,mask}, payload float32 [P,5] = {tsdf, weight, r, g, b}, records per destination
-        rank, payload voxels per destination rank), CUDA tensors grouped by destination rank.  Only reads the volume."""
+        rank, payload voxels per destination rank), CUDA tensors grouped by destination rank.  With float64 colour the
+        payload is float32 [P,8]: tsdf, weight and the r, g, b float64 words.  Only reads the volume."""
         import torch
         world = int(world)
         rec, pay = (C.c_int64 * world)(), (C.c_int64 * world)()
@@ -551,17 +601,22 @@ class B200TsdfVolume(_MapState):
         nrec, nvox = [int(x) for x in rec], [int(x) for x in pay]
         dev = torch.device("cuda", self.device)
         headers = torch.empty((sum(nrec), 4), dtype=torch.int32, device=dev)
-        payload = torch.empty((sum(nvox), VOXEL_PLANES), dtype=torch.float32, device=dev)
+        payload = torch.empty((sum(nvox), self._halo_words), dtype=torch.float32, device=dev)
         if headers.shape[0]:
             self._check(self._L.b2v_export_halo_device(self._h, world, rec, pay, headers.data_ptr(), payload.data_ptr(),
                                                        headers.shape[0], payload.shape[0]), "b2v_export_halo_device")
         return headers, payload, nrec, nvox
 
+    @property
+    def _halo_words(self) -> int:
+        """float32 words per voxel of a halo payload"""
+        return HALO_F64_WORDS if self.color_float64 else VOXEL_PLANES
+
     def _halo_args(self, headers, payload):
         import torch
         dev = torch.device("cuda", self.device)
         h = torch.as_tensor(headers, dtype=torch.int32).to(dev).contiguous().reshape(-1, 4)
-        x = torch.as_tensor(payload, dtype=torch.float32).to(dev).contiguous().reshape(-1, VOXEL_PLANES)
+        x = torch.as_tensor(payload, dtype=torch.float32).to(dev).contiguous().reshape(-1, self._halo_words)
         torch.cuda.current_stream(dev).synchronize()
         return h, x
 
@@ -599,6 +654,29 @@ class B200TsdfVolume(_MapState):
         self._check(self._L.b2v_extract_points(self._h, C.byref(n)), "b2v_extract_points")
         m = self._copy_mesh(n.value, 0)
         return PointCloud(m.vertices, m.vertex_colors, m.edge_ids)
+
+
+# float64-colour blocks (include/b2v.h B2V_BLOCK_BYTES_F64) as float32 words, and a halo payload voxel of such a volume
+RAW_F64_WORDS = 2 * BLOCK_VOXELS + 3 * 2 * BLOCK_VOXELS
+HALO_F64_WORDS = 2 + 3 * 2
+
+
+def _split_f64_blocks(raw):
+    """float64-colour blocks, float32 [n,4096] -> (vox float32 [n,2,512] tsdf and weight, rgb64 float64 [n,3,512])"""
+    raw = np.ascontiguousarray(raw, np.float32)
+    n = raw.shape[0]
+    vox = raw[:, :2 * BLOCK_VOXELS].reshape(n, 2, BLOCK_VOXELS).copy()
+    rgb64 = raw[:, 2 * BLOCK_VOXELS:].view(np.float64).reshape(n, 3, BLOCK_VOXELS).copy()
+    return vox, rgb64
+
+
+def _pack_f64_blocks(tw, rgb64):
+    """Inverse of _split_f64_blocks: tw float32 [n,2,512] (tsdf, weight), rgb64 float64 [n,3,512] -> [n,4096]"""
+    n = tw.shape[0]
+    raw = np.empty((n, RAW_F64_WORDS), np.float32)
+    raw[:, :2 * BLOCK_VOXELS] = np.asarray(tw, np.float32).reshape(n, 2 * BLOCK_VOXELS)
+    raw[:, 2 * BLOCK_VOXELS:].view(np.float64)[:] = np.asarray(rgb64, np.float64).reshape(n, 3 * BLOCK_VOXELS)
+    return raw
 
 
 def filter_shadow_points(depth, delta_depth=None, delta_x=2, delta_y=2, fill_value=-1, device=0):
