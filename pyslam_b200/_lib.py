@@ -51,6 +51,8 @@ EXPORTED_SYMBOLS = [
     "b2v_grid_upload_blocks", "b2v_sgrid_export_blocks", "b2v_sgrid_upload_blocks",
     "b2v_sgrid_set_label_overflow", "b2v_sgrid_label_storage", "b2v_sgrid_export_labels", "b2v_sgrid_upload_labels",
     "b2v_grid_set_input_order_sums",
+    "b2v_set_frame_store", "b2v_frame_store_clear", "b2v_frame_store_last", "b2v_frame_store_stats",
+    "b2v_integrate_stored",
 ]
 
 
@@ -204,6 +206,16 @@ def load() -> C.CDLL:
     L.b2v_set_input_event.argtypes = [vp, vp]
     L.b2v_set_group_size.restype = C.c_int
     L.b2v_set_group_size.argtypes = [vp, i32]
+    L.b2v_set_frame_store.restype = C.c_int
+    L.b2v_set_frame_store.argtypes = [vp, i32]
+    L.b2v_frame_store_clear.restype = C.c_int
+    L.b2v_frame_store_clear.argtypes = [vp]
+    L.b2v_frame_store_last.restype = C.c_int
+    L.b2v_frame_store_last.argtypes = [vp, vp, i32]
+    L.b2v_frame_store_stats.restype = C.c_int
+    L.b2v_frame_store_stats.argtypes = [vp, p_i64, p_i64]
+    L.b2v_integrate_stored.restype = C.c_int
+    L.b2v_integrate_stored.argtypes = [vp, i32, vp, vp, vp, vp]
     L.b2v_export_blocks.restype = i64
     L.b2v_export_blocks.argtypes = [vp, vp, vp, i64]
     L.b2v_upload_blocks.restype = C.c_int

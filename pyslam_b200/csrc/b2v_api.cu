@@ -187,6 +187,16 @@ struct b2v_volume {
     bool prof_enabled = false;
     std::vector<cudaEvent_t> prof_events;  // quadruples: allocate begin/end, integrate begin/end
     size_t prof_used = 0;
+    // frame store (b2v_set_frame_store): the packed texel image of each stored frame, slot s at s * store_H * store_W
+    // texels.  One address range reserved for store_max frames at the first stored frame's size and mapped as it
+    // fills, so a stored frame never moves.  Frames, not map state: reset, uploads and pool growth leave it as it is.
+    int32_t store_max = 0;               // 0: off
+    int32_t store_count = 0;             // filled slots, [0, store_count): their copies are enqueued
+    int store_H = 0, store_W = 0;        // size of every stored frame (0: none stored yet)
+    bool store_stopped = false;          // the device could not reserve or map more: no frame is stored any more
+    size_t store_map_limit = SIZE_MAX;   // B2V_FRAME_STORE_MAX_BYTES: the most the store maps (tests of that path)
+    VmmRange store;
+    std::vector<int32_t> store_last;     // slot of each frame of the most recent integrate call, or -1
 };
 
 // ---- the block pool: virtual memory management entry points of the driver ----
@@ -331,7 +341,7 @@ static int volume_clear_device(b2v_volume *v) {
     return B2V_OK;
 }
 
-extern "C" int b2v_version(void) { return 112; }
+extern "C" int b2v_version(void) { return 113; }
 
 extern "C" int b2v_selftest_division(int32_t device, uint64_t pairs, uint64_t *bad_reciprocals, uint64_t *bad_quotients) {
     if (cudaSetDevice(device) != cudaSuccess) return B2V_ERR_CUDA;
@@ -396,6 +406,7 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     if (const char *e = std::getenv("B2V_OVERLAP")) v->overlap = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_TMA")) v->use_tma = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_FUSE")) v->fuse = std::atoi(e) != 0;
+    if (const char *e = std::getenv("B2V_FRAME_STORE_MAX_BYTES")) v->store_map_limit = std::strtoull(e, nullptr, 10);
     if (const char *e = std::getenv("B2V_GROUP")) {
         const int n = std::atoi(e);
         if (n >= 1 && n <= kMaxGroup) v->group_frames = n;
@@ -722,16 +733,74 @@ static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d
     return B2V_OK;
 }
 
+static Texel *store_slot(const b2v_volume *v, int32_t slot) {
+    return reinterpret_cast<Texel *>(v->store.va) + static_cast<size_t>(slot) * v->store_H * v->store_W;
+}
+
+// map storage for the store's first `bytes` bytes (zeroed on `stream`); false, with nothing mapped past what was, when
+// the device cannot map it or it would pass store_map_limit
+static bool store_map(b2v_volume *v, size_t bytes, cudaStream_t stream) {
+    const size_t g = v->store.gran;
+    std::string err;   // not the volume's error: a store that cannot grow stops storing, the call goes on
+    return (bytes + g - 1) / g * g <= v->store_map_limit && vmm_map(&v->store, bytes, stream, &err);
+}
+
+// The store slots of the frames of an integrate call (v->store_last; -1: not stored), before anything is launched:
+// handed out in frame order while the store has room, to frames of the stored frames' size.  The first stored frame
+// sets that size and reserves the address range; the storage the call's frames need is mapped here (at least doubling
+// the mapping, else just what they need).  When the device cannot reserve or map it, the frames that fit in what is
+// mapped are stored and the store stops: later frames are not stored and integration goes on.  A slot counts as
+// filled (store_count) only once its copy is enqueued; the slots of groups a failing call did not reach go back to -1
+// (enqueue_frames).
+static void assign_store_slots(b2v_volume *v, int32_t n_frames, int H, int W, cudaStream_t stream) {
+    if (v->store_max == 0 || v->store_stopped) return;
+    if (v->store_H == 0) {
+        std::string err;
+        if (!vmm_reserve(&v->store, static_cast<size_t>(v->store_max) * H * W * sizeof(Texel), v->cfg.device, &err)) {
+            v->store_stopped = true;
+            return;
+        }
+        v->store_H = H;
+        v->store_W = W;
+    }
+    if (H != v->store_H || W != v->store_W) return;
+    const size_t pitch = static_cast<size_t>(H) * W * sizeof(Texel);
+    int32_t n = std::min(n_frames, v->store_max - v->store_count);
+    const size_t need = static_cast<size_t>(v->store_count + n) * pitch;
+    if (n > 0 && need > v->store.mapped) {
+        const size_t doubled = std::min(v->store.reserved, 2 * v->store.mapped);
+        if (!(doubled > need && store_map(v, doubled, stream)) && !store_map(v, need, stream)) {
+            v->store_stopped = true;
+            n = static_cast<int32_t>(std::min<size_t>(n, v->store.mapped / pitch - v->store_count));
+        }
+    }
+    for (int32_t f = 0; f < n; ++f) v->store_last[f] = v->store_count + f;
+}
+
 // Enqueues n_frames frames, contiguous in the caller's arrays, as groups in the group buffers: groups of up to
 // group_frames frames on the fused kernels when fusion is on and there are two frames or more, else groups of one
 // frame on the frame-by-frame kernels.  depth is float32 metres (u16_scale = 0) or raw uint16 widened on the device
 // to float32(depth) * u16_scale (u16_scale > 0).  Consumes the input event of b2v_set_input_event.
+// stored != nullptr: the frames are the frame store's slots stored[0..n_frames) (b2v_integrate_stored), at the stored
+// frames' size; depth and color are not read.  Each group's texel images are copied from the store into its staging
+// slots and the allocate kernels read depth from them (launch_allocate*, from_tex); the update is the same.
 static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, const void *depth, float u16_scale,
                           const uint8_t *color, int32_t height, int32_t width, const double K[4], const double *Tcw,
-                          void *stream) {
+                          void *stream, const int32_t *stored = nullptr) {
     const cudaEvent_t inputs_ready = v->input_event;  // one-shot: consumed by bad arguments too
     v->input_event = nullptr;
-    if (n_frames < 0 || (n_frames > 0 && (!depth || !color || !Tcw || !K)) || height <= 0 || width <= 0) {
+    v->store_last.assign(static_cast<size_t>(std::max(n_frames, 0)), -1);  // (also when the call fails)
+    // on every return: the slots of frames whose copies were not enqueued are not stored
+    struct UnfilledSlots {
+        b2v_volume *v;
+        ~UnfilledSlots() {
+            for (int32_t &s : v->store_last)
+                if (s >= v->store_count) s = -1;
+        }
+    } unfilled{v};
+    const bool replay = stored != nullptr;
+    if (n_frames < 0 || (n_frames > 0 && ((!replay && (!depth || !color)) || !Tcw || !K)) || height <= 0 ||
+        width <= 0) {
         v->err = std::string(what) + ": bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
@@ -742,20 +811,22 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
     }
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
     const size_t pixels = static_cast<size_t>(height) * width;
-    const bool dev_depth = is_device_pointer(depth), dev_color = is_device_pointer(color);
+    // (a replay reads no caller images)
+    const bool dev_depth = replay || is_device_pointer(depth), dev_color = replay || is_device_pointer(color);
     if (stream != nullptr && !(dev_depth && dev_color)) {
         v->err = std::string(what) + ": a caller stream requires device image pointers";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     cudaStream_t cs = stream ? static_cast<cudaStream_t>(stream) : v->compute;
     cudaStream_t as = v->overlap ? v->alloc : cs;  // stream of the allocate kernels
-    const bool u16 = u16_scale > 0.0f;
+    const bool u16 = !replay && u16_scale > 0.0f;
     const float *depth32 = static_cast<const float *>(depth);
     const uint16_t *depth16 = static_cast<const uint16_t *>(depth);
     {
         int rc = ensure_staging(v, pixels);
         if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
         if (rc != B2V_OK) return rc;
+        if (!replay) assign_store_slots(v, n_frames, height, width, as);
     }
     // This call's updates touch the blocks the previous call's did, and a block's running average depends on frame
     // order: on another stream they wait for the previous call's last update (on the same stream, stream order does
@@ -799,7 +870,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         // the group buffer (masks, union list, counters, texel images) was last used by group id - kGroupBufs
         B2V_CUDA(v, cudaStreamWaitEvent(as, v->ev_group_done[buf], 0));
         B2V_CUDA(v, cudaMemsetAsync(v->meta.counters + group_ctr(buf, 0), 0, kGroupCtrStride * sizeof(uint32_t), as));
-        if (g0 == 0 && (dev_depth || dev_color)) {
+        if (g0 == 0 && !replay && (dev_depth || dev_color)) {
             // one input fence per call: by default everything enqueued on the caller's stream so far (the inputs'
             // producers, earlier frames) happens before the allocate kernels.  A caller that knows better
             // (b2v_set_input_event: "the inputs are ready when this event fires") keeps the allocate kernels of this
@@ -844,11 +915,18 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         for (int k = 0; k < count; ++k) {
             const size_t f = static_cast<size_t>(g0 + k);
             // (widened) staging
-            const float *d_depth = dev_depth && !u16 ? depth32 + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
-            const uint8_t *d_color = dev_color ? color + pixels * 3 * f : stage_slot(v->d_color, pixels * 3, s0 + k);
+            const float *d_depth = nullptr;
+            const uint8_t *d_color = nullptr;
             Texel *tex = stage_slot(v->d_tex, texel_pitch(pixels), s0 + k);
-            const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s0 + k, as);
-            if (rc != B2V_OK) return rc;
+            if (replay) {  // the gather: the stored texel image into the frame's staging slot
+                B2V_CUDA(v, cudaMemcpyAsync(tex, store_slot(v, stored[f]), pixels * sizeof(Texel),
+                                            cudaMemcpyDeviceToDevice, as));
+            } else {
+                d_depth = dev_depth && !u16 ? depth32 + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
+                d_color = dev_color ? color + pixels * 3 * f : stage_slot(v->d_color, pixels * 3, s0 + k);
+                const int rc = rectify_frame(v, &d_depth, &d_color, height, width, s0 + k, as);
+                if (rc != B2V_OK) return rc;
+            }
             FrameParams P;
             fill_frame_params(&P, K, Tcw + 16 * f, height, width, v->geo);
             P.group_buf = buf;
@@ -863,7 +941,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             aargs.depth[k] = d_depth;
             aargs.color[k] = d_color;
             aargs.tex[k] = tex;
-            const FrameMaps *fm = frame_maps(v, d_depth, d_color, height, width);
+            const FrameMaps *fm = replay ? nullptr : frame_maps(v, d_depth, d_color, height, width);
             if (fm) aargs.maps[k] = *fm; else aargs.use_tma = 0;
             args.f[k] = P.E;
         }
@@ -878,11 +956,24 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             B2V_CUDA(v, cudaEventRecord(pe[0], as));
         }
         aargs.units = v->units;
-        B2V_CUDA(v, fused ? launch_allocate_group(aargs, v->table, v->meta, v->sm_count, as)
-                          : launch_allocate(aargs, v->table, v->meta, as));
+        B2V_CUDA(v, fused ? launch_allocate_group(aargs, v->table, v->meta, v->sm_count, as, replay)
+                          : launch_allocate(aargs, v->table, v->meta, as, replay));
         if (pe) B2V_CUDA(v, cudaEventRecord(pe[1], as));
         B2V_CUDA(v, cudaEventRecord(v->ev_galloc[buf], as));
         v->launches += fused ? 2 : 1;  // (+ the expand kernel of a fused group)
+        if (!replay) {
+            // the frame store: copy the packed texel images of the group's stored frames (mapped by
+            // assign_store_slots) on the allocate stream, after the pack and before the next group in this buffer
+            // overwrites the staging slots (its allocate kernels wait on this stream).  Enqueued after ev_galloc: with
+            // overlap on, the update does not wait for the copies; with it off they share its stream.
+            for (int k = 0; k < count; ++k) {
+                const int32_t slot = v->store_last[g0 + k];
+                if (slot < 0) continue;
+                B2V_CUDA(v, cudaMemcpyAsync(store_slot(v, slot), aargs.tex[k], pixels * sizeof(Texel),
+                                            cudaMemcpyDeviceToDevice, as));
+                v->store_count = slot + 1;   // filled: slots are handed out and copied in frame order
+            }
+        }
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
         if (v->growable && v->meta.pool_capacity < v->meta.capacity) {
             // in group order on one stream, each after its own allocation: the first group skipped is the first that
@@ -925,6 +1016,72 @@ extern "C" int b2v_integrate_batch_u16(b2v_volume *v, int32_t n_frames, const ui
     }
     return enqueue_frames(v, "b2v_integrate_batch_u16", n_frames, depth, depth_scale, color, height, width, K, Tcw,
                           stream);
+}
+
+// ---- frame store ----
+
+// empties the store and releases its memory, after every call that may still read or write it
+static int frame_store_release(b2v_volume *v) {
+    B2V_CUDA(v, cudaSetDevice(v->cfg.device));
+    B2V_CUDA(v, cudaDeviceSynchronize());   // replays gather on the caller's stream when overlap is off
+    vmm_release(&v->store);
+    v->store_count = 0;
+    v->store_H = v->store_W = 0;
+    v->store_stopped = false;
+    std::fill(v->store_last.begin(), v->store_last.end(), -1);
+    return B2V_OK;
+}
+
+extern "C" int b2v_set_frame_store(b2v_volume *v, int32_t max_frames) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    if (max_frames < 0) {
+        v->err = "b2v_set_frame_store: max_frames must be >= 0";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    const int rc = frame_store_release(v);
+    if (rc != B2V_OK) return rc;
+    v->store_max = max_frames;
+    return B2V_OK;
+}
+
+extern "C" int b2v_frame_store_clear(b2v_volume *v) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    return frame_store_release(v);
+}
+
+extern "C" int b2v_frame_store_last(b2v_volume *v, int32_t *slots, int32_t n) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    if (n != static_cast<int32_t>(v->store_last.size()) || (n > 0 && !slots)) {
+        v->err = "b2v_frame_store_last: n must be the frame count of the most recent integrate call";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    std::copy(v->store_last.begin(), v->store_last.end(), slots);
+    return B2V_OK;
+}
+
+extern "C" int b2v_frame_store_stats(b2v_volume *v, int64_t *frames, int64_t *bytes) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    if (frames) *frames = v->store_count;
+    if (bytes) *bytes = static_cast<int64_t>(v->store.mapped);
+    return B2V_OK;
+}
+
+extern "C" int b2v_integrate_stored(b2v_volume *v, int32_t n_frames, const int32_t *slots, const double K[4],
+                                    const double *Tcw, void *stream) {
+    if (!v) return B2V_ERR_INVALID_ARGUMENT;
+    v->store_last.assign(static_cast<size_t>(std::max(n_frames, 0)), -1);
+    if (n_frames > 0 && !slots) {
+        v->err = "b2v_integrate_stored: bad arguments";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    for (int32_t f = 0; f < n_frames; ++f)
+        if (slots[f] < 0 || slots[f] >= v->store_count) {
+            v->err = "b2v_integrate_stored: slot " + std::to_string(slots[f]) + " holds no frame (the store holds " +
+                     std::to_string(v->store_count) + ")";
+            return B2V_ERR_INVALID_ARGUMENT;
+        }
+    return enqueue_frames(v, "b2v_integrate_stored", n_frames, nullptr, 0.0f, nullptr, std::max(v->store_H, 1),
+                          std::max(v->store_W, 1), K, Tcw, stream, slots);
 }
 
 extern "C" int b2v_set_input_event(b2v_volume *v, void *event) {

@@ -292,13 +292,15 @@ struct GroupAllocArgs {
     int32_t count, use_tma;
 };
 static_assert(sizeof(GroupAllocArgs) < 32000, "kernel parameter space");
-// a one-frame group (frame 0 of args), with the frame-by-frame allocate_kernel
+// a one-frame group (frame 0 of args), with the frame-by-frame allocate_kernel.  from_tex: the frame's texel image is
+// already in args.tex[0] (a frame replayed from the frame store): depth, colour and maps are not read, nothing is packed
 cudaError_t launch_allocate(const GroupAllocArgs &args, const HashTable &table, const PoolMeta &meta,
-                            cudaStream_t stream);
+                            cudaStream_t stream, bool from_tex);
 // all frames of a group in ONE launch (blockIdx.z = frame): the per-frame latency chains overlap.  It collects the
 // group's units in args.units; a second kernel then touches each block of those units once for the whole group.
+// from_tex: as above, for every frame of the group
 cudaError_t launch_allocate_group(const GroupAllocArgs &args, const HashTable &table,
-                                  const PoolMeta &meta, int sm_count, cudaStream_t stream);
+                                  const PoolMeta &meta, int sm_count, cudaStream_t stream, bool from_tex);
 // projective TSDF + colour update of every block touched by the one-frame group in group buffer group_buf
 // (frame 0 of args)
 // color_f64: the volume's colour type (TsdfBlock), here and in every launcher below that takes it

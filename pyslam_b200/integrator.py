@@ -20,7 +20,7 @@ from types import SimpleNamespace
 
 import numpy as np
 
-from . import map_state, shard_plugin, sharding
+from . import keyframe_store, map_state, shard_plugin, sharding
 from .volume import B200TsdfVolume
 
 # defaults copied by value from the reference's parameter table (pyslam/config_parameters.py:311,
@@ -54,6 +54,9 @@ DEFAULT_PARAMETERS = {
     # keep each voxel's colour as Open3D does, a float64 running mean: voxel, mesh and point-cloud colours equal
     # Open3D's bit for bit, at 16 KiB per block instead of 10 KiB (INTEGRATION.md section 2)
     "kVolumetricIntegrationB200ColorFloat64": False,
+    # keep the packed frames of up to this many keyframes on the GPU (8 bytes per pixel: 2.46 MB per 640x480 keyframe),
+    # so that rebuild(map) sends only the keyframes' new poses to the integrator (keyframe_store.py); 0 = off
+    "kVolumetricIntegrationB200KeyframeStoreFrames": 0,
 }
 
 
@@ -252,8 +255,29 @@ def make_integrator_class(Base, api):
 
         def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
                      viewer_queue=None, **kwargs):
+            # the table of stored keyframes is created here, in the parent, before the base class spawns the
+            # integrator process, which receives it with the rest of the plugin
+            n = int(self._parent_parameter("kVolumetricIntegrationB200KeyframeStoreFrames", kwargs))
+            self._b200_keyframe_table = keyframe_store.StoredKeyframeTable(n) if n > 0 else None
             super().__init__(camera, environment_type, sensor_type, volumetric_integrator_type,
                              viewer_queue, **kwargs)
+
+        @staticmethod
+        def _parent_parameter(name, kwargs):
+            """A parameter as the parent process sees it: a constructor keyword, else the `parameters` dict keyword,
+            else pySLAM's Parameters class, else the default."""
+            if name in kwargs:
+                return kwargs[name]
+            if name in (kwargs.get("parameters") or {}):
+                return kwargs["parameters"][name]
+            return getattr(getattr(api, "Parameters", None), name, DEFAULT_PARAMETERS[name])
+
+        def add_task(self, task):
+            """Every task the front end enqueues (keyframes and rebuild(map) alike, base.py:1216-1232): an INTEGRATE
+            task of a keyframe the integrator has stored travels without its images (keyframe_store.light_task)."""
+            if getattr(self, "_b200_keyframe_table", None) is not None:
+                task = keyframe_store.light_task(task, self._b200_keyframe_table, TaskType.INTEGRATE)
+            super().add_task(task)
 
         # -- runs inside the integrator process: the CUDA context is created here, never in the parent
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
@@ -278,6 +302,10 @@ def make_integrator_class(Base, api):
                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None,
                 volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]),
                 color_float64=bool(p["kVolumetricIntegrationB200ColorFloat64"]), **self._map_placement())
+            self._store_frames = int(p["kVolumetricIntegrationB200KeyframeStoreFrames"])
+            if self._store_frames > 0:
+                self.volume.set_frame_store(self._store_frames)
+            self._stored_slots = {}         # keyframe_store.keyframe_key -> slot of the keyframes stored here
             self.last_output = None
             self.last_integrated_id = -1
             self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call
@@ -316,18 +344,92 @@ def make_integrator_class(Base, api):
 
         def _integrate_sharded(self, frames, K4, fused):
             """The frames on every rank's shard: one fused batch when the unsharded plugin fuses them, else one call
-            per frame.  Rank 0 uploads each batch once (raw uint16 depth stays 16-bit) and broadcasts it."""
+            per frame.  Rank 0 uploads each batch once (raw uint16 depth stays 16-bit) and broadcasts it.  Every rank
+            stores the same frames in the same slots; rank 0's are recorded."""
             for part in ([frames] if fused else [[f] for f in frames]):
                 scale = part[0][3]
-                self._shards.run(
+                slots = self._shards.run(
                     "integrate", dict(K=K4, poses=np.stack([np.asarray(f[0].pose, np.float64) for f in part]),
                                       scale=scale),
                     dict(depths=np.ascontiguousarray(np.stack([f[2] for f in part]),
                                                      np.float32 if scale is None else np.uint16),
                          colors=np.ascontiguousarray(np.stack([f[1] for f in part]), np.uint8)))
+                self._record_stored([f[0] for f in part], slots)
 
         def _op_integrate(self, meta, depths, colors):
             self.volume.integrate_batch(depths, colors, meta["K"], meta["poses"], depth_scale=meta["scale"])
+            return self.volume.last_stored_slots() if getattr(self, "_store_frames", 0) else None
+
+        def _op_integrate_stored(self, meta):
+            self.volume.integrate_stored(meta["slots"], meta["K"], meta["poses"])
+
+        def _record_stored(self, kds, slots):
+            """Note the store slots of keyframes just integrated (slots: last_stored_slots(), or None with the store
+            off) and publish them to the parent's table."""
+            if slots is None:
+                return
+            table = getattr(self, "_b200_keyframe_table", None)
+            for kd, slot in zip(kds, slots):
+                if slot >= 0:
+                    self._stored_slots[keyframe_store.keyframe_key(kd)] = int(slot)
+                    if table is not None:
+                        table.publish(int(slot), kd)
+
+        def _integrate_images(self, tasks):
+            """Today's path for tasks that carry their images; the keyframes integrated, in order."""
+            frames = []
+            for t in tasks:
+                kd = t.keyframe_data
+                color, depth, scale = self._prepare_frame(kd)
+                if color is not None and depth is not None:
+                    frames.append((kd, color, depth, scale))
+            if not frames:
+                return []
+            K4 = tuple(self._intrinsics())
+            same = all(f[1].shape == frames[0][1].shape and f[2].shape == frames[0][2].shape
+                       and f[2].dtype == frames[0][2].dtype and f[3] == frames[0][3]
+                       for f in frames)
+            store = getattr(self, "_store_frames", 0) > 0
+            if self._shards is not None:
+                self._integrate_sharded(frames, K4, len(frames) > 1 and same)
+            elif len(frames) > 1 and same:
+                # one C call: groups of frames fused per block visit (b2v_integrate_batch)
+                self.volume.integrate_batch(np.stack([f[2] for f in frames]),
+                                            np.stack([f[1] for f in frames]), K4,
+                                            np.stack([np.asarray(f[0].pose, np.float64) for f in frames]),
+                                            depth_scale=frames[0][3])
+                self._record_stored([f[0] for f in frames], self.volume.last_stored_slots() if store else None)
+            else:
+                for kd, color, depth, scale in frames:
+                    # north_star call: integrate(depth, color, K, pose = Tcw)
+                    self.volume.integrate(depth, color, K4, kd.pose, depth_scale=scale)
+                    self._record_stored([kd], self.volume.last_stored_slots() if store else None)
+            return [f[0] for f in frames]
+
+        def _integrate_stored(self, tasks):
+            """Light tasks (keyframe_store): the stored frames with the tasks' poses, in one call; the keyframes
+            integrated, in order.  A keyframe whose frame is not stored here is logged and left out."""
+            kds, slots = [], []
+            for t in tasks:
+                kd = t.keyframe_data
+                slot = self._stored_slots.get(keyframe_store.keyframe_key(kd))
+                if slot is None:
+                    getattr(Base, "print", print)(
+                        f"VolumetricIntegratorB200: ERROR: keyframe {kd.id} (timestamp {kd.timestamp}) came without "
+                        "images, but its frame is not in the frame store: it was not integrated")
+                    continue
+                kds.append(kd)
+                slots.append(slot)
+            if not kds:
+                return []
+            K4 = tuple(self._intrinsics())
+            slots = np.asarray(slots, np.int32)
+            poses = np.stack([np.asarray(kd.pose, np.float64) for kd in kds])
+            if self._shards is not None:
+                self._shards.run("integrate_stored", dict(K=K4, poses=poses, slots=slots))
+            else:
+                self.volume.integrate_stored(slots, K4, poses)
+            return kds
 
         def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
                                is_running, load_request_completed, load_request_condition,
@@ -369,31 +471,13 @@ def make_integrator_class(Base, api):
                                     break
                                 tasks.append(nxt)
                             self.last_input_task = tasks[-1]
-                            frames = []
-                            for t in tasks:
-                                kd = t.keyframe_data
-                                color, depth, scale = self._prepare_frame(kd)
-                                if color is not None and depth is not None:
-                                    frames.append((kd, color, depth, scale))
-                            if frames:
-                                K4 = tuple(self._intrinsics())
-                                same = all(f[1].shape == frames[0][1].shape and f[2].shape == frames[0][2].shape
-                                           and f[2].dtype == frames[0][2].dtype and f[3] == frames[0][3]
-                                           for f in frames)
-                                if self._shards is not None:
-                                    self._integrate_sharded(frames, K4, len(frames) > 1 and same)
-                                elif len(frames) > 1 and same:
-                                    # one C call: groups of frames fused per block visit (b2v_integrate_batch)
-                                    self.volume.integrate_batch(np.stack([f[2] for f in frames]),
-                                                                np.stack([f[1] for f in frames]), K4,
-                                                                np.stack([np.asarray(f[0].pose, np.float64) for f in frames]),
-                                                                depth_scale=frames[0][3])
-                                else:
-                                    for kd, color, depth, scale in frames:
-                                        # north_star call: integrate(depth, color, K, pose = Tcw)
-                                        self.volume.integrate(depth, color, K4, kd.pose, depth_scale=scale)
-                                self.last_integrated_id = frames[-1][0].id
-                                self.integrated_frames = getattr(self, "integrated_frames", 0) + len(frames)
+                            # light tasks (keyframe_store) and image-carrying ones may alternate: runs in order
+                            done = []
+                            for stored, run in keyframe_store.split_runs(tasks):
+                                done += self._integrate_stored(run) if stored else self._integrate_images(run)
+                            if done:
+                                self.last_integrated_id = done[-1].id
+                                self.integrated_frames = getattr(self, "integrated_frames", 0) + len(done)
                                 do_output = True
                                 if self.last_output is not None:
                                     dt = time.perf_counter() - self.last_output.timestamp

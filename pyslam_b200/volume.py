@@ -212,6 +212,7 @@ class B200TsdfVolume(_MapState):
         self._held, self._held_bytes = {}, 0
         self._input_event_set = False     # set_input_event named the next call's input event
         self._producer_event = None       # torch.cuda.Event: device inputs' producers on torch's current stream
+        self._last_frames = 0             # frames of the most recent integrate call (last_stored_slots)
 
     # ---- lifetime ----
     def close(self):
@@ -360,8 +361,9 @@ class B200TsdfVolume(_MapState):
             rc = self._release_held()
             if rc not in (_lib.B2V_OK, _lib.B2V_ERR_CAPACITY):
                 self._check(rc, "b2v_synchronize")
-        if _is_torch_cuda(inputs[0]):
+        if inputs and _is_torch_cuda(inputs[0]):
             self._order_after_producer(inputs[0], stream)
+        self._last_frames = max(int(args[0]), 0)
         try:
             rc = fn(self._h, *args)
         finally:
@@ -369,6 +371,45 @@ class B200TsdfVolume(_MapState):
         self._check(rc, what)
         self._held.update(new)
         self._held_bytes += new_bytes
+
+    # ---- frame store (rebuild(map) from keyframes on the GPU) ----
+    def set_frame_store(self, max_frames: int):
+        """Keep the packed image of up to `max_frames` integrated frames on the GPU (8 bytes per pixel, 2.46 MB per
+        640x480 frame), so that `integrate_stored` can integrate them again with new poses without their images.
+        0 turns the store off (the default).  Frames are stored in call order while there is room, at the size of the
+        first stored frame; nothing is evicted.  reset() and load_state() keep the store.  Empties the store and
+        synchronises (b2v_set_frame_store)."""
+        self._check(self._L.b2v_set_frame_store(self._h, int(max_frames)), "b2v_set_frame_store")
+
+    def clear_frame_store(self):
+        """Empty the frame store and release its memory; synchronises."""
+        self._check(self._L.b2v_frame_store_clear(self._h), "b2v_frame_store_clear")
+
+    def last_stored_slots(self) -> np.ndarray:
+        """int32 [n]: the store slot of each frame of the most recent integrate / integrate_batch call, -1 where the
+        frame was not stored (store off or full, another frame size; an integrate_stored call stores nothing)."""
+        slots = np.full(self._last_frames, -1, np.int32)
+        self._check(self._L.b2v_frame_store_last(self._h, slots.ctypes.data, len(slots)), "b2v_frame_store_last")
+        return slots
+
+    def frame_store_stats(self):
+        """(frames the store holds, device bytes it has mapped for them)."""
+        n, b = C.c_int64(0), C.c_int64(0)
+        self._check(self._L.b2v_frame_store_stats(self._h, C.byref(n), C.byref(b)), "b2v_frame_store_stats")
+        return int(n.value), int(b.value)
+
+    def integrate_stored(self, slots, K, poses, stream=None):
+        """Integrate stored frames again (slots from `last_stored_slots`) with poses [n,4,4] Tcw: the map equals
+        the one `integrate_batch` of the same frames' images at those poses gives, bit for bit.  Asynchronous, like
+        integrate_batch; there are no images to hold."""
+        sl = np.ascontiguousarray(np.asarray(slots).reshape(-1), dtype=np.int32)
+        K4 = _as_K4(K)
+        T = np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(-1, 16))
+        if T.shape[0] != len(sl):
+            raise RuntimeError("integrate_stored: one pose per slot")
+        self._enqueue("b2v_integrate_stored", self._L.b2v_integrate_stored,
+                      (len(sl), sl.ctypes.data, K4.ctypes.data, T.ctypes.data,
+                       C.c_void_p(stream) if stream else None), (), stream)
 
     def synchronize(self):
         """Wait for the work in flight; the inputs held for it are released."""
