@@ -53,6 +53,8 @@ EXPORTED_SYMBOLS = [
     "b2v_grid_set_input_order_sums",
     "b2v_set_frame_store", "b2v_frame_store_clear", "b2v_frame_store_last", "b2v_frame_store_stats",
     "b2v_integrate_stored",
+    *(f"{g}_{n}" for g in ("b2v_grid", "b2v_sgrid")
+      for n in ("set_frame_store", "frame_store_clear", "frame_store_last", "frame_store_stats", "stage_stored")),
 ]
 
 
@@ -296,6 +298,13 @@ def load() -> C.CDLL:
     L.b2v_grid_set_frame.argtypes = [vp, vp, i32, C.c_float, vp, i32, i32, i32, C.POINTER(B2VFrame)]
     L.b2v_sgrid_set_frame.restype = C.c_int
     L.b2v_sgrid_set_frame.argtypes = [vp, vp, i32, C.c_float, vp, vp, vp, i32, i32, i32, C.POINTER(B2VFrame)]
+    for g in ("b2v_grid", "b2v_sgrid"):
+        for name, args in (("set_frame_store", [vp, i32]), ("frame_store_clear", [vp]),
+                           ("frame_store_last", [vp, C.POINTER(i32)]), ("frame_store_stats", [vp, p_i64, p_i64]),
+                           ("stage_stored", [vp, i32, C.POINTER(B2VFrame)])):
+            fn = getattr(L, f"{g}_{name}")
+            fn.restype = C.c_int
+            fn.argtypes = args
     L.b2v_sgrid_remap_instance_ids.restype = C.c_int
     L.b2v_sgrid_remap_instance_ids.argtypes = [vp, C.POINTER(vp)]
     _lib = L

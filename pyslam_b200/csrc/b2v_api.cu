@@ -187,16 +187,8 @@ struct b2v_volume {
     bool prof_enabled = false;
     std::vector<cudaEvent_t> prof_events;  // quadruples: allocate begin/end, integrate begin/end
     size_t prof_used = 0;
-    // frame store (b2v_set_frame_store): the packed texel image of each stored frame, slot s at s * store_H * store_W
-    // texels.  One address range reserved for store_max frames at the first stored frame's size and mapped as it
-    // fills, so a stored frame never moves.  Frames, not map state: reset, uploads and pool growth leave it as it is.
-    int32_t store_max = 0;               // 0: off
-    int32_t store_count = 0;             // filled slots, [0, store_count): their copies are enqueued
-    int store_H = 0, store_W = 0;        // size of every stored frame (0: none stored yet)
-    bool store_stopped = false;          // the device could not reserve or map more: no frame is stored any more
-    size_t store_map_limit = SIZE_MAX;   // B2V_FRAME_STORE_MAX_BYTES: the most the store maps (tests of that path)
-    VmmRange store;
-    std::vector<int32_t> store_last;     // slot of each frame of the most recent integrate call, or -1
+    // frame store (b2v_set_frame_store): the packed texel image of each stored frame, H * W texels per slot
+    FrameStore store;
 };
 
 // ---- the block pool: virtual memory management entry points of the driver ----
@@ -304,6 +296,51 @@ void b2v::vmm_release(VmmRange *r) {
     r->reserved = r->mapped = 0;
 }
 
+// ---- frame store ----
+
+b2v::FrameStore::FrameStore() {
+    if (const char *e = std::getenv("B2V_FRAME_STORE_MAX_BYTES")) map_limit = std::strtoull(e, nullptr, 10);
+}
+
+void b2v::FrameStore::assign(int32_t n_frames, int fH, int fW, size_t fpitch, int device, cudaStream_t stream) {
+    if (max == 0 || stopped) return;
+    std::string err;   // not the owner's error: a store that cannot grow stops storing, the call goes on
+    if (H == 0) {
+        if (!vmm_reserve(&range, static_cast<size_t>(max) * fpitch, device, &err)) {
+            stopped = true;
+            return;
+        }
+        H = fH;
+        W = fW;
+        pitch = fpitch;
+    }
+    if (fH != H || fW != W) return;
+    // map the store's first `bytes` bytes; false, with nothing mapped past what was, past map_limit or on failure
+    auto map = [&](size_t bytes) {
+        const size_t g = range.gran;
+        return (bytes + g - 1) / g * g <= map_limit && vmm_map(&range, bytes, stream, &err);
+    };
+    int32_t n = std::min(n_frames, max - count);
+    const size_t need = static_cast<size_t>(count + n) * pitch;
+    if (n > 0 && need > range.mapped) {
+        const size_t doubled = std::min(range.reserved, 2 * range.mapped);
+        if (!(doubled > need && map(doubled)) && !map(need)) {
+            stopped = true;
+            n = static_cast<int32_t>(std::min<size_t>(n, range.mapped / pitch - count));
+        }
+    }
+    for (int32_t f = 0; f < n; ++f) last[f] = count + f;
+}
+
+void b2v::FrameStore::release() {
+    vmm_release(&range);
+    count = 0;
+    H = W = 0;
+    pitch = 0;
+    stopped = false;
+    std::fill(last.begin(), last.end(), -1);
+}
+
 // reserve the address range of meta.capacity blocks
 static size_t block_bytes(const b2v_volume *v) { return tsdf_block_bytes(v->cfg.color_f64 != 0); }
 
@@ -406,7 +443,6 @@ extern "C" int b2v_create(const b2v_config *cfg, b2v_volume **out) {
     if (const char *e = std::getenv("B2V_OVERLAP")) v->overlap = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_TMA")) v->use_tma = std::atoi(e) != 0;
     if (const char *e = std::getenv("B2V_FUSE")) v->fuse = std::atoi(e) != 0;
-    if (const char *e = std::getenv("B2V_FRAME_STORE_MAX_BYTES")) v->store_map_limit = std::strtoull(e, nullptr, 10);
     if (const char *e = std::getenv("B2V_GROUP")) {
         const int n = std::atoi(e);
         if (n >= 1 && n <= kMaxGroup) v->group_frames = n;
@@ -733,50 +769,6 @@ static int rectify_frame(b2v_volume *v, const float **d_depth, const uint8_t **d
     return B2V_OK;
 }
 
-static Texel *store_slot(const b2v_volume *v, int32_t slot) {
-    return reinterpret_cast<Texel *>(v->store.va) + static_cast<size_t>(slot) * v->store_H * v->store_W;
-}
-
-// map storage for the store's first `bytes` bytes (zeroed on `stream`); false, with nothing mapped past what was, when
-// the device cannot map it or it would pass store_map_limit
-static bool store_map(b2v_volume *v, size_t bytes, cudaStream_t stream) {
-    const size_t g = v->store.gran;
-    std::string err;   // not the volume's error: a store that cannot grow stops storing, the call goes on
-    return (bytes + g - 1) / g * g <= v->store_map_limit && vmm_map(&v->store, bytes, stream, &err);
-}
-
-// The store slots of the frames of an integrate call (v->store_last; -1: not stored), before anything is launched:
-// handed out in frame order while the store has room, to frames of the stored frames' size.  The first stored frame
-// sets that size and reserves the address range; the storage the call's frames need is mapped here (at least doubling
-// the mapping, else just what they need).  When the device cannot reserve or map it, the frames that fit in what is
-// mapped are stored and the store stops: later frames are not stored and integration goes on.  A slot counts as
-// filled (store_count) only once its copy is enqueued; the slots of groups a failing call did not reach go back to -1
-// (enqueue_frames).
-static void assign_store_slots(b2v_volume *v, int32_t n_frames, int H, int W, cudaStream_t stream) {
-    if (v->store_max == 0 || v->store_stopped) return;
-    if (v->store_H == 0) {
-        std::string err;
-        if (!vmm_reserve(&v->store, static_cast<size_t>(v->store_max) * H * W * sizeof(Texel), v->cfg.device, &err)) {
-            v->store_stopped = true;
-            return;
-        }
-        v->store_H = H;
-        v->store_W = W;
-    }
-    if (H != v->store_H || W != v->store_W) return;
-    const size_t pitch = static_cast<size_t>(H) * W * sizeof(Texel);
-    int32_t n = std::min(n_frames, v->store_max - v->store_count);
-    const size_t need = static_cast<size_t>(v->store_count + n) * pitch;
-    if (n > 0 && need > v->store.mapped) {
-        const size_t doubled = std::min(v->store.reserved, 2 * v->store.mapped);
-        if (!(doubled > need && store_map(v, doubled, stream)) && !store_map(v, need, stream)) {
-            v->store_stopped = true;
-            n = static_cast<int32_t>(std::min<size_t>(n, v->store.mapped / pitch - v->store_count));
-        }
-    }
-    for (int32_t f = 0; f < n; ++f) v->store_last[f] = v->store_count + f;
-}
-
 // Enqueues n_frames frames, contiguous in the caller's arrays, as groups in the group buffers: groups of up to
 // group_frames frames on the fused kernels when fusion is on and there are two frames or more, else groups of one
 // frame on the frame-by-frame kernels.  depth is float32 metres (u16_scale = 0) or raw uint16 widened on the device
@@ -789,15 +781,12 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
                           void *stream, const int32_t *stored = nullptr) {
     const cudaEvent_t inputs_ready = v->input_event;  // one-shot: consumed by bad arguments too
     v->input_event = nullptr;
-    v->store_last.assign(static_cast<size_t>(std::max(n_frames, 0)), -1);  // (also when the call fails)
+    v->store.begin_call(n_frames);  // (also when the call fails)
     // on every return: the slots of frames whose copies were not enqueued are not stored
     struct UnfilledSlots {
-        b2v_volume *v;
-        ~UnfilledSlots() {
-            for (int32_t &s : v->store_last)
-                if (s >= v->store_count) s = -1;
-        }
-    } unfilled{v};
+        FrameStore &s;
+        ~UnfilledSlots() { s.drop_unfilled(); }
+    } unfilled{v->store};
     const bool replay = stored != nullptr;
     if (n_frames < 0 || (n_frames > 0 && ((!replay && (!depth || !color)) || !Tcw || !K)) || height <= 0 ||
         width <= 0) {
@@ -826,7 +815,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         int rc = ensure_staging(v, pixels);
         if (rc == B2V_OK && u16) rc = ensure_staging16(v, pixels);
         if (rc != B2V_OK) return rc;
-        if (!replay) assign_store_slots(v, n_frames, height, width, as);
+        if (!replay) v->store.assign(n_frames, height, width, pixels * sizeof(Texel), v->cfg.device, as);
     }
     // This call's updates touch the blocks the previous call's did, and a block's running average depends on frame
     // order: on another stream they wait for the previous call's last update (on the same stream, stream order does
@@ -919,7 +908,7 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
             const uint8_t *d_color = nullptr;
             Texel *tex = stage_slot(v->d_tex, texel_pitch(pixels), s0 + k);
             if (replay) {  // the gather: the stored texel image into the frame's staging slot
-                B2V_CUDA(v, cudaMemcpyAsync(tex, store_slot(v, stored[f]), pixels * sizeof(Texel),
+                B2V_CUDA(v, cudaMemcpyAsync(tex, v->store.slot(stored[f]), pixels * sizeof(Texel),
                                             cudaMemcpyDeviceToDevice, as));
             } else {
                 d_depth = dev_depth && !u16 ? depth32 + pixels * f : stage_slot(v->d_depth, pixels, s0 + k);
@@ -963,15 +952,15 @@ static int enqueue_frames(b2v_volume *v, const char *what, int32_t n_frames, con
         v->launches += fused ? 2 : 1;  // (+ the expand kernel of a fused group)
         if (!replay) {
             // the frame store: copy the packed texel images of the group's stored frames (mapped by
-            // assign_store_slots) on the allocate stream, after the pack and before the next group in this buffer
+            // FrameStore::assign) on the allocate stream, after the pack and before the next group in this buffer
             // overwrites the staging slots (its allocate kernels wait on this stream).  Enqueued after ev_galloc: with
             // overlap on, the update does not wait for the copies; with it off they share its stream.
             for (int k = 0; k < count; ++k) {
-                const int32_t slot = v->store_last[g0 + k];
+                const int32_t slot = v->store.last[g0 + k];
                 if (slot < 0) continue;
-                B2V_CUDA(v, cudaMemcpyAsync(store_slot(v, slot), aargs.tex[k], pixels * sizeof(Texel),
+                B2V_CUDA(v, cudaMemcpyAsync(v->store.slot(slot), aargs.tex[k], pixels * sizeof(Texel),
                                             cudaMemcpyDeviceToDevice, as));
-                v->store_count = slot + 1;   // filled: slots are handed out and copied in frame order
+                v->store.filled(slot);
             }
         }
         if (v->overlap) B2V_CUDA(v, cudaStreamWaitEvent(cs, v->ev_galloc[buf], 0));
@@ -1024,11 +1013,7 @@ extern "C" int b2v_integrate_batch_u16(b2v_volume *v, int32_t n_frames, const ui
 static int frame_store_release(b2v_volume *v) {
     B2V_CUDA(v, cudaSetDevice(v->cfg.device));
     B2V_CUDA(v, cudaDeviceSynchronize());   // replays gather on the caller's stream when overlap is off
-    vmm_release(&v->store);
-    v->store_count = 0;
-    v->store_H = v->store_W = 0;
-    v->store_stopped = false;
-    std::fill(v->store_last.begin(), v->store_last.end(), -1);
+    v->store.release();
     return B2V_OK;
 }
 
@@ -1040,7 +1025,7 @@ extern "C" int b2v_set_frame_store(b2v_volume *v, int32_t max_frames) {
     }
     const int rc = frame_store_release(v);
     if (rc != B2V_OK) return rc;
-    v->store_max = max_frames;
+    v->store.max = max_frames;
     return B2V_OK;
 }
 
@@ -1051,37 +1036,37 @@ extern "C" int b2v_frame_store_clear(b2v_volume *v) {
 
 extern "C" int b2v_frame_store_last(b2v_volume *v, int32_t *slots, int32_t n) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    if (n != static_cast<int32_t>(v->store_last.size()) || (n > 0 && !slots)) {
+    if (n != static_cast<int32_t>(v->store.last.size()) || (n > 0 && !slots)) {
         v->err = "b2v_frame_store_last: n must be the frame count of the most recent integrate call";
         return B2V_ERR_INVALID_ARGUMENT;
     }
-    std::copy(v->store_last.begin(), v->store_last.end(), slots);
+    std::copy(v->store.last.begin(), v->store.last.end(), slots);
     return B2V_OK;
 }
 
 extern "C" int b2v_frame_store_stats(b2v_volume *v, int64_t *frames, int64_t *bytes) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    if (frames) *frames = v->store_count;
-    if (bytes) *bytes = static_cast<int64_t>(v->store.mapped);
+    if (frames) *frames = v->store.count;
+    if (bytes) *bytes = static_cast<int64_t>(v->store.range.mapped);
     return B2V_OK;
 }
 
 extern "C" int b2v_integrate_stored(b2v_volume *v, int32_t n_frames, const int32_t *slots, const double K[4],
                                     const double *Tcw, void *stream) {
     if (!v) return B2V_ERR_INVALID_ARGUMENT;
-    v->store_last.assign(static_cast<size_t>(std::max(n_frames, 0)), -1);
+    v->store.begin_call(n_frames);
     if (n_frames > 0 && !slots) {
         v->err = "b2v_integrate_stored: bad arguments";
         return B2V_ERR_INVALID_ARGUMENT;
     }
     for (int32_t f = 0; f < n_frames; ++f)
-        if (slots[f] < 0 || slots[f] >= v->store_count) {
+        if (!v->store.holds(slots[f])) {
             v->err = "b2v_integrate_stored: slot " + std::to_string(slots[f]) + " holds no frame (the store holds " +
-                     std::to_string(v->store_count) + ")";
+                     std::to_string(v->store.count) + ")";
             return B2V_ERR_INVALID_ARGUMENT;
         }
-    return enqueue_frames(v, "b2v_integrate_stored", n_frames, nullptr, 0.0f, nullptr, std::max(v->store_H, 1),
-                          std::max(v->store_W, 1), K, Tcw, stream, slots);
+    return enqueue_frames(v, "b2v_integrate_stored", n_frames, nullptr, 0.0f, nullptr, std::max(v->store.H, 1),
+                          std::max(v->store.W, 1), K, Tcw, stream, slots);
 }
 
 extern "C" int b2v_set_input_event(b2v_volume *v, void *event) {

@@ -773,25 +773,16 @@ int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scal
     else if (frame.mapx.get() && (H != frame.map_h || W != frame.map_w))
         bad = "set_frame: rectification maps were installed for a different image size";
     else if (filter_shadow_points && (H <= 2 || W <= 2)) bad = "set_frame: image too small for the shadow filter";
+    frame_store.begin_call(1);   // (also when the call fails)
     if (bad) {
         err = bad;
         return B2V_ERR_INVALID_ARGUMENT;
     }
     B2V_CUDA(this, cudaSetDevice(device));
-    frame.staged = b2v_frame{};
     const size_t pixels = static_cast<size_t>(H) * W;
-    // synchronise when the last buffer of a group is short, as stage_input does
-    if (pixels * 3 > frame.rgb.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
-    B2V_CUDA(this, frame.raw.reserve(pixels));
-    B2V_CUDA(this, frame.depth.reserve(pixels));
-    B2V_CUDA(this, frame.filtered.reserve(pixels));
-    B2V_CUDA(this, frame.shadow_scratch.reserve(kShadowScratchBytes));
-    B2V_CUDA(this, frame.rgb.reserve(pixels * 3));
-    if (cls) {
-        if (pixels > frame.obj.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
-        B2V_CUDA(this, frame.cls.reserve(pixels));
-        B2V_CUDA(this, frame.inst.reserve(pixels));
-        B2V_CUDA(this, frame.obj.reserve(pixels));
+    {
+        const int rc = reserve_frame(pixels, cls != nullptr);
+        if (rc != B2V_OK) return rc;
     }
     cudaStream_t s = stream;
     const bool rect = frame.mapx.get() != nullptr;
@@ -833,19 +824,100 @@ int BlockGridCore::set_frame(const void *depth, bool depth_u16, float depth_scal
     if (e == cudaSuccess && filter_shadow_points)
         e = launch_filter_shadow_points(frame.depth.get(), H, W, 2, 2, -1.0f, frame.filtered.get(),
                                         frame.shadow_scratch.get(), s);
+    // the frame store: the staged images into the next slot, before the synchronise below
+    int32_t stored = -1;
+    if (e == cudaSuccess && frame_store.max > 0) {
+        frame_store.assign(1, H, W, grid_record_pitch(pixels, frame_labels), device, s);
+        if (frame_store.last[0] >= 0) {
+            e = launch_grid_frame_pack(frame.depth.get(), filter_shadow_points ? frame.filtered.get() : nullptr,
+                                       frame.rgb.get(), cls ? frame.cls.get() : nullptr,
+                                       inst ? frame.inst.get() : nullptr, pixels, frame_labels,
+                                       frame_store.slot(frame_store.last[0]), s);
+            if (e == cudaSuccess) stored = frame_store.last[0];
+        }
+    }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) {
+        frame_store.drop_unfilled();
         err = std::string("set_frame: ") + cudaGetErrorString(e);
         return B2V_ERR_CUDA;
     }
+    if (stored >= 0) {
+        frame_store.filled(stored);
+        store_flags.resize(static_cast<size_t>(frame_store.count));
+        store_flags[stored] = static_cast<uint8_t>((cls ? kStoredClass : 0) | (inst ? kStoredInstance : 0) |
+                                                   (filter_shadow_points ? kStoredFiltered : 0));
+    }
+    finish_frame(H, W, filter_shadow_points, cls != nullptr, inst != nullptr, out);
+    return B2V_OK;
+}
+
+int BlockGridCore::reserve_frame(size_t pixels, bool labels) {
+    frame.staged = b2v_frame{};
+    // synchronise when the last buffer of a group is short, as stage_input does
+    if (pixels * 3 > frame.rgb.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+    B2V_CUDA(this, frame.raw.reserve(pixels));
+    B2V_CUDA(this, frame.depth.reserve(pixels));
+    B2V_CUDA(this, frame.filtered.reserve(pixels));
+    B2V_CUDA(this, frame.shadow_scratch.reserve(kShadowScratchBytes));
+    B2V_CUDA(this, frame.rgb.reserve(pixels * 3));
+    if (labels) {
+        if (pixels > frame.obj.size()) B2V_CUDA(this, cudaStreamSynchronize(stream));
+        B2V_CUDA(this, frame.cls.reserve(pixels));
+        B2V_CUDA(this, frame.inst.reserve(pixels));
+        B2V_CUDA(this, frame.obj.reserve(pixels));
+    }
+    return B2V_OK;
+}
+
+void BlockGridCore::finish_frame(int H, int W, bool filtered, bool cls, bool inst, b2v_frame *out) {
     frame.staged.depth = frame.depth.get();
-    frame.staged.filtered_depth = filter_shadow_points ? frame.filtered.get() : frame.depth.get();
+    frame.staged.filtered_depth = filtered ? frame.filtered.get() : frame.depth.get();
     frame.staged.color = frame.rgb.get();
     frame.staged.class_image = cls ? frame.cls.get() : nullptr;
     frame.staged.instance_image = inst ? frame.inst.get() : nullptr;
     frame.staged.height = H;
     frame.staged.width = W;
     *out = frame.staged;
+}
+
+int BlockGridCore::set_frame_store(int32_t max_frames) {
+    if (max_frames < 0) {
+        err = "set_frame_store: max_frames must be >= 0";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(this, cudaSetDevice(device));
+    B2V_CUDA(this, cudaStreamSynchronize(stream));
+    frame_store.release();
+    store_flags.clear();
+    frame_store.max = max_frames;
+    return B2V_OK;
+}
+
+int BlockGridCore::stage_stored(int32_t slot, b2v_frame *out) {
+    if (!out || !frame_store.holds(slot)) {
+        err = "stage_stored: slot " + std::to_string(slot) + " holds no frame (the store holds " +
+              std::to_string(frame_store.count) + ")";
+        return B2V_ERR_INVALID_ARGUMENT;
+    }
+    B2V_CUDA(this, cudaSetDevice(device));
+    const size_t pixels = static_cast<size_t>(frame_store.H) * frame_store.W;
+    const uint8_t fl = store_flags[slot];
+    const bool filtered = fl & kStoredFiltered, cls = fl & kStoredClass, inst = fl & kStoredInstance;
+    {
+        const int rc = reserve_frame(pixels, cls);
+        if (rc != B2V_OK) return rc;
+    }
+    cudaError_t e = launch_grid_frame_unpack(frame_store.slot(slot), pixels, frame_labels, frame.depth.get(),
+                                             filtered ? frame.filtered.get() : nullptr, frame.rgb.get(),
+                                             cls ? frame.cls.get() : nullptr, inst ? frame.inst.get() : nullptr,
+                                             stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) {
+        err = std::string("stage_stored: ") + cudaGetErrorString(e);
+        return B2V_ERR_CUDA;
+    }
+    finish_frame(frame_store.H, frame_store.W, filtered, cls, inst, out);
     return B2V_OK;
 }
 
@@ -1148,6 +1220,34 @@ extern "C" int b2v_grid_set_frame(b2v_grid *g, const void *depth, int32_t depth_
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     return g->set_frame(depth, depth_u16 != 0, depth_scale, color, nullptr, nullptr, height, width,
                         filter_shadow_points != 0, out);
+}
+
+extern "C" int b2v_grid_set_frame_store(b2v_grid *g, int32_t max_frames) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame_store(max_frames);
+}
+
+extern "C" int b2v_grid_frame_store_clear(b2v_grid *g) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame_store(g->frame_store.max);
+}
+
+extern "C" int b2v_grid_frame_store_last(b2v_grid *g, int32_t *slot) {
+    if (!g || !slot) return B2V_ERR_INVALID_ARGUMENT;
+    *slot = g->frame_store.last.empty() ? -1 : g->frame_store.last[0];
+    return B2V_OK;
+}
+
+extern "C" int b2v_grid_frame_store_stats(b2v_grid *g, int64_t *frames, int64_t *bytes) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (frames) *frames = g->frame_store.count;
+    if (bytes) *bytes = static_cast<int64_t>(g->frame_store.range.mapped);
+    return B2V_OK;
+}
+
+extern "C" int b2v_grid_stage_stored(b2v_grid *g, int32_t slot, b2v_frame *out) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->stage_stored(slot, out);
 }
 
 extern "C" int b2v_grid_synchronize(b2v_grid *g) {

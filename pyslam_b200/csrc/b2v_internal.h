@@ -84,6 +84,42 @@ bool vmm_reserve(VmmRange *r, size_t bytes, int device, std::string *err);
 bool vmm_map(VmmRange *r, size_t bytes, cudaStream_t stream, std::string *err);
 void vmm_release(VmmRange *r);
 
+// ---- frame store: the frames a map keeps on the device for a loop-closure rebuild (b2v_api.cu) ----
+// Slot s of a store holds one frame of the stored frames' size at s * pitch bytes of one address range, reserved for
+// `max` frames at the first stored frame and mapped as the store fills, so a stored frame never moves.  Frames, not
+// map state: the owner's reset, uploads and growth leave it as it is.  The owner packs a frame into slot(s) and calls
+// filled(s) once that copy is enqueued.
+struct FrameStore {
+    int32_t max = 0;               // 0: off
+    int32_t count = 0;             // filled slots, [0, count): their copies are enqueued
+    int H = 0, W = 0;              // size of every stored frame (0: none stored yet)
+    size_t pitch = 0;              // bytes per slot
+    bool stopped = false;          // the device could not reserve or map more: no frame is stored any more
+    size_t map_limit = SIZE_MAX;   // B2V_FRAME_STORE_MAX_BYTES: the most the store maps (tests of that path)
+    VmmRange range;
+    std::vector<int32_t> last;     // slot of each frame of the owner's most recent call, or -1
+
+    FrameStore();   // reads B2V_FRAME_STORE_MAX_BYTES
+    void *slot(int32_t s) const { return reinterpret_cast<char *>(range.va) + static_cast<size_t>(s) * pitch; }
+    // last := n times -1 (every call that may store frames starts with it, and so does one that stores none)
+    void begin_call(int32_t n) { last.assign(static_cast<size_t>(std::max(n, 0)), -1); }
+    // The slots of the first n entries of `last`, before anything is launched: handed out in frame order while the
+    // store has room, to frames of the stored frames' size.  The first stored frame sets that size and reserves the
+    // address range (pitch bytes per slot); the storage the frames need is mapped here (zeroed on `stream`; at least
+    // doubling the mapping, else just what they need).  When the device cannot reserve or map it, the frames that fit
+    // in what is mapped get slots and the store stops: later frames are not stored and the owner's call goes on.
+    void assign(int32_t n, int H, int W, size_t pitch, int device, cudaStream_t stream);
+    void filled(int32_t s) { count = s + 1; }   // slots are handed out and filled in frame order
+    // on every return of a call: the slots whose copies were not enqueued go back to -1
+    void drop_unfilled() {
+        for (int32_t &s : last)
+            if (s >= count) s = -1;
+    }
+    bool holds(int32_t s) const { return s >= 0 && s < count; }
+    // empties the store and releases its memory; the caller first waits for every call that may read or write it
+    void release();
+};
+
 // Texel of the update kernels, one per pixel of a frame, packed by the allocate kernels: {depth, r | g << 8 | b << 16}.
 // depth is 0 where the pixel is invalid (0, or beyond depth_trunc).  The depth-to-camera-distance multiplier is not
 // in the texel: the update kernels read it from the lambda image at the same pixel (one image per set of intrinsics).
@@ -608,6 +644,22 @@ struct BlockGridCore {
     // are checked before anything is touched.
     int set_frame(const void *depth, bool depth_u16, float depth_scale, const uint8_t *color, const int32_t *cls,
                   const int32_t *inst, int H, int W, bool filter_shadow_points, b2v_frame *out);
+
+    // Frame store (b2v_grid_set_frame_store / b2v_sgrid_set_frame_store): with it on, each successful set_frame packs
+    // its staged images into the next slot (launch_grid_frame_pack), one record per pixel: 8 bytes, or 16 with the
+    // label images of the semantic grids (frame_labels).  stage_stored unpacks a slot back into `frame`.
+    FrameStore frame_store;
+    bool frame_labels = false;   // semantic grids: records carry the class and instance images
+    enum : uint8_t { kStoredClass = 1, kStoredInstance = 2, kStoredFiltered = 4 };
+    std::vector<uint8_t> store_flags;   // per filled slot: which images set_frame staged
+    int set_frame_store(int32_t max_frames);   // empties the store (synchronises)
+    // set_frame / stage_stored: frame.staged := {}, the frame buffers sized for `pixels` (label buffers with labels);
+    // then frame.staged := the staged images and *out := frame.staged
+    int reserve_frame(size_t pixels, bool labels);
+    void finish_frame(int H, int W, bool filtered, bool cls, bool inst, b2v_frame *out);
+    // *out := the b2v_frame set_frame returned for the slot's frame, its images unpacked into `frame`.  A slot the
+    // store does not hold changes nothing.  Synchronises.
+    int stage_stored(int32_t slot, b2v_frame *out);
 };
 
 template <typename MapStorage, typename Replay> int BlockGridCore::resolve(MapStorage map_storage, Replay replay) {
@@ -639,6 +691,18 @@ int BlockGridCore::upload_blocks(int64_t n, const int32_t *keys4, const BlockArr
 
 // raw uint16 depth -> float32 metres (b2v_prep.cu)
 cudaError_t launch_depth_u16_to_f32(const uint16_t *src, float *dst, size_t n, float scale, cudaStream_t stream);
+
+// Frame-store records of the grids (b2v_prep.cu): per pixel {depth bits, r, g, b, flags} (8 bytes), followed with
+// labels by {class, instance} (16 bytes).  flags bit 0: the shadow filter set the pixel, i.e. filtered != depth
+// bitwise; the filter writes only `m ? -1.0f : d`, so unpack rebuilds filtered = flag ? -1.0f : depth exactly.
+// filtered / cls / inst NULL: not packed (unpack: not written).  `rec` is 16-byte aligned.
+constexpr size_t grid_record_pitch(size_t pixels, bool labels) {   // bytes per slot: whole 4-pixel groups
+    return (pixels + 3) / 4 * 4 * (labels ? 16 : 8);
+}
+cudaError_t launch_grid_frame_pack(const float *depth, const float *filtered, const uint8_t *rgb, const int32_t *cls,
+                                   const int32_t *inst, size_t pixels, bool labels, void *rec, cudaStream_t stream);
+cudaError_t launch_grid_frame_unpack(const void *rec, size_t pixels, bool labels, float *depth, float *filtered,
+                                     uint8_t *rgb, int32_t *cls, int32_t *inst, cudaStream_t stream);
 
 // filter_shadow_points (pyslam/utilities/depth.py:103-146) on the device; scratch: 64 + 16384 bytes
 constexpr size_t kShadowScratchBytes = 64 + 4096 * sizeof(uint32_t);

@@ -274,6 +274,164 @@ __global__ void remap_instance_ids_kernel(const int32_t *__restrict__ src, const
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// frame-store records of the grids (b2v_internal.h, launch_grid_frame_pack): one thread per group of 4 pixels, with
+// 16-byte loads and stores of depth, filtered depth, labels and records (colour: three 4-byte words); the pixels of a
+// last partial group one by one.  Word 1 of a record: r | g << 8 | b << 16 | flags << 24.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t record_word1(float d, float f, uint32_t rgb) {
+    return rgb | (__float_as_uint(f) != __float_as_uint(d) ? 1u << 24 : 0u);
+}
+
+template <bool Labels>
+__global__ void __launch_bounds__(256)
+grid_frame_pack_kernel(const float *__restrict__ depth, const float *__restrict__ filtered,
+                       const uint8_t *__restrict__ rgb, const int32_t *__restrict__ cls,
+                       const int32_t *__restrict__ inst, const size_t n, uint32_t *__restrict__ rec) {
+    constexpr int kWords = Labels ? 4 : 2;   // record words per pixel
+    const size_t groups = (n + 3) / 4;
+    for (size_t q = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < groups;
+         q += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const size_t p0 = 4 * q;
+        uint32_t *r = rec + p0 * kWords;
+        if (p0 + 4 <= n) {
+            const float4 d = __ldg(reinterpret_cast<const float4 *>(depth + p0));
+            const float4 f = filtered ? __ldg(reinterpret_cast<const float4 *>(filtered + p0)) : d;
+            const uint32_t *cw = reinterpret_cast<const uint32_t *>(rgb + 3 * p0);
+            const uint32_t w0 = __ldg(cw), w1 = __ldg(cw + 1), w2 = __ldg(cw + 2);
+            const uint32_t c0 = w0 & 0xFFFFFFu, c1 = (w0 >> 24) | ((w1 & 0xFFFFu) << 8),
+                           c2 = (w1 >> 16) | ((w2 & 0xFFu) << 16), c3 = w2 >> 8;
+            const uint4 a = make_uint4(__float_as_uint(d.x), record_word1(d.x, f.x, c0), __float_as_uint(d.y),
+                                       record_word1(d.y, f.y, c1));
+            const uint4 b = make_uint4(__float_as_uint(d.z), record_word1(d.z, f.z, c2), __float_as_uint(d.w),
+                                       record_word1(d.w, f.w, c3));
+            if constexpr (Labels) {
+                if (cls) {
+                    const int4 k = __ldg(reinterpret_cast<const int4 *>(cls + p0));
+                    const int4 m = inst ? __ldg(reinterpret_cast<const int4 *>(inst + p0)) : make_int4(0, 0, 0, 0);
+                    uint4 *o = reinterpret_cast<uint4 *>(r);
+                    o[0] = make_uint4(a.x, a.y, k.x, m.x);
+                    o[1] = make_uint4(a.z, a.w, k.y, m.y);
+                    o[2] = make_uint4(b.x, b.y, k.z, m.z);
+                    o[3] = make_uint4(b.z, b.w, k.w, m.w);
+                } else {   // the label half is not written
+                    uint2 *o = reinterpret_cast<uint2 *>(r);
+                    o[0] = make_uint2(a.x, a.y);
+                    o[2] = make_uint2(a.z, a.w);
+                    o[4] = make_uint2(b.x, b.y);
+                    o[6] = make_uint2(b.z, b.w);
+                }
+            } else {
+                reinterpret_cast<uint4 *>(r)[0] = a;
+                reinterpret_cast<uint4 *>(r)[1] = b;
+            }
+        } else {
+            for (size_t p = p0; p < n; ++p, r += kWords) {
+                const float d = depth[p], f = filtered ? filtered[p] : d;
+                const uint8_t *c = rgb + 3 * p;
+                r[0] = __float_as_uint(d);
+                r[1] = record_word1(d, f, c[0] | (static_cast<uint32_t>(c[1]) << 8) | (static_cast<uint32_t>(c[2]) << 16));
+                if constexpr (Labels) {
+                    if (cls) {
+                        r[2] = static_cast<uint32_t>(cls[p]);
+                        r[3] = inst ? static_cast<uint32_t>(inst[p]) : 0u;
+                    }
+                }
+            }
+        }
+    }
+}
+
+// the bits of the filtered depth: -1.0f where the filter set the pixel, else the depth's bits (NaN payloads included)
+__device__ __forceinline__ uint32_t record_filtered(uint32_t w0, uint32_t w1) {
+    return (w1 >> 24) & 1u ? 0xBF800000u : w0;
+}
+
+template <bool Labels>
+__global__ void __launch_bounds__(256)
+grid_frame_unpack_kernel(const uint32_t *__restrict__ rec, const size_t n, float *__restrict__ depth,
+                         float *__restrict__ filtered, uint8_t *__restrict__ rgb, int32_t *__restrict__ cls,
+                         int32_t *__restrict__ inst) {
+    constexpr int kWords = Labels ? 4 : 2;
+    const size_t groups = (n + 3) / 4;
+    for (size_t q = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < groups;
+         q += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const size_t p0 = 4 * q;
+        const uint32_t *r = rec + p0 * kWords;
+        if (p0 + 4 <= n) {
+            uint4 px[4];   // {depth bits, word 1, class, instance} of each pixel
+            if constexpr (Labels) {
+                const uint4 *in = reinterpret_cast<const uint4 *>(r);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) px[k] = __ldg(in + k);
+            } else {
+                const uint4 a = __ldg(reinterpret_cast<const uint4 *>(r)), b = __ldg(reinterpret_cast<const uint4 *>(r) + 1);
+                px[0] = make_uint4(a.x, a.y, 0, 0);
+                px[1] = make_uint4(a.z, a.w, 0, 0);
+                px[2] = make_uint4(b.x, b.y, 0, 0);
+                px[3] = make_uint4(b.z, b.w, 0, 0);
+            }
+            *reinterpret_cast<uint4 *>(depth + p0) = make_uint4(px[0].x, px[1].x, px[2].x, px[3].x);
+            if (filtered)
+                *reinterpret_cast<uint4 *>(filtered + p0) =
+                    make_uint4(record_filtered(px[0].x, px[0].y), record_filtered(px[1].x, px[1].y),
+                                record_filtered(px[2].x, px[2].y), record_filtered(px[3].x, px[3].y));
+            const uint32_t c0 = px[0].y & 0xFFFFFFu, c1 = px[1].y & 0xFFFFFFu, c2 = px[2].y & 0xFFFFFFu,
+                           c3 = px[3].y & 0xFFFFFFu;
+            uint32_t *cw = reinterpret_cast<uint32_t *>(rgb + 3 * p0);
+            cw[0] = c0 | (c1 << 24);
+            cw[1] = (c1 >> 8) | (c2 << 16);
+            cw[2] = (c2 >> 16) | (c3 << 8);
+            if constexpr (Labels) {
+                if (cls) *reinterpret_cast<uint4 *>(cls + p0) = make_uint4(px[0].z, px[1].z, px[2].z, px[3].z);
+                if (inst) *reinterpret_cast<uint4 *>(inst + p0) = make_uint4(px[0].w, px[1].w, px[2].w, px[3].w);
+            }
+        } else {
+            for (size_t p = p0; p < n; ++p, r += kWords) {
+                const uint32_t w0 = r[0], w1 = r[1];
+                depth[p] = __uint_as_float(w0);
+                if (filtered) filtered[p] = __uint_as_float(record_filtered(w0, w1));
+                rgb[3 * p] = static_cast<uint8_t>(w1);
+                rgb[3 * p + 1] = static_cast<uint8_t>(w1 >> 8);
+                rgb[3 * p + 2] = static_cast<uint8_t>(w1 >> 16);
+                if constexpr (Labels) {
+                    if (cls) cls[p] = static_cast<int32_t>(r[2]);
+                    if (inst) inst[p] = static_cast<int32_t>(r[3]);
+                }
+            }
+        }
+    }
+}
+
+static unsigned record_ctas(size_t pixels) {
+    return static_cast<unsigned>(std::min<size_t>((pixels + 4 * 256 - 1) / (4 * 256), 2368));
+}
+
+cudaError_t launch_grid_frame_pack(const float *depth, const float *filtered, const uint8_t *rgb, const int32_t *cls,
+                                   const int32_t *inst, size_t pixels, bool labels, void *rec, cudaStream_t stream) {
+    if (pixels == 0) return cudaSuccess;
+    uint32_t *r = static_cast<uint32_t *>(rec);
+    if (labels)
+        grid_frame_pack_kernel<true><<<record_ctas(pixels), 256, 0, stream>>>(depth, filtered, rgb, cls, inst, pixels, r);
+    else
+        grid_frame_pack_kernel<false><<<record_ctas(pixels), 256, 0, stream>>>(depth, filtered, rgb, nullptr, nullptr,
+                                                                                pixels, r);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_grid_frame_unpack(const void *rec, size_t pixels, bool labels, float *depth, float *filtered,
+                                     uint8_t *rgb, int32_t *cls, int32_t *inst, cudaStream_t stream) {
+    if (pixels == 0) return cudaSuccess;
+    const uint32_t *r = static_cast<const uint32_t *>(rec);
+    if (labels)
+        grid_frame_unpack_kernel<true><<<record_ctas(pixels), 256, 0, stream>>>(r, pixels, depth, filtered, rgb, cls,
+                                                                                 inst);
+    else
+        grid_frame_unpack_kernel<false><<<record_ctas(pixels), 256, 0, stream>>>(r, pixels, depth, filtered, rgb,
+                                                                                  nullptr, nullptr);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_remap_instance_ids(const int32_t *src, size_t n, const int32_t *map_inst, const int32_t *map_obj,
                                       int n_map, int32_t *dst, cudaStream_t stream) {
     if (n == 0) return cudaSuccess;

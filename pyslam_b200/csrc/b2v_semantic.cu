@@ -977,6 +977,7 @@ extern "C" int b2v_sgrid_create_ex(double voxel_size, int32_t block_size, uint32
     b2v_sgrid *g = new (std::nothrow) b2v_sgrid();
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     g->G.kind = kind;
+    g->frame_labels = true;
     // class defaults (voxel_data_semantic.h:107-108, 251-254)
     g->G.depth_threshold = kind == B2V_SEM_VOTING ? 10.0f : 5.0f;
     g->G.depth_decay_rate = 0.07f;
@@ -1692,6 +1693,34 @@ extern "C" int b2v_sgrid_set_frame(b2v_sgrid *g, const void *depth, int32_t dept
     if (!g) return B2V_ERR_INVALID_ARGUMENT;
     return g->set_frame(depth, depth_u16 != 0, depth_scale, color, class_image, instance_image, height, width,
                         filter_shadow_points != 0, out);
+}
+
+extern "C" int b2v_sgrid_set_frame_store(b2v_sgrid *g, int32_t max_frames) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame_store(max_frames);
+}
+
+extern "C" int b2v_sgrid_frame_store_clear(b2v_sgrid *g) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->set_frame_store(g->frame_store.max);
+}
+
+extern "C" int b2v_sgrid_frame_store_last(b2v_sgrid *g, int32_t *slot) {
+    if (!g || !slot) return B2V_ERR_INVALID_ARGUMENT;
+    *slot = g->frame_store.last.empty() ? -1 : g->frame_store.last[0];
+    return B2V_OK;
+}
+
+extern "C" int b2v_sgrid_frame_store_stats(b2v_sgrid *g, int64_t *frames, int64_t *bytes) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    if (frames) *frames = g->frame_store.count;
+    if (bytes) *bytes = static_cast<int64_t>(g->frame_store.range.mapped);
+    return B2V_OK;
+}
+
+extern "C" int b2v_sgrid_stage_stored(b2v_sgrid *g, int32_t slot, b2v_frame *out) {
+    if (!g) return B2V_ERR_INVALID_ARGUMENT;
+    return g->stage_stored(slot, out);
 }
 
 extern "C" int b2v_sgrid_remap_instance_ids(b2v_sgrid *g, const int32_t **object_image) {

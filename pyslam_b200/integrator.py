@@ -55,7 +55,8 @@ DEFAULT_PARAMETERS = {
     # Open3D's bit for bit, at 16 KiB per block instead of 10 KiB (INTEGRATION.md section 2)
     "kVolumetricIntegrationB200ColorFloat64": False,
     # keep the packed frames of up to this many keyframes on the GPU (8 bytes per pixel: 2.46 MB per 640x480 keyframe),
-    # so that rebuild(map) sends only the keyframes' new poses to the integrator (keyframe_store.py); 0 = off
+    # so that rebuild(map) sends only the keyframes' new poses to the integrator (keyframe_store.py); 0 = off.  The
+    # grid plugins take the same parameter (integrator_semantic.py)
     "kVolumetricIntegrationB200KeyframeStoreFrames": 0,
 }
 
@@ -105,7 +106,66 @@ def raw_depth(depth, camera, use_cpp: bool):
 
 
 class B200PluginSetup:
-    """Set-up every B200 plugin shares; mixed in before pySLAM's `VolumetricIntegratorBase`."""
+    """Set-up every B200 plugin shares; mixed in before pySLAM's `VolumetricIntegratorBase`.  A plugin class sets
+    `_api` and `_defaults` (its parameter table)."""
+
+    # the stored-keyframe table publishes each slot's label images (keyframe_store.label_flags)
+    _STORE_LABELS = False
+
+    def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type, viewer_queue=None,
+                 **kwargs):
+        # the table of stored keyframes is created here, in the parent, before the base class spawns the
+        # integrator process, which receives it with the rest of the plugin
+        n = int(self._parent_parameter("kVolumetricIntegrationB200KeyframeStoreFrames", kwargs))
+        self._b200_keyframe_table = (keyframe_store.StoredKeyframeTable(n, labels=self._STORE_LABELS) if n > 0
+                                     else None)
+        super().__init__(camera, environment_type, sensor_type, volumetric_integrator_type, viewer_queue, **kwargs)
+
+    @classmethod
+    def _parent_parameter(cls, name, kwargs):
+        """A parameter as the parent process sees it: a constructor keyword, else the `parameters` dict keyword,
+        else pySLAM's Parameters class, else the default."""
+        if name in kwargs:
+            return kwargs[name]
+        if name in (kwargs.get("parameters") or {}):
+            return kwargs["parameters"][name]
+        return getattr(getattr(cls._api, "Parameters", None), name, cls._defaults[name])
+
+    def add_task(self, task):
+        """Every task the front end enqueues (keyframes and rebuild(map) alike, base.py:1216-1232): an INTEGRATE
+        task of a keyframe the integrator has stored travels without its images (keyframe_store.light_task)."""
+        if getattr(self, "_b200_keyframe_table", None) is not None:
+            task = keyframe_store.light_task(task, self._b200_keyframe_table,
+                                             self._api.VolumetricIntegrationTaskType.INTEGRATE)
+        super().add_task(task)
+
+    def _init_frame_store(self):
+        """In the integrator process: the map's frame store per kVolumetricIntegrationB200KeyframeStoreFrames."""
+        self._store_frames = int(self.b200_parameters["kVolumetricIntegrationB200KeyframeStoreFrames"])
+        if self._store_frames > 0:
+            self.volume.set_frame_store(self._store_frames)
+        self._stored_slots = {}         # keyframe_store.keyframe_key -> slot of the keyframes stored here
+
+    def _record_stored(self, kds, slots):
+        """Note the store slots of keyframes just integrated (slots: the map's last stored slots, or None with the
+        store off) and publish them to the parent's table."""
+        if slots is None:
+            return
+        table = getattr(self, "_b200_keyframe_table", None)
+        for kd, slot in zip(kds, slots):
+            if slot >= 0:
+                self._stored_slots[keyframe_store.keyframe_key(kd)] = int(slot)
+                if table is not None:
+                    table.publish(int(slot), kd)
+
+    def _stored_slot(self, kd):
+        """The store slot of a light task's keyframe; None, logged, when its frame is not stored here."""
+        slot = self._stored_slots.get(keyframe_store.keyframe_key(kd))
+        if slot is None:
+            getattr(type(self), "print", print)(
+                f"{type(self).__name__}: ERROR: keyframe {kd.id} (timestamp {kd.timestamp}) came without "
+                "images, but its frame is not in the frame store: it was not integrated")
+        return slot
 
     def _merge_parameters(self, defaults, parameters_dict, constructor_kwargs):
         """self.b200_parameters: `defaults`, overridden by parameters_dict, then by constructor_kwargs (known keys)."""
@@ -251,33 +311,8 @@ def make_integrator_class(Base, api):
         """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
 
         _api = api
+        _defaults = DEFAULT_PARAMETERS
         _SHARD_KIND = "tsdf"
-
-        def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
-                     viewer_queue=None, **kwargs):
-            # the table of stored keyframes is created here, in the parent, before the base class spawns the
-            # integrator process, which receives it with the rest of the plugin
-            n = int(self._parent_parameter("kVolumetricIntegrationB200KeyframeStoreFrames", kwargs))
-            self._b200_keyframe_table = keyframe_store.StoredKeyframeTable(n) if n > 0 else None
-            super().__init__(camera, environment_type, sensor_type, volumetric_integrator_type,
-                             viewer_queue, **kwargs)
-
-        @staticmethod
-        def _parent_parameter(name, kwargs):
-            """A parameter as the parent process sees it: a constructor keyword, else the `parameters` dict keyword,
-            else pySLAM's Parameters class, else the default."""
-            if name in kwargs:
-                return kwargs[name]
-            if name in (kwargs.get("parameters") or {}):
-                return kwargs["parameters"][name]
-            return getattr(getattr(api, "Parameters", None), name, DEFAULT_PARAMETERS[name])
-
-        def add_task(self, task):
-            """Every task the front end enqueues (keyframes and rebuild(map) alike, base.py:1216-1232): an INTEGRATE
-            task of a keyframe the integrator has stored travels without its images (keyframe_store.light_task)."""
-            if getattr(self, "_b200_keyframe_table", None) is not None:
-                task = keyframe_store.light_task(task, self._b200_keyframe_table, TaskType.INTEGRATE)
-            super().add_task(task)
 
         # -- runs inside the integrator process: the CUDA context is created here, never in the parent
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
@@ -302,10 +337,7 @@ def make_integrator_class(Base, api):
                 max_capacity_blocks=int(p["kVolumetricIntegrationB200MaxCapacityBlocks"]) or None,
                 volume_unit_resolution=int(p["kVolumetricIntegrationB200UnitResolution"]),
                 color_float64=bool(p["kVolumetricIntegrationB200ColorFloat64"]), **self._map_placement())
-            self._store_frames = int(p["kVolumetricIntegrationB200KeyframeStoreFrames"])
-            if self._store_frames > 0:
-                self.volume.set_frame_store(self._store_frames)
-            self._stored_slots = {}         # keyframe_store.keyframe_key -> slot of the keyframes stored here
+            self._init_frame_store()
             self.last_output = None
             self.last_integrated_id = -1
             self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call
@@ -345,35 +377,27 @@ def make_integrator_class(Base, api):
         def _integrate_sharded(self, frames, K4, fused):
             """The frames on every rank's shard: one fused batch when the unsharded plugin fuses them, else one call
             per frame.  Rank 0 uploads each batch once (raw uint16 depth stays 16-bit) and broadcasts it.  Every rank
-            stores the same frames in the same slots; rank 0's are recorded."""
+            stores the same frames in the same slots while every rank's store has room; rank 0's are recorded only
+            when every rank's store holds as many frames as rank 0's (a rank whose store stopped early never catches
+            up, so its slots can no longer be replayed)."""
             for part in ([frames] if fused else [[f] for f in frames]):
                 scale = part[0][3]
-                slots = self._shards.run(
+                self._shards.run(
                     "integrate", dict(K=K4, poses=np.stack([np.asarray(f[0].pose, np.float64) for f in part]),
                                       scale=scale),
                     dict(depths=np.ascontiguousarray(np.stack([f[2] for f in part]),
                                                      np.float32 if scale is None else np.uint16),
                          colors=np.ascontiguousarray(np.stack([f[1] for f in part]), np.uint8)))
-                self._record_stored([f[0] for f in part], slots)
+                if self._store_frames > 0 and self._shards.agreed() >= 0:
+                    self._record_stored([f[0] for f in part], self.volume.last_stored_slots())
 
         def _op_integrate(self, meta, depths, colors):
+            """Every rank's frames stored so far (-1 with the store off): rank 0 checks that they agree."""
             self.volume.integrate_batch(depths, colors, meta["K"], meta["poses"], depth_scale=meta["scale"])
-            return self.volume.last_stored_slots() if getattr(self, "_store_frames", 0) else None
+            return self.volume.frame_store_stats()[0] if getattr(self, "_store_frames", 0) else -1
 
         def _op_integrate_stored(self, meta):
             self.volume.integrate_stored(meta["slots"], meta["K"], meta["poses"])
-
-        def _record_stored(self, kds, slots):
-            """Note the store slots of keyframes just integrated (slots: last_stored_slots(), or None with the store
-            off) and publish them to the parent's table."""
-            if slots is None:
-                return
-            table = getattr(self, "_b200_keyframe_table", None)
-            for kd, slot in zip(kds, slots):
-                if slot >= 0:
-                    self._stored_slots[keyframe_store.keyframe_key(kd)] = int(slot)
-                    if table is not None:
-                        table.publish(int(slot), kd)
 
         def _integrate_images(self, tasks):
             """Today's path for tasks that carry their images; the keyframes integrated, in order."""
@@ -412,11 +436,8 @@ def make_integrator_class(Base, api):
             kds, slots = [], []
             for t in tasks:
                 kd = t.keyframe_data
-                slot = self._stored_slots.get(keyframe_store.keyframe_key(kd))
+                slot = self._stored_slot(kd)
                 if slot is None:
-                    getattr(Base, "print", print)(
-                        f"VolumetricIntegratorB200: ERROR: keyframe {kd.id} (timestamp {kd.timestamp}) came without "
-                        "images, but its frame is not in the frame store: it was not integrated")
                     continue
                 kds.append(kd)
                 slots.append(slot)

@@ -32,7 +32,7 @@ from types import SimpleNamespace
 
 import numpy as np
 
-from . import sharding
+from . import keyframe_store, sharding
 from .integrator import B200PluginSetup, raw_depth, write_ply_points
 from .volume import (CameraFrustrum, VoxelBlockGrid, VoxelBlockSemanticGrid, VoxelBlockSemanticProbabilisticGrid,
                      filter_shadow_points, remap_instance_ids)
@@ -82,6 +82,10 @@ DEFAULT_PARAMETERS = {
     # SAVE also writes the grid's state beside dense_map.ply (dense_map.state.npz), which LOAD restores; off by
     # default: the file is as large as the map (78 KiB per Bayesian block)
     "kVolumetricIntegrationB200SaveMapState": False,
+    # keep what set_frame staged for up to this many keyframes on the GPU, so that rebuild(map) sends only the
+    # keyframes' new poses to the integrator (keyframe_store.py); 0 = off.  16 bytes per pixel on the semantic grids
+    # (4.9 MB per 640x480 keyframe), 8 on the point-average grid (2.46 MB)
+    "kVolumetricIntegrationB200KeyframeStoreFrames": 0,
 }
 
 
@@ -113,11 +117,7 @@ def make_semantic_integrator_class(Base, api):
         _api = api
         _SHARD_KIND = "semantic"
         _LABELS = True     # the grid takes class and instance images
-
-        def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type,
-                     viewer_queue=None, **kwargs):
-            super().__init__(camera, environment_type, sensor_type, volumetric_integrator_type,
-                             viewer_queue, **kwargs)
+        _STORE_LABELS = True
 
         # -- runs inside the integrator process: the CUDA context is created here, never in the parent
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
@@ -144,6 +144,7 @@ def make_semantic_integrator_class(Base, api):
             self.last_integrated_id = -1
             self.last_instance_map = {}
             self._init_gpu_rectify()
+            self._init_frame_store()
 
         def _after_load(self):
             """The restored grid has no association yet, and until the next keyframe the output represents it as
@@ -188,13 +189,22 @@ def make_semantic_integrator_class(Base, api):
 
         def _integrate_raw(self, kd, depth, scale, use_instances):
             """The loop body on the raw images: one set_frame uploads, rectifies and shadow-filters them on the
-            device; association (or carving), the instance remap and the integration read the staged images."""
+            device (and stores them, with the frame store on); the rest reads the staged images (_integrate_staged)."""
+            flt = bool(self.b200_parameters["kVolumetricIntegrationVoxelGridShadowPointsFilter"])
+            fr = self.volume.set_frame(depth, kd.img, class_image=kd.semantic_img,
+                                       instance_image=kd.semantic_instances_img if use_instances else None,
+                                       depth_scale=scale, filter_shadow_points=flt)
+            return self._integrate_staged(kd, fr, use_instances)
+
+        def _integrate_stored(self, kd, slot):
+            """The loop body on a stored frame (a light task): staged again from the frame store, then as on the
+            images it was stored from; its instance image is associated when it was staged."""
+            fr = self.volume.stage_stored(slot)
+            return self._integrate_staged(kd, fr, fr.instance_image is not None)
+
+        def _integrate_staged(self, kd, fr, use_instances):
+            """Association (or carving), the instance remap and the integration on the staged frame `fr`."""
             p = self.b200_parameters
-            flt = bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"])
-            classes, instances = kd.semantic_img, kd.semantic_instances_img
-            fr = self.volume.set_frame(depth, kd.img, class_image=classes,
-                                       instance_image=instances if use_instances else None, depth_scale=scale,
-                                       filter_shadow_points=flt)
             self.integrated_instance_ids = False
             self.camera_frustrum.set_T_cw(kd.pose)
             carve_thr = float(p["kVolumetricIntegrationVoxelGridCarvingDepthThreshold"])
@@ -219,20 +229,43 @@ def make_semantic_integrator_class(Base, api):
             return True
 
         def _integrate_keyframe(self, kd):
-            """The reference loop body for one keyframe (:300-461): on the raw images, or on the ones the base class
-            prepared on the host; on every rank's shard of a sharded grid."""
-            raw = self._raw_frame(kd)
+            """The reference loop body for one keyframe (:300-461): on the raw images, on the ones the base class
+            prepared on the host, or, for a light task, on its stored frame; on every rank's shard of a sharded grid.
+            With the frame store on, host-prepared frames of the frustum's size are staged like raw ones (no maps are
+            installed then, so set_frame only uploads and filters them) and stored."""
+            if getattr(kd, keyframe_store.STORED_FLAG, False):
+                slot = self._stored_slot(kd)
+                if slot is None:
+                    return False
+                if self._shards is not None:
+                    self._shards.run("frame_stored", dict(id=kd.id, pose=np.asarray(kd.pose, np.float64), slot=slot))
+                    return True
+                return self._integrate_stored(kd, slot)
+            src, raw, prepared = kd, self._raw_frame(kd), None
+            if raw is None:
+                rect = self.estimate_depth_if_needed_and_rectify(kd)
+                color, depth = rect[0], rect[1]
+                if color is None or depth is None:
+                    return False
+                kd = SimpleNamespace(id=kd.id, pose=kd.pose, img=color, depth=depth,
+                                     semantic_img=rect[3] if len(rect) > 3 else None,
+                                     semantic_instances_img=rect[4] if len(rect) > 4 else None)
+                if (self._store_frames > 0 and not self._gpu_rectify
+                        and np.shape(depth) == (self.camera_frustrum.height, self.camera_frustrum.width)):
+                    raw = (np.ascontiguousarray(depth, np.float32), None)
+                else:
+                    prepared = kd
             if self._shards is not None:
-                return self._integrate_keyframe_sharded(kd, raw)
-            if raw is not None:
-                return self._integrate_raw(kd, *raw, self._uses_instances(kd.semantic_img, kd.semantic_instances_img))
-            rect = self.estimate_depth_if_needed_and_rectify(kd)
-            color, depth = rect[0], rect[1]
-            classes = rect[3] if len(rect) > 3 else None
-            instances = rect[4] if len(rect) > 4 else None
-            if color is None or depth is None:
-                return False
-            return self._integrate_prepared(kd, color, depth, classes, instances)
+                slot = self._integrate_keyframe_sharded(kd, raw)
+            elif raw is not None:
+                self._integrate_raw(kd, *raw, self._uses_instances(kd.semantic_img, kd.semantic_instances_img))
+                slot = self.volume.last_stored_slot() if self._store_frames > 0 else -1
+            else:
+                self._integrate_prepared(prepared, prepared.img, prepared.depth, prepared.semantic_img,
+                                         prepared.semantic_instances_img)
+                slot = -1
+            self._record_stored([src], [slot])
+            return True
 
         def _labels(self, classes, instances, use_instances, raw):
             """The label images of a broadcast keyframe: none for the point-average grid; int32 (what set_frame
@@ -247,8 +280,10 @@ def make_semantic_integrator_class(Base, api):
             return out
 
         def _integrate_keyframe_sharded(self, kd, raw):
-            """Rank 0's part of INTEGRATE: broadcast the keyframe (raw images, or the host-prepared ones when the
-            frame takes the host path); every rank then runs the loop body on its shard (`_op_frame`)."""
+            """Rank 0's part of INTEGRATE: broadcast the keyframe (the images for set_frame when `raw`, else the
+            host-prepared ones); every rank then runs the loop body on its shard (`_op_frame`).  Returns the slot
+            every rank stored the frame in, or -1: a rank whose store stopped (each rank maps its own) stored it in
+            none, and a frame not in every rank's store cannot be replayed (`_op_frame_stored`)."""
             meta = dict(id=kd.id, pose=np.asarray(kd.pose, np.float64), raw=raw is not None)
             if raw is not None:
                 depth, scale = raw
@@ -257,22 +292,24 @@ def make_semantic_integrator_class(Base, api):
                 arrays = dict(depth=depth, img=kd.img,
                               **self._labels(kd.semantic_img, kd.semantic_instances_img, use, True))
             else:
-                rect = self.estimate_depth_if_needed_and_rectify(kd)
-                color, depth = rect[0], rect[1]
-                if color is None or depth is None:
-                    return False
-                arrays = dict(depth=depth, img=color, **self._labels(rect[3] if len(rect) > 3 else None,
-                                                                     rect[4] if len(rect) > 4 else None, False, False))
+                arrays = dict(depth=kd.depth, img=kd.img,
+                              **self._labels(kd.semantic_img, kd.semantic_instances_img, False, False))
             self._shards.run("frame", meta, arrays)
-            return True
+            return self._shards.agreed()
 
         def _op_frame(self, meta, depth, img, classes=None, instances=None):
             kd = SimpleNamespace(id=meta["id"], pose=meta["pose"], img=img, semantic_img=classes,
                                  semantic_instances_img=instances)
             if meta["raw"]:
-                return self._integrate_raw(kd, depth, meta["scale"], meta["use_instances"])
+                self._integrate_raw(kd, depth, meta["scale"], meta["use_instances"])
+                return self.volume.last_stored_slot() if self._store_frames > 0 else -1
             host = [x.cpu().numpy() if hasattr(x, "cpu") else x for x in (img, depth, classes, instances)]
-            return self._integrate_prepared(kd, *host)
+            self._integrate_prepared(kd, *host)
+            return -1
+
+        def _op_frame_stored(self, meta):
+            """A light task on every rank: the stored frame of slot meta["slot"] with pose meta["pose"]."""
+            self._integrate_stored(SimpleNamespace(id=meta["id"], pose=meta["pose"]), int(meta["slot"]))
 
         def _integrate_prepared(self, kd, color, depth, classes, instances):
             """The loop body on images the base class prepared on the host."""
@@ -421,16 +458,20 @@ def make_voxel_grid_integrator_class(Base, api):
         _defaults = dict(DEFAULT_PARAMETERS, kVolumetricIntegrationB200CapacityBlocks=1 << 17)
         _SHARD_KIND = "voxel_grid"
         _LABELS = False
+        _STORE_LABELS = False   # the point-average grid neither stores nor reads label images
 
         def _make_grid(self, p, side, constructor_kwargs):
             return VoxelBlockGrid(**dict(_grid_args(p, self.b200_set_parameters), **self._map_placement()),
                                   input_order_sums=bool(p["kVolumetricIntegrationB200InputOrderSums"]))
 
         def _integrate_raw(self, kd, depth, scale, use_instances):
-            """Staged raw images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
+            fr = self.volume.set_frame(depth, kd.img, depth_scale=scale, filter_shadow_points=bool(
+                self.b200_parameters["kVolumetricIntegrationVoxelGridShadowPointsFilter"]))
+            return self._integrate_staged(kd, fr, False)
+
+        def _integrate_staged(self, kd, fr, use_instances):
+            """Staged images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
             p = self.b200_parameters
-            fr = self.volume.set_frame(depth, kd.img, depth_scale=scale,
-                                       filter_shadow_points=bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"]))
             if p["kVolumetricIntegrationVoxelGridUseCarving"]:
                 self.camera_frustrum.set_T_cw(kd.pose)
                 self.volume.carve(self.camera_frustrum, fr.depth,

@@ -120,14 +120,20 @@ class ShardSide:
             dist.broadcast(flat, 0)
         return self._view(flat, tuple(shape), dtype)
 
-    def finish(self, err):
-        """The status all-reduce that ends every op; the first failing rank's message (None when all succeeded)."""
+    def finish(self, err, result=None):
+        """The status all-reduce that ends every op; the first failing rank's message (None when all succeeded).
+        It also gathers every rank's op result when that is an int (else -1) into `words`, rank by rank: a value each
+        rank computes for itself, such as the frame-store slot it filled, which rank 0 can check all ranks agree on."""
         import torch
         import torch.distributed as dist
-        flags = torch.zeros(self.world, dtype=torch.int32, device=self._torch_device)
+        flags = torch.zeros(2 * self.world, dtype=torch.int64, device=self._torch_device)
         flags[self.rank] = 1 if err else 0
+        word = result if isinstance(result, (int, np.integer)) and not isinstance(result, bool) else -1
+        flags[self.world + self.rank] = int(word)
         dist.all_reduce(flags)
-        failed = [r for r, f in enumerate(flags.cpu().tolist()) if f]
+        flags = flags.cpu().tolist()
+        self.words = flags[self.world:]
+        failed = [r for r, f in enumerate(flags[:self.world]) if f]
         if not failed:
             return None
         msg = [err if self.rank == failed[0] else None]
@@ -184,14 +190,20 @@ class ShardGroup(ShardSide):
             if p.poll() is not None:
                 raise RuntimeError(f"shard worker {r} exited with status {p.returncode}")
 
+    def agreed(self):
+        """The int result every rank returned from the last op, or -1 when the ranks' results differ."""
+        w = self.words
+        return w[0] if all(x == w[0] for x in w) else -1
+
     def _fail(self, msg):
         self._broken = msg
         self.close()
         raise RuntimeError(f"the shard group is down: {msg}")
 
     def run(self, op: str, meta: dict | None = None, arrays: dict | None = None):
-        """One op on every rank; rank 0's result.  RuntimeError when a rank failed (the group stays up) or the group
-        failed (it is then shut down and every later op raises)."""
+        """One op on every rank; rank 0's result (every rank's int result in `words`, see `finish`).  RuntimeError
+        when a rank failed (the group stays up) or the group failed (it is then shut down and every later op
+        raises)."""
         if self._closed:
             raise RuntimeError(f"the shard group is down: {self._broken or 'stopped'}")
         meta, arrays = meta or {}, arrays or {}
@@ -209,7 +221,7 @@ class ShardGroup(ShardSide):
             self._fail(f"{op}: {e}")
         result, err = _execute(self.plugin, op, meta, local, 0)
         try:
-            msg = self.finish(err)
+            msg = self.finish(err, result)
             if self._seq > 1:   # every worker has read the previous header
                 self.store.delete_key(f"{_OP_KEY}{self._seq - 1}")
         except Exception as e:
@@ -297,8 +309,8 @@ def serve(side: ShardSide):
             if plugin is None:
                 side.finish(f"rank {side.rank}: {op} before setup")
                 continue
-            _, err = _execute(plugin, op, meta, arrays, side.rank)
-            side.finish(err)
+            result, err = _execute(plugin, op, meta, arrays, side.rank)
+            side.finish(err, result)
     finally:
         if plugin is not None and getattr(plugin, "volume", None) is not None:
             plugin.volume.close()

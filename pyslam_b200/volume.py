@@ -1031,6 +1031,46 @@ class _BlockGrid(_MapState):
         self._frame = GridFrame(self, f)
         return self._frame
 
+    # ---- frame store (rebuild(map) from keyframes on the GPU) ----
+    def set_frame_store(self, max_frames: int):
+        """Keep what `set_frame` staged for up to `max_frames` frames on the GPU, so that `stage_stored` can stage them
+        again without their images: 8 bytes per pixel on the point-average grid (2.46 MB per 640x480 frame), 16 on the
+        semantic grids (4.9 MB).  0 turns the store off (the default).  Frames are stored in call order while there is
+        room, at the size of the first stored frame; nothing is evicted.  clear() and load_state() keep the store.
+        Empties the store and synchronises."""
+        self._check(self._c("set_frame_store")(self._h, int(max_frames)), self._P + "set_frame_store")
+
+    def clear_frame_store(self):
+        """Empty the frame store and release its memory; synchronises."""
+        self._check(self._c("frame_store_clear")(self._h), self._P + "frame_store_clear")
+
+    def last_stored_slot(self) -> int:
+        """The store slot of the most recent `set_frame`'s frame, or -1 (store off or full, another frame size, or a
+        failing call)."""
+        s = C.c_int32(-1)
+        self._check(self._c("frame_store_last")(self._h, C.byref(s)), self._P + "frame_store_last")
+        return int(s.value)
+
+    def frame_store_stats(self):
+        """(frames the store holds, device bytes it has mapped for them)."""
+        n, b = C.c_int64(0), C.c_int64(0)
+        self._check(self._c("frame_store_stats")(self._h, C.byref(n), C.byref(b)), self._P + "frame_store_stats")
+        return int(n.value), int(b.value)
+
+    def stage_stored(self, slot: int) -> GridFrame:
+        """Stage stored frame `slot` again (from `last_stored_slot`): the `GridFrame` the frame's `set_frame` returned,
+        its images bit for bit the same, so carving, the association, `remap_instance_ids` and `integrate_rgbd` give
+        the same map.  Like `set_frame`, earlier staged images go stale; a slot the store does not hold raises and
+        leaves the staged frame as it was."""
+        f = _lib.B2VFrame()
+        rc = self._c("stage_stored")(self._h, int(slot), C.byref(f))
+        if rc != _lib.B2V_ERR_INVALID_ARGUMENT:
+            self._frame_gen += 1
+            self._frame = None
+        self._check(rc, self._P + "stage_stored")
+        self._frame = GridFrame(self, f)
+        return self._frame
+
     def carve(self, camera_frustrum, depth_image, depth_threshold: float = 1e-2):
         """carve(camera_frustrum, depth_image, depth_threshold) (voxel_block_grid.hpp:616-622): reset voxels
         in the frustum that lie in front of the observed depth by more than the threshold.  Like the
