@@ -111,6 +111,8 @@ class B200PluginSetup:
 
     # the stored-keyframe table publishes each slot's label images (keyframe_store.label_flags)
     _STORE_LABELS = False
+    # a non-INTEGRATE task met while draining a backlog: handled by the next volume_integration call
+    _deferred_task, _has_deferred = None, False
 
     def __init__(self, camera, environment_type, sensor_type, volumetric_integrator_type, viewer_queue=None,
                  **kwargs):
@@ -147,10 +149,8 @@ class B200PluginSetup:
         self._stored_slots = {}         # keyframe_store.keyframe_key -> slot of the keyframes stored here
 
     def _record_stored(self, kds, slots):
-        """Note the store slots of keyframes just integrated (slots: the map's last stored slots, or None with the
-        store off) and publish them to the parent's table."""
-        if slots is None:
-            return
+        """Note the store slots of keyframes just integrated (-1: not stored) and publish them to the parent's
+        table."""
         table = getattr(self, "_b200_keyframe_table", None)
         for kd, slot in zip(kds, slots):
             if slot >= 0:
@@ -178,6 +178,14 @@ class B200PluginSetup:
         # the keys the caller set (the rest hold the plugin's defaults)
         self.b200_set_parameters = {k for k in defaults if k in (parameters_dict or {}) or k in (constructor_kwargs or {})}
         return p
+
+    def _environment_side(self, environment_type):
+        """"Indoor" or "Outdoor", the suffix of the parameters that depend on the environment: indoor unless pySLAM's
+        DatasetEnvironmentType says otherwise."""
+        env_t = getattr(self._api, "DatasetEnvironmentType", None)
+        if env_t is not None and hasattr(env_t, "INDOOR") and environment_type != env_t.INDOOR:
+            return "Outdoor"
+        return "Indoor"
 
     def _init_gpu_rectify(self):
         """Raw frames go to the device when the base class computed undistortion maps (base.py:766-778) and no depth
@@ -241,6 +249,13 @@ class B200PluginSetup:
             return getattr(self, "_op_" + op)(meta or {}, **arrays)
         return self._shards.run(op, meta, arrays)
 
+    def _agreed(self, result):
+        """The int `result` of the last `_map_call` when every rank computed the same (each computes its own, such as
+        the frame-store slot it filled), else -1 (ShardGroup.agreed); on one map, `result`."""
+        if getattr(self, "_shards", None) is None:
+            return result
+        return self._shards.agreed()
+
     def _op_reset(self, meta):
         self.volume.reset()
 
@@ -250,10 +265,6 @@ class B200PluginSetup:
     def _op_load_state(self, meta):
         self.volume.load_state(meta["paths"])
         self._after_load()
-
-    def _stop_shards(self):
-        if getattr(self, "_shards", None) is not None:
-            self._shards.close()
 
     def load(self, path):
         """The LOAD task of the map saved in directory `path`, the mirror of the base class's `save(path)`: it reads
@@ -298,14 +309,99 @@ class B200PluginSetup:
         c = self.camera
         return c.fx, c.fy, c.cx, c.cy
 
+    def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
+                           is_running, load_request_completed, load_request_condition,
+                           save_request_completed, save_request_condition,
+                           time_volumetric_integration):
+        """One task of the integrator process (base.py:905-915): RESET from the management queue first, then the next
+        task.  The plugin class provides `_integrate_tasks` (INTEGRATE), `_write_ply` (SAVE) and `_make_output`."""
+        api = self._api
+        TaskType = api.VolumetricIntegrationTaskType
+        t_start = time.perf_counter()
+        last_output = None
+        do_output = False
+        try:
+            if is_running.value == 1:
+                # management queue first: RESET
+                task = None
+                try:
+                    task = q_management.get_nowait()
+                except Exception:
+                    pass
+                if task is not None and task.task_type == TaskType.RESET:
+                    self._map_call("reset")
+                if self._has_deferred:
+                    self.last_input_task, self._deferred_task, self._has_deferred = self._deferred_task, None, False
+                else:
+                    self.last_input_task = q_in.get()  # blocking
+                if self.last_input_task is None:
+                    is_running.value = 0  # a None asks the loop to exit
+                else:
+                    ttype = self.last_input_task.task_type
+                    if ttype == TaskType.INTEGRATE:
+                        # backlog (rebuild(map), base.py:1242-1318): drain the consecutive INTEGRATE tasks that are
+                        # already queued, up to kVolumetricIntegrationB200MaxBatch (the grid plugins have no such
+                        # parameter and take one per call); anything else waits for the next call
+                        tasks = [self.last_input_task]
+                        max_batch = int(self.b200_parameters.get("kVolumetricIntegrationB200MaxBatch", 1))
+                        while len(tasks) < max_batch:
+                            try:
+                                nxt = q_in.get_nowait()
+                            except Exception:
+                                break
+                            if nxt is None or nxt.task_type != TaskType.INTEGRATE:
+                                self._deferred_task, self._has_deferred = nxt, True
+                                break
+                            tasks.append(nxt)
+                        self.last_input_task = tasks[-1]
+                        done = self._integrate_tasks(tasks)
+                        if done:
+                            self.last_integrated_id = done[-1].id
+                            self.integrated_frames = getattr(self, "integrated_frames", 0) + len(done)
+                            do_output = True
+                            if self.last_output is not None:
+                                dt = time.perf_counter() - self.last_output.timestamp
+                                if dt < self.b200_parameters["kVolumetricIntegrationOutputTimeInterval"]:
+                                    do_output = False
+                    elif ttype == TaskType.SAVE:
+                        self._write_ply(self.last_input_task.load_save_path)
+                        self._save_map_state(self.last_input_task.load_save_path)
+                        last_output = api.VolumetricIntegrationOutput(ttype)
+                    elif ttype == TaskType.LOAD:
+                        self._load_map_state(self.last_input_task, load_request_completed, load_request_condition)
+                    elif ttype == TaskType.UPDATE_OUTPUT:
+                        do_output = True
+                    if do_output:
+                        last_output = self._make_output(ttype)
+                        self.last_output = last_output
+                    if is_running.value == 1 and last_output is not None:
+                        if last_output.task_type in (TaskType.INTEGRATE, TaskType.UPDATE_OUTPUT):
+                            with q_out_condition:
+                                last_output.timestamp = time.perf_counter()
+                                q_out.put(last_output)
+                                q_out_condition.notify_all()
+                        elif last_output.task_type == TaskType.SAVE:
+                            with save_request_condition:
+                                save_request_completed.value = 1
+                                save_request_condition.notify_all()
+        except Exception as e:  # the reference logs and keeps the loop alive (tsdf.py:303-307)
+            printer = getattr(type(self), "print", print)
+            printer(f"{type(self).__name__}: EXCEPTION: {e} !!!")
+            printer(traceback.format_exc())
+        time_volumetric_integration.value = time.perf_counter() - t_start
+
+    def _stop_volume_integrator_implementation(self):
+        if getattr(self, "_shards", None) is not None:
+            self._shards.close()
+        if getattr(self, "volume", None) is not None:
+            self.volume.close()
+
 
 def make_integrator_class(Base, api):
     """Build the plugin class against a base class and an `api` namespace providing
     `VolumetricIntegrationTaskType`, `VolumetricIntegrationOutput`, `VolumetricIntegrationMesh`,
     `VolumetricIntegrationPointCloud`, `DatasetEnvironmentType` (or None) and `Parameters` (or None); optionally
     `VolumetricIntegrationTask`, the task type `load` enqueues (else a namespace with the task's fields)."""
-
-    TaskType = api.VolumetricIntegrationTaskType
 
     class VolumetricIntegratorB200(B200PluginSetup, Base):
         """TSDF + colour integration on an H100 (replaces VolumetricIntegratorTsdf + Open3D)."""
@@ -318,13 +414,8 @@ def make_integrator_class(Base, api):
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
             Base.init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs)
             p = self._merge_parameters(DEFAULT_PARAMETERS, parameters_dict, constructor_kwargs)
-            outdoor = False
-            env_t = getattr(api, "DatasetEnvironmentType", None)
-            if env_t is not None and hasattr(env_t, "INDOOR"):
-                outdoor = environment_type != env_t.INDOOR
-            self.volumetric_integration_depth_trunc = (
-                p["kVolumetricIntegrationTsdfDepthTruncOutdoor"] if outdoor
-                else p["kVolumetricIntegrationTsdfDepthTruncIndoor"])
+            self.volumetric_integration_depth_trunc = p[
+                f"kVolumetricIntegrationTsdfDepthTrunc{self._environment_side(environment_type)}"]
             self._start_map()
 
         def _build_map(self):
@@ -340,8 +431,6 @@ def make_integrator_class(Base, api):
             self._init_frame_store()
             self.last_output = None
             self.last_integrated_id = -1
-            self._deferred_task = None      # a non-INTEGRATE task met while draining a backlog: handled next call
-            self._has_deferred = False
             self._init_gpu_rectify()
 
         def _prepare_frame(self, kd):
@@ -374,33 +463,31 @@ def make_integrator_class(Base, api):
                 return self.volume.extract_point_cloud()
             return sharding.extract_point_cloud_sharded(self.volume)
 
-        def _integrate_sharded(self, frames, K4, fused):
-            """The frames on every rank's shard: one fused batch when the unsharded plugin fuses them, else one call
-            per frame.  Rank 0 uploads each batch once (raw uint16 depth stays 16-bit) and broadcasts it.  Every rank
-            stores the same frames in the same slots while every rank's store has room; rank 0's are recorded only
-            when every rank's store holds as many frames as rank 0's (a rank whose store stopped early never catches
-            up, so its slots can no longer be replayed)."""
-            for part in ([frames] if fused else [[f] for f in frames]):
-                scale = part[0][3]
-                self._shards.run(
-                    "integrate", dict(K=K4, poses=np.stack([np.asarray(f[0].pose, np.float64) for f in part]),
-                                      scale=scale),
-                    dict(depths=np.ascontiguousarray(np.stack([f[2] for f in part]),
-                                                     np.float32 if scale is None else np.uint16),
-                         colors=np.ascontiguousarray(np.stack([f[1] for f in part]), np.uint8)))
-                if self._store_frames > 0 and self._shards.agreed() >= 0:
-                    self._record_stored([f[0] for f in part], self.volume.last_stored_slots())
-
         def _op_integrate(self, meta, depths, colors):
-            """Every rank's frames stored so far (-1 with the store off): rank 0 checks that they agree."""
+            """The last store slot the call filled (-1: none, or the store is off): rank 0 records the call's slots only
+            when every rank filled the same.  Slots are filled in call order, so a rank's store holds that slot + 1
+            frames, and a rank whose store stopped early (each rank maps its own) never agrees again."""
             self.volume.integrate_batch(depths, colors, meta["K"], meta["poses"], depth_scale=meta["scale"])
-            return self.volume.frame_store_stats()[0] if getattr(self, "_store_frames", 0) else -1
+            return int(self.volume.last_stored_slots().max()) if getattr(self, "_store_frames", 0) else -1
 
         def _op_integrate_stored(self, meta):
             self.volume.integrate_stored(meta["slots"], meta["K"], meta["poses"])
 
+        def _integrate_tasks(self, tasks):
+            """Light tasks (keyframe_store) and image-carrying ones may alternate in a drained backlog: their runs in
+            order; the keyframes integrated, in order."""
+            done = []
+            for stored, run in keyframe_store.split_runs(tasks):
+                done += self._integrate_stored(run) if stored else self._integrate_images(run)
+            return done
+
         def _integrate_images(self, tasks):
-            """Today's path for tasks that carry their images; the keyframes integrated, in order."""
+            """Tasks that carry their images: one fused integrate_batch when there are several frames of one shape,
+            dtype and depth scale, else one integrate_batch per frame.  On a sharded map rank 0 uploads each batch
+            once (raw uint16 depth stays 16-bit) and broadcasts it.  Every rank stores the same frames in the same
+            slots while every rank's store has room; rank 0's are recorded only when every rank's store holds as many
+            frames as rank 0's (a rank whose store stopped early never catches up, so its slots can no longer be
+            replayed).  The keyframes integrated, in order."""
             frames = []
             for t in tasks:
                 kd = t.keyframe_data
@@ -414,20 +501,19 @@ def make_integrator_class(Base, api):
                        and f[2].dtype == frames[0][2].dtype and f[3] == frames[0][3]
                        for f in frames)
             store = getattr(self, "_store_frames", 0) > 0
-            if self._shards is not None:
-                self._integrate_sharded(frames, K4, len(frames) > 1 and same)
-            elif len(frames) > 1 and same:
-                # one C call: groups of frames fused per block visit (b2v_integrate_batch)
-                self.volume.integrate_batch(np.stack([f[2] for f in frames]),
-                                            np.stack([f[1] for f in frames]), K4,
-                                            np.stack([np.asarray(f[0].pose, np.float64) for f in frames]),
-                                            depth_scale=frames[0][3])
-                self._record_stored([f[0] for f in frames], self.volume.last_stored_slots() if store else None)
-            else:
-                for kd, color, depth, scale in frames:
-                    # north_star call: integrate(depth, color, K, pose = Tcw)
-                    self.volume.integrate(depth, color, K4, kd.pose, depth_scale=scale)
-                    self._record_stored([kd], self.volume.last_stored_slots() if store else None)
+            # one C call per part: groups of frames fused per block visit (b2v_integrate_batch); a lone frame is a
+            # one-frame batch of views, not a copy
+            for part in ([frames] if len(frames) > 1 and same else [[f] for f in frames]):
+                scale = part[0][3]
+                depths = np.stack([f[2] for f in part]) if len(part) > 1 else part[0][2][None]
+                colors = np.stack([f[1] for f in part]) if len(part) > 1 else part[0][1][None]
+                n = self._map_call(
+                    "integrate", dict(K=K4, poses=np.stack([np.asarray(f[0].pose, np.float64) for f in part]),
+                                      scale=scale),
+                    depths=np.ascontiguousarray(depths, np.float32 if scale is None else np.uint16),
+                    colors=np.ascontiguousarray(colors, np.uint8))
+                if store and self._agreed(n) >= 0:
+                    self._record_stored([f[0] for f in part], self.volume.last_stored_slots())
             return [f[0] for f in frames]
 
         def _integrate_stored(self, tasks):
@@ -446,114 +532,30 @@ def make_integrator_class(Base, api):
             K4 = tuple(self._intrinsics())
             slots = np.asarray(slots, np.int32)
             poses = np.stack([np.asarray(kd.pose, np.float64) for kd in kds])
-            if self._shards is not None:
-                self._shards.run("integrate_stored", dict(K=K4, poses=poses, slots=slots))
-            else:
-                self.volume.integrate_stored(slots, K4, poses)
+            self._map_call("integrate_stored", dict(K=K4, poses=poses, slots=slots))
             return kds
 
-        def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
-                               is_running, load_request_completed, load_request_condition,
-                               save_request_completed, save_request_condition,
-                               time_volumetric_integration):
-            t_start = time.perf_counter()
-            last_output = None
-            do_output = False
-            try:
-                if is_running.value == 1:
-                    # management queue first: RESET
-                    task = None
-                    try:
-                        task = q_management.get_nowait()
-                    except Exception:
-                        pass
-                    if task is not None and task.task_type == TaskType.RESET:
-                        self._map_call("reset")
-                    if self._has_deferred:
-                        self.last_input_task, self._deferred_task, self._has_deferred = self._deferred_task, None, False
-                    else:
-                        self.last_input_task = q_in.get()  # blocking
-                    if self.last_input_task is None:
-                        is_running.value = 0  # a None asks the loop to exit
-                    else:
-                        ttype = self.last_input_task.task_type
-                        if ttype == TaskType.INTEGRATE:
-                            # backlog (rebuild(map), base.py:1242-1318): drain the consecutive INTEGRATE tasks that
-                            # are already queued into one fused batch; anything else waits for the next call
-                            tasks = [self.last_input_task]
-                            max_batch = int(self.b200_parameters["kVolumetricIntegrationB200MaxBatch"])
-                            while len(tasks) < max_batch:
-                                try:
-                                    nxt = q_in.get_nowait()
-                                except Exception:
-                                    break
-                                if nxt is None or nxt.task_type != TaskType.INTEGRATE:
-                                    self._deferred_task, self._has_deferred = nxt, True
-                                    break
-                                tasks.append(nxt)
-                            self.last_input_task = tasks[-1]
-                            # light tasks (keyframe_store) and image-carrying ones may alternate: runs in order
-                            done = []
-                            for stored, run in keyframe_store.split_runs(tasks):
-                                done += self._integrate_stored(run) if stored else self._integrate_images(run)
-                            if done:
-                                self.last_integrated_id = done[-1].id
-                                self.integrated_frames = getattr(self, "integrated_frames", 0) + len(done)
-                                do_output = True
-                                if self.last_output is not None:
-                                    dt = time.perf_counter() - self.last_output.timestamp
-                                    if dt < self.b200_parameters["kVolumetricIntegrationOutputTimeInterval"]:
-                                        do_output = False
-                        elif ttype == TaskType.SAVE:
-                            path = self.last_input_task.load_save_path
-                            if self.b200_parameters["kVolumetricIntegrationTsdfExtractMesh"]:
-                                m = self._map_call("mesh")
-                                write_ply_mesh(path, m.vertices, m.triangles, m.vertex_colors)
-                            else:
-                                pc = self._map_call("points")
-                                write_ply_points(path, pc.points, pc.colors)
-                            self._save_map_state(path)
-                            last_output = api.VolumetricIntegrationOutput(ttype)
-                        elif ttype == TaskType.LOAD:
-                            self._load_map_state(self.last_input_task, load_request_completed, load_request_condition)
-                        elif ttype == TaskType.UPDATE_OUTPUT:
-                            do_output = True
-                        if do_output:
-                            last_output = self._make_output(ttype)
-                            self.last_output = last_output
-                        if is_running.value == 1 and last_output is not None:
-                            if last_output.task_type in (TaskType.INTEGRATE, TaskType.UPDATE_OUTPUT):
-                                with q_out_condition:
-                                    last_output.timestamp = time.perf_counter()
-                                    q_out.put(last_output)
-                                    q_out_condition.notify_all()
-                            elif last_output.task_type == TaskType.SAVE:
-                                with save_request_condition:
-                                    save_request_completed.value = 1
-                                    save_request_condition.notify_all()
-            except Exception as e:  # the reference logs and keeps the loop alive (tsdf.py:303-307)
-                printer = getattr(Base, "print", print)
-                printer(f"VolumetricIntegratorB200: EXCEPTION: {e} !!!")
-                printer(traceback.format_exc())
-            time_volumetric_integration.value = time.perf_counter() - t_start
-
-        def _stop_volume_integrator_implementation(self):
-            self._stop_shards()
-            if getattr(self, "volume", None) is not None:
-                self.volume.close()
+        def _write_ply(self, path):
+            """SAVE's dense_map.ply: the mesh, or the point cloud (kVolumetricIntegrationTsdfExtractMesh)."""
+            if self.b200_parameters["kVolumetricIntegrationTsdfExtractMesh"]:
+                m = self._map_call("mesh")
+                write_ply_mesh(path, m.vertices, m.triangles, m.vertex_colors)
+            else:
+                pc = self._map_call("points")
+                write_ply_points(path, pc.points, pc.colors)
 
     return VolumetricIntegratorB200
 
 
-def load_pyslam_plugin():
-    """Build the plugin against the real pySLAM types (requires pySLAM on sys.path).
-    INTEGRATION.md shows the three-line registration in the reference's factory / enum."""
+def pyslam_api():
+    """pySLAM's dense-integration module and the `api` namespace of its types that the plugin classes are built
+    against (requires pySLAM on sys.path)."""
     from pyslam.config_parameters import Parameters
     from pyslam.dense import volumetric_integrator_base as B
     from pyslam.io.dataset_types import DatasetEnvironmentType
     from pyslam.slam import USE_CPP   # C++ core: raw depth reaches the integrator unscaled (base.py:29, 1008-1012)
 
-    api = SimpleNamespace(
+    return B, SimpleNamespace(
         USE_CPP=bool(USE_CPP),
         VolumetricIntegrationTaskType=B.VolumetricIntegrationTaskType,
         VolumetricIntegrationTask=B.VolumetricIntegrationTask,
@@ -561,4 +563,10 @@ def load_pyslam_plugin():
         VolumetricIntegrationMesh=B.VolumetricIntegrationMesh,
         VolumetricIntegrationPointCloud=B.VolumetricIntegrationPointCloud,
         DatasetEnvironmentType=DatasetEnvironmentType, Parameters=Parameters)
+
+
+def load_pyslam_plugin():
+    """Build the plugin against the real pySLAM types (requires pySLAM on sys.path).
+    INTEGRATION.md shows the three-line registration in the reference's factory / enum."""
+    B, api = pyslam_api()
     return make_integrator_class(B.VolumetricIntegratorBase, api)

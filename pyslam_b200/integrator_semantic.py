@@ -25,15 +25,12 @@ class ids, object ids.
 
 from __future__ import annotations
 
-import time
-import traceback
-
 from types import SimpleNamespace
 
 import numpy as np
 
 from . import keyframe_store, sharding
-from .integrator import B200PluginSetup, raw_depth, write_ply_points
+from .integrator import B200PluginSetup, pyslam_api, raw_depth, write_ply_points
 from .volume import (CameraFrustrum, VoxelBlockGrid, VoxelBlockSemanticGrid, VoxelBlockSemanticProbabilisticGrid,
                      filter_shadow_points, remap_instance_ids)
 
@@ -108,7 +105,6 @@ def _grid_args(p, set_keys=()):
 
 def make_semantic_integrator_class(Base, api):
     """Build the semantic plugin class against a base class and an `api` namespace (see `integrator.py`)."""
-    TaskType = api.VolumetricIntegrationTaskType
 
     class VolumetricIntegratorB200SemanticGrid(B200PluginSetup, Base):
         """GPU semantic voxel-grid integrator; `use_semantic_probabilistic` selects Bayesian fusion (:131-141)."""
@@ -123,11 +119,7 @@ def make_semantic_integrator_class(Base, api):
         def init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs):
             Base.init(self, camera, environment_type, sensor_type, parameters_dict, constructor_kwargs)
             p = self._merge_parameters(self._defaults, parameters_dict, constructor_kwargs)
-            indoor = True
-            env_t = getattr(api, "DatasetEnvironmentType", None)
-            if env_t is not None and hasattr(env_t, "INDOOR"):
-                indoor = environment_type == env_t.INDOOR
-            self._side = "Indoor" if indoor else "Outdoor"
+            self._side = self._environment_side(environment_type)
             self._probabilistic = bool((constructor_kwargs or {}).get("use_semantic_probabilistic", False))
             self.volumetric_integration_depth_trunc = p[f"kVolumetricIntegrationTsdfDepthTrunc{self._side}"]
             self._start_map()
@@ -194,13 +186,13 @@ def make_semantic_integrator_class(Base, api):
             fr = self.volume.set_frame(depth, kd.img, class_image=kd.semantic_img,
                                        instance_image=kd.semantic_instances_img if use_instances else None,
                                        depth_scale=scale, filter_shadow_points=flt)
-            return self._integrate_staged(kd, fr, use_instances)
+            self._integrate_staged(kd, fr, use_instances)
 
         def _integrate_stored(self, kd, slot):
             """The loop body on a stored frame (a light task): staged again from the frame store, then as on the
             images it was stored from; its instance image is associated when it was staged."""
             fr = self.volume.stage_stored(slot)
-            return self._integrate_staged(kd, fr, fr.instance_image is not None)
+            self._integrate_staged(kd, fr, fr.instance_image is not None)
 
         def _integrate_staged(self, kd, fr, use_instances):
             """Association (or carving), the instance remap and the integration on the staged frame `fr`."""
@@ -225,50 +217,48 @@ def make_semantic_integrator_class(Base, api):
                 fr.filtered_depth, fr.color, (fx, fy, cx, cy), Twc, class_image=fr.class_image,
                 object_image=object_image, max_depth=self.volumetric_integration_depth_trunc,
                 use_depths=bool(p["kVolumetricSemanticProbabilisticIntegrationUseDepth"]), filter_shadow_points=False)
-            self.last_integrated_id = kd.id
-            return True
+
+        def _integrate_tasks(self, tasks):
+            """The keyframes integrated, in order (one task per call: the grid plugins drain no backlog)."""
+            return [t.keyframe_data for t in tasks if self._integrate_keyframe(t.keyframe_data)]
 
         def _integrate_keyframe(self, kd):
-            """The reference loop body for one keyframe (:300-461): on the raw images, on the ones the base class
-            prepared on the host, or, for a light task, on its stored frame; on every rank's shard of a sharded grid.
-            With the frame store on, host-prepared frames of the frustum's size are staged like raw ones (no maps are
-            installed then, so set_frame only uploads and filters them) and stored."""
+            """The reference loop body for one keyframe (:300-461), on this grid or on every rank's shard: on the raw
+            images (the images for set_frame), on the ones the base class prepared on the host, or, for a light task,
+            on its stored frame.  With the frame store on, host-prepared frames of the frustum's size are staged like
+            raw ones (no maps are installed then, so set_frame only uploads and filters them) and stored.  Whether the
+            keyframe was integrated."""
+            pose = np.asarray(kd.pose, np.float64)
             if getattr(kd, keyframe_store.STORED_FLAG, False):
                 slot = self._stored_slot(kd)
-                if slot is None:
-                    return False
-                if self._shards is not None:
-                    self._shards.run("frame_stored", dict(id=kd.id, pose=np.asarray(kd.pose, np.float64), slot=slot))
-                    return True
-                return self._integrate_stored(kd, slot)
-            src, raw, prepared = kd, self._raw_frame(kd), None
+                if slot is not None:
+                    self._map_call("frame_stored", dict(id=kd.id, pose=pose, slot=slot))
+                return slot is not None
+            src, raw = kd, self._raw_frame(kd)
             if raw is None:
                 rect = self.estimate_depth_if_needed_and_rectify(kd)
                 color, depth = rect[0], rect[1]
                 if color is None or depth is None:
                     return False
-                kd = SimpleNamespace(id=kd.id, pose=kd.pose, img=color, depth=depth,
+                kd = SimpleNamespace(id=kd.id, img=color, depth=depth,
                                      semantic_img=rect[3] if len(rect) > 3 else None,
                                      semantic_instances_img=rect[4] if len(rect) > 4 else None)
                 if (self._store_frames > 0 and not self._gpu_rectify
                         and np.shape(depth) == (self.camera_frustrum.height, self.camera_frustrum.width)):
                     raw = (np.ascontiguousarray(depth, np.float32), None)
-                else:
-                    prepared = kd
-            if self._shards is not None:
-                slot = self._integrate_keyframe_sharded(kd, raw)
-            elif raw is not None:
-                self._integrate_raw(kd, *raw, self._uses_instances(kd.semantic_img, kd.semantic_instances_img))
-                slot = self.volume.last_stored_slot() if self._store_frames > 0 else -1
-            else:
-                self._integrate_prepared(prepared, prepared.img, prepared.depth, prepared.semantic_img,
-                                         prepared.semantic_instances_img)
-                slot = -1
+            is_raw = raw is not None
+            depth, scale = raw if is_raw else (kd.depth, None)
+            use = is_raw and self._uses_instances(kd.semantic_img, kd.semantic_instances_img)
+            meta = dict(id=kd.id, pose=pose, raw=is_raw, scale=scale, use_instances=use)
+            arrays = self._labels(kd.semantic_img, kd.semantic_instances_img, use, is_raw)
+            # the slot every rank stored the frame in, or -1: a rank whose store stopped (each rank maps its own)
+            # stored it in none, and a frame not in every rank's store cannot be replayed (_op_frame_stored)
+            slot = self._agreed(self._map_call("frame", meta, depth=depth, img=kd.img, **arrays))
             self._record_stored([src], [slot])
             return True
 
         def _labels(self, classes, instances, use_instances, raw):
-            """The label images of a broadcast keyframe: none for the point-average grid; int32 (what set_frame
+            """The label images of a keyframe for `_op_frame`: none for the point-average grid; int32 (what set_frame
             converts them to) on the raw path, where an empty image is no image."""
             if not self._LABELS:
                 return {}
@@ -279,25 +269,9 @@ def make_semantic_integrator_class(Base, api):
                 out[name] = img
             return out
 
-        def _integrate_keyframe_sharded(self, kd, raw):
-            """Rank 0's part of INTEGRATE: broadcast the keyframe (the images for set_frame when `raw`, else the
-            host-prepared ones); every rank then runs the loop body on its shard (`_op_frame`).  Returns the slot
-            every rank stored the frame in, or -1: a rank whose store stopped (each rank maps its own) stored it in
-            none, and a frame not in every rank's store cannot be replayed (`_op_frame_stored`)."""
-            meta = dict(id=kd.id, pose=np.asarray(kd.pose, np.float64), raw=raw is not None)
-            if raw is not None:
-                depth, scale = raw
-                use = self._uses_instances(kd.semantic_img, kd.semantic_instances_img)
-                meta.update(scale=scale, use_instances=use)
-                arrays = dict(depth=depth, img=kd.img,
-                              **self._labels(kd.semantic_img, kd.semantic_instances_img, use, True))
-            else:
-                arrays = dict(depth=kd.depth, img=kd.img,
-                              **self._labels(kd.semantic_img, kd.semantic_instances_img, False, False))
-            self._shards.run("frame", meta, arrays)
-            return self._shards.agreed()
-
         def _op_frame(self, meta, depth, img, classes=None, instances=None):
+            """One keyframe on this map (every rank's shard): the images for set_frame when meta["raw"], else the
+            host-prepared ones.  The frame-store slot of its frame, or -1."""
             kd = SimpleNamespace(id=meta["id"], pose=meta["pose"], img=img, semantic_img=classes,
                                  semantic_instances_img=instances)
             if meta["raw"]:
@@ -308,7 +282,8 @@ def make_semantic_integrator_class(Base, api):
             return -1
 
         def _op_frame_stored(self, meta):
-            """A light task on every rank: the stored frame of slot meta["slot"] with pose meta["pose"]."""
+            """A light task on this map (every rank's shard): the stored frame of slot meta["slot"] with pose
+            meta["pose"]."""
             self._integrate_stored(SimpleNamespace(id=meta["id"], pose=meta["pose"]), int(meta["slot"]))
 
         def _integrate_prepared(self, kd, color, depth, classes, instances):
@@ -340,8 +315,6 @@ def make_semantic_integrator_class(Base, api):
                 depth, color, (fx, fy, cx, cy), Twc, class_image=classes, object_image=object_image,
                 max_depth=self.volumetric_integration_depth_trunc,
                 use_depths=bool(p["kVolumetricSemanticProbabilisticIntegrationUseDepth"]), filter_shadow_points=flt)
-            self.last_integrated_id = kd.id
-            return True
 
         def _make_output(self, task_type):
             p = self.b200_parameters
@@ -379,77 +352,20 @@ def make_semantic_integrator_class(Base, api):
                 return self.volume.get_object_segments(**meta)
             return sharding.get_object_segments_sharded(self.volume, **meta)
 
-        def volume_integration(self, q_in, q_out, q_out_condition, q_management, viewer_queue,
-                               is_running, load_request_completed, load_request_condition,
-                               save_request_completed, save_request_condition,
-                               time_volumetric_integration):
-            t_start = time.perf_counter()
-            last_output = None
-            do_output = False
-            try:
-                if is_running.value == 1:
-                    task = None
-                    try:
-                        task = q_management.get_nowait()
-                    except Exception:
-                        pass
-                    if task is not None and task.task_type == TaskType.RESET:
-                        self._map_call("reset")
-                    self.last_input_task = q_in.get()  # blocking
-                    if self.last_input_task is None:
-                        is_running.value = 0
-                    else:
-                        ttype = self.last_input_task.task_type
-                        if ttype == TaskType.INTEGRATE:
-                            if self._integrate_keyframe(self.last_input_task.keyframe_data):
-                                do_output = True
-                                if self.last_output is not None:
-                                    dt = time.perf_counter() - self.last_output.timestamp
-                                    if dt < self.b200_parameters["kVolumetricIntegrationOutputTimeInterval"]:
-                                        do_output = False
-                        elif ttype == TaskType.SAVE:
-                            p = self.b200_parameters
-                            v = self._map_call("voxels", dict(
-                                min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
-                                min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"])))
-                            if len(v.points):
-                                write_ply_points(self.last_input_task.load_save_path, v.points, v.colors)
-                            self._save_map_state(self.last_input_task.load_save_path)
-                            last_output = api.VolumetricIntegrationOutput(ttype)
-                        elif ttype == TaskType.LOAD:
-                            self._load_map_state(self.last_input_task, load_request_completed, load_request_condition)
-                        elif ttype == TaskType.UPDATE_OUTPUT:
-                            do_output = True
-                        if do_output:
-                            last_output = self._make_output(ttype)
-                            self.last_output = last_output
-                        if is_running.value == 1 and last_output is not None:
-                            if last_output.task_type in (TaskType.INTEGRATE, TaskType.UPDATE_OUTPUT):
-                                with q_out_condition:
-                                    last_output.timestamp = time.perf_counter()
-                                    q_out.put(last_output)
-                                    q_out_condition.notify_all()
-                            elif last_output.task_type == TaskType.SAVE:
-                                with save_request_condition:
-                                    save_request_completed.value = 1
-                                    save_request_condition.notify_all()
-            except Exception as e:  # the reference logs and keeps the loop alive (:720-730)
-                printer = getattr(Base, "print", print)
-                printer(f"VolumetricIntegratorB200SemanticGrid: EXCEPTION: {e} !!!")
-                printer(traceback.format_exc())
-            time_volumetric_integration.value = time.perf_counter() - t_start
-
-        def _stop_volume_integrator_implementation(self):
-            self._stop_shards()
-            if getattr(self, "volume", None) is not None:
-                self.volume.close()
+        def _write_ply(self, path):
+            """SAVE's dense_map.ply: the voxels' points, when there are any."""
+            p = self.b200_parameters
+            v = self._map_call("voxels", dict(min_count=int(p["kVolumetricIntegrationVoxelGridMinCount"]),
+                                              min_confidence=float(p["kVolumetricIntegrationVoxelGridMinConfidence"])))
+            if len(v.points):
+                write_ply_points(path, v.points, v.colors)
 
     return VolumetricIntegratorB200SemanticGrid
 
 
 def make_voxel_grid_integrator_class(Base, api):
     """The point-average backend (`VolumetricIntegratorVoxelGrid`, pyslam/dense/volumetric_integrator_voxel_grid.py)
-    on the GPU compat grid.  Same task loop as the semantic class; the loop body is reference :232-300: optional
+    on the GPU compat grid.  Same task loop as the other plugins (B200PluginSetup); the loop body is reference :232-300: optional
     shadow filter -> depth2pointcloud -> world transform -> optional carve (with the UNFILTERED depth, :283-296) ->
     integrate, all of which `VoxelBlockGrid.carve` / `integrate_rgbd` do on the device."""
     SemanticCls = make_semantic_integrator_class(Base, api)
@@ -467,7 +383,7 @@ def make_voxel_grid_integrator_class(Base, api):
         def _integrate_raw(self, kd, depth, scale, use_instances):
             fr = self.volume.set_frame(depth, kd.img, depth_scale=scale, filter_shadow_points=bool(
                 self.b200_parameters["kVolumetricIntegrationVoxelGridShadowPointsFilter"]))
-            return self._integrate_staged(kd, fr, False)
+            self._integrate_staged(kd, fr, False)
 
         def _integrate_staged(self, kd, fr, use_instances):
             """Staged images: carve with the UNFILTERED depth, integrate the filtered one (:283-296)."""
@@ -480,8 +396,6 @@ def make_voxel_grid_integrator_class(Base, api):
             Twc = np.linalg.inv(np.asarray(kd.pose, np.float64).reshape(4, 4))
             self.volume.integrate_rgbd(fr.filtered_depth, fr.color, (fx, fy, cx, cy), Twc,
                                        max_depth=self.volumetric_integration_depth_trunc, filter_shadow_points=False)
-            self.last_integrated_id = kd.id
-            return True
 
         def _integrate_prepared(self, kd, color, depth, classes, instances):
             p = self.b200_parameters
@@ -495,8 +409,6 @@ def make_voxel_grid_integrator_class(Base, api):
             self.volume.integrate_rgbd(depth, color, (fx, fy, cx, cy), Twc,
                                        max_depth=self.volumetric_integration_depth_trunc,
                                        filter_shadow_points=bool(p["kVolumetricIntegrationVoxelGridShadowPointsFilter"]))
-            self.last_integrated_id = kd.id
-            return True
 
         def _make_output(self, task_type):
             v = self._map_call("voxels", dict(min_count=int(self.b200_parameters["kVolumetricIntegrationVoxelGridMinCount"])))
@@ -509,22 +421,8 @@ def make_voxel_grid_integrator_class(Base, api):
 
 def load_pyslam_semantic_plugin():
     """The semantic plugin built against the real pySLAM types (requires pySLAM on sys.path)."""
-    from types import SimpleNamespace
-
-    from pyslam.config_parameters import Parameters
-    from pyslam.dense import volumetric_integrator_base as B
-    from pyslam.io.dataset_types import DatasetEnvironmentType
-    from pyslam.slam import USE_CPP   # C++ core: raw depth reaches the integrator unscaled (base.py:29, 1008-1012)
-
-    api = SimpleNamespace(
-        USE_CPP=bool(USE_CPP),
-        VolumetricIntegrationTaskType=B.VolumetricIntegrationTaskType,
-        VolumetricIntegrationTask=B.VolumetricIntegrationTask,
-        VolumetricIntegrationOutput=B.VolumetricIntegrationOutput,
-        VolumetricIntegrationMesh=B.VolumetricIntegrationMesh,
-        VolumetricIntegrationPointCloud=B.VolumetricIntegrationPointCloud,
-        VolumetricIntegrationObjectList=B.VolumetricIntegrationObjectList,
-        DatasetEnvironmentType=DatasetEnvironmentType, Parameters=Parameters)
+    B, api = pyslam_api()
+    api.VolumetricIntegrationObjectList = B.VolumetricIntegrationObjectList
     try:   # colours of the viewer: semantic palette and per-object id colours (reference :535-575)
         from pyslam.semantics.semantic_mapping_shared import SemanticMappingShared
         from pyslam.utilities.colors import IdsColorTable

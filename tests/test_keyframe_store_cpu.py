@@ -29,10 +29,6 @@ class _StoreVolume:
             self.last.append(self.count if self.count < self.max_frames else -1)
             self.count += self.count < self.max_frames
 
-    def integrate(self, depth, color, K, pose, depth_scale=None):
-        self._store(1)
-        self.calls.append(("integrate", int(color[0, 0, 0])))
-
     def integrate_batch(self, depths, colors, K, poses, depth_scale=None):
         self._store(len(depths))
         self.calls.append(("integrate_batch", [int(c[0, 0, 0]) for c in colors]))
@@ -124,7 +120,7 @@ def test_store_off_passes_every_task_through(monkeypatch):
     assert [c[0] for c in integ.volume.calls] == ["integrate_batch", "integrate_batch"]
 
 
-def test_mixed_backlog_is_split_into_runs_in_order(monkeypatch):
+def test_mixed_backlog_is_split_into_runs_in_order_with_one_frame_batches(monkeypatch):
     tasks = [P.VolumetricIntegrationTask(_kd(i), INTEGRATE) for i in range(7)]
     stored = [True, True, False, True, False, False, True]
     tasks = [KS.light_task(t, SimpleNamespace(lookup=lambda kd: 0), INTEGRATE) if s else t
@@ -132,7 +128,8 @@ def test_mixed_backlog_is_split_into_runs_in_order(monkeypatch):
     runs = KS.split_runs(tasks)
     assert [(s, [t.keyframe_data.id for t in r]) for s, r in runs] == [
         (True, [0, 1]), (False, [2]), (True, [3]), (False, [4, 5]), (True, [6])]
-    # through the plugin: one integrate_stored call per stored run, today's path for the others, in queue order
+    # through the plugin: one integrate_stored call per stored run, integrate_batch for the others (a lone frame is a
+    # one-frame batch), in queue order
     integ = _plugin(monkeypatch, 8)
     for i in range(7):
         integ.add_keyframe_data(_kd(i))
@@ -145,7 +142,7 @@ def test_mixed_backlog_is_split_into_runs_in_order(monkeypatch):
         integ.add_keyframe_data(kd)
     integ.run_pending()
     calls = [(c[0], c[1]) for c in integ.volume.calls]
-    assert calls == [("integrate_stored", [0, 1]), ("integrate", 12), ("integrate_stored", [3]),
+    assert calls == [("integrate_stored", [0, 1]), ("integrate_batch", [12]), ("integrate_stored", [3]),
                      ("integrate_batch", [14, 15]), ("integrate_stored", [6])]
     assert np.array_equal(integ.volume.calls[0][2], np.stack([_kd(0).pose * 3, _kd(1).pose * 3]))
     assert integ.last_integrated_id == 6

@@ -174,9 +174,6 @@ class _StateVolume:
     def __init__(self, **kw):
         self.value = np.zeros(3)
 
-    def integrate(self, depth, color, K, pose, depth_scale=None):
-        self.value = self.value + 1
-
     def integrate_batch(self, depths, colors, K, poses, depth_scale=None):
         self.value = self.value + len(depths)
 

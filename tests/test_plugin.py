@@ -19,14 +19,11 @@ class _FakeVolume:
         self.calls = []
         self.closed = False
 
-    def integrate(self, depth, color, K, pose, depth_scale=None):
-        assert color.dtype == np.uint8 and (depth.dtype == np.float32 or (depth_scale and depth.dtype == np.uint16))
-        self.calls.append(("integrate", tuple(K), np.asarray(pose).copy(), color[0, 0].copy()))
-        self.last_depth, self.last_scale = depth, depth_scale
-
     def integrate_batch(self, depths, colors, K, poses, depth_scale=None):
         assert colors.dtype == np.uint8 and depths.shape[0] == colors.shape[0] == poses.shape[0]
-        self.calls.append(("integrate_batch", tuple(K), np.asarray(poses).copy(), int(depths.shape[0])))
+        assert depths.dtype == np.float32 or (depth_scale and depths.dtype == np.uint16)
+        self.calls.append(("integrate_batch", tuple(K), np.asarray(poses).copy(), int(depths.shape[0]),
+                           colors[0, 0, 0].copy()))
         self.last_depth, self.last_scale = depths, depth_scale
 
     def reset(self):
@@ -52,7 +49,7 @@ def _camera(cfg):
                            height=cfg.height, D=None)
 
 
-def test_adapter_task_flow_with_fake_volume(monkeypatch, tmp_path):
+def test_adapter_task_flow_with_fake_volume_one_frame_batches(monkeypatch, tmp_path):
     monkeypatch.setattr(I, "B200TsdfVolume", _FakeVolume)
     Cls = P.standalone_integrator_class()
     cfg = S.CONFIGS["T0"]
@@ -64,15 +61,17 @@ def test_adapter_task_flow_with_fake_volume(monkeypatch, tmp_path):
     kd = P.VolumetricIntegrationKeyframeData(id=7, pose=T, img=bgr, depth=(d * 1000).astype(np.uint16))
     integ.add_keyframe_data(kd)
     integ.step()
-    name, K, pose, px = integ.volume.calls[0]
-    assert name == "integrate" and K == (cfg.fx, cfg.fy, cfg.cx, cfg.cy) and np.array_equal(pose, T)
+    name, K, poses, n, px = integ.volume.calls[0]
+    assert name == "integrate_batch" and n == 1 and K == (cfg.fx, cfg.fy, cfg.cx, cfg.cy)
+    assert np.array_equal(poses[0], T)
     assert np.array_equal(px, c[0, 0])  # BGR -> RGB before the volume sees it (base.py:1054)
     out = integ.pop_output()             # first integrate always produces an output
     assert out.id == 7 and out.mesh.triangles.shape == (1, 3) and out.point_cloud is None
     # a second frame inside the output interval integrates but does not extract
     integ.add_keyframe_data(kd)
     integ.step()
-    assert integ.pop_output() is None and integ.volume.calls[-1][0] == "integrate"
+    assert integ.pop_output() is None and integ.volume.calls[-1][0] == "integrate_batch"
+    assert integ.volume.calls[-1][3] == 1
     # UPDATE_OUTPUT forces an extraction
     integ.add_update_output_task()
     integ.step()
@@ -91,7 +90,7 @@ def test_adapter_task_flow_with_fake_volume(monkeypatch, tmp_path):
     assert ("reset",) in integ.volume.calls
     # exceptions inside a task are logged and do not kill the loop (tsdf.py:303-307)
     integ.add_keyframe_data(P.VolumetricIntegrationKeyframeData(id=9, pose=T, img=bgr[:3], depth=d))
-    monkeypatch.setattr(_FakeVolume, "integrate", lambda *a, **k: (_ for _ in ()).throw(RuntimeError("x")))
+    monkeypatch.setattr(_FakeVolume, "integrate_batch", lambda *a, **k: (_ for _ in ()).throw(RuntimeError("x")))
     integ.step()
     assert integ.is_running.value == 1
     integ.add_task(None)
@@ -101,7 +100,7 @@ def test_adapter_task_flow_with_fake_volume(monkeypatch, tmp_path):
     assert integ.volume.closed
 
 
-def test_backlog_is_drained_into_one_fused_batch(monkeypatch):
+def test_backlog_is_drained_into_one_fused_batch_lone_frames_into_one_frame_batches(monkeypatch):
     """rebuild(map) re-enqueues every keyframe (base.py:1242-1318): consecutive INTEGRATE tasks already in the queue
     go to ONE integrate_batch call (bounded); a task of another type met while draining is handled by the next
     call, in order; output cadence and RESET semantics are unchanged."""
@@ -121,7 +120,7 @@ def test_backlog_is_drained_into_one_fused_batch(monkeypatch):
     integ.add_update_output_task()
     integ.add_keyframe_data(P.VolumetricIntegrationKeyframeData(id=6, pose=T, img=bgr, depth=d))
     integ.step()                                   # frames 0..3 (bounded by MaxBatch) in one call
-    name, K, P4, n = integ.volume.calls[0]
+    name, K, P4, n, _ = integ.volume.calls[0]
     assert name == "integrate_batch" and n == 4 and np.array_equal(P4, np.stack(poses[:4]))
     assert integ.pop_output().id == 3              # the first output carries the last integrated id
     integ.step()                                   # frames 4, 5; the UPDATE_OUTPUT task is met and deferred
@@ -131,13 +130,15 @@ def test_backlog_is_drained_into_one_fused_batch(monkeypatch):
     assert integ.pop_output().task_type == P.VolumetricIntegrationTaskType.UPDATE_OUTPUT
     assert [cl[0] for cl in integ.volume.calls if cl[0].startswith("integrate")] == ["integrate_batch"] * 2
     integ.step()                                   # frame 6 alone: the single-frame call
-    assert integ.volume.calls[-1][0] == "integrate" and integ.integrated_frames == 7
+    assert integ.volume.calls[-1][0] == "integrate_batch" and integ.volume.calls[-1][3] == 1
+    assert integ.integrated_frames == 7
     # MaxBatch = 1 restores one task per call
     integ2 = Cls(_camera(cfg), P.DatasetEnvironmentType.INDOOR, None, "B200_TSDF", kVolumetricIntegrationB200MaxBatch=1)
     for i in range(3):
         integ2.add_keyframe_data(P.VolumetricIntegrationKeyframeData(id=i, pose=T, img=bgr, depth=d))
     integ2.run_pending()
-    assert [cl[0] for cl in integ2.volume.calls if cl[0].startswith("integrate")] == ["integrate"] * 3
+    assert [(cl[0], cl[3]) for cl in integ2.volume.calls
+            if cl[0].startswith("integrate")] == [("integrate_batch", 1)] * 3
 
 
 def test_outdoor_depth_trunc_and_point_cloud_mode(monkeypatch):
@@ -186,7 +187,7 @@ def test_adapter_end_to_end_on_gpu(tmp_path):
     integ.quit()
 
 
-def test_adapter_gpu_rectification_hands_raw_frames_to_the_volume(monkeypatch):
+def test_adapter_gpu_rectification_hands_raw_frames_to_the_volume_as_one_frame_batches(monkeypatch):
     """With calibration maps the adapter installs them on the volume (swap_rb=True) and passes the RAW BGR
     image and float32 depth; with the option off it goes through the base class's CPU remap."""
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", "remap_T0.npz"))
@@ -204,15 +205,15 @@ def test_adapter_gpu_rectification_hands_raw_frames_to_the_volume(monkeypatch):
     kd = P.VolumetricIntegrationKeyframeData(id=1, pose=g["Tcw"], img=g["bgr"], depth=g["depth"])
     integ.add_keyframe_data(kd)
     integ.step()
-    call = [c for c in integ.volume.calls if c[0] == "integrate"][-1]
-    assert np.array_equal(call[3], g["bgr"][0, 0])   # raw BGR, untouched
+    call = [c for c in integ.volume.calls if c[0] == "integrate_batch" and c[3] == 1][-1]
+    assert np.array_equal(call[4], g["bgr"][0, 0])   # raw BGR, untouched
     # raw uint16 depth: python core -> depth.astype(float32) on the host; C++ core (USE_CPP) -> the uint16 image goes
     # to the GPU with depth_scale = camera.depth_factor (base.py:1007-1015 multiplies by self.camera.depth_factor)
     raw16 = np.round(g["depth"] * 5000.0).astype(np.uint16)
     integ.add_keyframe_data(P.VolumetricIntegrationKeyframeData(id=2, pose=g["Tcw"], img=g["bgr"], depth=raw16))
     integ.step()
-    assert integ.volume.last_depth.dtype == np.float32 and integ.volume.last_scale is None
-    assert np.array_equal(integ.volume.last_depth, raw16.astype(np.float32))
+    assert integ.volume.last_depth[0].dtype == np.float32 and integ.volume.last_scale is None
+    assert np.array_equal(integ.volume.last_depth[0], raw16.astype(np.float32))
     api_cpp = SimpleNamespace(**{**vars(P.API), "USE_CPP": True})
     ClsCpp = I.make_integrator_class(P.StandaloneIntegratorBase, api_cpp)
     cam = _camera(cfg)
@@ -220,7 +221,7 @@ def test_adapter_gpu_rectification_hands_raw_frames_to_the_volume(monkeypatch):
     integ_cpp = ClsCpp(cam, P.DatasetEnvironmentType.INDOOR, None, "B200_TSDF", calib_maps=(g["map1"], g["map2"]))
     integ_cpp.add_keyframe_data(P.VolumetricIntegrationKeyframeData(id=3, pose=g["Tcw"], img=g["bgr"], depth=raw16))
     integ_cpp.step()
-    assert integ_cpp.volume.last_depth.dtype == np.uint16 and integ_cpp.volume.last_scale == np.float32(1.0 / 5000.0)
+    assert integ_cpp.volume.last_depth[0].dtype == np.uint16 and integ_cpp.volume.last_scale == np.float32(1.0 / 5000.0)
     cv2 = pytest.importorskip("cv2")
     del cv2
     integ2 = Cls(_camera(cfg), P.DatasetEnvironmentType.INDOOR, None, "B200_TSDF",
@@ -228,8 +229,8 @@ def test_adapter_gpu_rectification_hands_raw_frames_to_the_volume(monkeypatch):
     assert not any(c[0] == "rect" for c in integ2.volume.calls)
     integ2.add_keyframe_data(kd)
     integ2.step()
-    call = [c for c in integ2.volume.calls if c[0] == "integrate"][-1]
-    assert np.array_equal(call[3], g["rgb_u"][0, 0])  # CPU-rectified RGB
+    call = [c for c in integ2.volume.calls if c[0] == "integrate_batch" and c[3] == 1][-1]
+    assert np.array_equal(call[4], g["rgb_u"][0, 0])  # CPU-rectified RGB
 
 
 @pytest.mark.gpu

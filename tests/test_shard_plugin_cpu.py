@@ -41,10 +41,6 @@ class _RecVolume:
         self.calls.append(call)
         self._log()
 
-    def integrate(self, depth, color, K, pose, depth_scale=None):
-        # the single map's one-frame call is the batch entry point with one frame (B200TsdfVolume.integrate)
-        self.integrate_batch(np.asarray(depth)[None], np.asarray(color)[None], K, np.asarray(pose)[None], depth_scale)
-
     def integrate_batch(self, depths, colors, K, poses, depth_scale=None):
         poses = np.asarray(poses, np.float64).reshape(-1, 4, 4)
         if self.rank == 1 and poses[0, 0, 3] == 99.0:
